@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — samples/sec of one training step of the hot path on B200.
+"""bench.py — samples/sec of one training step of the hot path on H100.
 
 Default workload = BASELINE.json configs[1]: DeepFM Criteo-shape, 39 categorical fields x 25,641
 rows (~1.0 M rows), emb_dim 16, MLP 300-300-300, batch 4096 per GPU (weak scaling).
@@ -13,10 +13,16 @@ interaction / MLP forward -> BCE -> backward (dense-gradient scatter-add, GEMM d
 clip_grad_norm_(10) -> Adam over every parameter.
 
     python bench.py --gpus N --steps K --warmup W          # this repo's CUDA path
-    python bench.py --impl reference ...                   # the UNMODIFIED reference (baseline/_ref) on host CPU
+    python bench.py --impl reference ...                   # the UNMODIFIED reference (oracle/_ref) on host CPU
     python bench.py --impl reference-gpu ...               # the unmodified reference, eager, on cuda:0
 
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for every field.
+`--dump-outputs DIR` also writes what the timed step computed in its last timed step (its loss and the
+parameters it left behind, large tables as a fixed seeded row sample) as DIR/<name>.npy, so that two builds
+can be compared output for output on identical inputs.  Gradient scatters and bias-gradient sums use float
+atomics, whose order varies from run to run; Adam amplifies those last-bit differences step by step, so
+compare short runs (two runs of `--steps 5 --warmup 2` of the same build agree to ~3e-5 relative, while after
+200 steps they have drifted apart).
 """
 import argparse
 import json
@@ -64,7 +70,9 @@ def parse():
     ap.add_argument("--steps-only", action="store_true", help="skip the per-kernel / stress / CPU legs (profiling)")
     ap.add_argument("--precision", default="tf32x3", choices=["fp32", "tf32x3", "tf32", "bf16"],
                     help="arithmetic of the dense GEMMs: fp32 FFMA, 3xTF32 (fp32-class, the parity mode), 1xTF32, or "
-                         "bf16 operands with fp32 accumulation (BASELINE configs[1]) on tcgen05")
+                         "bf16 operands with fp32 accumulation (BASELINE configs[1]) on wgmma")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last timed step's loss and parameters as DIR/<name>.npy")
     a = ap.parse_args()
     if a.batch <= 0:
         a.batch = DEFAULT_BATCH[a.workload] if a.workload != "dlrm" else max(DLRM_GLOBAL_BATCH // max(a.gpus, 1), 1)
@@ -130,7 +138,7 @@ def workload_config(args, n_gpus):
     width = DIM + (1 if w in ("deepfm", "xdeepfm") else 0)          # + the D=1 LogisticRegression tables
     arena_mb = rows * width * 4 / 1e6 / (1 if n_gpus == 1 or args.dp_only else n_gpus)
     return {"workload": name, "global_batch": args.batch * n_gpus, "per_gpu_batch": args.batch, "parallelism": par,
-            "cache": "working set (4 fp32 arenas x %.0f MB per GPU: params, grads, Adam m/v) exceeds the 126 MB L2; "
+            "cache": "working set (4 fp32 arenas x %.0f MB per GPU: params, grads, Adam m/v) exceeds the 50 MB L2; "
                      "%d distinct index batches are rotated" % (arena_mb, args.nbatches)}
 
 
@@ -234,9 +242,9 @@ class ClockSampler(object):
 
 
 # ------------------------------------------------------------------------------------------
-# Reference arms: the UNMODIFIED reference from baseline/_ref (its own model class, its own
+# Reference arms: the UNMODIFIED reference from oracle/_ref (its own model class, its own
 # BaseModel.train_step), on the host CPU or eager on cuda:0.  Falls back to the oracle port when
-# baseline/_ref is absent.
+# oracle/_ref is absent.
 # ------------------------------------------------------------------------------------------
 def build_reference_model(args, gpu):
     """(model, feature_map) of the reference's own class for the workload, from a synthetic FeatureMap."""
@@ -290,7 +298,7 @@ def cpu_reference_run(args, steps, warmup, seconds=None, threads=None):
         step = model.train_step
         batches = reference_batches(fm, make_batches(4, batch, specs=make_specs(args)))
         kind = "reference"
-    except ImportError:       # no baseline/_ref on this machine: the oracle restatement (same ATen ops)
+    except ImportError:       # no oracle/_ref on this machine: the oracle restatement (same ATen ops)
         import torch
         from oracle import fuxictr_oracle as O
         from fuxictr_b200 import zoo
@@ -348,7 +356,7 @@ def cpu_reference_run(args, steps, warmup, seconds=None, threads=None):
 
 
 def cpu_baseline_entry(r, args, how):
-    what = ("the unmodified reference (baseline/_ref: model_zoo class + BaseModel.train_step)" if r["kind"] == "reference"
+    what = ("the unmodified reference (oracle/_ref: model_zoo class + BaseModel.train_step)" if r["kind"] == "reference"
             else "oracle port of the reference's ATen path")
     return {"value": r["value"], "unit": "samples/s", "cores": r["cores"], "kind": r["kind"],
             "sample": "%d train steps of batch %d %s on %d of %d host threads (fastest of the sweep %s); %s"
@@ -373,7 +381,7 @@ def run_reference_arm(args):
 
 
 def reference_gpu_eager(args, steps=30, warmup=5):
-    """The unmodified reference on the SAME B200, eager CUDA, no patching: the GPU-vs-GPU bar
+    """The unmodified reference on the SAME GPU, eager CUDA, no patching: the GPU-vs-GPU bar
     (SURVEY.md 8d).  Reported with the `loss.item()` sync of train_epoch (rank_model.py:342) and without."""
     from fuxictr_b200 import patch
     patch.disable()
@@ -411,7 +419,7 @@ def run_reference_gpu_arm(args):
 
 
 # ------------------------------------------------------------------------------------------
-# B200 arm
+# b200 arm: this repository's kernels
 # ------------------------------------------------------------------------------------------
 def time_kernel(fn, reps, stream_sync=None):
     """Average device duration (ms) of `fn` over `reps` back-to-back launches.  The launches are
@@ -529,7 +537,7 @@ def kernel_rooflines(model, fm, dev_batch, peaks, args, with_gather=True):
     if mode != "fp32":
         x3 = mode == "tf32x3"
         # dense TF32 = half the measured bf16 rate; bf16 operands are measured against the bf16 rate itself
-        tf32_peak = peaks.get("bf16_tflops", 1590.0) / (1.0 if mode == "bf16" else 2.0)
+        tf32_peak = peaks.get("bf16_tflops", 989.0) / (1.0 if mode == "bf16" else 2.0)
         # the largest dense contraction of the workload: (in, out) widths of that Linear
         K_, N_ = {"deepfm": (nf * DIM, HIDDEN[0]), "dlrm": (DLRM_TOP[0], DLRM_TOP[1]),
                   "dcnv2": (nf * DIM, nf * DIM), "din": (fm.sum_emb_out_dim(), DIN_HIDDEN[0]),
@@ -593,9 +601,37 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as fd:
             p = json.load(fd)
-        return {"hbm_gbs": float(p["hbm_gbs"]), "bf16_tflops": float(p.get("bf16_tflops", 1590.0)),
+        return {"hbm_gbs": float(p["hbm_gbs"]), "bf16_tflops": float(p.get("bf16_tflops", 989.0)),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet (dense, 700 W), not measured"}
+
+
+DUMP_ROW_SAMPLE = 4096          # rows kept of a parameter with more rows than this (fixed seed)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(path, model, loss_dev):
+    """DIR/<name>.npy of what the timed path computed in its last step: `loss` (float64, shape (1,)) and every
+    parameter of the model as that step left it (`param.<state_dict key>`, float32).  A parameter with more
+    than DUMP_ROW_SAMPLE rows is written as the rows picked by a fixed-seed draw (the same rows in every run),
+    so that the whole dump stays within DUMP_MAX_BYTES."""
+    import numpy as np
+    import torch
+    out = OrderedDict()
+    out["loss"] = loss_dev.detach().double().reshape(1).cpu().numpy()
+    gen = torch.Generator().manual_seed(0)
+    for name, p in model.state_dict().items():
+        t = p.detach()
+        if t.dim() >= 1 and t.shape[0] > DUMP_ROW_SAMPLE:
+            rows = torch.randint(0, t.shape[0], (DUMP_ROW_SAMPLE,), generator=gen)
+            t = t[rows.to(t.device)]
+        out["param." + name] = t.float().cpu().numpy()
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_MAX_BYTES))
+    os.makedirs(path, exist_ok=True)
+    for name, arr in out.items():
+        np.save(os.path.join(path, name + ".npy"), arr)
 
 
 def build_model(args, local, world):
@@ -742,6 +778,8 @@ def run_b200_arm(args):
         sampler.wait_first()
     t_w0 = time.time()
     ms_total = timed(False, args.steps, warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, pipe.loss_dev)
     ms_e2e = timed(True, args.steps, warmup)
     t_w1 = time.time()
     windows, clock_note = [(t_w0, t_w1)], "rows sampled inside the two timed regions"
@@ -797,7 +835,7 @@ def run_b200_arm(args):
         flops = sum(2.0 * v["shape_MNK"][0] * v["shape_MNK"][1] * v["shape_MNK"][2] for v in gem)
         ms = sum(v["ms"] for v in gem)
         passes = gem[0]["passes"] if gem else 1
-        roofline = {"kernel": "gemm_tf32_kernel (first MLP layer: forward + dgrad + wgrad launches)", "bound": "tensor",
+        roofline = {"kernel": "gemm_tc_kernel (first MLP layer: forward + dgrad + wgrad launches)", "bound": "tensor",
                     "achieved": flops / ms / 1e9, "peak": tf32_peak, "unit": "TFLOP/s", "frac": flops / ms / 1e9 / tf32_peak,
                     "frac_counting_3xTF32_passes": flops * passes / ms / 1e9 / tf32_peak, "passes": passes,
                     "algorithmic_flops": flops, "traffic": None,
@@ -810,22 +848,13 @@ def run_b200_arm(args):
                     "algorithmic_bytes": k["algorithmic_bytes"] if k else None, "traffic": None,
                     "peak_source": peaks["source"]}
     roofline["share_of_step"] = share
-    # dram__bytes_read+write of one `ncu --set full` capture of the same command, N = 1 only (a shard of
-    # the arena is a different launch: never reuse the N = 1 figure there)
-    tpath = os.path.join(ROOT, "profiles", "r2_step_kernels_traffic.json")
-    if world == 1 and args.workload == "deepfm" and os.path.exists(tpath):
-        with open(tpath) as fd:
-            cap = json.load(fd).get({"adam_step": "adam_kernel", "gemm": "gemm_tf32_kernel"}.get(dom, dom))
-        if cap:
-            roofline["traffic"] = (cap["dram_read_MB"] + cap["dram_write_MB"]) * 1e6
-            roofline["traffic_source"] = "profiles/r2_step_kernels_traffic.json (ncu --set full, per launch)"
     line = {"metric": METRICS[args.workload], "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps,
             "warmup": warmup, "ms_per_step": step_ms, "higher_is_better": True,
             "scaling": "weak" if args.workload == "deepfm" else "strong",
             "vs_baseline": None,
             "dtype": {"fp32": "f32", "tf32x3": "f32 (3xTF32 tensor-core GEMMs, fp32 everything else)",
                       "tf32": "tf32 GEMMs, f32 elsewhere",
-                      "bf16": "bf16 GEMM operands (fp32 accumulation in TMEM), f32 tables / optimizer"}[args.precision],
+                      "bf16": "bf16 GEMM operands (fp32 accumulation), f32 tables / optimizer"}[args.precision],
             # `config` names the WORKLOAD only (both arms print the same dict); how this arm computes it:
             "data": "synthetic", "config": workload_config(args, world),
             "matmul": args.precision,

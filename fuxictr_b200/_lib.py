@@ -68,8 +68,8 @@ class b2_gemm_desc(ctypes.Structure):
 
 class b2_gemm_plan(ctypes.Structure):
     """struct b2_gemm_plan of include/fuxictr_b200.h."""
-    _fields_ = [(k, c_int32) for k in ("bn", "splits", "stages", "nacc", "nmain", "tmem_cols", "grid", "threads",
-                                       "tiles_m", "tiles_n", "tma_store", "passes", "kb_per_split", "pad_")] + \
+    _fields_ = [(k, c_int32) for k in ("bn", "splits", "stages", "cstages", "grid", "threads", "tiles_m", "tiles_n",
+                                       "passes", "kb_per_split")] + \
                [("smem_bytes", c_int64)]
 
 
@@ -173,7 +173,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             "fuxictr_b200: %s is missing. Build it with `python -m fuxictr_b200.build` "
-            "(needs nvcc); there is no CPU fallback for the B200 hot path." % LIB_PATH)
+            "(needs nvcc); there is no CPU fallback for the H100 hot path." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError here == header/library mismatch: fail loudly

@@ -1,6 +1,6 @@
 """Flat HBM arenas for parameters, gradients and Adam state + the fused dense optimizer.
 
-B200-first memory layout: every trainable tensor of a model is a 16-byte-aligned slice
+H100-first memory layout: every trainable tensor of a model is a 16-byte-aligned slice
 of ONE fp32 arena `P`; its gradient is the same slice of arena `G`; Adam's moments are
 the same slices of `M` and `V`.  The Parameter *objects* are kept (the reference builds
 its optimizer and state_dict around them, rank_model.py:92, 417-433) — only their

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a C-ABI library (libfuxictr_b200.so) with plain nvcc.
+"""In-tree build of the sm_90a (H100) C-ABI library (libfuxictr_b200.so) with plain nvcc.
 
 The library has no torch / Python dependency: it is what a C, Go or Python (ctypes)
 host binds.  `python -m fuxictr_b200.build` or `__graft_entry__.build()` runs this.
@@ -14,21 +14,19 @@ CSRC = os.path.join(HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 LIB = os.path.join(HERE, "libfuxictr_b200.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
 ]
-if os.environ.get("B2_BUILD_PROBE", "0") != "0":     # timing probes of gemm_tc.cu (tools/gemm_probe.py, gemm_trace.py)
-    NVCC_FLAGS.append("-DB2_GEMM_PROBE")
 
 
 def _nvcc():
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found; cannot build the sm_100a library")
+    raise RuntimeError("nvcc not found; cannot build the sm_90a library")
 
 
 def _digest():
@@ -43,7 +41,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu for sm_100a and link libfuxictr_b200.so next to this file."""
+    """Compile every .cu for sm_90a and link libfuxictr_b200.so next to this file."""
     stamp = os.path.join(HERE, "build", "stamp")
     digest = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(stamp):

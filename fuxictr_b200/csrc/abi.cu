@@ -11,7 +11,7 @@ int b2_fail(int code, const char* fmt, ...) {
   return code;
 }
 
-extern "C" B2_API const char* b2_version(void) { return "fuxictr_b200 0.1.0 (sm_100a)"; }
+extern "C" B2_API const char* b2_version(void) { return "fuxictr_b200 0.1.0 (sm_90a)"; }
 
 extern "C" B2_API const char* b2_last_error(void) { return b2_tls_error; }
 

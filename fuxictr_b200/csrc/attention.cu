@@ -1,4 +1,4 @@
-// attention.cu — Dice activation and the non-GEMM parts of DIN target attention, sm_100a.
+// attention.cu — Dice activation and the non-GEMM parts of DIN target attention, sm_90a.
 //
 // Reference semantics (reczoo/FuxiCTR v2.3.10):
 //   Dice.forward           fuxictr/pytorch/layers/activations.py:37,49-50

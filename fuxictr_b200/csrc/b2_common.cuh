@@ -1,4 +1,4 @@
-// b2_common.cuh — shared device/host helpers for the sm_100a kernels.
+// b2_common.cuh — shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -8,7 +8,7 @@
 
 #include "../../include/fuxictr_b200.h"
 
-#define B2_NUM_SMS 148  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+#define B2_NUM_SMS 132  // H100 SXM: 132 SMs; grids are sized in multiples of this
 
 // ---- per-thread last-error string (no C++ exceptions cross the ABI) --------
 extern thread_local char b2_tls_error[512];
@@ -31,7 +31,7 @@ static inline int64_t b2_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b
 // ---- programmatic dependent launch (on by default; B2_PDL=0 launches plainly) --------------------
 // The step is a chain of ~45 short kernels; with PDL a kernel's CTAs are scheduled while its predecessor
 // drains and sit at griddepcontrol.wait (which returns only when the predecessor has COMPLETED and its
-// writes are visible), so the launch latency — and, for the GEMM, the barrier/TMEM/tensormap prologue —
+// writes are visible), so the launch latency — and, for the GEMM, the barrier/tensormap prologue —
 // overlaps the predecessor's tail.  Captured into CUDA graphs as programmatic dependency edges.
 #include <stdlib.h>
 static inline bool b2_pdl_on() {
@@ -112,7 +112,7 @@ __device__ __forceinline__ void b2_red_add(float* p, float x) {
 }
 
 // 3xTF32 split: small(x) = rna_tf32(x - big(x)), big(x) = x with the 13 low mantissa bits cleared (what
-// kind::tf32 reads from a raw fp32 operand).  x - big(x) is exact; rounding it to a tf32-representable
+// the GEMM feeds the tensor core as the tf32 operand).  x - big(x) is exact; rounding it to a tf32-representable
 // value HERE (round-to-nearest) makes the hardware truncation of the small operand a no-op, so the
 // residual of the split is unbiased instead of always toward zero.
 __device__ __forceinline__ float b2_tf32_small(float v) {

@@ -1,5 +1,5 @@
 // cin.cu — one Compressed-Interaction-Network layer without ever materialising the
-// (B, F*H, D) Hadamard tensor, sm_100a.
+// (B, F*H, D) Hadamard tensor, sm_90a.
 //
 // Reference (reczoo/FuxiCTR v2.3.10), fuxictr/pytorch/layers/interactions/compressed_interaction_net.py:70-73:
 //     hadamard = einsum("bhd,bmd->bhmd", X_0, X_i).view(B, F*H, D)

@@ -1,5 +1,5 @@
 // dense.cu — fp32 dense layer (parity path), elementwise backward helpers, fused
-// logit+BCE, and the dense clip+Adam step, sm_100a.
+// logit+BCE, and the dense clip+Adam step, sm_90a.
 //
 // Reference semantics (reczoo/FuxiCTR v2.3.10):
 //   MLP_Block                fuxictr/pytorch/layers/blocks/mlp_block.py:64-96   (nn.Linear + act)
@@ -8,7 +8,7 @@
 //   BaseModel.train_step     fuxictr/pytorch/models/rank_model.py:316-322       (clip + Adam)
 //
 // The fp32 GEMM here is the 1e-5-parity path: plain FFMA with fp32 accumulate, the
-// same arithmetic class as the reference's ATen addmm.  The tensor-core (tcgen05)
+// same arithmetic class as the reference's ATen addmm.  The tensor-core (wgmma)
 // GEMM for the bf16 throughput path lives in gemm_tc.cu.
 #include "b2_common.cuh"
 #include "adam_common.cuh"
@@ -347,7 +347,7 @@ extern "C" B2_API int b2_logit_bce_fwd(const float* t0, const float* t1, const f
 
 // ---------------------------------------------------------------------------------
 // Dense clip_grad_norm_ + Adam over a flat fp32 arena (rank_model.py:321-322).
-// HBM-bound streaming: float4, grid = whole waves of 148 SMs.
+// HBM-bound streaming: float4, grid = whole waves of B2_NUM_SMS (132) SMs.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {

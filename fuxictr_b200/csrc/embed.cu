@@ -1,5 +1,5 @@
 // embed.cu — fused multi-field embedding gather / scatter-add and the D=1
-// LogisticRegression gather-reduce, sm_100a.
+// LogisticRegression gather-reduce, sm_90a.
 //
 // Reference semantics (reczoo/FuxiCTR v2.3.10):
 //   FeatureEmbeddingDict.forward   fuxictr/pytorch/layers/embeddings/feature_embedding.py:261-297
@@ -24,8 +24,8 @@ __device__ __forceinline__ typename VecT<VEC>::type b2_ld_row(const typename Vec
   return __ldg(p);
 }
 // mode 0: plain read-only load; 1: L1::no_allocate (one-touch); 2: read-only load with the L2::64B
-// prefetch-size hint — a D=16 row is exactly one 64-byte sector pair.  Measured: no gain in this kernel
-// (3773 vs 3755 GB/s, profiles/r1_gather_ceiling.md), kept selectable through B2_GATHER_STREAM=2.
+// prefetch-size hint — a D=16 row is exactly one 64-byte sector pair.  Not the default (its gain on the
+// H100 is not measured), kept selectable through B2_GATHER_STREAM=2.
 template <>
 __device__ __forceinline__ float4 b2_ld_row<4>(const float4* p, int mode) {
   if (mode == 2) {

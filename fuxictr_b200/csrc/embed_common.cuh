@@ -124,7 +124,7 @@ __host__ __device__ static inline size_t pack_smem_bytes(int nfields) {
   return sizeof(b2_field) * nfields + sizeof(int32_t) * (nfields + 1);
 }
 
-// Grid sized in whole waves of 148 SMs x 8 resident 256-thread CTAs, capped by the work.
+// Grid sized in whole waves of B2_NUM_SMS (132) SMs x 8 resident 256-thread CTAs, capped by the work.
 static inline int grid_for(int64_t nthreads_needed, int block) {
   int64_t blocks = b2_ceil_div(nthreads_needed, block);
   const int64_t wave = (int64_t) B2_NUM_SMS * 8;

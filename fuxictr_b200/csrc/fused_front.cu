@@ -1,4 +1,4 @@
-// fused_front.cu — the whole "sparse front" of an FM-style model in one launch each way, sm_100a.
+// fused_front.cu — the whole "sparse front" of an FM-style model in one launch each way, sm_90a.
 //
 // Forward  (b2_front_fwd): for every sample, in ONE kernel
 //   * the multi-field embedding gather, written as the stacked (B, F, D) tensor

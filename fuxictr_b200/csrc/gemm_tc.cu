@@ -1,37 +1,33 @@
-// gemm_tc.cu — TMA-fed tcgen05 (5th-gen tensor core) GEMM with TMEM accumulator and a
-// fused epilogue, sm_100a.  The dense contraction behind MLP_Block
+// gemm_tc.cu — TMA-fed wgmma (Hopper tensor core) GEMM with register accumulators and a fused
+// epilogue, sm_90a.  The dense contraction behind MLP_Block
 // (fuxictr/pytorch/layers/blocks/mlp_block.py:74-85), CrossNetV2's d x d Linear
 // (fuxictr/pytorch/layers/interactions/cross_net.py:126-129) and CIN's 1x1 Conv1d
 // (fuxictr/pytorch/layers/interactions/compressed_interaction_net.py:72).
 //
 //   C[m, n] = epi( sum_k A(m, k) * B(n, k) )
 // Each operand is either K-major (memory (rows, K), K contiguous) or MN-major (memory (K, rows),
-// rows contiguous): the tensor core reads both through its shared-memory matrix descriptor, so
-// the dgrad (dX = dZ W) and wgrad (dW = dZ^T X) contractions of a Linear layer consume W, dZ and X
-// exactly as they lie in memory — no transpose pass.
+// rows contiguous).  TMA copies both exactly as they lie in memory, so the dgrad (dX = dZ W) and wgrad
+// (dW = dZ^T X) contractions of a Linear layer need no transpose pass in HBM.
 //
-// Arithmetic: tcgen05.mma kind::tf32 reads the fp32 operands straight from shared memory
-// (the tensor core ignores the low 13 mantissa bits) and accumulates in fp32 in TMEM.
-//   precision 1 ("tf32"):   one pass, ~1e-3 relative — at least the bf16 the config names.
+// Arithmetic: wgmma .tf32 on fp32 operands, fp32 accumulation in registers.
+//   precision 1 ("tf32"):   one pass on big(x) = x with the 13 low mantissa bits cleared, ~1e-3 relative.
 //   precision 3 ("tf32x3"): error-compensated 3xTF32: with x = big(x) + small(x),
 //        A.B ~= A_big.B_big + A_big.B_small + A_small.B_big
-//     where big() is the hardware truncation itself and small = rna_tf32(x - big(x)) — fp32-class accuracy
-//     (the 1e-5 parity bar) on tensor cores.  The small tiles are made in shared memory by the helper
-//     warps (B2_GEMM_X3_INLINE: the GEMM then reads only the fp32 operands) or loaded from HBM (a_small /
-//     b_small of the descriptor, produced by b2_split_tf32 or a previous epilogue).
-//   bf16 operands (elem_dtype B2_BF16): kind::f16, 64-element k-blocks, fp32 accumulation.
+//     where small = rna_tf32(x - big(x)) — fp32-class accuracy (the 1e-5 parity bar) on tensor cores.  The
+//     main product of every k-block is accumulated from zero and added to the running sum in fp32
+//     round-to-nearest, so the error does not grow with the length of the contraction.
+//   bf16 operands (elem_dtype B2_BF16): wgmma .bf16, 64-element k-blocks, fp32 accumulation.
 //
-// Structure (persistent: at most one CTA per SM, striding over the 128 x BN output tiles x K splits):
-//   warp 0      TMA producer: cp.async.bulk.tensor 128B-swizzled tiles into a 2-4-stage mbarrier ring
-//   warp 1      TMEM allocator + tcgen05.mma issuer (one elect.sync lane), tcgen05.commit -> mbarriers
-//   warps 2-5   epilogue: tcgen05.ld (32 lanes x 32 columns per warp) -> smem transpose -> fused epilogue ->
-//               TMA tensor store of the finished 32 x 32 chunk (register stores for split-K / accumulate / c_pre)
-//   warps 6-9   helpers: (inline 3xTF32) A -> As, B -> Bs in shared memory, then every second epilogue chunk
-//   TMEM holds 1 or 2 accumulator stages (full/empty mbarriers), so a CTA with several tiles never
-//   drains its pipelines between them; in one-tile CTAs the epilogue's patches reuse the dead ring.
-//   Kernels of a step are chained with programmatic dependent launch (prologue under the predecessor's tail).
-// Where the time goes (probe build, DESIGN.md section 5): SS-mode operand fetch from shared memory and the
-// short MMA issue queue bound the main loop; the output burst bounds the epilogue.
+// Structure (one CTA per 128 x BN output tile and K split; 384 threads):
+//   warpgroup 0    thread 0 issues cp.async.bulk.tensor loads of the raw operand tiles into a 3-stage
+//                  mbarrier ring; the whole warpgroup converts each raw tile (either major, fp32 or bf16)
+//                  into the K-major 128B-swizzled tiles wgmma reads — big and small parts for 3xTF32 —
+//                  in a second 3-stage ring.  wgmma reads tf32 operands from shared memory only in K-major
+//                  form, so this pass is what lets MN-major operands stay as they lie in HBM.
+//   warpgroups 1-2 64 rows each: wgmma m64nBNk8 (tf32) / k16 (bf16) from the converted tiles, then the fused
+//                  epilogue straight from the accumulator registers (each quad of lanes writes 32 contiguous
+//                  bytes of one output row).
+// Kernels of a step are chained with programmatic dependent launch (prologue under the predecessor's tail).
 // Every mbarrier wait is bounded: a pipeline bug traps with a message instead of hanging the GPU.
 #include "b2_common.cuh"
 #include <string.h>
@@ -39,31 +35,16 @@
 #include <cuda.h>  // CUtensorMap + enums only; cuTensorMapEncodeTiled is resolved at run time
 
 namespace tc {
-constexpr int BM = 128;          // UMMA M (cta_group::1): TMEM lane == output row
-constexpr int BK = 32;           // fp32 elements per k-block == one 128-byte swizzle row (bf16: 64)
-constexpr int UMMA_K_BYTES = 32; // kind::tf32: K = 8 elements of 4 bytes per instruction
-constexpr int MAX_STAGES = 4;  // 4 stages of (A,B) for one pass; 3 stages of (A,As,B,Bs) for 3xTF32
-constexpr int A_BYTES = BM * 128;
-constexpr int NTHREADS = 320;   // producer, MMA issuer, 4 epilogue warps, 4 helper warps (second half of the epilogue
-                                // columns; with B2_GEMM_X3_INLINE they first make the 3xTF32 small parts in shared memory)
-constexpr int PATCH_BYTES = 8 * 32 * 33 * 4;   // epilogue transpose patches (one per epilogue / helper warp)
-
-// Timing probes (tools/gemm_probe.py, tools/gemm_trace.py): compiled in only with -DB2_GEMM_PROBE
-// (B2_BUILD_PROBE=1 python -m fuxictr_b200.build); the product build has no debug hooks.
-#ifdef B2_GEMM_PROBE
-#define B2_DBG(bit) ((p.dbg & (bit)) != 0)
-#define B2_STAMP(cond, idx) do { if (p.trace != nullptr && blockIdx.x == 0 && (cond)) p.trace[idx] = clock64(); } while (0)
-#else
-#define B2_DBG(bit) false
-#define B2_STAMP(cond, idx) do { } while (0)
-#endif
+constexpr int BM = 128;          // two consumer warpgroups x wgmma M = 64
+constexpr int NTHREADS = 384;    // converter warpgroup + two wgmma warpgroups
+constexpr int RSTAGES = 3;       // raw TMA tiles in flight
+constexpr int CSTAGES = 3;       // converted tiles in flight
 
 struct Params {
-  CUtensorMap map_a[2];   // [0] the operand, [1] its 3xTF32 small part
-  CUtensorMap map_b[2];
-  CUtensorMap map_c;      // C as a (N, M) tensor with 32 x 32 boxes: the epilogue's TMA store (tma_store != 0)
+  CUtensorMap map_a;
+  CUtensorMap map_b;
   float* c;
-  float* c_small;         // optional: tf32_small(C) for the consumer's 3xTF32 operand
+  float* c_small;         // optional: tf32_small(C) (or the bf16 copy of C) for the consumer's operand
   float* c_pre;           // optional: acc + bias BEFORE mul/add/act (CrossNetV2 saves it for its backward)
   int64_t ldc;
   const float* bias;
@@ -71,19 +52,11 @@ struct Params {
   const float* add;
   const float* ybwd;      // optional (M, N) ld = ldc: C = act_bwd'(ybwd) * (...)   (activation backward)
   float* colsum;          // optional (N): += column sums of C (bias gradient)
-  int M, N, K, bn, nseg, act, act_bwd, beta, kb_per_split;
+  int M, N, K, act, act_bwd, beta, kb_per_split;
   int a_mn, b_mn;         // operand is MN-major (memory (K, rows))
-  int esz;                // operand element bytes: 4 = fp32 read as tf32 (kind::tf32), 2 = bf16 (kind::f16)
-  int64_t ld_aux;         // leading dimension of c_small (fp32 small part, or the bf16 copy of C when esz == 2)
-  int nmain;      // TMEM accumulators for the main (big x big) product: its K range is cut in nmain chunks
-  int tiles_m, tiles_n, splits;   // tile grid; CTAs stride over tiles_m * tiles_n * splits work items
-  int nacc;       // accumulator stages in TMEM (2: the epilogue of a tile overlaps the next main loop)
-  int stages;     // operand ring depth (<= MAX_STAGES), chosen by the host to fit 227 KB
-  long long* trace;   // probe build only: CTA 0 writes clock64() stamps of its loops here (B2_GEMM_TRACE)
-  int dbg;        // probe build only: B2_GEMM_DBG bits (timing experiments; results are wrong when set)
-  int tma_store;  // the epilogue hands finished 32 x 32 chunks to cp.async.bulk.tensor stores (plain C output only)
-  int inline_split;  // 3xTF32 with the small parts computed in shared memory by warps 6..9 (no As/Bs in HBM)
-  int tmem_cols;  // power of two >= (nmain + (nseg > 1)) * bn
+  int esz;                // operand element bytes: 4 = fp32 (tf32 passes), 2 = bf16
+  int64_t ld_aux;         // leading dimension of c_small
+  int tiles_m, tiles_n, splits;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -131,536 +104,294 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-// One elected lane of a fully converged warp (elect.sync): unlike `lane == 0`, the compiler knows the
-// enclosing control flow is warp-uniform, so descriptors / coordinates stay in uniform registers and
-// every UTCHMMA / UTMALDG is a single instruction instead of a per-instruction election loop.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// K-major, 128-byte swizzle, tile rows are 128 B apart, 8-row groups 1024 B apart.
+// wgmma shared-memory matrix descriptor of a K-major, 128B-swizzled tile: rows 128 B apart, 8-row swizzle
+// atoms 1024 B apart (SBO); the leading byte offset is unused for swizzled K-major layouts.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr) {
   uint64_t d = 0;
   d |= (uint64_t) ((addr & 0x3FFFFu) >> 4);  // start address  [0,14)
-  d |= (uint64_t) 0 << 16;                   // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t) 1 << 16;                   // leading byte offset [16,30)
   d |= (uint64_t) (1024 >> 4) << 32;         // stride byte offset [32,46)
-  d |= (uint64_t) 1 << 46;                   // descriptor version (sm_100)
-  d |= (uint64_t) 2 << 61;                   // layout: SWIZZLE_128B
+  d |= (uint64_t) 1 << 62;                   // layout: SWIZZLE_128B
   return d;
 }
-// MN-major: the tile is a row of [128 bytes of MN-elements x bke k-rows] boxes (what one TMA box writes:
-// k-row r at r * 128 B), boxes box_bytes apart = LBO.
-//   16-bit operands: SWIZZLE_128B, swizzle atom = 8 k-rows (1024 B) = SBO.
-//   32-bit operands (tf32): the ONLY MN-major layout the tensor core accepts is SWIZZLE_128B_BASE32B
-//   (32-byte swizzle granules, atom = 4 k-rows = 512 B = SBO); its TMA twin is SWIZZLE_128B_ATOM_32B.
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t addr, uint32_t box_bytes, int esz) {
-  uint64_t d = 0;
-  d |= (uint64_t) ((addr & 0x3FFFFu) >> 4);      // start address  [0,14)
-  d |= (uint64_t) (box_bytes >> 4) << 16;        // leading byte offset [16,30): next 128-byte-wide MN block
-  d |= (uint64_t) ((esz == 4 ? 512 : 1024) >> 4) << 32;   // stride byte offset [32,46): next swizzle atom along K
-  d |= (uint64_t) 1 << 46;                       // descriptor version (sm_100)
-  d |= (uint64_t) (esz == 4 ? 1 : 2) << 61;      // layout: SWIZZLE_128B_BASE32B (1) / SWIZZLE_128B (2)
-  return d;
-}
+// Byte offset of 16-byte chunk `c` (0..7) of row `r` in a K-major 128B-swizzled tile (1024-byte aligned base).
+__device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t) (r * 128 + ((c ^ (r & 7)) << 4)); }
 __device__ __forceinline__ float tf32_small(float v) { return b2_tf32_small(v); }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ float tf32_big(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// wgmma.mma_async m64nNk8 (tf32) / m64nNk16 (bf16), both operands from shared memory, fp32 accumulators
+// d[] in the wgmma fragment layout; scale_d == 0 overwrites the accumulators.
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 
-// One lane's share of the epilogue: column n of 32 consecutive rows (mrow0 ...), values in t[].
-// `store_c` false: everything but the store of C itself (the caller hands the chunk to a TMA store).
-__device__ __forceinline__ void epilogue_store(const Params& p, float (&t)[32], int mrow0, int n, bool split, bool store_c) {
-  float* cp = p.c + (int64_t) mrow0 * p.ldc + n;
-  if (split) {
+// 16 bytes of K-major fp32 operand -> the converted tile: big part (13 low mantissa bits cleared) and, for
+// 3xTF32, the small part at the same offset in the small tile.
+template <bool X3>
+__device__ __forceinline__ void store_split(uint8_t* dst, uint32_t small_off, uint32_t off, const float4& v) {
+  *reinterpret_cast<float4*>(dst + off) = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
+  if (X3)
+    *reinterpret_cast<float4*>(dst + small_off + off) =
+        make_float4(tf32_small(v.x), tf32_small(v.y), tf32_small(v.z), tf32_small(v.w));
+}
+
+// One operand's k-block as TMA wrote it -> K-major 128B-swizzled tile of `rows` rows, by the 128 threads of
+// the converter warpgroup.  Raw layouts: K-major (rows, 128 B of k); MN-major (k, rows): 32 fp32 or 64 bf16
+// k-rows of `rows` elements, transposed here in registers (4 x 4 fp32 or 8 x 8 bf16 per thread).
+template <bool X3>
+__device__ __forceinline__ void convert_tile(const uint8_t* src, uint8_t* dst, uint32_t small_off, int rows, int mn,
+                                             int esz, int ct) {
+  if (esz == 2) {
+    if (!mn) {
+      for (int q = ct; q < rows * 8; q += 128)
+        *reinterpret_cast<uint4*>(dst + swz(q >> 3, q & 7)) = *reinterpret_cast<const uint4*>(src + 16 * q);
+    } else {
+      for (int b = ct; b < rows; b += 128) {
+        const int kq = b & 7, r0 = (b >> 3) * 8;
+        uint4 v[8];
 #pragma unroll
-    for (int r = 0; r < 32; ++r)
-      if (mrow0 + r < p.M) b2_red_add(cp + (int64_t) r * p.ldc, t[r]);
-  } else {
-    if (p.c_pre != nullptr) {
-      float* pp = p.c_pre + (int64_t) mrow0 * p.ldc + n;
+        for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const uint4*>(src + ((8 * kq + j) * rows + r0) * 2);
 #pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) pp[(int64_t) r * p.ldc] = t[r];
-    }
-    if (p.mul != nullptr) {
-      const float* mp = p.mul + (int64_t) mrow0 * p.ldc + n;
+        for (int i = 0; i < 8; ++i) {
+          uint32_t w[4];
 #pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) t[r] *= __ldg(mp + (int64_t) r * p.ldc);
-    }
-    if (p.add != nullptr) {
-      const float* ap = p.add + (int64_t) mrow0 * p.ldc + n;
-#pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) t[r] += __ldg(ap + (int64_t) r * p.ldc);
-    }
-    if (p.act == B2_ACT_RELU) {
-#pragma unroll
-      for (int r = 0; r < 32; ++r) t[r] = fmaxf(t[r], 0.f);
-    } else if (p.act == B2_ACT_SIGMOID) {
-#pragma unroll
-      for (int r = 0; r < 32; ++r) t[r] = 1.f / (1.f + expf(-t[r]));
-    }
-    if (p.ybwd != nullptr) {   // activation backward of the PRODUCER of this gradient, fused
-      const float* yp = p.ybwd + (int64_t) mrow0 * p.ldc + n;
-      if (p.act_bwd == B2_ACT_RELU) {
-#pragma unroll
-        for (int r = 0; r < 32; ++r)
-          if (mrow0 + r < p.M) t[r] = (__ldg(yp + (int64_t) r * p.ldc) > 0.f) ? t[r] : 0.f;
-      } else if (p.act_bwd == B2_ACT_SIGMOID) {
-#pragma unroll
-        for (int r = 0; r < 32; ++r)
-          if (mrow0 + r < p.M) {
-            const float yv = __ldg(yp + (int64_t) r * p.ldc);
-            t[r] = t[r] * ((1.f - yv) * yv);
+          for (int j = 0; j < 8; j += 2) {
+            const uint32_t lo = reinterpret_cast<const uint16_t*>(&v[j])[i];
+            const uint32_t hi = reinterpret_cast<const uint16_t*>(&v[j + 1])[i];
+            w[j >> 1] = lo | (hi << 16);
           }
+          *reinterpret_cast<uint4*>(dst + swz(r0 + i, kq)) = make_uint4(w[0], w[1], w[2], w[3]);
+        }
       }
     }
-    if (p.beta) {
+    return;
+  }
+  if (!mn) {
+    for (int q = ct; q < rows * 8; q += 128)
+      store_split<X3>(dst, small_off, swz(q >> 3, q & 7), *reinterpret_cast<const float4*>(src + 16 * q));
+  } else {
+    for (int b = ct; b < 2 * rows; b += 128) {
+      const int kq = b & 7, r0 = (b >> 3) * 4;
+      float4 v[4];
 #pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) t[r] += cp[(int64_t) r * p.ldc];
-    }
-    if (store_c) {
-#pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) cp[(int64_t) r * p.ldc] = t[r];   // 128 contiguous bytes per row
-    }
-    if (p.c_small != nullptr && p.esz == 4) {   // the consumer's 3xTF32 small part, produced where C is produced
-      float* sp = p.c_small + (int64_t) mrow0 * p.ld_aux + n;
-#pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) sp[(int64_t) r * p.ld_aux] = tf32_small(t[r]);
-    } else if (p.c_small != nullptr) {          // bf16 mode: the consumer's bf16 operand (round-to-nearest-even)
-      __nv_bfloat16* sp = reinterpret_cast<__nv_bfloat16*>(p.c_small) + (int64_t) mrow0 * p.ld_aux + n;
-#pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) sp[(int64_t) r * p.ld_aux] = __float2bfloat16_rn(t[r]);
-    }
-    if (p.colsum != nullptr) {    // bias gradient: this lane owns column n of 32 rows
-      float cs = 0.f;
-#pragma unroll
-      for (int r = 0; r < 32; ++r)
-        if (mrow0 + r < p.M) cs += t[r];
-      b2_red_add(p.colsum + n, cs);
+      for (int j = 0; j < 4; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((4 * kq + j) * rows + r0) * 4);
+      store_split<X3>(dst, small_off, swz(r0 + 0, kq), make_float4(v[0].x, v[1].x, v[2].x, v[3].x));
+      store_split<X3>(dst, small_off, swz(r0 + 1, kq), make_float4(v[0].y, v[1].y, v[2].y, v[3].y));
+      store_split<X3>(dst, small_off, swz(r0 + 2, kq), make_float4(v[0].z, v[1].z, v[2].z, v[3].z));
+      store_split<X3>(dst, small_off, swz(r0 + 3, kq), make_float4(v[0].w, v[1].w, v[2].w, v[3].w));
     }
   }
 }
 
-// Persistent tile loop: CTA c works on tiles c, c + gridDim.x, ... (one tile per CTA when the problem
-// has no more tiles than SMs).  Three pipelines run through all of a CTA's tiles without draining:
-//   smem ring      full[s] / empty[s]            TMA producer  <->  MMA issuer
-//   TMEM stages    tmem_full[a] / tmem_empty[a]  MMA issuer    <->  epilogue warps (a < nacc = 1 or 2)
-// so the barrier / TMEM / descriptor prologue is paid once per CTA, the producer prefetches the next
-// tile's operands during an epilogue, and with nacc = 2 the epilogue of tile j overlaps the main loop
-// of tile j + 1.
+// One output element (m, n) of the fused epilogue, t = accumulator + bias; returns what enters the column sum.
+__device__ __forceinline__ float epilogue_elem(const Params& p, int m, int n, float t) {
+  const int64_t o = (int64_t) m * p.ldc + n;
+  if (p.splits > 1) {          // split-K: partial sums of a plain linear output (C was zeroed by the host)
+    b2_red_add(p.c + o, t);
+    return 0.f;
+  }
+  if (p.c_pre != nullptr) p.c_pre[o] = t;
+  if (p.mul != nullptr) t *= __ldg(p.mul + o);
+  if (p.add != nullptr) t += __ldg(p.add + o);
+  if (p.act == B2_ACT_RELU) t = fmaxf(t, 0.f);
+  else if (p.act == B2_ACT_SIGMOID) t = 1.f / (1.f + expf(-t));
+  if (p.ybwd != nullptr) {     // activation backward of the PRODUCER of this gradient, fused
+    const float yv = __ldg(p.ybwd + o);
+    if (p.act_bwd == B2_ACT_RELU) t = (yv > 0.f) ? t : 0.f;
+    else if (p.act_bwd == B2_ACT_SIGMOID) t = t * ((1.f - yv) * yv);
+  }
+  if (p.beta) t += p.c[o];
+  p.c[o] = t;
+  if (p.c_small != nullptr) {
+    const int64_t oa = (int64_t) m * p.ld_aux + n;
+    if (p.esz == 4) p.c_small[oa] = tf32_small(t);   // the consumer's 3xTF32 small part, produced where C is
+    else reinterpret_cast<__nv_bfloat16*>(p.c_small)[oa] = __float2bfloat16_rn(t);   // bf16 mode operand
+  }
+  return t;
+}
+
+template <int BN, bool X3>
 __global__ void __launch_bounds__(NTHREADS, 1)
-gemm_tf32_kernel(const __grid_constant__ Params p) {
+gemm_tc_kernel(const __grid_constant__ Params p) {
+  constexpr int NR = BN / 2;                            // accumulators per thread: 64 x BN per warpgroup
+  constexpr uint32_t TILE_BYTES = (BM + BN) * 128;      // one k-block of A and B (raw, or converted big part)
+  constexpr uint32_t CONV_BYTES = (X3 ? 2 : 1) * TILE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte aligned bases: align by hand (1 KB of slack is requested).
-  // (pointer arithmetic on smem_raw keeps the shared address space visible to the compiler)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const uint32_t b_bytes = (uint32_t) p.bn * 128u;
-  const bool x3 = p.nseg > 1;
-  const int STAGES = p.stages;
-  const uint32_t stage_bytes = (x3 ? 2u : 1u) * (A_BYTES + b_bytes);
-  const uint32_t off_as = A_BYTES, off_b = (x3 ? 2u : 1u) * A_BYTES, off_bs = off_b + b_bytes;
-  // The 8 epilogue transpose patches (32 x 33 floats each) follow the ring — or, when every CTA has exactly
-  // one tile, lie ON the ring: the accumulator is complete only after every MMA has read its operands and
-  // nothing is loaded afterwards, so the ring is dead by then and its bytes buy one more stage instead.
-  const bool single_tile = p.tiles_m * p.tiles_n * p.splits <= (int) gridDim.x;
-  float* patch_base = reinterpret_cast<float*>(smem + (single_tile ? 0u : STAGES * stage_bytes));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes + (single_tile ? 0 : PATCH_BYTES));
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * MAX_STAGES + 4);
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + MAX_STAGES),
-                 tfull0 = smem_u32(bars + 2 * MAX_STAGES), tempty0 = smem_u32(bars + 2 * MAX_STAGES + 2),
-                 conv0 = smem_u32(bars + 2 * MAX_STAGES + 4);
-  const bool inl = p.inline_split != 0;
+  uint8_t* raw0 = smem;
+  uint8_t* conv0 = smem + RSTAGES * TILE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(conv0 + CSTAGES * CONV_BYTES);
+  const uint32_t rfull0 = smem_u32(bars), cfull0 = smem_u32(bars + RSTAGES),
+                 cempty0 = smem_u32(bars + RSTAGES + CSTAGES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bke = 128 / p.esz;                      // k elements per k-block: one 128-byte swizzle row
-  const int mnb = 128 / p.esz;                      // MN elements per MN-major box (128 bytes wide)
-  const uint32_t box_bytes = (uint32_t) bke * 128u; // one MN-major box: bke k-rows x 128 B
   const int num_kb_total = (p.K + bke - 1) / bke;
   const int tiles_mn = p.tiles_m * p.tiles_n;
-  const int total_tiles = tiles_mn * p.splits;
-  const int acc_cols = (p.nmain + (x3 ? 1 : 0)) * p.bn;   // TMEM columns of one accumulator stage
-  // Warps 6..9 take every second 32-column chunk of the epilogue (TMEM lane quadrant = warp % 4, like warps
-  // 2..5).  With the inline split they are the converters first, so they help only when this CTA has a
-  // single tile (otherwise they are already converting the next tile's operands).
-  const bool helpers = (!inl || total_tiles <= (int) gridDim.x) && !B2_DBG(32);
+  const int z = blockIdx.x / tiles_mn, rr = blockIdx.x - z * tiles_mn;
+  const int m0 = (rr / p.tiles_n) * BM, n0 = (rr % p.tiles_n) * BN;
+  const int kb_begin = z * p.kb_per_split;
+  const int nkb = min(num_kb_total, kb_begin + p.kb_per_split) - kb_begin;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < ((x3 && !inl) ? 2 : 1); ++s) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_a[s])) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_b[s])) : "memory");
-    }
-    if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_c)) : "memory");
-    for (int s = 0; s < MAX_STAGES; ++s) {
-      mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-      mbar_init(conv0 + 8 * s, 4);      // one arrival per converter warp
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, helpers ? 8 : 4);    // one arrival per warp that reads the accumulator
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_a)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_b)) : "memory");
+    for (int s = 0; s < RSTAGES; ++s) mbar_init(rfull0 + 8 * s, 1);
+    for (int s = 0; s < CSTAGES; ++s) {
+      mbar_init(cfull0 + 8 * s, 4);      // one arrival per converter warp
+      mbar_init(cempty0 + 8 * s, 8);     // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {  // whole warp: allocate TMEM columns for the accumulator stage(s)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t) p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  B2_STAMP(threadIdx.x == 0, 640);
-  // PDL: everything above touched only shared memory, TMEM and the kernel parameters; from here on the
+  // PDL: everything above touched only shared memory and the kernel parameters; from here on the
   // predecessor's outputs are read.  Let the successor begin ITS prologue once every CTA got this far.
   b2_pdl_trigger();
   b2_pdl_wait();
 
-  // One warp's share of a tile's epilogue: 32-column chunks first, first + step, ... of TMEM lane quadrant
-  // warp % 4.  Each warp owns a 32 x 33-float patch to transpose its TMEM rows, so that one store
-  // instruction writes 128 contiguous bytes of ONE output row instead of 16 bytes of 32 different rows
-  // (partial-sector writes to untouched lines cost an L2 fill each — measured 19 us per tile before this).
-  auto epilogue_tile = [&](int t, int j, int first, int step) {
-    const int q = warp & 3;
-    const bool split = p.splits > 1;
-    float* patch = patch_base + (warp - 2) * (32 * 33);
-    const int z = t / tiles_mn, rr = t - z * tiles_mn;
-    const int m0 = (rr / p.tiles_n) * BM, n0 = (rr % p.tiles_n) * p.bn;
-    const int kb_begin = z * p.kb_per_split;
-    const int nkb = min(num_kb_total, kb_begin + p.kb_per_split) - kb_begin;
-    const int nmain = min(p.nmain, nkb);
-    const int nslots = nmain + (x3 ? 1 : 0);
-    const int acc = (p.nacc == 2) ? (j & 1) : 0;
-    const uint32_t use = (uint32_t) (p.nacc == 2 ? (j >> 1) : j);
-    B2_STAMP(lane == 0, 512 + 4 * warp + 0);
-    mbar_wait(tfull0 + 8 * acc, use & 1u, 2);
-    B2_STAMP(lane == 0, 512 + 4 * warp + 1);
-    tc_fence_after();
-    const uint32_t tacc = tmem_base + (uint32_t) (acc * acc_cols) + ((uint32_t) (q * 32) << 16);
-    if (first >= p.bn) {          // a helper warp with no chunk in a narrow tile still owes its arrival
+  if (warp < 4) {
+    // ---------------- warpgroup 0: TMA (thread 0) and operand conversion ----------------
+    const int ct = threadIdx.x;
+    auto load = [&](int i) {
+      const int s = i % RSTAGES, kb = kb_begin + i;
+      const uint32_t dst = smem_u32(raw0 + s * TILE_BYTES), bar = rfull0 + 8 * s;
+      mbar_expect_tx(bar, TILE_BYTES);   // out-of-range parts of a box arrive zero-filled and count in full
+      if (p.a_mn) tma_load_2d(dst, &p.map_a, bar, m0, kb * bke);
+      else tma_load_2d(dst, &p.map_a, bar, kb * bke, m0);
+      if (p.b_mn) tma_load_2d(dst + BM * 128, &p.map_b, bar, n0, kb * bke);
+      else tma_load_2d(dst + BM * 128, &p.map_b, bar, kb * bke, n0);
+    };
+    if (ct == 0)
+      for (int i = 0; i < RSTAGES && i < nkb; ++i) load(i);
+    for (int i = 0; i < nkb; ++i) {
+      const int rs = i % RSTAGES, cs = i % CSTAGES;
+      mbar_wait(rfull0 + 8 * rs, (uint32_t) (i / RSTAGES) & 1u, 0);
+      mbar_wait(cempty0 + 8 * cs, ((uint32_t) (i / CSTAGES) & 1u) ^ 1u, 1);
+      const uint8_t* src = raw0 + rs * TILE_BYTES;
+      uint8_t* dst = conv0 + cs * CONV_BYTES;
+      convert_tile<X3>(src, dst, TILE_BYTES, BM, p.a_mn, p.esz, ct);
+      convert_tile<X3>(src + BM * 128, dst + BM * 128, TILE_BYTES, BN, p.b_mn, p.esz, ct);
+      // generic-proxy stores -> visible to wgmma (async proxy) before the consumers are told
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
+      if (lane == 0) mbar_arrive(cfull0 + 8 * cs);
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // every converter thread is done with raw stage rs
+      if (ct == 0 && i + RSTAGES < nkb) load(i + RSTAGES);
     }
-    for (int c0 = first; c0 < p.bn; c0 += step) {
-      uint32_t v[32];
-      __syncwarp();  // tcgen05.ld is warp-collective; also fences the previous patch reads
-      tmem_ld32(tacc + (uint32_t) c0, v);
-      for (int sl = 1; sl < nslots; ++sl) {  // fp32 round-to-nearest sum of the accumulation chains
-        uint32_t w[32];
-        tmem_ld32(tacc + (uint32_t) (sl * p.bn + c0), w);
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj) v[jj] = __float_as_uint(__uint_as_float(v[jj]) + __uint_as_float(w[jj]));
-      }
-      if (c0 + step >= p.bn) {      // this warp's last TMEM read of the tile: hand the accumulator stage back
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      }
-#pragma unroll
-      for (int jj = 0; jj < 32; ++jj) patch[lane * 33 + jj] = __uint_as_float(v[jj]);  // row = lane
-      __syncwarp();
-      const int n = n0 + c0 + lane;  // this lane's output column for the whole chunk
-      const bool n_ok = n < p.N;
-      const float bv = (n_ok && p.bias != nullptr && z == 0) ? __ldg(p.bias + n) : 0.f;
-      float tt[32];
-#pragma unroll
-      for (int r = 0; r < 32; ++r) tt[r] = patch[r * 33 + lane] + bv;  // 32 independent LDS in flight
-      const int mrow0 = m0 + q * 32;
-      if (!p.tma_store) {
-        if (n_ok && !B2_DBG(2)) epilogue_store(p, tt, mrow0, n, split, true);
-      } else {
-        // TMA store: the finished chunk goes back into the warp's patch as a dense 32 x 32 box (row = output
-        // row, 128 B per row) and ONE bulk tensor store writes it; rows >= M and columns >= N are clipped by
-        // the tensor map, so nothing here is predicated on the tile edges.
-        if (n_ok) epilogue_store(p, tt, mrow0, n, split, false);
-        __syncwarp();                  // every lane has read its column out of the 33-pitch patch
-#pragma unroll
-        for (int r = 0; r < 32; ++r) patch[r * 32 + lane] = tt[r];
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0 && !B2_DBG(2)) {
-          tma_store_2d(&p.map_c, smem_u32(patch), n0 + c0, mrow0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the patch is rewritten by the next chunk
-        }
-        __syncwarp();
-      }
-    }
-    if (p.tma_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    B2_STAMP(lane == 0, 512 + 4 * warp + 2);
-  };
-
-  if (warp == 0) {
-    // ---------------- TMA producer (the warp loops converged; one elected lane issues) ----------------
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const int z = t / tiles_mn, r = t - z * tiles_mn;
-      const int m0 = (r / p.tiles_n) * BM, n0 = (r % p.tiles_n) * p.bn;
-      const int kb_begin = z * p.kb_per_split;
-      const int kb_end = min(num_kb_total, kb_begin + p.kb_per_split);
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        B2_STAMP(lane == 0 && kb - kb_begin < 60, 4 * (kb - kb_begin) + 0);
-        mbar_wait(empty0 + 8 * stage, phase ^ 1, 0);
-        B2_STAMP(lane == 0 && kb - kb_begin < 60, 4 * (kb - kb_begin) + 1);
-        const uint32_t a_dst = smem_base + stage * stage_bytes;
-        const uint32_t full = full0 + 8 * stage;
-        if (B2_DBG(16) && elect_one()) mbar_arrive(full);      // probe: no operand traffic at all
-        if (!B2_DBG(16) && elect_one()) {
-          mbar_expect_tx(full, inl ? (A_BYTES + b_bytes) : stage_bytes);
-          // every operand tile is loaded ONCE per k-block; 3xTF32 reuses them for its 3 products.
-          // K-major operand: one box (128 B of k x rows).  MN-major operand: one box per 128 B of rows
-          // (coordinates {row, k}); out-of-range boxes arrive zero-filled.
-          for (int s = 0; s < ((x3 && !inl) ? 2 : 1); ++s) {
-            const uint32_t a_t = a_dst + (s ? off_as : 0u), b_t = a_dst + (s ? off_bs : off_b);
-            if (!p.a_mn) {
-              tma_load_2d(a_t, &p.map_a[s], full, kb * bke, m0);
-            } else {
-              for (int j = 0; j < BM / mnb; ++j) tma_load_2d(a_t + j * box_bytes, &p.map_a[s], full, m0 + mnb * j, kb * bke);
-            }
-            if (!p.b_mn) {
-              tma_load_2d(b_t, &p.map_b[s], full, kb * bke, n0);
-            } else {
-              for (int j = 0; j < p.bn / mnb; ++j) tma_load_2d(b_t + j * box_bytes, &p.map_b[s], full, n0 + mnb * j, kb * bke);
-            }
-          }
-        }
-        __syncwarp();
-        B2_STAMP(lane == 0 && kb - kb_begin < 60, 4 * (kb - kb_begin) + 2);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer (the warp loops converged; one elected lane issues) ----------------
-    // instruction descriptor: D=f32, A=B=tf32 | bf16, operand majors, N = bn, M = 128
-    const uint32_t fmt = (p.esz == 2) ? 1u : 2u;   // operand format: kind::f16 1 = BF16; kind::tf32 2 = TF32
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t) (p.a_mn ? 1 : 0) << 15) |
-                           ((uint32_t) (p.b_mn ? 1 : 0) << 16) | ((uint32_t) (p.bn >> 3) << 17) |
-                           ((uint32_t) (BM >> 4) << 24);
-    // one instruction consumes 32 bytes of K per row (8 tf32 / 16 bf16 elements): 32 bytes along a
-    // K-major swizzle row (+2 in the (addr >> 4) field), or 8 / 16 k-rows of an MN-major tile
-    const uint32_t mn_step = (p.esz == 2) ? 2048u : 1024u;
-    const uint32_t ak = p.a_mn ? (mn_step >> 4) : (uint32_t) (UMMA_K_BYTES >> 4);
-    const uint32_t bk = p.b_mn ? (mn_step >> 4) : (uint32_t) (UMMA_K_BYTES >> 4);
-    // The tensor core adds each instruction's 8 products into the fp32 accumulator with
-    // truncation, so rounding error grows with the length of one accumulation chain and with
-    // the magnitude of the accumulator.  For 3xTF32 the K range of the main product is
-    // therefore cut into `nmain` chains held in separate TMEM column ranges, and the two small
-    // correction products get a range of their own; the epilogue adds the ranges in fp32 RN.
-    //
-    // The elected lane is the instruction stream behind every MMA of the CTA, so its scalar work per
-    // k-block is on the critical path: descriptors are built once (stage 0) and advanced by 32-bit
-    // adds on their low word (the 14-bit start-address field never carries), the chain boundaries
-    // are tracked incrementally, and the bf16 / TF32 / 3xTF32 loops are separate.
-    const uint64_t a0 = p.a_mn ? make_smem_desc_mn(smem_base, box_bytes, p.esz) : make_smem_desc(smem_base);
-    const uint64_t b0 = p.b_mn ? make_smem_desc_mn(smem_base + off_b, box_bytes, p.esz) : make_smem_desc(smem_base + off_b);
-    const uint64_t as0 = p.a_mn ? make_smem_desc_mn(smem_base + off_as, box_bytes, p.esz) : make_smem_desc(smem_base + off_as);
-    const uint64_t bs0 = p.b_mn ? make_smem_desc_mn(smem_base + off_bs, box_bytes, p.esz) : make_smem_desc(smem_base + off_bs);
-    const uint32_t a_hi = (uint32_t) (a0 >> 32), b_hi = (uint32_t) (b0 >> 32);
-    const uint32_t as_hi = (uint32_t) (as0 >> 32), bs_hi = (uint32_t) (bs0 >> 32);
-    const uint32_t stage_units = stage_bytes >> 4;
-#define B2_DESC(hi, lo) ((((uint64_t) (hi)) << 32) | (uint64_t) (uint32_t) (lo))
-    int stage = 0;
-    uint32_t phase = 0, so = 0;      // so: this stage's offset in descriptor units
-    int j = 0;                        // this CTA's tile counter
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
-      const int z = t / tiles_mn;
-      const int kb_begin = z * p.kb_per_split;
-      const int nkb = min(num_kb_total, kb_begin + p.kb_per_split) - kb_begin;
-      const int nmain = min(p.nmain, nkb);        // a short last K split may hold fewer k-blocks than chains
-      const int acc = (p.nacc == 2) ? (j & 1) : 0;
-      const uint32_t use = (uint32_t) (p.nacc == 2 ? (j >> 1) : j);
-      mbar_wait(tempty0 + 8 * acc, (use & 1u) ^ 1u, 3);    // the epilogue drained this accumulator stage
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + (uint32_t) (acc * acc_cols);
-      const uint32_t d_corr = tacc + (uint32_t) (nmain * p.bn);
-      // chain c covers k-blocks [ceil(c nkb / nmain), ceil((c+1) nkb / nmain)): divisions only at the boundaries
-      int slot = 0, this_start = 0, next_start = (nkb + nmain - 1) / nmain;
-      const uint32_t ready0 = inl ? conv0 : full0;           // operands (and their small parts) are in place
-      mbar_wait(ready0 + 8 * stage, phase, 1);
-      for (int i = 0; i < nkb; ++i) {
-        if (i == next_start) {
-          ++slot;
-          this_start = next_start;
-          next_start = ((slot + 1) * nkb + nmain - 1) / nmain;
-        }
-        const uint32_t keep = (i == this_start) ? 0u : 1u;      // first k-block of a chain overwrites
-        const uint32_t d_main = tacc + (uint32_t) (slot * p.bn);
-        const uint32_t al = (uint32_t) a0 + so, bl = (uint32_t) b0 + so;
-        const uint32_t asl = (uint32_t) as0 + so, bsl = (uint32_t) bs0 + so;
-        int nstage = stage + 1;
-        uint32_t nphase = phase;
-        if (nstage == STAGES) { nstage = 0; nphase ^= 1; }
-        // The tensor pipe's instruction queue is short: whatever this thread does between the last MMA of
-        // one k-block and the first of the next is a bubble (measured ~380 cycles per k-block against 576 of
-        // MMA work).  So each k-block is issued in two halves and the look at the NEXT stage's barrier sits
-        // between them, under the queued instructions of the first half.
-#define B2_ISSUE_HALF(K0)                                                                                      \
-        if (elect_one()) {                                                                                     \
-          if (B2_DBG(4)) {        /* probe: no tensor work, only the pipeline hand-offs */                      \
-          } else if (p.esz == 2) {                                                                             \
-            _Pragma("unroll") for (int k = (K0); k < (K0) + 2; ++k)                                            \
-              umma_bf16(d_main, B2_DESC(a_hi, al + k * ak), B2_DESC(b_hi, bl + k * bk), idesc, (k > 0) ? 1u : keep); \
-          } else if (!x3) {                                                                                    \
-            _Pragma("unroll") for (int k = (K0); k < (K0) + 2; ++k)                                            \
-              umma_tf32(d_main, B2_DESC(a_hi, al + k * ak), B2_DESC(b_hi, bl + k * bk), idesc, (k > 0) ? 1u : keep); \
-          } else {                                                                                             \
-            _Pragma("unroll") for (int k = (K0); k < (K0) + 2; ++k) {                                          \
-              const uint64_t ad = B2_DESC(a_hi, al + k * ak), bd = B2_DESC(b_hi, bl + k * bk);                 \
-              umma_tf32(d_main, ad, bd, idesc, (k > 0) ? 1u : keep);                                   /* A_big . B_big */   \
-              umma_tf32(d_corr, ad, B2_DESC(bs_hi, bsl + k * bk), idesc, (i > 0 || k > 0) ? 1u : 0u); /* A_big . B_small */ \
-              umma_tf32(d_corr, B2_DESC(as_hi, asl + k * ak), bd, idesc, 1u);                          /* A_small . B_big */ \
-            }                                                                                                  \
-          }                                                                                                    \
-          if ((K0) == 2) {                                                                                     \
-            umma_commit(empty0 + 8 * stage);                      /* frees this smem slot once the MMAs have read it */ \
-            if (i == nkb - 1) umma_commit(tfull0 + 8 * acc);      /* ... and the last one: accumulator complete */      \
-          }                                                                                                    \
-        }                                                                                                      \
-        __syncwarp();
-        B2_STAMP(lane == 0 && i < 60, 256 + 4 * i + 0);
-        B2_ISSUE_HALF(0)
-        B2_STAMP(lane == 0 && i < 60, 256 + 4 * i + 1);
-        // non-blocking look at the next stage under the queued first half; block for it only after the
-        // second half is queued too (a blocking wait here would hold back MMAs whose operands are present)
-        const bool more = i + 1 < nkb;
-        const bool next_ready = more && __all_sync(0xffffffffu, mbar_try_wait(ready0 + 8 * nstage, nphase));
-        B2_ISSUE_HALF(2)
-#undef B2_ISSUE_HALF
-        B2_STAMP(lane == 0 && i < 60, 256 + 4 * i + 2);
-        if (more && !next_ready) mbar_wait(ready0 + 8 * nstage, nphase, 1);
-        B2_STAMP(lane == 0 && i < 60, 256 + 4 * i + 3);
-        so += stage_units;
-        stage = nstage;
-        phase = nphase;
-        if (stage == 0) so = 0;
-      }
-    }
-#undef B2_DESC
-  } else if (warp < 6) {
-    // ---------------- epilogue warps 2..5: TMEM lane quadrant = warp % 4 ----------------
-    int j = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j)
-      epilogue_tile(t, j, 0, helpers ? 64 : 32);
   } else {
-    // ---------------- helper warps 6..9 ----------------
-    // Inline 3xTF32: small = x - tf32(x), element for element.  The small tiles have their operand's own
-    // shared-memory layout (whatever the swizzle), so the conversion is a flat 16-byte-per-lane pass:
-    // A -> As, B -> Bs.  Generic-proxy stores are made visible to the tensor core (async proxy) by
-    // fence.proxy.async before the arrival the MMA warp waits on.  Then (or only) the odd epilogue chunks.
-    const int cw = threadIdx.x - 6 * 32;          // 0..127
-    const int b_chunks = (int) (b_bytes >> 4);
-    int stage = 0;
-    uint32_t phase = 0;
-    int j = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
-      const int z = t / tiles_mn;
-      const int kb_begin = z * p.kb_per_split;
-      const int nkb = min(num_kb_total, kb_begin + p.kb_per_split) - kb_begin;
-      for (int i = 0; inl && i < nkb; ++i) {
-        mbar_wait(full0 + 8 * stage, phase, 4);
-        uint8_t* sb = smem + (size_t) stage * stage_bytes;
-        if (!B2_DBG(1)) {
-          float4 v[A_BYTES / 16 / 128];
+    // ---------------- warpgroups 1-2: wgmma on rows 64 g .. 64 g + 63 of the tile, then the epilogue ----------
+    const int g = (warp >> 2) - 1;
+    float acc[NR];
+    float part[X3 ? NR : 1], corr[X3 ? NR : 1];
 #pragma unroll
-          for (int u = 0; u < A_BYTES / 16 / 128; ++u) v[u] = *reinterpret_cast<const float4*>(sb + 16 * (cw + 128 * u));
+    for (int r = 0; r < NR; ++r) acc[r] = 0.f;
 #pragma unroll
-          for (int u = 0; u < A_BYTES / 16 / 128; ++u) {
-            float4 w;
-            w.x = tf32_small(v[u].x); w.y = tf32_small(v[u].y); w.z = tf32_small(v[u].z); w.w = tf32_small(v[u].w);
-            *reinterpret_cast<float4*>(sb + off_as + 16 * (cw + 128 * u)) = w;
-          }
+    for (int r = 0; r < (X3 ? NR : 1); ++r) { part[r] = 0.f; corr[r] = 0.f; }
+    for (int i = 0; i < nkb; ++i) {
+      const int cs = i % CSTAGES;
+      mbar_wait(cfull0 + 8 * cs, (uint32_t) (i / CSTAGES) & 1u, 2);
+      const uint32_t base = smem_u32(conv0 + cs * CONV_BYTES);
+      // one instruction consumes 32 bytes of K per row (8 tf32 / 16 bf16): +2 in the (addr >> 4) field
+      const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + BM * 128);
+      wgmma_fence();
+      if constexpr (X3) {
+        const uint64_t asd = ad + (TILE_BYTES >> 4), bsd = bd + (TILE_BYTES >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_tf32(part, ad + 2 * k, bd + 2 * k, k > 0 ? 1u : 0u);   // A_big . B_big
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_tf32(corr, ad + 2 * k, bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                  // A_big . B_small
+          wgmma_tf32(corr, asd + 2 * k, bd + 2 * k, 1u);                                         // A_small . B_big
         }
-        for (int c = cw; c < (B2_DBG(1) ? 0 : b_chunks); c += 256) {
-          const float4 v0 = *reinterpret_cast<const float4*>(sb + off_b + 16 * c);
-          const bool two = c + 128 < b_chunks;
-          float4 v1 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (two) v1 = *reinterpret_cast<const float4*>(sb + off_b + 16 * (c + 128));
-          float4 w;
-          w.x = tf32_small(v0.x); w.y = tf32_small(v0.y); w.z = tf32_small(v0.z); w.w = tf32_small(v0.w);
-          *reinterpret_cast<float4*>(sb + off_bs + 16 * c) = w;
-          if (two) {
-            w.x = tf32_small(v1.x); w.y = tf32_small(v1.y); w.z = tf32_small(v1.z); w.w = tf32_small(v1.w);
-            *reinterpret_cast<float4*>(sb + off_bs + 16 * (c + 128)) = w;
-          }
+      } else {
+        if (p.esz == 2) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_tf32(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(conv0 + 8 * stage);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (helpers) epilogue_tile(t, j, 32, 64);
+      wgmma_commit();
+      wgmma_wait0();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(cempty0 + 8 * cs);     // the converted stage may be overwritten
+      if constexpr (X3) {
+#pragma unroll
+        for (int r = 0; r < NR; ++r) acc[r] += part[r];   // this k-block's main product, fp32 round-to-nearest
+      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t) p.tmem_cols)
-                 : "memory");
+    if constexpr (X3) {
+#pragma unroll
+      for (int r = 0; r < NR; ++r) acc[r] += corr[r];
+    }
+    // wgmma fragment: d[4j + 2h + e] is row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e of the warpgroup
+    const int row0 = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+        const bool n_ok = n < p.N;
+        const float bv = (n_ok && p.bias != nullptr && z == 0) ? __ldg(p.bias + n) : 0.f;
+        float cs = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = row0 + 8 * h;
+          if (n_ok && m < p.M) cs += epilogue_elem(p, m, n, acc[4 * j + 2 * h + e] + bv);
+        }
+        if (p.colsum != nullptr) {    // bias gradient: the 8 lanes of one column, then one red.add per warp
+          cs += __shfl_xor_sync(0xffffffffu, cs, 4);
+          cs += __shfl_xor_sync(0xffffffffu, cs, 8);
+          cs += __shfl_xor_sync(0xffffffffu, cs, 16);
+          if (lane < 4 && n_ok) b2_red_add(p.colsum + n, cs);
+        }
+      }
+    }
   }
 }
 
@@ -877,7 +608,8 @@ static b2_encode_tiled_fn b2_get_encode() {
 }
 
 // K-major operand: memory (rows, K), K contiguous, leading dimension ld; box = 128 B of k x box_rows rows.
-// MN-major operand: memory (K, rows), rows contiguous, leading dimension ld; box = 128 B of rows x (128/esz) k.
+// MN-major operand: memory (K, rows), rows contiguous, leading dimension ld; box = box_rows rows x 128 B of k.
+// Unswizzled: the converter warpgroup writes the swizzled layout wgmma reads.
 static int encode_operand(CUtensorMap* map, const void* base, int64_t rows, int64_t K, int64_t ld,
                           int mn_major, int box_rows, int esz) {
   b2_encode_tiled_fn enc = b2_get_encode();
@@ -890,12 +622,11 @@ static int encode_operand(CUtensorMap* map, const void* base, int64_t rows, int6
     box[0] = per128; box[1] = (cuuint32_t) box_rows;
   } else {
     dims[0] = (cuuint64_t) rows; dims[1] = (cuuint64_t) K;
-    box[0] = per128; box[1] = per128;
+    box[0] = (cuuint32_t) box_rows; box[1] = per128;
   }
   CUresult r = enc(map, esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                    const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   (mn_major && esz == 4) ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return b2_fail(B2_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int) r);
   return B2_OK;
 }
@@ -911,8 +642,26 @@ extern "C" B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const fl
           N < (1ll << 31) && K < (1ll << 31)) ? 1 : 0;
 }
 
-// plan != NULL: fill in the launch plan (tile shape, ring depth, TMEM, shared memory) and return without
+// plan != NULL: fill in the launch plan (tile shape, ring depths, shared memory) and return without
 // touching the device — pure host arithmetic, so the CPU test-suite can sweep it (tests/test_abi.py).
+template <int BN, bool X3>
+static size_t gemm_smem_bytes() {
+  const size_t tile = (size_t) (tc::BM + BN) * 128;
+  return tc::RSTAGES * tile + tc::CSTAGES * (X3 ? 2 : 1) * tile + 1024 + 128;   // + alignment slack, mbarriers
+}
+template <int BN, bool X3>
+static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
+  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, X3>;
+  const size_t smem = gemm_smem_bytes<BN, X3>();
+  // opt-in to > 48 KB of dynamic shared memory: an idempotent per-process property of each instantiation
+  // (C++11 guarantees the initialiser runs once, thread-safely)
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+  if (attr_rc != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: smem attribute: %s", cudaGetErrorString(attr_rc));
+  B2_LAUNCH(kern, grid, tc::NTHREADS, smem, st, p);
+  B2_CUDA_LAUNCH_CHECK("b2_gemm_tc");
+  return B2_OK;
+}
+
 static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan) {
   B2_REQUIRE(d != nullptr, "NULL descriptor");
   const void* a = d->a; const void* b = d->b; float* c = d->c;
@@ -930,6 +679,8 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   B2_REQUIRE(esz == 4 || d->a_small == nullptr, "bf16 operands are single-pass (no small parts)");
   const bool inline_split = (d->flags & B2_GEMM_X3_INLINE) != 0;
   B2_REQUIRE(!inline_split || (esz == 4 && d->a_small == nullptr), "B2_GEMM_X3_INLINE: fp32 operands, no small parts");
+  // The small parts are always derived from the fp32 operands in shared memory (the converter warpgroup).  A
+  // caller's a_small / b_small hold the same values (b2_tf32_small of the operand) and select 3xTF32 alone.
   const bool three_pass = inline_split || d->a_small != nullptr;
   const int64_t ld_aux = d->ld_aux > 0 ? d->ld_aux : ldc;
   B2_REQUIRE(d->c_small == nullptr || ld_aux >= N, "ld_aux too small");
@@ -938,8 +689,8 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
     return b2_fail(B2_E_UNSUPPORTED, "operands are not TMA-addressable (16-byte base, 16-byte row pitch)");
   cudaStream_t st = (cudaStream_t) stream;
 
-  // Tile-shape choice: BN in {32..256 step 32}; the kernel is bound by L2->SM operand traffic,
-  // so minimise waves x per-CTA operand bytes, where one wave = 148 CTAs (one per SM).
+  // Tile-shape choice: BN in {32, 64, 128} (3xTF32: <= 64, its three accumulator sets live in registers);
+  // minimise waves x per-CTA work, where one wave = 132 CTAs (one per SM).
   const int bke = 128 / esz;
   const int64_t tiles_m = b2_ceil_div(M, tc::BM);
   const int64_t num_kb = b2_ceil_div(K, bke);
@@ -948,61 +699,35 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
                        d->c_small == nullptr && d->c_pre == nullptr && d->colsum == nullptr);
   int best_bn = 0, best_split = 1;
   double best_cost = 1e300;
-  // 3xTF32: (chains + 1 correction range) x bn <= 512 TMEM columns and 3 stages of {A, As, B, Bs} <= 227 KB:
-  // bn <= 128 keeps 3-4 chains, bn = 160 keeps 2 (used when it saves a whole wave, e.g. 8192 x 624 x 624)
-  const int x3_bn_max = [] { const char* e = getenv("B2_X3_BN_MAX"); return e ? atoi(e) : 160; }();
-  const int bn_max = three_pass ? x3_bn_max : 256;
-  // cycles per k-block (128 bytes of K): the tensor pipe needs passes x 4 instructions x bn/2, the L2->SM
-  // fabric (~6300 B/cycle chip-wide, ~43 per SM) needs the operand bytes — 3xTF32 with small parts from HBM
-  // moves them twice
+  const int bn_max = three_pass ? 64 : 128;
+  // cycles per k-block: the tensor pipe needs passes x 4 instructions x bn/2 (m64 per warpgroup, two in
+  // parallel), the converter warpgroup moves (128 + bn) rows of 128 bytes (2x for the small parts)
   const double mma_per_bn = (three_pass ? 3.0 : 1.0) * 2.0;
-  const double l2_per_row = 3.0 * ((three_pass && !inline_split) ? 2.0 : 1.0);
-  const int bn_step = (d->b_mn_major && esz == 2) ? 64 : 32;   // an MN-major box is 128 bytes of rows
-  for (int bn = bn_step; bn <= bn_max; bn += bn_step) {
+  const double conv_per_row = three_pass ? 4.0 : 3.0;
+  for (int bn = 32; bn <= bn_max; bn *= 2) {
     const int64_t tiles_n = b2_ceil_div(N, bn);
     for (int split = 1; split <= 32; split *= 2) {
       if (split > 1 && (!linear || num_kb / split < 8)) break;
       const int64_t ctas = tiles_m * tiles_n * split;
       const int64_t waves = b2_ceil_div(ctas, B2_NUM_SMS);
       const double kb = (double) b2_ceil_div(num_kb, split);
-      // per-CTA time ~ fixed prologue/epilogue + k-blocks x bytes per k-block
-      const double per_kb = fmax(mma_per_bn * bn, l2_per_row * (double) (tc::BM + bn));
+      const double per_kb = fmax(mma_per_bn * bn, conv_per_row * (double) (tc::BM + bn));
       const double cost = (double) waves * (10000.0 + kb * per_kb);
       if (cost < best_cost) { best_cost = cost; best_bn = bn; best_split = split; }
     }
   }
   tc::Params p;
-  const int nseg = three_pass ? 3 : 1;
-  const void* as[2] = {a, d->a_small};
-  const void* bs[2] = {b, d->b_small};
-  for (int s = 0; plan == nullptr && s < (d->a_small != nullptr ? 2 : 1); ++s) {
-    int rc = encode_operand(&p.map_a[s], as[s], M, K, lda, d->a_mn_major, tc::BM, esz);
+  memset(&p, 0, sizeof(p));
+  if (plan == nullptr) {
+    int rc = encode_operand(&p.map_a, a, M, K, lda, d->a_mn_major, tc::BM, esz);
     if (rc != B2_OK) return rc;
-    rc = encode_operand(&p.map_b[s], bs[s], N, K, ldb, d->b_mn_major, best_bn, esz);
+    rc = encode_operand(&p.map_b, b, N, K, ldb, d->b_mn_major, best_bn, esz);
     if (rc != B2_OK) return rc;
-  }
-  // TMA-store epilogue for a plain C output (no split-K reduction, no accumulate, no second output):
-  // C is described as an (N, M) fp32 tensor with pitch ldc and written in 32 x 32 boxes
-  p.tma_store = 0;
-  if (best_split == 1 && !d->beta_accumulate && d->c_small == nullptr && d->c_pre == nullptr && tma_ok(c, ldc)) {
-    b2_encode_tiled_fn enc = plan != nullptr ? nullptr : b2_get_encode();
-    cuuint64_t dims[2] = {(cuuint64_t) N, (cuuint64_t) M}, strides[1] = {(cuuint64_t) ldc * 4};
-    cuuint32_t box[2] = {32, 32}, estr[2] = {1, 1};
-    if (plan != nullptr) p.tma_store = 1;
-    if (enc != nullptr &&
-        enc(&p.map_c, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
-      p.tma_store = 1;
-  }
-  {
-    static const bool off = [] { const char* e = getenv("B2_GEMM_TMA_STORE"); return e != nullptr && atoi(e) == 0; }();
-    if (off) p.tma_store = 0;
   }
   p.c = c; p.c_small = reinterpret_cast<float*>(d->c_small); p.c_pre = d->c_pre; p.ldc = ldc; p.ld_aux = ld_aux;
   p.bias = d->bias; p.mul = d->mul; p.add = d->add;
   p.ybwd = d->ybwd; p.colsum = d->colsum;
-  p.M = (int) M; p.N = (int) N; p.K = (int) K; p.bn = best_bn; p.nseg = nseg; p.inline_split = inline_split ? 1 : 0; p.act = d->act;
-  p.act_bwd = d->act_bwd; p.esz = esz;
+  p.M = (int) M; p.N = (int) N; p.K = (int) K; p.act = d->act; p.act_bwd = d->act_bwd; p.esz = esz;
   p.a_mn = d->a_mn_major ? 1 : 0; p.b_mn = d->b_mn_major ? 1 : 0;
   p.beta = d->beta_accumulate ? 1 : 0;
   p.kb_per_split = (int) b2_ceil_div(num_kb, best_split);
@@ -1010,81 +735,38 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   const int64_t tiles_n = b2_ceil_div(N, best_bn);
   const int64_t total_tiles = tiles_m * tiles_n * splits;
   B2_REQUIRE(total_tiles < (1ll << 31), "too many tiles");
-  const bool multi = total_tiles > B2_NUM_SMS;        // some CTA processes more than one tile
-  if (nseg == 1) {
-    p.nmain = 1;
-  } else {
-    // Accumulation chains of the main product: the truncating accumulator loses accuracy with the LENGTH of
-    // a chain, so the K range is cut into as many chains as TMEM holds (<= 4).  Fewer, longer chains were
-    // measured (B2_X3_CHAIN_KB = k-blocks per chain): 0.003 ms faster per step, but 64 per chain gives
-    // 2.1-2.8e-6 vs fp64 at K = 8,192 and even 16 per chain breaks the 1e-5 MLP-chain parity at 500-wide
-    // layers — the default (0) keeps every chain TMEM has room for.
-    static const int chain_kb = [] { const char* e = getenv("B2_X3_CHAIN_KB"); return e ? atoi(e) : 0; }();
-    const int fit = 512 / best_bn - 1;                 // all of TMEM: nmain main chains + 1 correction
-    p.nmain = chain_kb > 0 ? (int) b2_ceil_div(p.kb_per_split, chain_kb) : fit;
-    if (p.nmain > fit) p.nmain = fit;
-    if (p.nmain > 4) p.nmain = 4;
-    if (p.nmain > p.kb_per_split) p.nmain = p.kb_per_split;
-    if (p.nmain < 1) p.nmain = 1;
-  }
-  // Two accumulator stages (the epilogue of tile j under the main loop of tile j+1) when a CTA has
-  // several tiles and both stages fit the 512 TMEM columns; 3xTF32 gives up chains for it only down to 2
-  // (or to the k-block count of a short contraction).
-  p.nacc = 1;
-  if (multi) {
-    int nm = p.nmain;
-    const int corr = nseg > 1 ? 1 : 0;
-    while (nm > 1 && 2 * (nm + corr) * best_bn > 512) --nm;
-    const int floor_nm = (nseg > 1) ? (p.nmain < 2 ? p.nmain : 2) : 1;
-    if (2 * (nm + corr) * best_bn <= 512 && nm >= floor_nm) { p.nmain = nm; p.nacc = 2; }
-  }
-  {
-    const int need = p.nacc * (p.nmain + (nseg > 1 ? 1 : 0)) * best_bn;
-    int cols = 32;
-    while (cols < need) cols <<= 1;
-    p.tmem_cols = cols;
-  }
   p.tiles_m = (int) tiles_m; p.tiles_n = (int) tiles_n; p.splits = splits;
-  if (plan == nullptr && splits > 1 && !p.beta && !(d->flags & B2_GEMM_C_IS_ZERO)) {
+  size_t smem = 0;
+  switch (best_bn * 2 + (three_pass ? 1 : 0)) {
+    case 64: smem = gemm_smem_bytes<32, false>(); break;
+    case 65: smem = gemm_smem_bytes<32, true>(); break;
+    case 128: smem = gemm_smem_bytes<64, false>(); break;
+    case 129: smem = gemm_smem_bytes<64, true>(); break;
+    default: smem = gemm_smem_bytes<128, false>(); break;
+  }
+  B2_REQUIRE(smem <= (size_t) 227 * 1024, "tile does not fit shared memory");
+  if (plan != nullptr) {
+    plan->bn = best_bn; plan->splits = splits; plan->stages = tc::RSTAGES; plan->cstages = tc::CSTAGES;
+    plan->grid = (int) total_tiles; plan->threads = tc::NTHREADS; plan->tiles_m = p.tiles_m; plan->tiles_n = p.tiles_n;
+    plan->passes = three_pass ? 3 : 1; plan->kb_per_split = p.kb_per_split; plan->smem_bytes = (int64_t) smem;
+    return B2_OK;
+  }
+  if (splits > 1 && !p.beta && !(d->flags & B2_GEMM_C_IS_ZERO)) {
     cudaError_t e = cudaMemset2DAsync(c, (size_t) ldc * 4, 0, (size_t) N * 4, (size_t) M, st);
     if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
   }
-  if (plan == nullptr && d->colsum != nullptr && !(d->flags & B2_GEMM_COLSUM_IS_ZERO)) {
+  if (d->colsum != nullptr && !(d->flags & B2_GEMM_COLSUM_IS_ZERO)) {
     cudaError_t e = cudaMemsetAsync(d->colsum, 0, sizeof(float) * (size_t) N, st);
     if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
   }
-  // operand ring: 4 stages of {A, B}, or 3 of {A, As, B, Bs} for 3xTF32 — one fewer when the widest
-  // 3xTF32 tile (bn = 160) would not leave room for the epilogue patches under 227 KB
-  const size_t stage_bytes = (nseg > 1 ? (size_t) 2 : (size_t) 1) * (tc::A_BYTES + (size_t) best_bn * 128);
-  const int grid = (int) (total_tiles < B2_NUM_SMS ? total_tiles : B2_NUM_SMS);     // persistent: at most one CTA per SM
-  // (one tile per CTA: the epilogue patches reuse the ring, see the kernel)
-  const size_t fixed_bytes = (total_tiles <= grid ? 0 : tc::PATCH_BYTES) + 1024 + 192;
-  p.dbg = 0; p.trace = nullptr;
-#ifdef B2_GEMM_PROBE
-  { const char* e = getenv("B2_GEMM_DBG"); p.dbg = e ? atoi(e) : 0; }
-  { const char* e = getenv("B2_GEMM_TRACE"); p.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 0)) : nullptr; }
-#endif
-  p.stages = tc::MAX_STAGES;       // as deep as 227 KB allows (3xTF32 stages are twice the size)
-  if (p.dbg & 8) p.stages = 2;
-  while (p.stages > 2 && p.stages * stage_bytes + fixed_bytes > (size_t) 227 * 1024) --p.stages;
-  B2_REQUIRE(p.stages * stage_bytes + fixed_bytes <= (size_t) 227 * 1024, "tile does not fit shared memory");
-  B2_REQUIRE(p.stages * stage_bytes >= (size_t) tc::PATCH_BYTES, "ring smaller than the epilogue patches");
-  const size_t smem = p.stages * stage_bytes + fixed_bytes;
-  if (plan != nullptr) {
-    plan->bn = p.bn; plan->splits = p.splits; plan->stages = p.stages; plan->nacc = p.nacc; plan->nmain = p.nmain;
-    plan->tmem_cols = p.tmem_cols; plan->grid = grid; plan->threads = tc::NTHREADS; plan->tiles_m = p.tiles_m;
-    plan->tiles_n = p.tiles_n; plan->tma_store = p.tma_store; plan->passes = nseg; plan->kb_per_split = p.kb_per_split;
-    plan->smem_bytes = (int64_t) smem;
-    return B2_OK;
+  const int grid = (int) total_tiles;
+  switch (best_bn * 2 + (three_pass ? 1 : 0)) {
+    case 64: return gemm_launch<32, false>(p, grid, st);
+    case 65: return gemm_launch<32, true>(p, grid, st);
+    case 128: return gemm_launch<64, false>(p, grid, st);
+    case 129: return gemm_launch<64, true>(p, grid, st);
+    default: return gemm_launch<128, false>(p, grid, st);
   }
-  // opt-in to > 48 KB of dynamic shared memory: an idempotent per-process property of the kernel
-  // (C++11 guarantees the initialiser runs once, thread-safely)
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(
-      tc::gemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (attr_rc != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: smem attribute: %s", cudaGetErrorString(attr_rc));
-  B2_LAUNCH(tc::gemm_tf32_kernel, grid, tc::NTHREADS, smem, st, p);
-  B2_CUDA_LAUNCH_CHECK("b2_gemm_tc");
-  return B2_OK;
 }
 
 extern "C" B2_API int b2_gemm_tc_ex(const b2_gemm_desc* d, void* stream) { return gemm_tc_impl(d, stream, nullptr); }

@@ -1,4 +1,4 @@
-// interact.cu — feature-interaction kernels over the (fields x emb_dim) tile, sm_100a.
+// interact.cu — feature-interaction kernels over the (fields x emb_dim) tile, sm_90a.
 //
 // Reference semantics (reczoo/FuxiCTR v2.3.10):
 //   InnerProductInteraction.forward  fuxictr/pytorch/layers/interactions/inner_product.py:41-70

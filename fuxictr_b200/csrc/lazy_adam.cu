@@ -1,5 +1,5 @@
 // lazy_adam.cu — row-wise evaluation of the reference's DENSE Adam semantics for embedding tables
-// (see b2_lazy_ctx in include/fuxictr_b200.h), sm_100a.
+// (see b2_lazy_ctx in include/fuxictr_b200.h), sm_90a.
 //
 // BaseModel.train_step (fuxictr/pytorch/models/rank_model.py:321-322) clips and then lets
 // torch.optim.Adam update EVERY row of every table, although only ~B*F rows carry a gradient.  A row

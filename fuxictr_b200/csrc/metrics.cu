@@ -1,4 +1,4 @@
-// metrics.cu — device-resident evaluation metrics (SURVEY.md 8f row 3), sm_100a.
+// metrics.cu — device-resident evaluation metrics (SURVEY.md 8f row 3), sm_90a.
 //
 // BaseModel.evaluate (fuxictr/pytorch/models/rank_model.py:350-381) copies y_pred / y_true to the
 // host after EVERY batch, grows Python lists, and hands float64 arrays to sklearn's log_loss and

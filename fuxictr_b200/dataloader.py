@@ -3,7 +3,7 @@
 The reference's loaders hold a split as ONE (N, input_length + n_labels) numpy matrix
 (`np.column_stack` over features + labels: npz_dataloader.py:63-66, parquet_dataloader.py:65-74),
 hand single ROWS to torch's DataLoader, re-stack them with `default_collate`, and slice the batch
-into per-feature column views (`BatchCollator`, npz_dataloader.py:111-125).  The B200 input path
+into per-feature column views (`BatchCollator`, npz_dataloader.py:111-125).  The H100 input path
 (pipeline.TrainPipeline) wants exactly that (B, W) matrix, pinned, before it is sliced — so these
 loaders skip the row-by-row round trip:
 

@@ -372,13 +372,14 @@ def gemm_f32(a, b, out, a_t=False, b_t=False, bias=None, act=B2_ACT_NONE, mul=No
 
 # Matmul arithmetic of the dense layers:
 #   "fp32"   FFMA SIMT kernel (b2_gemm_f32)                       — bit-for-bit the reference's class
-#   "tf32x3" tcgen05 tensor cores, error-compensated 3xTF32       — fp32-class accuracy (1e-5 parity)
-#   "tf32"   tcgen05 tensor cores, single TF32 pass (10-bit mantissa, >= the bf16 of BASELINE configs[1])
-#   "bf16"   tcgen05 kind::f16 on bf16 copies of the operands, fp32 accumulation (BASELINE configs[1] "bf16");
+#   "tf32x3" wgmma tensor cores, error-compensated 3xTF32         — fp32-class accuracy (1e-5 parity)
+#   "tf32"   wgmma tensor cores, single TF32 pass (10-bit mantissa, >= the bf16 of BASELINE configs[1])
+#   "bf16"   wgmma .bf16 on bf16 copies of the operands, fp32 accumulation (BASELINE configs[1] "bf16");
 #            activations / weights / gradients stay fp32 in HBM, every producer also emits the bf16 operand
 #            3xTF32 reads the fp32 operands alone and derives the small parts in shared memory inside the
-#            GEMM (B2_GEMM_X3_INLINE, default); set_x3_inline(False) / B2_X3_INLINE=0 selects the older
-#            layout where every producer also writes its small part to HBM (kept as the A/B baseline)
+#            GEMM (B2_GEMM_X3_INLINE, default); set_x3_inline(False) / B2_X3_INLINE=0 exercises the ABI's other
+#            3xTF32 form: producers also write small parts to HBM and pass them as a_small / b_small, which the
+#            GEMM does not read — extra launches and traffic for identical results, kept for testing that form
 _MATMUL = {"mode": "fp32", "x3_inline": os.environ.get("B2_X3_INLINE", "1") != "0"}
 
 
@@ -425,7 +426,7 @@ def transpose_f32(t, want_small):
 def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=None, act=B2_ACT_NONE,
             mul=None, add=None, ybwd=None, act_bwd=B2_ACT_NONE, out_small=None, colsum=None, accumulate=False,
             out_pre=None, out_is_zero=False):
-    """out (M,N) = epi(sum_k A(m,k) B(n,k)) on the tcgen05 kernel (b2_gemm_tc_ex).  a is (M,K), or (K,M) when
+    """out (M,N) = epi(sum_k A(m,k) B(n,k)) on the wgmma kernel (b2_gemm_tc_ex).  a is (M,K), or (K,M) when
     a_mn (MN-major: the tensor is consumed as it lies, no transpose); b is (N,K), or (K,N) when b_mn.
     a_small / b_small: the operands' 3xTF32 small parts (both or neither).  Epilogue extras: ybwd/act_bwd
     (activation backward of the gradient's producer), out_small (3xTF32 small part of out), colsum (N)."""
@@ -593,9 +594,9 @@ def _tc_layer_ok(weight):
 class _LinearAct(torch.autograd.Function):
     """y = act(x W^T + b): nn.Linear (+ReLU/Sigmoid) of MLP_Block (mlp_block.py:74-80).
 
-    Three arithmetic paths: the N = 1 output head (GEMV kernels), the tcgen05 tensor-core GEMM
-    (TF32 / 3xTF32; dX and dW consume W, dZ and X as they lie in memory through MN-major operand
-    descriptors — no transposes), and the fp32 SIMT GEMM.  The backward fuses activation-backward,
+    Three arithmetic paths: the N = 1 output head (GEMV kernels), the wgmma tensor-core GEMM
+    (TF32 / 3xTF32; dX and dW consume W, dZ and X as they lie in memory as MN-major operands —
+    no transposes in HBM), and the fp32 SIMT GEMM.  The backward fuses activation-backward,
     the 3xTF32 split and the bias gradient into a single pass over dY."""
 
     @staticmethod

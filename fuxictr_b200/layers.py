@@ -2,7 +2,7 @@
 
 Same class names, constructor signatures, child-module names (hence state_dict keys),
 initialisation order and forward signatures as ``fuxictr.pytorch.layers`` — the modules
-are *parameter containers*; their forwards dispatch to the sm_100a kernels of
+are *parameter containers*; their forwards dispatch to the sm_90a kernels of
 libfuxictr_b200.so through fuxictr_b200.functional.  CUDA tensors are required: a CPU
 tensor raises (there is no CPU implementation on this path).
 
@@ -158,7 +158,7 @@ class FeatureEmbeddingDict(nn.Module):
         if kind in ("categorical", "sequence"):
             if self.use_pretrain and "pretrained_emb" in spec:
                 raise NotImplementedError(
-                    "feature %s: pretrained_emb is outside the B200 hot path "
+                    "feature %s: pretrained_emb is outside the H100 hot path "
                     "(SURVEY.md section 2 row 2); keep the reference module for it" % name)
             return nn.Embedding(spec["vocab_size"], width, padding_idx=spec.get("padding_idx", None))
         return None

@@ -25,7 +25,7 @@ def _check_metrics(metrics):
             continue
         if m in ("gAUC", "avgAUC", "MRR") or m.startswith("NDCG"):
             raise NotImplementedError("metric={} is a per-group host metric of the reference "
-                                      "(fuxictr/metrics.py:49-72); not on the B200 path.".format(m))
+                                      "(fuxictr/metrics.py:49-72); not on the H100 path.".format(m))
         raise ValueError("metric={} not supported.".format(m))       # metrics.py:52
 
 

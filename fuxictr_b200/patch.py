@@ -1,4 +1,4 @@
-"""enable(): route the UNMODIFIED reference's hot-path layers through the B200 kernels.
+"""enable(): route the UNMODIFIED reference's hot-path layers through the H100 kernels.
 
 On a machine that has reczoo/FuxiCTR installed, ``import fuxictr_b200.patch as p; p.enable()``
 (before or after building a model) swaps the ``forward`` of the reference's own layer classes —

@@ -68,7 +68,7 @@ class RankModel(nn.Module):
         self._optimizer_name = "Adam" if str(optimizer).lower() == "adam" else optimizer
         self.optimizer = getattr(torch.optim, self._optimizer_name)(self.parameters(), lr=lr)
         if loss not in self._LOSSES:
-            raise NotImplementedError("loss={} is not supported on the B200 path.".format(loss))
+            raise NotImplementedError("loss={} is not supported on the H100 path.".format(loss))
         self.loss_fn = torch.nn.functional.binary_cross_entropy
 
     def reset_parameters(self):
@@ -152,7 +152,7 @@ class RankModel(nn.Module):
         self.materialize_tables()
         return predict_generator(self, data_generator)
 
-    # -- B200 extension: flat arenas + 2-kernel clip/Adam -------------------------------------
+    # -- H100 extension: flat arenas + 2-kernel clip/Adam -------------------------------------
     def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=True):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
@@ -363,7 +363,7 @@ class DCNv2(RankModel):
                                     embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
                                     **kwargs)
         if use_low_rank_mixture:
-            raise NotImplementedError("CrossNetMix is outside the B200 hot path (SURVEY.md section 2 row 6)")
+            raise NotImplementedError("CrossNetMix is outside the H100 hot path (SURVEY.md section 2 row 6)")
         if model_structure not in self._STRUCTURES:
             raise AssertionError("model_structure={} not supported!".format(model_structure))
         self.model_structure = model_structure

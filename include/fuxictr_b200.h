@@ -1,5 +1,5 @@
 /*
- * fuxictr_b200.h — C-ABI of the B200 (sm_100a) hot path for FuxiCTR models.
+ * fuxictr_b200.h — C-ABI of the H100 (sm_90a) hot path for FuxiCTR models.
  *
  * The reference (reczoo/FuxiCTR v2.3.10) has no FFI: its hot path is a set of
  * torch.nn.Module classes that dispatch to stock ATen ops.  Every entry point
@@ -64,12 +64,12 @@ extern "C" {
 B2_API const char* b2_version(void);
 B2_API const char* b2_last_error(void);
 /* Returns the compute capability major*10+minor of `device`, or a negative
- * error.  The library only contains sm_100a code. */
+ * error.  The library only contains sm_90a code. */
 B2_API int b2_device_cc(int device);
 /* Sets cudaLimitMaxL2FetchGranularity (32, 64 or 128 bytes) on the current device: how much L2 pulls
  * from HBM around a missing 32-byte sector.  Embedding rows are 64 bytes (D=16 fp32) at random
- * addresses; with 128-byte fetches every row read costs 128 bytes of DRAM traffic
- * (profiles/r1_gather_ceiling.md).  A context-wide hint; no effect on results. */
+ * addresses; with 128-byte fetches every row read costs 128 bytes of DRAM traffic.  A context-wide hint;
+ * no effect on results. */
 B2_API int b2_set_l2_fetch_granularity(int bytes);
 
 /*
@@ -361,7 +361,7 @@ B2_API int b2_din_softmax_bwd(const float* p, const float* g, const unsigned cha
  *           (CrossNetV2: mul = x_0, add = x_i).  NULL = absent.
  *   beta_accumulate != 0: C += result (used for gradient accumulation).
  * math: B2_F32 = fp32 FMA (parity path); B2_BF16 = operands rounded to bf16,
- * fp32 accumulate, on tcgen05 tensor cores when shapes allow.
+ * fp32 accumulate, on wgmma tensor cores when shapes allow.
  */
 B2_API int b2_gemm_f32(const float* a, int64_t a_rs, int64_t a_cs, const float* b, int64_t b_rs,
                 int64_t b_cs, float* c, int64_t ldc, int64_t M, int64_t N, int64_t K,
@@ -371,10 +371,11 @@ B2_API int b2_gemm_f32(const float* a, int64_t a_rs, int64_t a_cs, const float* 
 /*
  * Tensor-core dense layer: same contract as b2_gemm_f32 for the K-major case
  *   C[m,n] = epi( sum_k A[m,k] * B[n,k] + bias[n] ),  A (M,K) ld=lda, B (N,K) ld=ldb, fp32,
- * computed by a TMA-fed tcgen05.mma kind::tf32 kernel with the accumulator in TMEM.
+ * computed by a TMA-fed wgmma .tf32 kernel with the accumulators in registers.
  *   a_small == b_small == NULL : single-pass TF32 (operand mantissas truncated to 10 bits).
- *   a_small, b_small given      : error-compensated 3xTF32 (fp32-class accuracy); they hold
- *                                 x - tf32_trunc(x) of A and B (same shapes/lds), see b2_split_tf32.
+ *   a_small, b_small given      : error-compensated 3xTF32 (fp32-class accuracy).  The pointers act as a
+ *                                 mode flag: their contents are NOT read (the kernel derives the small
+ *                                 parts of A and B itself); only their TMA alignment is checked.
  * Operands must be TMA-addressable (16-byte aligned base, ld % 4 == 0): b2_gemm_tc_supported()
  * says whether they are; otherwise B2_E_UNSUPPORTED is returned and the caller uses b2_gemm_f32.
  */
@@ -387,8 +388,8 @@ B2_API int b2_gemm_tc(const float* a, int64_t lda, const float* b, int64_t ldb, 
 
 /*
  * The general tensor-core contraction:  C[m,n] = epi( sum_k A(m,k) * B(n,k) ).
- * Operand layouts (the tensor core reads either through its shared-memory matrix descriptor, so
- * no transpose pass is ever needed):
+ * Operand layouts (TMA loads either as it lies and the kernel re-lays it out in shared memory, so
+ * no transpose pass in global memory is ever needed):
  *   a_mn_major == 0:  A in memory (M, K), k contiguous, leading dimension lda   ("K-major")
  *   a_mn_major != 0:  A in memory (K, M), m contiguous, leading dimension lda   ("MN-major")
  *   likewise b_mn_major for B: (N, K) or (K, N).
@@ -402,10 +403,10 @@ B2_API int b2_gemm_tc(const float* a, int64_t lda, const float* b, int64_t ldb, 
  *                                  sigmoid_backward of the reference's autograd);
  *   C = v (+ C if beta_accumulate);  c_small = v - tf32_trunc(v) (the consumer's 3xTF32 operand);
  *   colsum[n] = sum_m v  (bias gradient; the call zeroes colsum first).
- * mul, add, ybwd, c_small share C's leading dimension.  a_small/b_small: 3xTF32 small parts of the
- * operands (same layout as the operands) or both NULL for single-pass TF32.
+ * mul, add, ybwd, c_small share C's leading dimension.  a_small/b_small: both non-NULL selects 3xTF32
+ * (contents not read, see b2_gemm_tc; B2_GEMM_X3_INLINE selects it without them), both NULL single-pass TF32.
  * elem_dtype == B2_BF16 (BASELINE configs[1] "bf16"): a and b hold bf16 (row pitch a multiple of 16
- * bytes, i.e. leading dimensions % 8 == 0), one pass of tcgen05.mma kind::f16 with fp32 accumulation;
+ * bytes, i.e. leading dimensions % 8 == 0), one pass of wgmma .bf16 with fp32 accumulation;
  * C stays fp32 and c_small, if given, receives C rounded to bf16 (leading dimension ld_aux) — the
  * next contraction's operand.  b2_to_bf16 makes that operand for tensors no epilogue produced.
  */
@@ -427,7 +428,7 @@ typedef struct b2_gemm_desc {
   int32_t a_mn_major, b_mn_major;
   int32_t act, act_bwd;
   int32_t beta_accumulate;
-  int32_t elem_dtype;     /* B2_F32 (kind::tf32 on raw fp32) or B2_BF16 (kind::f16, fp32 accumulation) */
+  int32_t elem_dtype;     /* B2_F32 (wgmma .tf32 passes on fp32) or B2_BF16 (wgmma .bf16, fp32 accumulation) */
   int64_t ld_aux;         /* leading dimension of c_small (0 = ldc) */
   int64_t flags;          /* B2_GEMM_*: the caller vouches an output is already all-zero (skips its memset) */
 } b2_gemm_desc;
@@ -436,10 +437,10 @@ typedef struct b2_gemm_desc {
 #define B2_GEMM_X3_INLINE 4      /* 3xTF32 from the fp32 operands alone: the small parts are made in shared memory */
 B2_API int b2_gemm_tc_ex(const b2_gemm_desc* desc, void* stream);
 /* The launch plan b2_gemm_tc_ex would use for `desc` (pure host arithmetic: no device call, no stream): lets a
-   host-only test check that every plan fits the SM (<= 227 KB of shared memory, <= 512 TMEM columns). */
+   host-only test check that every plan fits the SM (<= 227 KB of shared memory).  stages: raw TMA tiles in
+   flight; cstages: converted (swizzled, split) tiles in flight; grid: one CTA per tile and K split. */
 typedef struct b2_gemm_plan {
-  int32_t bn, splits, stages, nacc, nmain, tmem_cols, grid, threads, tiles_m, tiles_n, tma_store, passes, kb_per_split;
-  int32_t pad_;
+  int32_t bn, splits, stages, cstages, grid, threads, tiles_m, tiles_n, passes, kb_per_split;
   int64_t smem_bytes;
 } b2_gemm_plan;
 B2_API int b2_gemm_tc_plan(const b2_gemm_desc* desc, b2_gemm_plan* plan);

@@ -124,9 +124,9 @@ def _plan(M, N, K, a_mn=False, b_mn=False, mode="tf32x3", epilogue=False, lda=No
 
 def test_gemm_plans_fit_the_sm():
     """Host-only: for a sweep of shapes, operand majors, arithmetic modes and epilogues the launch plan of
-    the tcgen05 GEMM stays inside one SM — <= 227 KB of dynamic shared memory, <= 512 TMEM columns, a ring
-    of >= 2 stages, at most one CTA per SM, tiles that cover the problem.  (A 239 KB plan once reached the
-    GPU as `invalid argument`; this sweep runs without one.)"""
+    the wgmma GEMM stays inside one SM — <= 227 KB of dynamic shared memory, rings of >= 2 stages, accumulator
+    tiles that fit the registers, one CTA per tile, tiles that cover the problem.  (A 239 KB plan once reached
+    the GPU as `invalid argument`; this sweep runs without one.)"""
     import itertools
     shapes = [(4096, 300, 624), (4096, 624, 300), (300, 624, 4096), (8192, 624, 624), (624, 624, 8192), (2048, 500, 432),
               (65536, 64, 415), (64, 415, 65536), (128, 32, 32), (76, 44, 36), (1, 16, 8), (130, 18, 40), (4096, 1024, 1024),
@@ -140,20 +140,18 @@ def test_gemm_plans_fit_the_sm():
         p = _plan(M, N, K, a_mn, b_mn, mode, epi)
         tag = (M, N, K, a_mn, b_mn, mode, epi)
         assert 1024 <= p.smem_bytes <= 227 * 1024, tag
-        assert 2 <= p.stages <= 4, tag
-        assert p.tmem_cols in (32, 64, 128, 256, 512), tag
-        slots = p.nmain + (1 if p.passes == 3 else 0)
-        assert p.nacc in (1, 2) and p.nacc * slots * p.bn <= p.tmem_cols <= 512, tag
-        assert p.bn % 32 == 0 and 32 <= p.bn <= 256, tag
-        if b_mn and esz == 2:
-            assert p.bn % 64 == 0, tag
+        assert 2 <= p.stages <= 4 and 2 <= p.cstages <= 4, tag
+        assert p.passes == (3 if mode.startswith("tf32x3") else 1), tag
+        assert p.bn in (32, 64, 128), tag
+        if p.passes == 3:
+            assert p.bn <= 64, tag        # main, partial and correction accumulators: 3 x bn/2 registers a thread
         assert p.tiles_m * 128 >= M and p.tiles_n * p.bn >= N and (p.tiles_n - 1) * p.bn < N, tag
         kb = -(-K // (128 // esz))
         assert p.splits >= 1 and p.splits * p.kb_per_split >= kb and (p.splits - 1) * p.kb_per_split < kb, tag
         if epi:
             assert p.splits == 1, tag     # a non-linear epilogue cannot be split over K
-        assert 1 <= p.grid <= 148 and p.grid <= p.tiles_m * p.tiles_n * p.splits, tag
-        assert p.threads == 320, tag
+        assert p.grid == p.tiles_m * p.tiles_n * p.splits, tag
+        assert p.threads == 384, tag
         checked += 1
     assert checked > 400
 

@@ -13,7 +13,7 @@ import torch
 
 from conftest import GOLDEN, ROOT
 
-from baseline import refenv  # noqa: E402  (the unmodified reference under baseline/_ref)
+from baseline import refenv  # noqa: E402  (the unmodified reference under oracle/_ref)
 HAVE_REF = refenv.available()
 FIXTURES = os.path.join(ROOT, "tests", "golden", "data")
 

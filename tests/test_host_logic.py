@@ -2,6 +2,8 @@
 state_dict keys (pinned by reference goldens), launch plans, and the refusal to compute
 on CPU tensors (there is no fallback path)."""
 
+import os
+
 import pytest
 import torch
 
@@ -130,7 +132,7 @@ def test_batch_views_alias_the_matrix_for_sequences_too():
 
 
 # ---------------------------------------------------------------------------------------------
-# Mirror constructors vs the LIVE reference (baseline/_ref): same seed => bit-identical state_dict
+# Mirror constructors vs the reference (stored from its own classes): same seed => bit-identical state_dict
 # (keys, shapes, registration order, RNG consumption order), over more configurations than the goldens.
 # ---------------------------------------------------------------------------------------------
 _SEQ_SPECS = [
@@ -168,28 +170,31 @@ _MIRROR_CASES = [
 ]
 
 
-@pytest.mark.parametrize("name,specs,kwargs", _MIRROR_CASES, ids=["%s-%d" % (c[0], i) for i, c in enumerate(_MIRROR_CASES)])
-def test_mirror_constructors_match_the_live_reference_seed_for_seed(name, specs, kwargs):
-    from baseline import refenv
-    if not refenv.available():
-        pytest.skip(refenv.why_unavailable())
-    refenv.import_reference()
-    ref_cls = refenv.load_model_class(name)
+def mirror_case_id(i):
+    return "%s-%d" % (_MIRROR_CASES[i][0], i)
+
+
+@pytest.mark.parametrize("name,specs,kwargs", _MIRROR_CASES, ids=[mirror_case_id(i) for i in range(len(_MIRROR_CASES))])
+def test_mirror_constructors_match_the_reference_seed_for_seed(name, specs, kwargs):
+    """What the reference's own classes built under the same seed is stored in tests/golden/mirror_init.json
+    (tests/golden/make_mirror_golden.py): keys, dtypes, shapes, SHA-256 of every tensor, module tree."""
+    import hashlib
+    import json
+    from conftest import GOLDEN
+    with open(os.path.join(GOLDEN, "mirror_init.json")) as fd:
+        ref = json.load(fd)[mirror_case_id(_MIRROR_CASES.index((name, specs, kwargs)))]
     emb_dim = kwargs["embedding_dim"]
     torch.manual_seed(4242)
-    ref = ref_cls(refenv.synthetic_feature_map(specs, embedding_dim=emb_dim), model_root="/tmp/b2_mirror/",
-                  metrics=["AUC"], verbose=0, gpu=-1, optimizer="adam", loss="binary_crossentropy", **kwargs)
-    torch.manual_seed(4242)
     ours = getattr(zoo, name)(FeatureMap.from_specs(specs, embedding_dim=emb_dim), gpu=-1, **kwargs)
-    sd_ref, sd = ref.state_dict(), ours.state_dict()
-    assert list(sd.keys()) == list(sd_ref.keys())
-    for k, v in sd_ref.items():
-        assert sd[k].dtype == v.dtype and sd[k].shape == v.shape, k
-        assert torch.equal(sd[k], v), k
+    sd = ours.state_dict()
+    assert list(sd.keys()) == [k for k, _, _, _ in ref["state_dict"]]
+    for k, dtype, shape, digest in ref["state_dict"]:
+        assert str(sd[k].dtype) == dtype and list(sd[k].shape) == shape, k
+        assert hashlib.sha256(sd[k].detach().contiguous().cpu().numpy().tobytes()).hexdigest() == digest, k
     # module tree: same names, and the same torch module type wherever the reference uses a stock one
-    ref_mods = dict(ref.named_modules())
+    ref_mods = ref["modules"]
     for mname, mod in ours.named_modules():
         assert mname in ref_mods, mname
-        if type(ref_mods[mname]).__module__.startswith("torch."):
-            assert type(mod) is type(ref_mods[mname]), mname
+        if ref_mods[mname] is not None:
+            assert type(mod).__module__ + "." + type(mod).__name__ == ref_mods[mname], mname
     assert set(ref_mods) == set(dict(ours.named_modules()))
