@@ -18,13 +18,18 @@
 //     round-to-nearest, so the error does not grow with the length of the contraction.
 //   bf16 operands (elem_dtype B2_BF16): wgmma .bf16, 64-element k-blocks, fp32 accumulation.
 //
-// Structure (one CTA per 128 x BN output tile and K split; 384 threads):
-//   warpgroup 0    thread 0 issues cp.async.bulk.tensor loads of the raw operand tiles into a 3-stage
-//                  mbarrier ring; the whole warpgroup converts each raw tile (either major, fp32 or bf16)
-//                  into the K-major 128B-swizzled tiles wgmma reads — big and small parts for 3xTF32 —
-//                  in a second 3-stage ring.  wgmma reads tf32 operands from shared memory only in K-major
-//                  form, so this pass is what lets MN-major operands stay as they lie in HBM.
-//   warpgroups 1-2 64 rows each: wgmma m64nBNk8 (tf32) / k16 (bf16) from the converted tiles, then the fused
+// Structure (one CTA per 128 x BN output tile and K split; 384 threads), one ring of 2-4 stages:
+//   K-major operands are loaded by TMA with the 128B swizzle, straight into the layout wgmma reads; wgmma
+//   .tf32 reads an fp32 value as its truncation big(x), so the raw tile is the big part (DESIGN.md §4).
+//   MN-major operands land unswizzled in a staging tile of the same stage; wgmma reads tf32 from shared memory
+//   only K-major, so they are transposed into the swizzled tile in shared memory and stay as they lie in HBM.
+//   warp 0         one thread issues the TMA loads of a stage as soon as the consumers release it.
+//   warps 1-3      converter: MN-major staging -> swizzled tile; 3xTF32: the small parts of A and B, written at
+//                  the offsets of the swizzled tile in their own tiles (no re-layout).
+//   warpgroups 1-2 64 rows each: wgmma m64nBNk8 (tf32) / k16 (bf16), both operands from shared memory.  3xTF32
+//                  commits each k-block as two groups, the main product and then the cross terms; the main
+//                  product is folded into the sum while the cross terms still run, and a stage is released
+//                  one k-block later.  The single-pass modes likewise keep one group in flight.  Then the fused
 //                  epilogue straight from the accumulator registers (each quad of lanes writes 32 contiguous
 //                  bytes of one output row).
 // Kernels of a step are chained with programmatic dependent launch (prologue under the predecessor's tail).
@@ -36,9 +41,26 @@
 
 namespace tc {
 constexpr int BM = 128;          // two consumer warpgroups x wgmma M = 64
-constexpr int NTHREADS = 384;    // converter warpgroup + two wgmma warpgroups
-constexpr int RSTAGES = 3;       // raw TMA tiles in flight
-constexpr int CSTAGES = 3;       // converted tiles in flight
+constexpr int NTHREADS = 384;    // producer / converter warpgroup + two wgmma warpgroups
+constexpr int NCONV = 96;        // converter threads (warps 1-3)
+enum Mode { TF32 = 0, BF16 = 1, X3 = 2 };
+
+// Shared memory of one pipeline stage: the swizzled A and B tiles wgmma reads, their small parts (3xTF32), and
+// unswizzled staging tiles where an MN-major operand lands.  Every tile starts 1024-byte aligned.
+template <int BN, int MODE>
+struct Ring {
+  static constexpr uint32_t A_BYTES = BM * 128, B_BYTES = BN * 128;
+  static constexpr uint32_t OFF_B = A_BYTES;
+  static constexpr uint32_t OFF_AS = OFF_B + B_BYTES;                               // A small (3xTF32)
+  static constexpr uint32_t OFF_BS = OFF_AS + (MODE == X3 ? A_BYTES : 0);           // B small (3xTF32)
+  static constexpr uint32_t OFF_SA = OFF_BS + (MODE == X3 ? B_BYTES : 0);           // A staging (MN-major)
+  static constexpr uint32_t OFF_SB = OFF_SA + A_BYTES;                              // B staging (MN-major)
+  static constexpr uint32_t STAGE = OFF_SB + B_BYTES;
+  static constexpr uint32_t EXTRA = 1024 + 128;                                     // alignment slack, mbarriers
+  static constexpr int STAGES = (227u * 1024u - EXTRA) / STAGE >= 4 ? 4 : (int) ((227u * 1024u - EXTRA) / STAGE);
+  static constexpr size_t SMEM = (size_t) STAGES * STAGE + EXTRA;
+  static_assert(STAGES >= 2, "ring does not fit shared memory");
+};
 
 struct Params {
   CUtensorMap map_a;
@@ -85,17 +107,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: ~2 s at 2 GHz, then report and trap (never hang the device).
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int which) {
+// Bounded wait: ~2 s at 2 GHz, then trap (never hang the device).  No printf: a function call anywhere in the
+// kernel makes ptxas serialise every wgmma (C7510).
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("b2 tc_gemm: mbarrier wait timed out (role %d, block %d,%d,%d)\n", which, blockIdx.x,
-             blockIdx.y, blockIdx.z);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar,
                                             int c0, int c1) {
@@ -121,6 +139,7 @@ __device__ __forceinline__ float tf32_big(float v) { return __uint_as_float(__fl
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // wgmma.mma_async m64nNk8 (tf32) / m64nNk16 (bf16), both operands from shared memory, fp32 accumulators
 // d[] in the wgmma fragment layout; scale_d == 0 overwrites the accumulators.
@@ -167,61 +186,59 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t a, uint64_t 
       : "l"(a), "l"(b), "r"(scale_d));
 }
 
-// 16 bytes of K-major fp32 operand -> the converted tile: big part (13 low mantissa bits cleared) and, for
-// 3xTF32, the small part at the same offset in the small tile.
-template <bool X3>
+// What the converter writes for 16 bytes of operand: bf16 as it is; for fp32 the big part (13 low mantissa bits
+// cleared), or the big part and, at the same offset in the small tile, the small part.
+enum Split { RAW = 0, BIG = 1, BIG_SMALL = 2 };
+template <int SPLIT>
 __device__ __forceinline__ void store_split(uint8_t* dst, uint32_t small_off, uint32_t off, const float4& v) {
+  static_assert(SPLIT != RAW, "fp32 tiles are stored split");
   *reinterpret_cast<float4*>(dst + off) = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
-  if (X3)
+  if (SPLIT == BIG_SMALL)
     *reinterpret_cast<float4*>(dst + small_off + off) =
         make_float4(tf32_small(v.x), tf32_small(v.y), tf32_small(v.z), tf32_small(v.w));
 }
 
-// One operand's k-block as TMA wrote it -> K-major 128B-swizzled tile of `rows` rows, by the 128 threads of
-// the converter warpgroup.  Raw layouts: K-major (rows, 128 B of k); MN-major (k, rows): 32 fp32 or 64 bf16
-// k-rows of `rows` elements, transposed here in registers (4 x 4 fp32 or 8 x 8 bf16 per thread).
-template <bool X3>
-__device__ __forceinline__ void convert_tile(const uint8_t* src, uint8_t* dst, uint32_t small_off, int rows, int mn,
-                                             int esz, int ct) {
-  if (esz == 2) {
-    if (!mn) {
-      for (int q = ct; q < rows * 8; q += 128)
-        *reinterpret_cast<uint4*>(dst + swz(q >> 3, q & 7)) = *reinterpret_cast<const uint4*>(src + 16 * q);
-    } else {
-      for (int b = ct; b < rows; b += 128) {
-        const int kq = b & 7, r0 = (b >> 3) * 8;
-        uint4 v[8];
+// One MN-major k-block as TMA wrote it — (k, rows): 32 fp32 or 64 bf16 k-rows of `rows` elements — into the
+// K-major 128B-swizzled tile of `rows` rows, transposed in registers (4 x 4 fp32 or 8 x 8 bf16 per thread).
+template <bool BF, int SPLIT>
+__device__ __forceinline__ void transpose_tile(const uint8_t* src, uint8_t* dst, uint32_t small_off, int rows, int ct) {
+  if constexpr (BF) {
+    for (int b = ct; b < rows; b += NCONV) {
+      const int kq = b & 7, r0 = (b >> 3) * 8;
+      uint4 v[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const uint4*>(src + ((8 * kq + j) * rows + r0) * 2);
+      for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const uint4*>(src + ((8 * kq + j) * rows + r0) * 2);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          uint32_t w[4];
+      for (int i = 0; i < 8; ++i) {
+        uint32_t w[4];
 #pragma unroll
-          for (int j = 0; j < 8; j += 2) {
-            const uint32_t lo = reinterpret_cast<const uint16_t*>(&v[j])[i];
-            const uint32_t hi = reinterpret_cast<const uint16_t*>(&v[j + 1])[i];
-            w[j >> 1] = lo | (hi << 16);
-          }
-          *reinterpret_cast<uint4*>(dst + swz(r0 + i, kq)) = make_uint4(w[0], w[1], w[2], w[3]);
+        for (int j = 0; j < 8; j += 2) {
+          const uint32_t lo = reinterpret_cast<const uint16_t*>(&v[j])[i];
+          const uint32_t hi = reinterpret_cast<const uint16_t*>(&v[j + 1])[i];
+          w[j >> 1] = lo | (hi << 16);
         }
+        *reinterpret_cast<uint4*>(dst + swz(r0 + i, kq)) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
-    return;
-  }
-  if (!mn) {
-    for (int q = ct; q < rows * 8; q += 128)
-      store_split<X3>(dst, small_off, swz(q >> 3, q & 7), *reinterpret_cast<const float4*>(src + 16 * q));
   } else {
-    for (int b = ct; b < 2 * rows; b += 128) {
+    for (int b = ct; b < 2 * rows; b += NCONV) {
       const int kq = b & 7, r0 = (b >> 3) * 4;
       float4 v[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((4 * kq + j) * rows + r0) * 4);
-      store_split<X3>(dst, small_off, swz(r0 + 0, kq), make_float4(v[0].x, v[1].x, v[2].x, v[3].x));
-      store_split<X3>(dst, small_off, swz(r0 + 1, kq), make_float4(v[0].y, v[1].y, v[2].y, v[3].y));
-      store_split<X3>(dst, small_off, swz(r0 + 2, kq), make_float4(v[0].z, v[1].z, v[2].z, v[3].z));
-      store_split<X3>(dst, small_off, swz(r0 + 3, kq), make_float4(v[0].w, v[1].w, v[2].w, v[3].w));
+      store_split<SPLIT>(dst, small_off, swz(r0 + 0, kq), make_float4(v[0].x, v[1].x, v[2].x, v[3].x));
+      store_split<SPLIT>(dst, small_off, swz(r0 + 1, kq), make_float4(v[0].y, v[1].y, v[2].y, v[3].y));
+      store_split<SPLIT>(dst, small_off, swz(r0 + 2, kq), make_float4(v[0].z, v[1].z, v[2].z, v[3].z));
+      store_split<SPLIT>(dst, small_off, swz(r0 + 3, kq), make_float4(v[0].w, v[1].w, v[2].w, v[3].w));
     }
+  }
+}
+
+// The small part of a swizzled fp32 tile, written at the same offsets of the small tile: no re-layout.
+__device__ __forceinline__ void small_tile(const uint8_t* src, uint8_t* dst, int rows, int ct) {
+  for (int q = ct; q < rows * 8; q += NCONV) {
+    const float4 v = *reinterpret_cast<const float4*>(src + 16 * q);
+    *reinterpret_cast<float4*>(dst + 16 * q) = make_float4(tf32_small(v.x), tf32_small(v.y), tf32_small(v.z), tf32_small(v.w));
   }
 }
 
@@ -252,37 +269,36 @@ __device__ __forceinline__ float epilogue_elem(const Params& p, int m, int n, fl
   return t;
 }
 
-template <int BN, bool X3>
+template <int BN, int MODE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
+  using R = Ring<BN, MODE>;
+  constexpr int S = R::STAGES;
   constexpr int NR = BN / 2;                            // accumulators per thread: 64 x BN per warpgroup
-  constexpr uint32_t TILE_BYTES = (BM + BN) * 128;      // one k-block of A and B (raw, or converted big part)
-  constexpr uint32_t CONV_BYTES = (X3 ? 2 : 1) * TILE_BYTES;
+  constexpr int BKE = MODE == BF16 ? 64 : 32;           // k elements per k-block: one 128-byte swizzle row
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte aligned bases: align by hand (1 KB of slack is requested).
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* raw0 = smem;
-  uint8_t* conv0 = smem + RSTAGES * TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(conv0 + CSTAGES * CONV_BYTES);
-  const uint32_t rfull0 = smem_u32(bars), cfull0 = smem_u32(bars + RSTAGES),
-                 cempty0 = smem_u32(bars + RSTAGES + CSTAGES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * R::STAGE);
+  // per stage: TMA landed; converter done; consumers done (the producer may refill it)
+  const uint32_t full0 = smem_u32(bars), conv0 = smem_u32(bars + S), empty0 = smem_u32(bars + 2 * S);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int bke = 128 / p.esz;                      // k elements per k-block: one 128-byte swizzle row
-  const int num_kb_total = (p.K + bke - 1) / bke;
+  const int num_kb_total = (p.K + BKE - 1) / BKE;
   const int tiles_mn = p.tiles_m * p.tiles_n;
   const int z = blockIdx.x / tiles_mn, rr = blockIdx.x - z * tiles_mn;
   const int m0 = (rr / p.tiles_n) * BM, n0 = (rr % p.tiles_n) * BN;
   const int kb_begin = z * p.kb_per_split;
   const int nkb = min(num_kb_total, kb_begin + p.kb_per_split) - kb_begin;
+  const bool conv = MODE == X3 || p.a_mn || p.b_mn;    // the converter has work in every stage
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.map_b)) : "memory");
-    for (int s = 0; s < RSTAGES; ++s) mbar_init(rfull0 + 8 * s, 1);
-    for (int s = 0; s < CSTAGES; ++s) {
-      mbar_init(cfull0 + 8 * s, 4);      // one arrival per converter warp
-      mbar_init(cempty0 + 8 * s, 8);     // one arrival per consumer warp
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full0 + 8 * s, 1);
+      mbar_init(conv0 + 8 * s, NCONV / 32);   // one arrival per converter warp
+      mbar_init(empty0 + 8 * s, 8);           // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -294,80 +310,107 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
   b2_pdl_wait();
 
   if (warp < 4) {
-    // ---------------- warpgroup 0: TMA (thread 0) and operand conversion ----------------
-    const int ct = threadIdx.x;
-    auto load = [&](int i) {
-      const int s = i % RSTAGES, kb = kb_begin + i;
-      const uint32_t dst = smem_u32(raw0 + s * TILE_BYTES), bar = rfull0 + 8 * s;
-      mbar_expect_tx(bar, TILE_BYTES);   // out-of-range parts of a box arrive zero-filled and count in full
-      if (p.a_mn) tma_load_2d(dst, &p.map_a, bar, m0, kb * bke);
-      else tma_load_2d(dst, &p.map_a, bar, kb * bke, m0);
-      if (p.b_mn) tma_load_2d(dst + BM * 128, &p.map_b, bar, n0, kb * bke);
-      else tma_load_2d(dst + BM * 128, &p.map_b, bar, kb * bke, n0);
-    };
-    if (ct == 0)
-      for (int i = 0; i < RSTAGES && i < nkb; ++i) load(i);
-    for (int i = 0; i < nkb; ++i) {
-      const int rs = i % RSTAGES, cs = i % CSTAGES;
-      mbar_wait(rfull0 + 8 * rs, (uint32_t) (i / RSTAGES) & 1u, 0);
-      mbar_wait(cempty0 + 8 * cs, ((uint32_t) (i / CSTAGES) & 1u) ^ 1u, 1);
-      const uint8_t* src = raw0 + rs * TILE_BYTES;
-      uint8_t* dst = conv0 + cs * CONV_BYTES;
-      convert_tile<X3>(src, dst, TILE_BYTES, BM, p.a_mn, p.esz, ct);
-      convert_tile<X3>(src + BM * 128, dst + BM * 128, TILE_BYTES, BN, p.b_mn, p.esz, ct);
-      // generic-proxy stores -> visible to wgmma (async proxy) before the consumers are told
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(cfull0 + 8 * cs);
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // every converter thread is done with raw stage rs
-      if (ct == 0 && i + RSTAGES < nkb) load(i + RSTAGES);
+    // ---------------- warpgroup 0: TMA producer (warp 0) and converter (warps 1-3) ----------------
+    if (warp == 0) {
+      if (lane == 0) {
+        for (int i = 0; i < nkb; ++i) {
+          const int s = i % S, kb = kb_begin + i;
+          if (i >= S) mbar_wait(empty0 + 8 * s, ((uint32_t) (i / S) & 1u) ^ 1u);
+          const uint32_t st = smem_u32(smem + s * R::STAGE), bar = full0 + 8 * s;
+          mbar_expect_tx(bar, R::A_BYTES + R::B_BYTES);   // out-of-range parts of a box arrive zero-filled, count in full
+          if (p.a_mn) tma_load_2d(st + R::OFF_SA, &p.map_a, bar, m0, kb * BKE);
+          else tma_load_2d(st, &p.map_a, bar, kb * BKE, m0);
+          if (p.b_mn) tma_load_2d(st + R::OFF_SB, &p.map_b, bar, n0, kb * BKE);
+          else tma_load_2d(st + R::OFF_B, &p.map_b, bar, kb * BKE, n0);
+        }
+      }
+    } else if (conv) {
+      const int ct = threadIdx.x - 32;
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % S;
+        mbar_wait(full0 + 8 * s, (uint32_t) (i / S) & 1u);
+        uint8_t* st = smem + s * R::STAGE;
+        if constexpr (MODE == BF16) {
+          if (p.a_mn) transpose_tile<true, RAW>(st + R::OFF_SA, st, 0, BM, ct);
+          if (p.b_mn) transpose_tile<true, RAW>(st + R::OFF_SB, st + R::OFF_B, 0, BN, ct);
+        } else if constexpr (MODE == TF32) {
+          if (p.a_mn) transpose_tile<false, BIG>(st + R::OFF_SA, st, 0, BM, ct);
+          if (p.b_mn) transpose_tile<false, BIG>(st + R::OFF_SB, st + R::OFF_B, 0, BN, ct);
+        } else {
+          if (p.a_mn) transpose_tile<false, BIG_SMALL>(st + R::OFF_SA, st, R::OFF_AS, BM, ct);
+          else small_tile(st, st + R::OFF_AS, BM, ct);
+          if (p.b_mn) transpose_tile<false, BIG_SMALL>(st + R::OFF_SB, st + R::OFF_B, R::OFF_BS - R::OFF_B, BN, ct);
+          else small_tile(st + R::OFF_B, st + R::OFF_BS, BN, ct);
+        }
+        // generic-proxy stores -> visible to wgmma (async proxy) before the consumers are told
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncwarp();
+        if (lane == 0) mbar_arrive(conv0 + 8 * s);
+      }
     }
   } else {
     // ---------------- warpgroups 1-2: wgmma on rows 64 g .. 64 g + 63 of the tile, then the epilogue ----------
     const int g = (warp >> 2) - 1;
+    auto ready = [&](int i) -> const uint8_t* {
+      const int s = i % S;
+      const uint32_t ph = (uint32_t) (i / S) & 1u;
+      mbar_wait(full0 + 8 * s, ph);
+      if (conv) mbar_wait(conv0 + 8 * s, ph);
+      return smem + s * R::STAGE;
+    };
+    auto release = [&](int i) {        // k-block i's wgmma group has completed: its stage may be refilled
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + 8 * (i % S));
+    };
     float acc[NR];
-    float part[X3 ? NR : 1], corr[X3 ? NR : 1];
 #pragma unroll
     for (int r = 0; r < NR; ++r) acc[r] = 0.f;
+    if constexpr (MODE == X3) {
+      float corr[NR], part[NR];
 #pragma unroll
-    for (int r = 0; r < (X3 ? NR : 1); ++r) { part[r] = 0.f; corr[r] = 0.f; }
-    for (int i = 0; i < nkb; ++i) {
-      const int cs = i % CSTAGES;
-      mbar_wait(cfull0 + 8 * cs, (uint32_t) (i / CSTAGES) & 1u, 2);
-      const uint32_t base = smem_u32(conv0 + cs * CONV_BYTES);
-      // one instruction consumes 32 bytes of K per row (8 tf32 / 16 bf16): +2 in the (addr >> 4) field
-      const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + BM * 128);
-      wgmma_fence();
-      if constexpr (X3) {
-        const uint64_t asd = ad + (TILE_BYTES >> 4), bsd = bd + (TILE_BYTES >> 4);
+      for (int r = 0; r < NR; ++r) { corr[r] = 0.f; part[r] = 0.f; }
+      for (int i = 0; i < nkb; ++i) {
+        const uint32_t base = smem_u32(ready(i));
+        // one instruction consumes 32 bytes of K per row (8 tf32): +2 in the (addr >> 4) field
+        const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R::OFF_B),
+                       asd = make_smem_desc(base + R::OFF_AS + g * 64 * 128), bsd = make_smem_desc(base + R::OFF_BS);
+        // two groups: the main product A_big.B_big from zero into part, then the cross terms into corr
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_tf32(part, ad + 2 * k, bd + 2 * k, k > 0 ? 1u : 0u);   // A_big . B_big
+        for (int k = 0; k < 4; ++k) wgmma_tf32(part, ad + 2 * k, bd + 2 * k, k > 0 ? 1u : 0u);        // A_big . B_big
+        wgmma_commit();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          wgmma_tf32(corr, ad + 2 * k, bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                  // A_big . B_small
-          wgmma_tf32(corr, asd + 2 * k, bd + 2 * k, 1u);                                         // A_small . B_big
+          wgmma_tf32(corr, ad + 2 * k, bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                    // A_big . B_small
+          wgmma_tf32(corr, asd + 2 * k, bd + 2 * k, 1u);                                           // A_small . B_big
         }
-      } else {
-        if (p.esz == 2) {
+        wgmma_commit();
+        // all but the cross group just committed are done: fold this k-block's main product (fp32
+        // round-to-nearest) while the cross terms run, and release the previous k-block's stage
+        wgmma_wait1();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_bf16(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
-        } else {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_tf32(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
-        }
+        for (int r = 0; r < NR; ++r) acc[r] += part[r];
+        if (i > 0) release(i - 1);
       }
-      wgmma_commit();
       wgmma_wait0();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(cempty0 + 8 * cs);     // the converted stage may be overwritten
-      if constexpr (X3) {
-#pragma unroll
-        for (int r = 0; r < NR; ++r) acc[r] += part[r];   // this k-block's main product, fp32 round-to-nearest
-      }
-    }
-    if constexpr (X3) {
 #pragma unroll
       for (int r = 0; r < NR; ++r) acc[r] += corr[r];
+    } else {
+      for (int i = 0; i < nkb; ++i) {
+        const uint32_t base = smem_u32(ready(i));
+        // one instruction consumes 32 bytes of K per row (8 tf32 / 16 bf16): +2 in the (addr >> 4) field
+        const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R::OFF_B);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if constexpr (MODE == BF16) wgmma_bf16(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
+          else wgmma_tf32(acc, ad + 2 * k, bd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait1();
+        if (i > 0) release(i - 1);
+      }
+      wgmma_wait0();
     }
     // wgmma fragment: d[4j + 2h + e] is row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e of the warpgroup
     const int row0 = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -609,7 +652,7 @@ static b2_encode_tiled_fn b2_get_encode() {
 
 // K-major operand: memory (rows, K), K contiguous, leading dimension ld; box = 128 B of k x box_rows rows.
 // MN-major operand: memory (K, rows), rows contiguous, leading dimension ld; box = box_rows rows x 128 B of k.
-// Unswizzled: the converter warpgroup writes the swizzled layout wgmma reads.
+// K-major boxes land 128B-swizzled, the layout wgmma reads; MN-major ones unswizzled, for the converter to transpose.
 static int encode_operand(CUtensorMap* map, const void* base, int64_t rows, int64_t K, int64_t ld,
                           int mn_major, int box_rows, int esz) {
   b2_encode_tiled_fn enc = b2_get_encode();
@@ -626,7 +669,8 @@ static int encode_operand(CUtensorMap* map, const void* base, int64_t rows, int6
   }
   CUresult r = enc(map, esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                    const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   mn_major ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return b2_fail(B2_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int) r);
   return B2_OK;
 }
@@ -644,15 +688,10 @@ extern "C" B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const fl
 
 // plan != NULL: fill in the launch plan (tile shape, ring depths, shared memory) and return without
 // touching the device — pure host arithmetic, so the CPU test-suite can sweep it (tests/test_abi.py).
-template <int BN, bool X3>
-static size_t gemm_smem_bytes() {
-  const size_t tile = (size_t) (tc::BM + BN) * 128;
-  return tc::RSTAGES * tile + tc::CSTAGES * (X3 ? 2 : 1) * tile + 1024 + 128;   // + alignment slack, mbarriers
-}
-template <int BN, bool X3>
+template <int BN, int MODE>
 static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
-  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, X3>;
-  const size_t smem = gemm_smem_bytes<BN, X3>();
+  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE>;
+  const size_t smem = tc::Ring<BN, MODE>::SMEM;
   // opt-in to > 48 KB of dynamic shared memory: an idempotent per-process property of each instantiation
   // (C++11 guarantees the initialiser runs once, thread-safely)
   static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
@@ -660,6 +699,28 @@ static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
   B2_LAUNCH(kern, grid, tc::NTHREADS, smem, st, p);
   B2_CUDA_LAUNCH_CHECK("b2_gemm_tc");
   return B2_OK;
+}
+
+// One kernel instantiation per tile width and arithmetic mode (tf32 and bf16 single pass, 3xTF32 up to bn = 64).
+struct GemmInst {
+  int (*launch)(const tc::Params&, int, cudaStream_t);
+  size_t smem;
+  int stages;
+};
+template <int BN, int MODE>
+static GemmInst gemm_inst_of() { return {gemm_launch<BN, MODE>, tc::Ring<BN, MODE>::SMEM, tc::Ring<BN, MODE>::STAGES}; }
+static GemmInst gemm_inst(int bn, int mode) {
+  switch (bn * 4 + mode) {
+    case 32 * 4 + tc::TF32: return gemm_inst_of<32, tc::TF32>();
+    case 64 * 4 + tc::TF32: return gemm_inst_of<64, tc::TF32>();
+    case 128 * 4 + tc::TF32: return gemm_inst_of<128, tc::TF32>();
+    case 32 * 4 + tc::BF16: return gemm_inst_of<32, tc::BF16>();
+    case 64 * 4 + tc::BF16: return gemm_inst_of<64, tc::BF16>();
+    case 128 * 4 + tc::BF16: return gemm_inst_of<128, tc::BF16>();
+    case 32 * 4 + tc::X3: return gemm_inst_of<32, tc::X3>();
+    case 64 * 4 + tc::X3: return gemm_inst_of<64, tc::X3>();
+    default: return {nullptr, 0, 0};
+  }
 }
 
 static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan) {
@@ -700,18 +761,23 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   int best_bn = 0, best_split = 1;
   double best_cost = 1e300;
   const int bn_max = three_pass ? 64 : 128;
-  // cycles per k-block: the tensor pipe needs passes x 4 instructions x bn/2 (m64 per warpgroup, two in
-  // parallel), the converter warpgroup moves (128 + bn) rows of 128 bytes (2x for the small parts)
-  const double mma_per_bn = (three_pass ? 3.0 : 1.0) * 2.0;
-  const double conv_per_row = three_pass ? 4.0 : 3.0;
   for (int bn = 32; bn <= bn_max; bn *= 2) {
+    // Cycles per k-block: the larger of the tensor pipe — passes x 4 instructions x bn/2 (m64 per warpgroup, two
+    // in parallel) — and shared memory at 128 B (one tile row) a cycle.  Shared-memory rows: TMA writes A and B;
+    // the converter reads and writes an MN-major tile again, and in 3xTF32 reads each tile and writes its small
+    // part (both in one pass for an MN-major tile); wgmma reads 64 rows of A and B per pass and warpgroup.
+    const bool mn_a = d->a_mn_major != 0, mn_b = d->b_mn_major != 0;
+    const double rows_tma = tc::BM + bn;
+    const double rows_conv = (mn_a ? 2.0 : 0.0) * tc::BM + (mn_b ? 2.0 : 0.0) * bn +
+                             (three_pass ? (mn_a ? 1.0 : 2.0) * tc::BM + (mn_b ? 1.0 : 2.0) * bn : 0.0);
+    const double rows_mma = (three_pass ? 3.0 : 1.0) * 2.0 * (64 + bn);
+    const double per_kb = fmax((three_pass ? 3.0 : 1.0) * 2.0 * bn, rows_tma + rows_conv + rows_mma);
     const int64_t tiles_n = b2_ceil_div(N, bn);
     for (int split = 1; split <= 32; split *= 2) {
       if (split > 1 && (!linear || num_kb / split < 8)) break;
       const int64_t ctas = tiles_m * tiles_n * split;
       const int64_t waves = b2_ceil_div(ctas, B2_NUM_SMS);
       const double kb = (double) b2_ceil_div(num_kb, split);
-      const double per_kb = fmax(mma_per_bn * bn, conv_per_row * (double) (tc::BM + bn));
       const double cost = (double) waves * (10000.0 + kb * per_kb);
       if (cost < best_cost) { best_cost = cost; best_bn = bn; best_split = split; }
     }
@@ -736,19 +802,13 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   const int64_t total_tiles = tiles_m * tiles_n * splits;
   B2_REQUIRE(total_tiles < (1ll << 31), "too many tiles");
   p.tiles_m = (int) tiles_m; p.tiles_n = (int) tiles_n; p.splits = splits;
-  size_t smem = 0;
-  switch (best_bn * 2 + (three_pass ? 1 : 0)) {
-    case 64: smem = gemm_smem_bytes<32, false>(); break;
-    case 65: smem = gemm_smem_bytes<32, true>(); break;
-    case 128: smem = gemm_smem_bytes<64, false>(); break;
-    case 129: smem = gemm_smem_bytes<64, true>(); break;
-    default: smem = gemm_smem_bytes<128, false>(); break;
-  }
-  B2_REQUIRE(smem <= (size_t) 227 * 1024, "tile does not fit shared memory");
+  const GemmInst inst = gemm_inst(best_bn, three_pass ? tc::X3 : (esz == 2 ? tc::BF16 : tc::TF32));
+  B2_REQUIRE(inst.launch != nullptr, "no GEMM instantiation for bn %d", best_bn);
+  B2_REQUIRE(inst.smem <= (size_t) 227 * 1024, "tile does not fit shared memory");
   if (plan != nullptr) {
-    plan->bn = best_bn; plan->splits = splits; plan->stages = tc::RSTAGES; plan->cstages = tc::CSTAGES;
+    plan->bn = best_bn; plan->splits = splits; plan->stages = inst.stages; plan->cstages = inst.stages;
     plan->grid = (int) total_tiles; plan->threads = tc::NTHREADS; plan->tiles_m = p.tiles_m; plan->tiles_n = p.tiles_n;
-    plan->passes = three_pass ? 3 : 1; plan->kb_per_split = p.kb_per_split; plan->smem_bytes = (int64_t) smem;
+    plan->passes = three_pass ? 3 : 1; plan->kb_per_split = p.kb_per_split; plan->smem_bytes = (int64_t) inst.smem;
     return B2_OK;
   }
   if (splits > 1 && !p.beta && !(d->flags & B2_GEMM_C_IS_ZERO)) {
@@ -759,14 +819,7 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
     cudaError_t e = cudaMemsetAsync(d->colsum, 0, sizeof(float) * (size_t) N, st);
     if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
   }
-  const int grid = (int) total_tiles;
-  switch (best_bn * 2 + (three_pass ? 1 : 0)) {
-    case 64: return gemm_launch<32, false>(p, grid, st);
-    case 65: return gemm_launch<32, true>(p, grid, st);
-    case 128: return gemm_launch<64, false>(p, grid, st);
-    case 129: return gemm_launch<64, true>(p, grid, st);
-    default: return gemm_launch<128, false>(p, grid, st);
-  }
+  return inst.launch(p, (int) total_tiles, st);
 }
 
 extern "C" B2_API int b2_gemm_tc_ex(const b2_gemm_desc* d, void* stream) { return gemm_tc_impl(d, stream, nullptr); }

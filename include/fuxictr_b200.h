@@ -437,8 +437,9 @@ typedef struct b2_gemm_desc {
 #define B2_GEMM_X3_INLINE 4      /* 3xTF32 from the fp32 operands alone: the small parts are made in shared memory */
 B2_API int b2_gemm_tc_ex(const b2_gemm_desc* desc, void* stream);
 /* The launch plan b2_gemm_tc_ex would use for `desc` (pure host arithmetic: no device call, no stream): lets a
-   host-only test check that every plan fits the SM (<= 227 KB of shared memory).  stages: raw TMA tiles in
-   flight; cstages: converted (swizzled, split) tiles in flight; grid: one CTA per tile and K split. */
+   host-only test check that every plan fits the SM (<= 227 KB of shared memory).  stages: k-blocks in flight in
+   the operand ring; cstages: the same ring (loaded and converted tiles share a stage); grid: one CTA per tile
+   and K split. */
 typedef struct b2_gemm_plan {
   int32_t bn, splits, stages, cstages, grid, threads, tiles_m, tiles_n, passes, kb_per_split;
   int64_t smem_bytes;
