@@ -102,6 +102,11 @@ class LazyTables(object):
     def __init__(self, arena, tables):
         self.arena = arena
         self.tables = list(tables)
+        rows = sum(int(p.shape[0]) for p in self.tables)
+        if rows > 2 ** 31 - 1:
+            # worklist entries and the row numbers the kernels compute are int32
+            raise ValueError("lazy tables: %d rows on this device; at most 2^31 - 1 are supported (row-shard the "
+                             "tables over more GPUs)" % rows)
         dev = arena.P.device
         base = 0
         descs = (_lib.b2_lazy_table * len(self.tables))()
@@ -123,30 +128,39 @@ class LazyTables(object):
         self.opt = None
         self._ctx_cache = {}
 
+    def _new_ctx(self, emb_tables, lr_tables):
+        """b2_lazy_ctx with field i of the launch reading emb_tables[i] (and lr_tables[i])."""
+        opt, a = self.opt, self.arena
+        ctx = _lib.b2_lazy_ctx()
+        ctx.last_step, ctx.sched = self.last_step.data_ptr(), self.sched.data_ptr()
+        ctx.step_dev, ctx.mark = opt.step_dev.data_ptr(), self.mark.data_ptr()
+        ctx.worklist, ctx.counter = self.worklist.data_ptr(), self.counter.data_ptr()
+        ctx.delta_m = (opt.M.data_ptr() - a.P.data_ptr()) // 4
+        ctx.delta_v = (opt.V.data_ptr() - a.P.data_ptr()) // 4
+        # the same float32 roundings as make_const() in csrc/lazy_adam.cu / adam_kernel in dense.cu:
+        # beta is rounded to fp32 FIRST, then 1 - beta is taken in double and rounded again
+        b1, b2 = float(np.float32(opt.betas[0])), float(np.float32(opt.betas[1]))
+        ctx.w1, ctx.beta2 = float(np.float32(1.0 - b1)), b2
+        ctx.w2, ctx.eps = float(np.float32(1.0 - b2)), opt.eps
+        ctx.worklist_capacity = self.capacity
+        for i, t in enumerate(emb_tables):
+            ctx.grow_emb[i] = t._b2_grow_base
+        for i, t in enumerate(lr_tables or ()):
+            ctx.grow_lr[i] = t._b2_grow_base
+        return ctx
+
     def ctx_for(self, plan, lr_plan, emb_tables, lr_tables):
         key = (id(plan), id(lr_plan))
         ctx = self._ctx_cache.get(key)
         if ctx is None:
-            opt, a = self.opt, self.arena
-            ctx = _lib.b2_lazy_ctx()
-            ctx.last_step, ctx.sched = self.last_step.data_ptr(), self.sched.data_ptr()
-            ctx.step_dev, ctx.mark = opt.step_dev.data_ptr(), self.mark.data_ptr()
-            ctx.worklist, ctx.counter = self.worklist.data_ptr(), self.counter.data_ptr()
-            ctx.delta_m = (opt.M.data_ptr() - a.P.data_ptr()) // 4
-            ctx.delta_v = (opt.V.data_ptr() - a.P.data_ptr()) // 4
-            # the same float32 roundings as make_const() in csrc/lazy_adam.cu / adam_kernel in dense.cu:
-            # beta is rounded to fp32 FIRST, then 1 - beta is taken in double and rounded again
-            b1, b2 = float(np.float32(opt.betas[0])), float(np.float32(opt.betas[1]))
-            ctx.w1, ctx.beta2 = float(np.float32(1.0 - b1)), b2
-            ctx.w2, ctx.eps = float(np.float32(1.0 - b2)), opt.eps
-            ctx.worklist_capacity = self.capacity
-            for i, f in enumerate(plan.fields):
-                ctx.grow_emb[i] = emb_tables[f.table_slot]._b2_grow_base
-            if lr_plan is not None:
-                for i, f in enumerate(lr_plan.fields):
-                    ctx.grow_lr[i] = lr_tables[f.table_slot]._b2_grow_base
+            ctx = self._new_ctx([emb_tables[f.table_slot] for f in plan.fields],
+                                [lr_tables[f.table_slot] for f in lr_plan.fields] if lr_plan is not None else None)
             self._ctx_cache[key] = ctx
         return ctx
+
+    def shard_ctx(self, emb_tables, lr_tables):
+        """The context of a sharded front (one shard table per field): rows are this rank's local rows."""
+        return self._new_ctx(emb_tables, lr_tables)
 
     def materialize(self):
         """Bring every row up to date (before reading the tables outside the kernels)."""
@@ -231,8 +245,25 @@ class FusedAdam(object):
             self.lazy.counter.zero_()
 
     _stepped = False
+    group = None                 # sharded: the PeerGroup (fuxictr_b200.sharded) that sums a buffer over the ranks
 
     def step(self):
+        """clip + Adam.  A row-sharded step sums one buffer over the ranks midway (the norm term of the
+        shards, and the dense gradients unless they are already being summed on the side stream)."""
+        for buf in self.step_phases():
+            self._sum_over_ranks(buf)
+
+    def _sum_over_ranks(self, buf):
+        if self.group is not None:
+            self.group.all_reduce_sum(buf)
+        else:
+            import torch.distributed as dist
+            dist.all_reduce(buf, op=dist.ReduceOp.SUM)
+
+    def step_phases(self):
+        """The step as a generator: it yields each buffer that has to be summed over the ranks (row-sharded
+        runs: once) and finishes the step when resumed.  step() sums through the group; a driver of several
+        virtual ranks in one process (sharded.lockstep_steps) sums across them in lock step instead."""
         a = self.arena
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         if not torch.cuda.is_current_stream_capturing():
@@ -253,21 +284,31 @@ class FusedAdam(object):
             a.G.mul_(1.0 / dist.get_world_size())          # mean over the global batch (rank_model.py:130)
         sumsq_ptr = ctypes.c_void_p(0)
         if self.sharded:
-            import torch.distributed as dist
-            world = dist.get_world_size()
+            if self.group is not None:
+                world = self.group.world
+            else:
+                import torch.distributed as dist
+                world = dist.get_world_size()
             slot = a._G_ext[a.numel:a.numel + 1]               # rides behind the dense slice
             slot.zero_()
             if self.max_norm is not None and a.tail_offset > 0:
-                _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr()), a.tail_offset,
-                          ctypes.c_void_p(slot.data_ptr()), st)   # this rank's shard part of ||g||^2
+                if self.lazy is not None:   # only the enqueued rows carry a gradient: no pass over the shards
+                    lz = self.lazy
+                    _lib.call("b2_lazy_sumsq", ctypes.c_void_p(lz.tables_dev.data_ptr()), len(lz.tables),
+                              ctypes.c_void_p(lz.worklist.data_ptr()), ctypes.c_void_p(lz.counter.data_ptr()),
+                              lz.capacity, (a.G.data_ptr() - a.P.data_ptr()) // 4, ctypes.c_void_p(slot.data_ptr()),
+                              st)
+                else:
+                    _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr()), a.tail_offset,
+                              ctypes.c_void_p(slot.data_ptr()), st)   # this rank's shard part of ||g||^2
             if self._early_pending:
                 # the dense gradients are already being summed on the side stream: only the norm scalar here
-                dist.all_reduce(slot, op=dist.ReduceOp.SUM)
+                yield slot
                 torch.cuda.current_stream().wait_stream(self._side)
                 self._early_pending = False
             else:
-                # ONE collective: dense gradients (to be averaged) + the shard norm term (to be summed)
-                dist.all_reduce(a._G_ext[a.tail_offset:a.numel + 1], op=dist.ReduceOp.SUM)
+                # ONE sum: dense gradients (to be averaged) + the shard norm term (to be summed)
+                yield a._G_ext[a.tail_offset:a.numel + 1]
             dense = a.G[a.tail_offset:]
             if dense.numel() > 0 and not self.dense_prescaled:
                 dense.mul_(1.0 / world)                          # mean over the global batch

@@ -17,7 +17,7 @@
 // pass, ceil(F / (32/LPR)) passes with all index loads, then all row loads, in flight together;
 // field sums are xor-shuffle reductions over the (fields x emb_dim) register tile.
 #include "embed_common.cuh"
-#include "adam_common.cuh"
+#include "lazy_replay.cuh"
 
 namespace {
 
@@ -51,8 +51,6 @@ front_fwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
   // lazy tables: steps completed so far; a row with last_step < done replays the missed
   // zero-gradient Adam updates in registers (never written back here)
   const int done = lazy ? (int) *lz.step_dev : 0;
-  const B2AdamConst ac = {lz.w1, lz.beta2, lz.w2, lz.eps};
-  const B2AdamSched* sched = reinterpret_cast<const B2AdamSched*>(lz.sched);
 
   for (int64_t b = warp; b < batch; b += nwarps) {
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -87,49 +85,15 @@ front_fwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
         }
       }
       if (lazy) {
-        int last_e[MAX_PASSES], last_l[MAX_PASSES];
+        int fu[MAX_PASSES];
+        bool on_e[MAX_PASSES], on_l[MAX_PASSES];
 #pragma unroll
-        for (int u = 0; u < MAX_PASSES; ++u) {   // all last_step loads in flight
-          const int f = f0 + u * rows_per_pass + rg;
-          last_e[u] = done;
-          last_l[u] = done;
-          if (f < F && ok[u]) {
-            if (lane_on) last_e[u] = __ldg(lz.last_step + lz.grow_emb[f] + row[u]);
-            if (has_lr && sub == 0) last_l[u] = __ldg(lz.last_step + lz.grow_lr[f] + row[u]);
-          }
+        for (int u = 0; u < MAX_PASSES; ++u) {
+          fu[u] = f0 + u * rows_per_pass + rg;
+          on_e[u] = ok[u] && lane_on;            // ok[u] implies f < F
+          on_l[u] = ok[u] && has_lr && sub == 0;
         }
-        float4 m4[MAX_PASSES], v4[MAX_PASSES];
-        float m1[MAX_PASSES], v1[MAX_PASSES];
-#pragma unroll
-        for (int u = 0; u < MAX_PASSES; ++u) {   // all moment loads of stale rows in flight
-          const int f = f0 + u * rows_per_pass + rg;
-          m4[u] = v4[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          m1[u] = v1[u] = 0.f;
-          if (last_e[u] < done) {
-            const float* pp = reinterpret_cast<const float*>(sf.f[f].table) + row[u] * dim + e;
-            m4[u] = *reinterpret_cast<const float4*>(pp + lz.delta_m);
-            v4[u] = *reinterpret_cast<const float4*>(pp + lz.delta_v);
-          }
-          if (last_l[u] < done) {
-            const float* pp = reinterpret_cast<const float*>(lf.f[f].table) + row[u];
-            m1[u] = pp[lz.delta_m];
-            v1[u] = pp[lz.delta_v];
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < MAX_PASSES; ++u) {   // replay the missed zero-gradient updates
-          for (int k = last_e[u] + 1; k <= done; ++k) {
-            const B2AdamSched sc = sched[k];
-            b2_adam_apply(v[u].x, 0.f, m4[u].x, v4[u].x, ac, sc.x, sc.y);
-            b2_adam_apply(v[u].y, 0.f, m4[u].y, v4[u].y, ac, sc.x, sc.y);
-            b2_adam_apply(v[u].z, 0.f, m4[u].z, v4[u].z, ac, sc.x, sc.y);
-            b2_adam_apply(v[u].w, 0.f, m4[u].w, v4[u].w, ac, sc.x, sc.y);
-          }
-          for (int k = last_l[u] + 1; k <= done; ++k) {
-            const B2AdamSched sc = sched[k];
-            b2_adam_apply(w[u], 0.f, m1[u], v1[u], ac, sc.x, sc.y);
-          }
-        }
+        b2_lazy_replay<MAX_PASSES>(lz, done, sf, lf, dim, e, fu, row, on_e, on_l, v, w);
       }
 #pragma unroll
       for (int u = 0; u < MAX_PASSES; ++u) {
@@ -224,13 +188,13 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
             b2_red_add(reinterpret_cast<float*>(const_cast<void*>(ld.table)) + row, gl);
             if (lazy) {   // first toucher of the LR row this step enqueues it
               const int grow = (int) (lz.grow_lr[f] + row);
-              if (atomicExch(lz.mark + grow, tmark) != tmark) enq_l = grow;
+              if (b2_lazy_claim(lz, grow, tmark)) enq_l = grow;
             }
           }
         }
         if (lazy && drow != nullptr && sub == 0) {   // first toucher of the embedding row enqueues it
           const int grow = (int) (lz.grow_emb[f] + row);
-          if (atomicExch(lz.mark + grow, tmark) != tmark) enq_e = grow;
+          if (b2_lazy_claim(lz, grow, tmark)) enq_e = grow;
         }
       }
       if (drow != nullptr && e < dim) {
@@ -245,26 +209,7 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
         }
       }
     }
-    if (lazy) {
-      // warp-aggregated append: one atomicAdd on the shared counter per warp, not per row
-      const unsigned me = __ballot_sync(0xffffffffu, enq_e >= 0);
-      const unsigned ml = __ballot_sync(0xffffffffu, enq_l >= 0);
-      const int ne = __popc(me), nl = __popc(ml);
-      if (ne + nl > 0) {
-        int base = 0;
-        if (lane == 0) base = atomicAdd(lz.counter, ne + nl);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        const unsigned lt = (1u << lane) - 1u;
-        if (enq_e >= 0) {
-          const int pos = base + __popc(me & lt);
-          if (pos < lz.worklist_capacity) lz.worklist[pos] = enq_e;
-        }
-        if (enq_l >= 0) {
-          const int pos = base + ne + __popc(ml & lt);
-          if (pos < lz.worklist_capacity) lz.worklist[pos] = enq_l;
-        }
-      }
-    }
+    if (lazy) b2_lazy_append(lz, enq_e, enq_l, lane);   // one atomicAdd per warp, not per row
     // warp-level aggregation of duplicate destination rows (see scatter_bwd_kernel)
     const unsigned peers = __match_any_sync(0xffffffffu, (unsigned long long) drow);
     unsigned gset = 0;

@@ -24,6 +24,7 @@
 //  fuxictr/pytorch/layers/blocks/logistic_regression.py:55-58); the reference has no multi-GPU path.
 // Cross-rank ordering (ids visible -> push -> pushes landed -> ... ) is the caller's barrier.
 #include "embed_common.cuh"
+#include "lazy_replay.cuh"
 
 namespace {
 struct PeerPtrs {
@@ -42,16 +43,21 @@ struct BcastDst { void* p[16]; };
 
 #define B2_OWN_ZERO (1 << 18)    // out-of-range id: the slot is defined as a zero row, no gradient
 
+constexpr int SERVE_U = 4;       // list entries a lane group serves at once (loads in flight)
+
 // Two phases per 256-item chunk.  SCAN: one thread per (requester, sample, field) candidate reads the id
 // and keeps it only when this rank owns the row — the (world-1)/world candidates that belong to other
 // ranks cost one coalesced 4-byte load each.  SERVE: the block walks the compacted list in shared memory
 // with dim/4 lanes per entry (gather the table row, 16-byte P2P stores into the requester's slot), and
 // appends the entries that will receive a gradient to the rank's owned-row list with ONE global atomic
 // per chunk (a per-warp atomic on the one counter serialises ~1e5 times per launch at 8 ranks).
-template <typename IdxT>
+// LAZY: the tables are lazily evaluated (b2_lazy_ctx) — a separate instantiation, so that the plain
+// push keeps its register budget (and occupancy).
+template <typename IdxT, bool LAZY>
 __global__ void __launch_bounds__(256)
 shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr,
-                  const __grid_constant__ PeerPtrs peers, int64_t batch_local, int64_t ids_stride,
+                  const __grid_constant__ PeerPtrs peers, const __grid_constant__ b2_lazy_ctx lz,
+                  int64_t batch_local, int64_t ids_stride,
                   int dim, int lpr_log2, int has_lr, int world, int rank,
                   int32_t* __restrict__ status, int4* __restrict__ owned, int32_t* __restrict__ owned_count,
                   int32_t owned_cap) {
@@ -71,6 +77,8 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
   const int e = sub * 4;
   const int64_t per_rank = batch_local * (int64_t) F;
   const int64_t nitems = per_rank * world;
+  const int done = LAZY ? (int) *lz.step_dev : 0;   // lazy tables: steps completed so far
+  const int gstride = 256 >> lpr_log2;               // lane groups per block
   for (int64_t base = (int64_t) blockIdx.x * 256; base < nitems; base += (int64_t) gridDim.x * 256) {
     if (threadIdx.x == 0) { s_front = 0; s_back = 0; }
     __syncthreads();
@@ -114,22 +122,40 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
     __syncthreads();
     const int nfront = s_front, nback = s_back;
     if (threadIdx.x == 0 && nfront > 0) s_gbase = atomicAdd(owned_count, nfront);
-    // ---- serve
+    // ---- serve: SERVE_U entries per lane group at once, all row loads (and for lazy tables all
+    // last_step and moment loads) in flight; a stale row is brought up to date in registers before
+    // it is stored (lazy_replay.cuh), an out-of-range id stores a zero row
     const int nserve = nfront + nback;
-    for (int k = threadIdx.x >> lpr_log2; k < nserve; k += 256 >> lpr_log2) {
-      const int4 it = list[k < nfront ? k : 255 - (k - nfront)];
-      const int p = it.x, f = it.w & 0xffff;
-      const int64_t bf = it.y, lrow = it.z;
-      if (it.w & B2_OWN_ZERO) {
-        if (e < dim) *reinterpret_cast<float4*>(peers.emb[p] + bf * dim + e) = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (has_lr && sub == 0) peers.lrw[p][bf] = 0.f;
-      } else {
-        if (e < dim) {
-          const float4 v = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(sf.f[f].table) + lrow * dim + e));
-          *reinterpret_cast<float4*>(peers.emb[p] + bf * dim + e) = v;   // P2P store
-        }
-        if (has_lr && sub == 0)
-          peers.lrw[p][bf] = __ldg(reinterpret_cast<const float*>(lf.f[f].table) + lrow);
+    for (int k0 = threadIdx.x >> lpr_log2; k0 < nserve; k0 += SERVE_U * gstride) {
+      int4 it[SERVE_U];
+      int f[SERVE_U];
+      int64_t lrow[SERVE_U];
+      bool on_e[SERVE_U], on_l[SERVE_U];
+      float4 v[SERVE_U];
+      float w[SERVE_U];
+#pragma unroll
+      for (int u = 0; u < SERVE_U; ++u) {
+        const int k = k0 + u * gstride;
+        it[u] = (k < nserve) ? list[k < nfront ? k : 255 - (k - nfront)] : make_int4(-1, 0, 0, B2_OWN_ZERO);
+        f[u] = it[u].w & 0xffff;
+        lrow[u] = it[u].z;
+        const bool row_ok = !(it[u].w & B2_OWN_ZERO);
+        on_e[u] = row_ok && e < dim;
+        on_l[u] = row_ok && has_lr && sub == 0;
+        v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        w[u] = 0.f;
+        if (on_e[u])
+          v[u] = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(sf.f[f[u]].table) + lrow[u] * dim + e));
+        if (on_l[u]) w[u] = __ldg(reinterpret_cast<const float*>(lf.f[f[u]].table) + lrow[u]);
+      }
+      if (LAZY) b2_lazy_replay<SERVE_U>(lz, done, sf, lf, dim, e, f, lrow, on_e, on_l, v, w);
+#pragma unroll
+      for (int u = 0; u < SERVE_U; ++u) {
+        const int p = it[u].x;
+        if (p < 0) continue;
+        const int64_t bf = it[u].y;
+        if (e < dim) *reinterpret_cast<float4*>(peers.emb[p] + bf * dim + e) = v[u];   // P2P store
+        if (has_lr && sub == 0) peers.lrw[p][bf] = w[u];
       }
     }
     __syncthreads();
@@ -143,7 +169,8 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
 
 __global__ void __launch_bounds__(256)
 shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr,
-                  const __grid_constant__ PeerPtrs peers, int dim, int lpr_log2, int has_lr, float scale,
+                  const __grid_constant__ PeerPtrs peers, const __grid_constant__ b2_lazy_ctx lz, int lazy,
+                  int dim, int lpr_log2, int has_lr, float scale,
                   const int4* __restrict__ owned, const int32_t* __restrict__ owned_count, int32_t owned_cap) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(emb, smem_raw);
@@ -162,10 +189,12 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
   const int64_t ngroups = ((int64_t) gridDim.x * blockDim.x) >> lpr_log2;
   const int64_t group = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> lpr_log2;
   const int64_t warp_first = group - my_group;
+  const int tmark = lazy ? (int) *lz.step_dev + 1 : 0;   // the optimizer step these gradients feed
   for (int64_t wbase = warp_first; wbase < nitems; wbase += ngroups) {
     const int64_t item = wbase + my_group;
     float* drow = nullptr;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    int enq_e = -1, enq_l = -1;   // local rows (global over this rank's lazy tables) this lane enqueues
     if (item < nitems) {
       const int4 it = __ldg(owned + item);
       const int p = it.x, f = it.w & 0xffff;
@@ -173,6 +202,11 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
       const b2_field& fd = sf.f[f];
       if ((it.w & B2_OWN_EMB) && fd.table != nullptr) {
         drow = reinterpret_cast<float*>(const_cast<void*>(fd.table)) + lrow * dim;
+        // several requesters may send gradients for this row: the first of them this step enqueues it
+        if (lazy && sub == 0) {
+          const int grow = (int) (lz.grow_emb[f] + lrow);
+          if (b2_lazy_claim(lz, grow, tmark)) enq_e = grow;
+        }
         if (e < dim) {
           v = *reinterpret_cast<const float4*>(peers.gemb[p] + bf * dim + e);  // P2P load
           v.x *= scale; v.y *= scale; v.z *= scale; v.w *= scale;
@@ -180,10 +214,16 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
       }
       if (has_lr && sub == 0 && (it.w & B2_OWN_LR)) {
         const b2_field& ld = lf.f[f];
-        if (ld.table != nullptr)
+        if (ld.table != nullptr) {
           b2_red_add(reinterpret_cast<float*>(const_cast<void*>(ld.table)) + lrow, peers.glogit[p][bf / F] * scale);
+          if (lazy) {
+            const int grow = (int) (lz.grow_lr[f] + lrow);
+            if (b2_lazy_claim(lz, grow, tmark)) enq_l = grow;
+          }
+        }
       }
     }
+    if (lazy) b2_lazy_append(lz, enq_e, enq_l, lane);
     const unsigned peers_mask = __match_any_sync(0xffffffffu, (unsigned long long) drow);
     unsigned gset = 0;
     for (int g = 0; g < groups_per_warp; ++g) gset |= ((peers_mask >> (g << lpr_log2)) & 1u) << g;
@@ -352,14 +392,32 @@ int check_shard_args(const b2_field* emb, int nfields, int world, int rank) {
     B2_REQUIRE(emb[i].dim == dim && emb[i].seq_len == 1, "field %d: one common dim, no sequences", i);
   return B2_OK;
 }
+
+template <typename IdxT, typename... Args>
+int launch_push(bool lazy, int grid, size_t smem, cudaStream_t st, Args... args) {
+  if (lazy) shard_push_kernel<IdxT, true><<<grid, 256, smem, st>>>(args...);
+  else shard_push_kernel<IdxT, false><<<grid, 256, smem, st>>>(args...);
+  return B2_OK;
+}
+
+int check_lazy(const b2_lazy_ctx* lz) {
+  if (lz == nullptr) return B2_OK;
+  B2_REQUIRE(lz->last_step && lz->sched && lz->step_dev && lz->mark && lz->worklist && lz->counter,
+             "lazy context: NULL last_step / sched / step_dev / mark / worklist / counter");
+  B2_REQUIRE(lz->worklist_capacity >= 1, "lazy context: worklist_capacity %d", lz->worklist_capacity);
+  return B2_OK;
+}
 }  // namespace
 
-extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                    int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                                    int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                                    float* const* peer_lrw, int32_t* status, int32_t* owned,
-                                    int32_t* owned_count, int32_t owned_capacity, void* stream) {
+extern "C" B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                       int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                                       int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                                       float* const* peer_lrw, int32_t* status, int32_t* owned,
+                                       int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                       void* stream) {
   int rc = check_shard_args(emb_fields, nfields, world, rank);
+  if (rc != B2_OK) return rc;
+  rc = check_lazy(lazy);
   if (rc != B2_OK) return rc;
   B2_REQUIRE(peer_ids && peer_emb && (lr_fields == nullptr || peer_lrw != nullptr), "NULL peer pointer array");
   B2_REQUIRE(owned == nullptr || (owned_count != nullptr && owned_capacity >= 1), "owned list needs a counter and a capacity");
@@ -388,21 +446,35 @@ extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* 
   const size_t smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
   const int grid = grid_for(batch_local * (int64_t) nfields * world, 256);
   int4* ow = reinterpret_cast<int4*>(owned);
+  static thread_local b2_lazy_ctx lz_none;
+  const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
   switch (idx_dtype) {
-    case B2_F64: shard_push_kernel<double><<<grid, 256, smem, st>>>(epack, lpack, pp, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
-    case B2_I64: shard_push_kernel<int64_t><<<grid, 256, smem, st>>>(epack, lpack, pp, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
-    case B2_I32: shard_push_kernel<int32_t><<<grid, 256, smem, st>>>(epack, lpack, pp, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
+    case B2_F64: rc = launch_push<double>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
+    case B2_I64: rc = launch_push<int64_t>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
+    case B2_I32: rc = launch_push<int32_t>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
   B2_CUDA_LAUNCH_CHECK("b2_shard_push");
   return B2_OK;
 }
 
-extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                    int64_t batch_local, int world, int rank, const float* const* peer_gemb,
-                                    const float* const* peer_glogit, float scale, const int32_t* owned,
-                                    const int32_t* owned_count, int32_t owned_capacity, void* stream) {
+extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                    int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                                    int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                                    float* const* peer_lrw, int32_t* status, int32_t* owned,
+                                    int32_t* owned_count, int32_t owned_capacity, void* stream) {
+  return b2_shard_push_ex(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_ids, idx_dtype, ids_stride,
+                          peer_emb, peer_lrw, status, owned, owned_count, owned_capacity, nullptr, stream);
+}
+
+extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                       int64_t batch_local, int world, int rank, const float* const* peer_gemb,
+                                       const float* const* peer_glogit, float scale, const int32_t* owned,
+                                       const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                       void* stream) {
   int rc = check_shard_args(emb_fields, nfields, world, rank);
+  if (rc != B2_OK) return rc;
+  rc = check_lazy(lazy);
   if (rc != B2_OK) return rc;
   B2_REQUIRE(peer_gemb && (lr_fields == nullptr || peer_glogit != nullptr), "NULL peer pointer array");
   B2_REQUIRE(owned && owned_count && owned_capacity >= 1 && ((uintptr_t) owned % 16) == 0, "bad owned list");
@@ -426,11 +498,21 @@ extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* 
   int64_t expect = batch_local * (int64_t) nfields * 2;
   if (expect > owned_capacity) expect = owned_capacity;
   const int grid = grid_for(expect << lpr_log2, 256);
-  shard_pull_kernel<<<grid, 256, smem, (cudaStream_t) stream>>>(epack, lpack, pp, dim, lpr_log2, has_lr, scale,
-                                                               reinterpret_cast<const int4*>(owned), owned_count,
-                                                               owned_capacity);
+  static thread_local b2_lazy_ctx lz_none;
+  const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
+  shard_pull_kernel<<<grid, 256, smem, (cudaStream_t) stream>>>(epack, lpack, pp, lz, lazy ? 1 : 0, dim, lpr_log2,
+                                                               has_lr, scale, reinterpret_cast<const int4*>(owned),
+                                                               owned_count, owned_capacity);
   B2_CUDA_LAUNCH_CHECK("b2_shard_pull");
   return B2_OK;
+}
+
+extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                    int64_t batch_local, int world, int rank, const float* const* peer_gemb,
+                                    const float* const* peer_glogit, float scale, const int32_t* owned,
+                                    const int32_t* owned_count, int32_t owned_capacity, void* stream) {
+  return b2_shard_pull_ex(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_gemb, peer_glogit, scale,
+                          owned, owned_count, owned_capacity, nullptr, stream);
 }
 
 extern "C" B2_API int b2_peer_bcast_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,

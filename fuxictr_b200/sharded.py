@@ -57,6 +57,10 @@ class PeerGroup(object):
     def barrier(self):
         raise NotImplementedError
 
+    def all_reduce_sum(self, buf):
+        """buf <- sum over the ranks of buf (in place, on the current stream)."""
+        raise NotImplementedError
+
 
 class SymmPeerGroup(PeerGroup):
     """One process per GPU; buffers come from torch.distributed symmetric memory (NVLink P2P)."""
@@ -80,6 +84,9 @@ class SymmPeerGroup(PeerGroup):
     def barrier(self):
         self._handles[0].barrier()      # device-side signal-pad barrier on the current stream
 
+    def all_reduce_sum(self, buf):
+        self._dist.all_reduce(buf, op=self._dist.ReduceOp.SUM, group=self.group)
+
 
 class VirtualPeerGroup(PeerGroup):
     """`world` virtual ranks in one process: buffers are ordinary tensors shared through a dict;
@@ -95,6 +102,34 @@ class VirtualPeerGroup(PeerGroup):
 
     def barrier(self):
         pass
+
+    def all_reduce_sum(self, buf):
+        """A sum over virtual ranks needs every rank's buffer at once: lockstep_steps() does it between the
+        phases of all ranks' optimizer steps.  One virtual rank is its own sum."""
+        if self.world != 1:
+            raise RuntimeError("virtual ranks sum over ranks in lock step: drive their optimizer steps with "
+                               "fuxictr_b200.sharded.lockstep_steps")
+
+
+def lockstep_steps(optimizers, combine=None):
+    """One FusedAdam step of every virtual rank, in lock step: each rank runs up to the point where its step
+    sums a buffer over the ranks (FusedAdam.step_phases), the buffers are summed in rank order and the
+    sum is written back to every rank, then every rank finishes.  `combine(bufs)` may replace that sum."""
+    phases = [opt.step_phases() for opt in optimizers]
+    while True:
+        bufs = [next(ph, None) for ph in phases]
+        if all(b is None for b in bufs):
+            return
+        if any(b is None for b in bufs):
+            raise RuntimeError("virtual ranks disagree on the number of cross-rank sums in a step")
+        if combine is not None:
+            combine(bufs)
+            continue
+        total = bufs[0].clone()
+        for b in bufs[1:]:
+            total.add_(b)
+        for b in bufs:
+            b.copy_(total)
 
 
 class _LazyPtrs(object):
@@ -161,6 +196,8 @@ class ShardedFront(object):
         # 1/world (default), or the caller seeds backward() with 1/world and sets pull_scale = 1
         self.pull_scale = 1.0 / g.world
         self.on_dense_grads_ready = None     # set by RankModel.use_fused_optimizer (overlapped dense all-reduce)
+        self._lazy_ctx = None                # b2_lazy_ctx when the shard tables are lazily evaluated (lazy_ctx())
+        self._lazy_owner = None
 
     # -- descriptors --------------------------------------------------------------------------
     def _descs(self, tables, dim):
@@ -183,13 +220,25 @@ class ShardedFront(object):
         _lib.call("b2_peer_bcast_ids", F2._ptr(src), self.src_code, self.B * self.W, _ptr_array(dst), g.world,
                   F2._stream())
 
+    def lazy_ctx(self):
+        """The b2_lazy_ctx of the shard tables when an optimizer evaluates them lazily (arena.LazyTables over
+        this rank's shard parameters), else None.  Built once per LazyTables."""
+        lazy = getattr(self.emb_tables[0], "_b2_lazy", None)
+        if lazy is None:
+            return None
+        if self._lazy_owner is not lazy:
+            self._lazy_ctx, self._lazy_owner = lazy.shard_ctx(self.emb_tables, self.lr_tables), lazy
+        return self._lazy_ctx
+
     def phase_push(self):
         g = self.group
         lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
-        _lib.call("b2_shard_push", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
+        lz = self.lazy_ctx()
+        _lib.call("b2_shard_push_ex", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.ids_ptrs), self.idx_code, self.W, _ptr_array(self.emb_ptrs),
                   _ptr_array(self.lrw_ptrs) if lr is not None else None, F2._ptr(self.status),
-                  F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap, F2._stream())
+                  F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
+                  ctypes.byref(lz) if lz is not None else None, F2._stream())
 
     def phase_reduce(self):
         """Local: logit (B,1) and field sums from the landed rows.  Returns (emb copy, logit, sums)."""
@@ -215,9 +264,11 @@ class ShardedFront(object):
     def phase_pull(self, emb_grads, lr_grads):
         g = self.group
         lr = self._descs(lr_grads, 1) if lr_grads else None
-        _lib.call("b2_shard_pull", self._descs(emb_grads, self.dim), lr, self.F, self.B, g.world, g.rank,
+        lz = self.lazy_ctx()        # lazy tables: the pull enqueues every row it scatters a gradient into
+        _lib.call("b2_shard_pull_ex", self._descs(emb_grads, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.gemb_ptrs), _ptr_array(self.glogit_ptrs) if lr is not None else None,
-                  self.pull_scale, F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap, F2._stream())
+                  self.pull_scale, F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
+                  ctypes.byref(lz) if lz is not None else None, F2._stream())
 
 
 class _ShardedFrontFn(torch.autograd.Function):

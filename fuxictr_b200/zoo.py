@@ -226,25 +226,26 @@ class RankModel(nn.Module):
 
     def use_fused_optimizer(self, lazy_tables=False):
         """Re-home parameters into one HBM arena and replace clip_grad_norm_ + torch Adam by
-        the two-kernel FusedAdam (same arithmetic; see arena.py).  Call after model_to_device().
-        lazy_tables=True (models whose tables are read only by the fused front: DeepFM, xDeepFM):
-        the dense Adam semantics of the tables are evaluated row-wise and lazily — bit-identical
-        results, O(batch) instead of O(vocabulary) optimizer traffic; call materialize_tables()
-        before reading table weights outside the kernels (state_dict, evaluation on other paths)."""
+        the two-kernel FusedAdam (same arithmetic; see arena.py).  Call after model_to_device()
+        (and after enable_sharding() for row-sharded tables).
+        lazy_tables=True (models whose every forward reads the tables through a replaying kernel:
+        `_replays_lazy_tables`, i.e. DeepFM, xDeepFM, DLRM; unsharded or row-sharded): the dense Adam
+        semantics of the tables are evaluated row-wise and lazily — bit-identical results, O(batch)
+        instead of O(vocabulary) optimizer traffic; call materialize_tables() before reading table
+        weights outside the kernels (state_dict() and evaluate() do)."""
         if self._optimizer_name != "Adam":
             raise NotImplementedError("the fused optimizer implements Adam only")
-        if lazy_tables:
-            if getattr(self, "_sharded_params", None):
-                raise NotImplementedError("lazy tables and row-sharding are not combined yet")
-            first = self._front_tables()
-            self._arena = ParamArena(self, first=first)
-            self._fused_optimizer = FusedAdam(self._arena, lr=self._lr, max_norm=self._max_gradient_norm)
-            self._lazy = self._fused_optimizer.enable_lazy(first)
-            self.optimizer = None
-            return self._fused_optimizer
+        if lazy_tables and not getattr(type(self), "_replays_lazy_tables", False):
+            # any other forward reads the tables through kernels that neither replay nor enqueue: the
+            # tables would silently stop training
+            raise NotImplementedError("%s reads its tables through kernels without the lazy replay; lazy tables "
+                                      "are implemented for DeepFM, xDeepFM and DLRM" % type(self).__name__)
         # tables first (the row shards of a sharded run, else every nn.Embedding weight): the dense
         # parameters then form one contiguous tail (one all-reduce, one 3xTF32 split launch per step)
-        first = getattr(self, "_sharded_params", None)
+        sharded = getattr(self, "_sharded_params", None)
+        first = list(sharded) if sharded else None
+        if lazy_tables and not first:
+            first = self._front_tables()
         if not first:
             first, seen = [], set()
             for m in self.modules():
@@ -253,13 +254,17 @@ class RankModel(nn.Module):
                     first.append(m.weight)
         self._arena = ParamArena(self, first=first)
         self._fused_optimizer = FusedAdam(self._arena, lr=self._lr, max_norm=self._max_gradient_norm)
-        self._fused_optimizer.sharded = bool(getattr(self, "_sharded_params", None))
+        if lazy_tables:
+            self._lazy = self._fused_optimizer.enable_lazy(first)
+        self._fused_optimizer.sharded = bool(sharded)
         self._fused_optimizer.dense_prescaled = getattr(self, "_loss_grad", None) is not None
         front = getattr(self, "_sharded_front", None)
-        if front is not None and front.group.world > 1 and hasattr(front.group, "group"):
-            # real ranks (not the single-process virtual harness): overlap the dense all-reduce with the pull
-            self._fused_optimizer.enable_dense_overlap()
-            front.on_dense_grads_ready = self._fused_optimizer.start_dense_allreduce
+        if front is not None:
+            self._fused_optimizer.group = front.group     # sums the norm term (and dense gradients) over the ranks
+            if front.group.world > 1 and hasattr(front.group, "group"):
+                # real ranks (not the single-process virtual harness): overlap the dense all-reduce with the pull
+                self._fused_optimizer.enable_dense_overlap()
+                front.on_dense_grads_ready = self._fused_optimizer.start_dense_allreduce
         self.optimizer = None
         return self._fused_optimizer
 
@@ -311,6 +316,7 @@ def _parse_regularizer(reg):
 class DeepFM(RankModel):
     """model_zoo/DeepFM/DeepFM_torch/src/DeepFM.py:41-88: y = sigmoid(FM(X, E) + MLP(flatten(E)))."""
     _routes_sharded_front = True
+    _replays_lazy_tables = True
 
     def __init__(self, feature_map, model_id="DeepFM", gpu=-1, learning_rate=1e-3, embedding_dim=10,
                  hidden_units=[64, 64, 64], hidden_activations="ReLU", net_dropout=0, batch_norm=False,
@@ -410,6 +416,7 @@ class DLRM(RankModel):
     numeric ones as one more "field"), pairwise dot (or concat) interaction, top MLP with the output
     activation inside it."""
     _routes_sharded_front = True
+    _replays_lazy_tables = True
 
     def __init__(self, feature_map, model_id="DLRM", gpu=-1, learning_rate=1e-3, embedding_dim=10,
                  top_mlp_units=[64, 64, 64], bottom_mlp_units=[64, 64, 64], top_mlp_activations="ReLU",
@@ -448,6 +455,11 @@ class DLRM(RankModel):
         if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables (SURVEY.md 8e, C5)
             from .sharded import sharded_front
             feat_emb, _ = sharded_front(self._sharded_front, self._batch_matrix(inputs))
+        elif getattr(self, "_lazy", None) is not None:     # lazy tables: read through the replaying front
+            fused = fused_front(self.embedding_layer, None, X, want_fm=False)
+            if fused is None:
+                raise RuntimeError("lazy tables are only readable through the fused front (unsupported config)")
+            feat_emb = fused[0]
         else:
             feat_emb = self.embedding_layer(X)
         dense_emb = None
@@ -518,6 +530,7 @@ class DIN(RankModel):
 
 class xDeepFM(RankModel):
     """model_zoo/xDeepFM/src/xDeepFM.py:41-97: y = sigmoid(LR(X) + CIN(E) [+ DNN(flatten(E))])."""
+    _replays_lazy_tables = True
 
     def __init__(self, feature_map, model_id="xDeepFM", gpu=-1, learning_rate=1e-3, embedding_dim=10,
                  dnn_hidden_units=[64, 64, 64], dnn_activations="ReLU", cin_hidden_units=[16, 16, 16],

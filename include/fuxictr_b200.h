@@ -162,6 +162,13 @@ B2_API int b2_lr_bwd(const b2_field* fields, int nfields, int64_t batch, int idx
  * scalars (sched[t], written by b2_adam_sched) and the same explicitly rounded arithmetic as the
  * dense pass, so the result is BIT-IDENTICAL to dense Adam (tests/test_gpu_parity.py).
  * Rows are numbered globally: table i owns rows [grow_base[i], grow_base[i] + vocab_i).
+ * Row-sharded tables (b2_shard_push_ex / b2_shard_pull_ex): the same protocol over the rows THIS rank
+ * owns.  The push replays a stale row before it stores it into the requester's buffer; the pull, where
+ * several requesters may send gradients for one row, enqueues the row once.  grow_emb / grow_lr and
+ * the worklist then count this rank's LOCAL rows (shard row r of table i is row grow_base[i] + r);
+ * worklist entries are int32, so a rank holds at most 2^31 - 1 lazy rows.
+ * The readers of a lazy table are these four kernels only; every other read of the parameters needs
+ * b2_lazy_materialize first.
  */
 typedef struct b2_lazy_ctx {
   const int32_t* last_step; /* [total rows] optimizer step each row is current for */
@@ -258,6 +265,21 @@ B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, 
                          int64_t batch_local, int world, int rank, const float* const* peer_gemb,
                          const float* const* peer_glogit, float scale, const int32_t* owned,
                          const int32_t* owned_count, int32_t owned_capacity, void* stream);
+/* Lazy tables (see b2_lazy_ctx): lazy == NULL is b2_shard_push / b2_shard_pull.  Otherwise the push
+ * brings every served row with last_step[grow] < *step_dev up to date in registers before the store
+ * (nothing is written back), and the pull appends every owned, non-padding row it scatters a gradient
+ * into to the worklist, once per step (claimed through mark).  grow = grow_emb[f] / grow_lr[f] + local
+ * row.  The caller zeroes lazy->counter before the pull of a step. */
+B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                            int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                            int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                            float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
+                            int32_t owned_capacity, const b2_lazy_ctx* lazy, void* stream);
+B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                            int64_t batch_local, int world, int rank, const float* const* peer_gemb,
+                            const float* const* peer_glogit, float scale, const int32_t* owned,
+                            const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                            void* stream);
 B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream);
 /* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
  * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world. */

@@ -4,7 +4,10 @@ restatement of the reference's BaseModel.train_step) run on the whole global bat
 mean loss, this rank's table shards and the replicated dense weights, within 1e-5 relative.
 
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/dist_sharded_check.py \
-        [--model DeepFM|DLRM] [--precision fp32|tf32x3] [--batch-local 64]
+        [--model DeepFM|DLRM] [--precision fp32|tf32x3] [--batch-local 64] [--lazy]
+
+--lazy evaluates the tables' dense Adam lazily (use_fused_optimizer(lazy_tables=True)): the push replays
+stale rows, the pull enqueues touched rows, and state_dict() brings every shard row up to date.
 
 Checker use of oracle/ only (tests/test_gpu_multirank.py launches this script).
 """
@@ -22,6 +25,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--model", default="DeepFM", choices=["DeepFM", "DLRM"])
 ap.add_argument("--precision", default="fp32", choices=["fp32", "tf32x3"])
 ap.add_argument("--batch-local", type=int, default=64)
+ap.add_argument("--lazy", action="store_true", help="lazily evaluated tables (dense Adam semantics, row-wise)")
 args = ap.parse_args()
 
 rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
@@ -76,7 +80,7 @@ trainer = O.OracleTrainer(state0, pred, spec_map, ["label"])
 ref_losses = [float(trainer.train_step(fm.batch_dict(b))) for b in batches]
 
 model.enable_sharding(SH.SymmPeerGroup(), B_l, NF + 1, torch.float64, want_fm=(args.model == "DeepFM"))
-model.use_fused_optimizer()
+model.use_fused_optimizer(lazy_tables=args.lazy)
 model.train()
 losses = []
 mine = [b[rank * B_l:(rank + 1) * B_l].contiguous().cuda() for b in batches]
@@ -95,7 +99,7 @@ tol = 1e-5
 ok = True
 err = rel(lt.cpu(), torch.tensor(ref_losses))
 ok &= err < tol
-print("[r%d] %s loss err %.2e" % (rank, args.model, err), flush=True)
+print("[r%d] %s%s loss err %.2e" % (rank, args.model, " lazy" if args.lazy else "", err), flush=True)
 worst = 0.0
 for k, v in model.state_dict().items():
     r = trainer.state[k].detach()
