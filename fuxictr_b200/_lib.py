@@ -51,6 +51,11 @@ class b2_field(ctypes.Structure):
     ]
 
 
+class b2_touch(ctypes.Structure):
+    """struct b2_touch of include/fuxictr_b200.h (24 bytes)."""
+    _fields_ = [("flags", c_void_p), ("base", c_void_p), ("n", c_int64)]
+
+
 _FIELD_P = ctypes.POINTER(b2_field)
 
 
@@ -83,12 +88,16 @@ SIGNATURES = {
     "b2_embed_gather_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_embed_gather_hot_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_embed_scatter_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p]),
+    "b2_embed_scatter_bwd_ex": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_lr_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_lr_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_lr_bwd_ex": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_front_fwd": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_front_bwd": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_front_bwd_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_lazy_sumsq": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "b2_lazy_adam_step": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_void_p]),
@@ -104,7 +113,7 @@ SIGNATURES = {
     "b2_shard_push_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2_shard_pull_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_float,
-                                 c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+                                 c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
     "b2_peer_bcast": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "b2_peer_bcast_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "b2_front_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
@@ -156,6 +165,9 @@ SIGNATURES = {
     "b2_sumsq": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
                              c_float, c_float, c_float, c_void_p, c_int, c_void_p]),
+    "b2_sumsq_ex": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
+    "b2_adam_step_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
+                                c_float, c_float, c_float, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
     "b2_logloss_sum": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_auc_workspace_bytes": (c_int, [c_int64, ctypes.POINTER(c_int64)]),
     "b2_auc": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),

@@ -29,6 +29,7 @@ class ParamArena(object):
     """Re-homes the trainable fp32 CUDA parameters of `module` into one flat buffer."""
 
     ALIGN = 4  # floats (16 bytes): every slice is float4-addressable
+    GRANULE = 16  # floats (64 bytes) per byte of `touched`
 
     def __init__(self, module, first=()):
         """`first`: parameters to place at the front of the arena (e.g. the row-sharded tables of a
@@ -54,6 +55,9 @@ class ParamArena(object):
         for i, p in enumerate(uniq):
             if i == n_first:
                 self.tail_offset = off
+            if i < n_first:
+                # tables start on a 64-byte granule of `touched`: a touched 16-float row then flags one granule, not two
+                off = (off + self.GRANULE - 1) // self.GRANULE * self.GRANULE
             slots.append((p, off))
             off += (p.numel() + self.ALIGN - 1) // self.ALIGN * self.ALIGN
         if n_first >= len(uniq):
@@ -69,6 +73,15 @@ class ParamArena(object):
         self.tail_params = uniq[n_first:]      # the dense (non-`first`) parameters, contiguous from tail_offset
         self.step_id = 0
         self.grads_are_zero = True
+        # Touched-granule flags of the table prefix G[:tail_offset] (b2_touch): one byte per 16 floats.  The
+        # backward kernels set the byte of every granule they add a table gradient into; FusedAdam's clip
+        # and Adam passes read G only there and clear the bytes again.  Invariant: every nonzero float of
+        # G[:tail_offset] lies in a flagged granule.  None: no table prefix, or lazy tables (own worklist).
+        self.touched, self.touch = None, None
+        if self.tail_offset > 0:
+            self.touched = torch.zeros((self.tail_offset + self.GRANULE - 1) // self.GRANULE, dtype=torch.uint8,
+                                       device=dev)
+            self.touch = _lib.b2_touch(self.touched.data_ptr(), self.G.data_ptr(), self.tail_offset)
         with torch.no_grad():
             for p, o in slots:
                 dst = self.P[o:o + p.numel()].view(p.shape)
@@ -79,6 +92,12 @@ class ParamArena(object):
 
     def grad_view(self, slot):
         return self.G[slot.offset:slot.offset + slot.numel].view(slot.shape)
+
+    def mark_slot(self, slot):
+        """Flag every granule of `slot` (its gradient is written by something that sets no flags)."""
+        if self.touched is not None and slot.offset < self.tail_offset:
+            end = min(slot.offset + slot.numel, self.tail_offset)
+            self.touched[slot.offset // 16:(end + 15) // 16].fill_(1)
 
     def begin_step(self, grads_zeroed):
         """Call once per training step before backward. `grads_zeroed`: G is already all-zero
@@ -207,6 +226,7 @@ class FusedAdam(object):
         self.lazy = LazyTables(self.arena, tables)
         self.lazy.opt = self
         self.lazy.sched = self.sched          # one schedule table for the dense and the lazy kernels
+        self.arena.touched, self.arena.touch = None, None    # the worklist says which rows carry a gradient
         return self.lazy
 
     def count_step(self, n=1):
@@ -278,10 +298,16 @@ class FusedAdam(object):
             g = p.grad
             if g is not None and g.data_ptr() != g_base + p._b2_slot.offset * 4:
                 a.grad_view(p._b2_slot).copy_(g)
+                a.mark_slot(p._b2_slot)
         if self.grad_allreduce:
             import torch.distributed as dist
             dist.all_reduce(a.G, op=dist.ReduceOp.SUM)   # one NCCL collective over the whole arena
             a.G.mul_(1.0 / dist.get_world_size())          # mean over the global batch (rank_model.py:130)
+            if a.touched is not None:                      # a granule any rank wrote may now be nonzero here
+                dist.all_reduce(a.touched, op=dist.ReduceOp.MAX)
+        # The table passes read G only in flagged granules and clear the flags with the gradients: only when
+        # the step zeroes G (otherwise the flags just accumulate, and the passes read everything).
+        flags = a.touched if (self.zero_grad_in_step and self.lazy is None) else None
         sumsq_ptr = ctypes.c_void_p(0)
         if self.sharded:
             if self.group is not None:
@@ -298,9 +324,12 @@ class FusedAdam(object):
                               ctypes.c_void_p(lz.worklist.data_ptr()), ctypes.c_void_p(lz.counter.data_ptr()),
                               lz.capacity, (a.G.data_ptr() - a.P.data_ptr()) // 4, ctypes.c_void_p(slot.data_ptr()),
                               st)
+                elif flags is not None:     # this rank's shard part of ||g||^2
+                    _lib.call("b2_sumsq_ex", ctypes.c_void_p(a.G.data_ptr()), a.tail_offset,
+                              ctypes.c_void_p(slot.data_ptr()), ctypes.c_void_p(flags.data_ptr()), a.tail_offset, st)
                 else:
                     _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr()), a.tail_offset,
-                              ctypes.c_void_p(slot.data_ptr()), st)   # this rank's shard part of ||g||^2
+                              ctypes.c_void_p(slot.data_ptr()), st)
             if self._early_pending:
                 # the dense gradients are already being summed on the side stream: only the norm scalar here
                 yield slot
@@ -330,12 +359,22 @@ class FusedAdam(object):
                 if a.numel > a.tail_offset:
                     _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr() + 4 * a.tail_offset),
                               a.numel - a.tail_offset, ctypes.c_void_p(self.sumsq.data_ptr()), st)
+            elif flags is not None:
+                _lib.call("b2_sumsq_ex", ctypes.c_void_p(a.G.data_ptr()), a.numel,
+                          ctypes.c_void_p(self.sumsq.data_ptr()), ctypes.c_void_p(flags.data_ptr()), a.tail_offset, st)
             else:
                 _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr()), a.numel,
                           ctypes.c_void_p(self.sumsq.data_ptr()), st)
             sumsq_ptr = ctypes.c_void_p(self.sumsq.data_ptr())
         vp = ctypes.c_void_p
         lo = 0
+        if flags is not None:
+            # tables: G loaded (and zeroed, and its flag cleared) only in the granules a backward wrote
+            _lib.call("b2_adam_step_ex", vp(a.P.data_ptr()), vp(a.G.data_ptr()), vp(self.M.data_ptr()),
+                      vp(self.V.data_ptr()), a.tail_offset, sumsq_ptr, float(self.max_norm or 0.0), self.lr,
+                      self.betas[0], self.betas[1], self.eps, vp(self.step_dev.data_ptr()), 1,
+                      vp(flags.data_ptr()), a.tail_offset, st)
+            lo = a.tail_offset
         if self.lazy is not None:
             _lib.call("b2_adam_sched", vp(self.step_dev.data_ptr()), self.lr, self.betas[0], self.betas[1],
                       vp(self.sched.data_ptr()), self.sched.shape[0], st)
@@ -357,8 +396,8 @@ class FusedAdam(object):
                       vp(self.step_dev.data_ptr()), vp(self.sched.data_ptr()),
                       1 if self.zero_grad_in_step else 0, st)
         elif n > 0:                             # dense pass: the two per-step scalars are computed in-kernel
-            _lib.call("b2_adam_step", vp(a.P.data_ptr()), vp(a.G.data_ptr()), vp(self.M.data_ptr()),
-                      vp(self.V.data_ptr()), n, sumsq_ptr, float(self.max_norm or 0.0), self.lr,
+            _lib.call("b2_adam_step", vp(a.P.data_ptr() + 4 * lo), vp(a.G.data_ptr() + 4 * lo),
+                      vp(self.M.data_ptr() + 4 * lo), vp(self.V.data_ptr() + 4 * lo), n, sumsq_ptr, float(self.max_norm or 0.0), self.lr,
                       self.betas[0], self.betas[1], self.eps, vp(self.step_dev.data_ptr()),
                       1 if self.zero_grad_in_step else 0, st)
         self._stepped = True

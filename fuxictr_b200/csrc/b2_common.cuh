@@ -99,6 +99,14 @@ __device__ __forceinline__ void b2_stg_stream(float4* p, const float4& v) {
 }
 
 // Vector reductions to global memory (sm_90+): one 16-byte / 8-byte atomic per lane.
+// Flags the 64-byte granule of the gradient element p if it lies in the flagged range (b2_touch).
+// A vector of at most 4 floats at its natural alignment never straddles two granules.  The lanes writing
+// one row call it for each of their vectors; only the row's first vector and the first vector of each
+// further granule store (row_start: p is the row's first element), so an aligned row costs one store.
+__device__ __forceinline__ void b2_touch_mark(const b2_touch& t, const float* p, bool row_start) {
+  const uint64_t o = (uint64_t) ((intptr_t) p - (intptr_t) t.base) >> 2;
+  if (o < (uint64_t) t.n && (row_start || (o & 15) == 0)) t.flags[o >> 4] = 1;
+}
 __device__ __forceinline__ void b2_red_add_v4(float* p, const float4& v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y),
                "f"(v.z), "f"(v.w)

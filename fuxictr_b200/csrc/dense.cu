@@ -349,18 +349,33 @@ extern "C" B2_API int b2_logit_bce_fwd(const float* t0, const float* t1, const f
 // Dense clip_grad_norm_ + Adam over a flat fp32 arena (rank_model.py:321-322).
 // HBM-bound streaming: float4, grid = whole waves of B2_NUM_SMS (132) SMs.
 // ---------------------------------------------------------------------------------
+constexpr int SUMSQ_UNROLL = 4;
+
+// flags (may be NULL): byte k covers float4s [4k, 4k + 4) of the first nf4; an unflagged granule is all
+// zero and is skipped, which leaves every thread's partial sum bit-identical to the full pass.
 __global__ void __launch_bounds__(256)
-sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {
+sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out,
+             const uint8_t* __restrict__ flags, int64_t nf4) {
   b2_pdl_wait();
   b2_pdl_trigger();
   __shared__ float red[32];
   float acc = 0.f;
   const int64_t n4 = n >> 2;
   const float4* g4 = reinterpret_cast<const float4*>(g);
-  for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n4;
-       i += (int64_t) gridDim.x * blockDim.x) {
-    const float4 v = b2_ldg_stream(g4 + i);
-    acc += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
+  // SUMSQ_UNROLL strided float4s per iteration, all flag loads and then all G loads in flight; they are added
+  // in the order of the plain loop, and a skipped or out-of-range float4 adds +0, which leaves acc unchanged.
+  const int64_t stride = (int64_t) gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += SUMSQ_UNROLL * stride) {
+    float4 v[SUMSQ_UNROLL];
+#pragma unroll
+    for (int u = 0; u < SUMSQ_UNROLL; ++u) {
+      const int64_t j = i + u * stride;
+      v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (j < n4 && (j >= nf4 || flags[j >> 2] != 0)) v[u] = b2_ldg_stream(g4 + j);
+    }
+#pragma unroll
+    for (int u = 0; u < SUMSQ_UNROLL; ++u)
+      acc += (v[u].x * v[u].x + v[u].y * v[u].y) + (v[u].z * v[u].z + v[u].w * v[u].w);
   }
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
     const float v = g[(n4 << 2) + threadIdx.x];
@@ -370,16 +385,24 @@ sumsq_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {
   if (threadIdx.x == 0) b2_red_add(out, t);
 }
 
-extern "C" B2_API int b2_sumsq(const float* g, int64_t n, float* out, void* stream) {
+extern "C" B2_API int b2_sumsq_ex(const float* g, int64_t n, float* out, const uint8_t* flags, int64_t n_flagged,
+                                  void* stream) {
   B2_REQUIRE(g && out, "NULL pointer");
   B2_REQUIRE(((uintptr_t) g % 16) == 0, "gradient arena must be 16-byte aligned");
+  B2_REQUIRE(flags == nullptr || (n_flagged >= 0 && n_flagged <= n && n_flagged % 4 == 0),
+             "n_flagged=%lld must be a multiple of 4 in [0, n=%lld]", (long long) n_flagged, (long long) n);
   if (n <= 0) return B2_OK;
   int64_t blocks = b2_ceil_div(n >> 2, 256 * 4);
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
-  B2_LAUNCH(sumsq_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, g, n, out);
+  const int64_t nf4 = flags != nullptr ? n_flagged >> 2 : 0;
+  B2_LAUNCH(sumsq_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, g, n, out, flags, nf4);
   B2_CUDA_LAUNCH_CHECK("b2_sumsq");
   return B2_OK;
+}
+
+extern "C" B2_API int b2_sumsq(const float* g, int64_t n, float* out, void* stream) {
+  return b2_sumsq_ex(g, n, out, nullptr, 0, stream);
 }
 
 // sched[step] is written first so that the dense pass and every later lazy catch-up of the same
@@ -397,7 +420,7 @@ __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
             float* __restrict__ v, int64_t n, const float* __restrict__ sumsq, float max_norm,
             float lr, float beta1, float beta2, float eps, const int64_t* __restrict__ step_dev,
-            int zero_grad, const B2AdamSched* __restrict__ sched) {
+            int zero_grad, const B2AdamSched* __restrict__ sched, uint8_t* __restrict__ flags, int64_t nf4) {
   b2_pdl_wait();
   b2_pdl_trigger();
   __shared__ B2AdamConst sc;
@@ -433,9 +456,18 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
   float4* g4 = reinterpret_cast<float4*>(g);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
-  for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n4;
-       i += (int64_t) gridDim.x * blockDim.x) {
-    float4 pp = p4[i], gg = g4[i], mm = m4[i], vv = v4[i];
+  // Warp-uniform trip count: the 4 lanes of a flagged granule (float4s 4k..4k+3, one warp) all read its
+  // flag before its first lane clears it.
+  const int lane = threadIdx.x & 31;
+  for (int64_t i0 = (int64_t) blockIdx.x * blockDim.x + (threadIdx.x & ~31); i0 < n4;
+       i0 += (int64_t) gridDim.x * blockDim.x) {
+    const int64_t i = i0 + lane;
+    const bool flagged = i < nf4;
+    const bool live = !flagged || flags[i >> 2] != 0;   // false: the granule's gradient is known to be zero
+    if (i0 < nf4) __syncwarp();
+    if (i >= n4) continue;
+    float4 pp = p4[i], mm = m4[i], vv = v4[i];
+    const float4 gg = live ? g4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     b2_adam_apply(pp.x, __fmul_rn(gg.x, clip), mm.x, vv.x, c, step_size, ibc2);   // g.mul_(clip_coef) first
     b2_adam_apply(pp.y, __fmul_rn(gg.y, clip), mm.y, vv.y, c, step_size, ibc2);
     b2_adam_apply(pp.z, __fmul_rn(gg.z, clip), mm.z, vv.z, c, step_size, ibc2);
@@ -443,6 +475,7 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
     p4[i] = pp; m4[i] = mm; v4[i] = vv;
     // zero_grad fused in; rows no sample touched are already zero (most of a table): skip their 16-byte store
     if (zero_grad && (gg.x != 0.f || gg.y != 0.f || gg.z != 0.f || gg.w != 0.f)) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (zero_grad && flagged && live && (i & 3) == 0) flags[i >> 2] = 0;   // the granule is all zero again
   }
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
     const int64_t i = (n4 << 2) + threadIdx.x;
@@ -453,22 +486,33 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
   }
 }
 
-extern "C" B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n,
-                            const float* sumsq, float max_norm, float lr, float beta1,
-                            float beta2, float eps, const int64_t* step_dev, int zero_grad,
-                            void* stream) {
+extern "C" B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n,
+                                      const float* sumsq, float max_norm, float lr, float beta1,
+                                      float beta2, float eps, const int64_t* step_dev, int zero_grad,
+                                      uint8_t* flags, int64_t n_flagged, void* stream) {
   B2_REQUIRE(p && g && m && v && step_dev, "NULL pointer");
   B2_REQUIRE((((uintptr_t) p | (uintptr_t) g | (uintptr_t) m | (uintptr_t) v) % 16) == 0,
              "arenas must be 16-byte aligned");
+  B2_REQUIRE(flags == nullptr || (n_flagged >= 0 && n_flagged <= n && n_flagged % 4 == 0),
+             "n_flagged=%lld must be a multiple of 4 in [0, n=%lld]", (long long) n_flagged, (long long) n);
   if (n <= 0) return B2_OK;
   int64_t blocks = b2_ceil_div(n >> 2, 256 * 2);
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
   const B2AdamSched* no_sched = nullptr;
+  const int64_t nf4 = flags != nullptr ? n_flagged >> 2 : 0;
   B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2,
-            eps, step_dev, zero_grad, no_sched);
+            eps, step_dev, zero_grad, no_sched, flags, nf4);
   B2_CUDA_LAUNCH_CHECK("b2_adam_step");
   return B2_OK;
+}
+
+extern "C" B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n,
+                            const float* sumsq, float max_norm, float lr, float beta1,
+                            float beta2, float eps, const int64_t* step_dev, int zero_grad,
+                            void* stream) {
+  return b2_adam_step_ex(p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2, eps, step_dev, zero_grad, nullptr, 0,
+                         stream);
 }
 
 extern "C" B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
@@ -493,7 +537,7 @@ extern "C" B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v,
   if (blocks < 1) blocks = 1;
   const B2AdamSched* sched_tab = reinterpret_cast<const B2AdamSched*>(sched);
   B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, 0.f, beta1, beta2,
-            eps, step_dev, zero_grad, sched_tab);
+            eps, step_dev, zero_grad, sched_tab, (uint8_t*) nullptr, (int64_t) 0);
   B2_CUDA_LAUNCH_CHECK("b2_adam_step_sched");
   return B2_OK;
 }

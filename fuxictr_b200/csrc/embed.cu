@@ -224,7 +224,7 @@ gather_general_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch, i
 template <typename IdxT, int VEC>
 __global__ void __launch_bounds__(256)
 scatter_bwd_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch, int lpr_log2,
-                   const float* __restrict__ mean_count) {
+                   const float* __restrict__ mean_count, const b2_touch tch) {
   using V = typename VecT<VEC>::type;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(pack, smem_raw);
@@ -304,7 +304,10 @@ scatter_bwd_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch, int 
         }
         v = acc;
       }
-      if (leader && e < dim) b2_vred(drow + e, v);
+      if (leader && e < dim) {
+        b2_vred(drow + e, v);
+        b2_touch_mark(tch, drow + e, e == 0);
+      }
     }
   }
 }
@@ -343,7 +346,7 @@ lr_fwd_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch,
 template <typename IdxT>
 __global__ void __launch_bounds__(256)
 lr_bwd_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch,
-              const float* __restrict__ gout, float* __restrict__ gbias) {
+              const float* __restrict__ gout, float* __restrict__ gbias, const b2_touch tch) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(pack, smem_raw);
   __shared__ float red[32];
@@ -361,8 +364,11 @@ lr_bwd_kernel(const __grid_constant__ B2FieldPack pack, int64_t batch,
     const float g = __ldg(gout + b);
     if (slot == 0) gb += g;
     const int64_t row = b2_load_index<IdxT>(fd.idx, b * fd.idx_stride + l);
-    if (row >= 0 && row < fd.vocab && row != (int64_t) fd.padding_idx)
-      b2_red_add(reinterpret_cast<float*>(const_cast<void*>(fd.table)) + row, g);
+    if (row >= 0 && row < fd.vocab && row != (int64_t) fd.padding_idx) {
+      float* dst = reinterpret_cast<float*>(const_cast<void*>(fd.table)) + row;
+      b2_red_add(dst, g);
+      b2_touch_mark(tch, dst, true);
+    }
   }
   if (gbias != nullptr) {
     const float t = b2_block_sum(gb, red);
@@ -424,16 +430,16 @@ static int launch_gather(const B2FieldPack& pack, int64_t batch, int vec, int ma
 
 template <typename IdxT>
 static int launch_scatter(const B2FieldPack& pack, int64_t batch, int vec, int max_dim,
-                          const float* mean_count, cudaStream_t st) {
+                          const float* mean_count, const b2_touch& tch, cudaStream_t st) {
   const int block = 256;
   const size_t smem = pack_smem_bytes(pack.nfields);
   int lpr_log2 = next_pow2_log2((max_dim + vec - 1) / vec);
   if (lpr_log2 > 5) lpr_log2 = 5;
   const int64_t nitems = batch * (int64_t) pack.nslots;
   const int grid = grid_for(nitems << lpr_log2, block);
-  if (vec == 4) scatter_bwd_kernel<IdxT, 4><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count);
-  else if (vec == 2) scatter_bwd_kernel<IdxT, 2><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count);
-  else scatter_bwd_kernel<IdxT, 1><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count);
+  if (vec == 4) scatter_bwd_kernel<IdxT, 4><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count, tch);
+  else if (vec == 2) scatter_bwd_kernel<IdxT, 2><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count, tch);
+  else scatter_bwd_kernel<IdxT, 1><<<grid, block, smem, st>>>(pack, batch, lpr_log2, mean_count, tch);
   B2_CUDA_LAUNCH_CHECK("b2_embed_scatter_bwd");
   return B2_OK;
 }
@@ -471,22 +477,31 @@ extern "C" B2_API int b2_embed_gather_hot_fwd(const b2_field* fields, int nfield
 extern "C" B2_API int b2_embed_scatter_bwd(const b2_field* fields, int nfields, int64_t batch,
                                     int idx_dtype, int elem_dtype, const float* mean_count,
                                     void* stream) {
+  return b2_embed_scatter_bwd_ex(fields, nfields, batch, idx_dtype, elem_dtype, mean_count, nullptr, stream);
+}
+
+extern "C" B2_API int b2_embed_scatter_bwd_ex(const b2_field* fields, int nfields, int64_t batch,
+                                              int idx_dtype, int elem_dtype, const float* mean_count,
+                                              const b2_touch* touch, void* stream) {
+  b2_touch tch;
+  int rc = b2_touch_arg(touch, tch);
+  if (rc != B2_OK) return rc;
   B2_REQUIRE(elem_dtype == B2_F32, "elem_dtype %d unsupported (only B2_F32)", elem_dtype);
   B2_REQUIRE(batch >= 0, "negative batch");
   if (batch == 0) return B2_OK;
   static thread_local B2FieldPack pack;
   int vec, max_dim;
   bool any_pooled;
-  int rc = build_pack(pack, fields, nfields, true, true, &vec, &max_dim, &any_pooled);
+  rc = build_pack(pack, fields, nfields, true, true, &vec, &max_dim, &any_pooled);
   if (rc != B2_OK) return rc;
   for (int i = 0; i < nfields; ++i)
     if (fields[i].seq_len > 1 && fields[i].pool == B2_POOL_MEAN)
       B2_REQUIRE(mean_count != nullptr, "field %d: POOL_MEAN needs mean_count", i);
   cudaStream_t st = (cudaStream_t) stream;
   switch (idx_dtype) {
-    case B2_F64: return launch_scatter<double>(pack, batch, vec, max_dim, mean_count, st);
-    case B2_I64: return launch_scatter<int64_t>(pack, batch, vec, max_dim, mean_count, st);
-    case B2_I32: return launch_scatter<int32_t>(pack, batch, vec, max_dim, mean_count, st);
+    case B2_F64: return launch_scatter<double>(pack, batch, vec, max_dim, mean_count, tch, st);
+    case B2_I64: return launch_scatter<int64_t>(pack, batch, vec, max_dim, mean_count, tch, st);
+    case B2_I32: return launch_scatter<int32_t>(pack, batch, vec, max_dim, mean_count, tch, st);
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
 }
@@ -502,10 +517,10 @@ static int launch_lr_fwd(const B2FieldPack& pack, int64_t batch, const float* bi
 }
 template <typename IdxT>
 static int launch_lr_bwd(const B2FieldPack& pack, int64_t batch, const float* gout, float* gbias,
-                         cudaStream_t st) {
+                         const b2_touch& tch, cudaStream_t st) {
   const int block = 256;
   const int grid = grid_for(batch * (int64_t) pack.nslots, block);
-  lr_bwd_kernel<IdxT><<<grid, block, pack_smem_bytes(pack.nfields), st>>>(pack, batch, gout, gbias);
+  lr_bwd_kernel<IdxT><<<grid, block, pack_smem_bytes(pack.nfields), st>>>(pack, batch, gout, gbias, tch);
   B2_CUDA_LAUNCH_CHECK("b2_lr_bwd");
   return B2_OK;
 }
@@ -529,17 +544,25 @@ extern "C" B2_API int b2_lr_fwd(const b2_field* fields, int nfields, int64_t bat
 
 extern "C" B2_API int b2_lr_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
                          const float* gout, float* gbias, void* stream) {
+  return b2_lr_bwd_ex(fields, nfields, batch, idx_dtype, gout, gbias, nullptr, stream);
+}
+
+extern "C" B2_API int b2_lr_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
+                                   const float* gout, float* gbias, const b2_touch* touch, void* stream) {
+  b2_touch tch;
+  int rc = b2_touch_arg(touch, tch);
+  if (rc != B2_OK) return rc;
   B2_REQUIRE(gout != nullptr, "gout is NULL");
   B2_REQUIRE(batch >= 0, "negative batch");
   if (batch == 0) return B2_OK;
   static thread_local B2FieldPack pack;
-  int rc = build_pack(pack, fields, nfields, true, false, nullptr, nullptr, nullptr);
+  rc = build_pack(pack, fields, nfields, true, false, nullptr, nullptr, nullptr);
   if (rc != B2_OK) return rc;
   cudaStream_t st = (cudaStream_t) stream;
   switch (idx_dtype) {
-    case B2_F64: return launch_lr_bwd<double>(pack, batch, gout, gbias, st);
-    case B2_I64: return launch_lr_bwd<int64_t>(pack, batch, gout, gbias, st);
-    case B2_I32: return launch_lr_bwd<int32_t>(pack, batch, gout, gbias, st);
+    case B2_F64: return launch_lr_bwd<double>(pack, batch, gout, gbias, tch, st);
+    case B2_I64: return launch_lr_bwd<int64_t>(pack, batch, gout, gbias, tch, st);
+    case B2_I32: return launch_lr_bwd<int32_t>(pack, batch, gout, gbias, tch, st);
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
 }

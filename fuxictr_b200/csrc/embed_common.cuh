@@ -133,3 +133,12 @@ static inline int grid_for(int64_t nthreads_needed, int block) {
   return (int) blocks;
 }
 
+// The touched-granule descriptor a backward launch takes by value (b2_touch); NULL = one that marks nothing.
+static inline int b2_touch_arg(const b2_touch* touch, b2_touch& out) {
+  out = b2_touch{nullptr, nullptr, 0};
+  if (touch == nullptr || touch->flags == nullptr || touch->n <= 0) return B2_OK;
+  B2_REQUIRE(touch->base != nullptr && ((uintptr_t) touch->base % 16) == 0, "touch: base must be 16-byte aligned");
+  out = *touch;
+  return B2_OK;
+}
+

@@ -143,7 +143,7 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
                  int64_t batch, int dim, int lpr_log2, int has_lr, int want_fm,
                  const float* __restrict__ emb_saved, const float* __restrict__ gx_base,
                  const float* __restrict__ sums, const float* __restrict__ glogit,
-                 float* __restrict__ gbias) {
+                 float* __restrict__ gbias, const b2_touch tch) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ float red[32];
   const SmemFields sf = b2_stage_fields(emb, smem_raw);
@@ -185,7 +185,9 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
         if (has_lr && sub == 0) {
           const b2_field& ld = lf.f[f];
           if (ld.table != nullptr && row != (int64_t) ld.padding_idx) {
-            b2_red_add(reinterpret_cast<float*>(const_cast<void*>(ld.table)) + row, gl);
+            float* dst = reinterpret_cast<float*>(const_cast<void*>(ld.table)) + row;
+            b2_red_add(dst, gl);
+            b2_touch_mark(tch, dst, true);
             if (lazy) {   // first toucher of the LR row this step enqueues it
               const int grow = (int) (lz.grow_lr[f] + row);
               if (b2_lazy_claim(lz, grow, tmark)) enq_l = grow;
@@ -229,7 +231,10 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
       }
       v = acc;
     }
-    if (leader && e < dim) b2_red_add_v4(drow + e, v);
+    if (leader && e < dim) {
+      b2_red_add_v4(drow + e, v);
+      b2_touch_mark(tch, drow + e, e == 0);
+    }
   }
   if (gbias != nullptr) {
     const float t = b2_block_sum(gb_acc, red);
@@ -258,12 +263,12 @@ template <typename IdxT>
 int launch_front_bwd(const B2FieldPack& emb, const B2FieldPack& lr, const b2_lazy_ctx& lz, int lazy,
                      int64_t batch, int dim, int has_lr,
                      int want_fm, const float* emb_saved, const float* gx, const float* sums,
-                     const float* glogit, float* gbias, cudaStream_t st) {
+                     const float* glogit, float* gbias, const b2_touch& tch, cudaStream_t st) {
   int lpr_log2 = next_pow2_log2((dim + 3) / 4);
   const size_t smem = ((pack_smem_bytes(emb.nfields) + 15) & ~(size_t) 15) + pack_smem_bytes(emb.nfields) + 16;
   const int grid = grid_for((batch * (int64_t) emb.nfields) << lpr_log2, 256);
   auto kfn = front_bwd_kernel<IdxT>;
-  B2_LAUNCH(kfn, grid, 256, smem, st, emb, lr, lz, lazy, batch, dim, lpr_log2, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias);
+  B2_LAUNCH(kfn, grid, 256, smem, st, emb, lr, lz, lazy, batch, dim, lpr_log2, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, tch);
   B2_CUDA_LAUNCH_CHECK("b2_front_bwd");
   return B2_OK;
 }
@@ -340,7 +345,18 @@ extern "C" B2_API int b2_front_bwd(const b2_field* emb_fields, const b2_field* l
                                    int64_t batch, int idx_dtype, int want_fm, const float* emb_saved,
                                    const float* gx, const float* sums, const float* glogit, float* gbias,
                                    const b2_lazy_ctx* lazy, void* stream) {
+  return b2_front_bwd_ex(emb_fields, lr_fields, nfields, batch, idx_dtype, want_fm, emb_saved, gx, sums, glogit,
+                         gbias, lazy, nullptr, stream);
+}
+
+extern "C" B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                      int64_t batch, int idx_dtype, int want_fm, const float* emb_saved,
+                                      const float* gx, const float* sums, const float* glogit, float* gbias,
+                                      const b2_lazy_ctx* lazy, const b2_touch* touch, void* stream) {
   int rc = check_front(emb_fields, lr_fields, nfields, true);
+  if (rc != B2_OK) return rc;
+  b2_touch tch;
+  rc = b2_touch_arg(touch, tch);
   if (rc != B2_OK) return rc;
   B2_REQUIRE(batch >= 0, "negative batch");
   B2_REQUIRE(gx != nullptr, "gx (gradient arena base) is NULL");
@@ -357,9 +373,9 @@ extern "C" B2_API int b2_front_bwd(const b2_field* emb_fields, const b2_field* l
   const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
   const int lzf = lazy ? 1 : 0;
   switch (idx_dtype) {
-    case B2_F64: return launch_front_bwd<double>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, st);
-    case B2_I64: return launch_front_bwd<int64_t>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, st);
-    case B2_I32: return launch_front_bwd<int32_t>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, st);
+    case B2_F64: return launch_front_bwd<double>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, tch, st);
+    case B2_I64: return launch_front_bwd<int64_t>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, tch, st);
+    case B2_I32: return launch_front_bwd<int32_t>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, tch, st);
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
 }

@@ -171,7 +171,8 @@ __global__ void __launch_bounds__(256)
 shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr,
                   const __grid_constant__ PeerPtrs peers, const __grid_constant__ b2_lazy_ctx lz, int lazy,
                   int dim, int lpr_log2, int has_lr, float scale,
-                  const int4* __restrict__ owned, const int32_t* __restrict__ owned_count, int32_t owned_cap) {
+                  const int4* __restrict__ owned, const int32_t* __restrict__ owned_count, int32_t owned_cap,
+                  const b2_touch tch) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(emb, smem_raw);
   SmemFields lf;
@@ -215,7 +216,9 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
       if (has_lr && sub == 0 && (it.w & B2_OWN_LR)) {
         const b2_field& ld = lf.f[f];
         if (ld.table != nullptr) {
-          b2_red_add(reinterpret_cast<float*>(const_cast<void*>(ld.table)) + lrow, peers.glogit[p][bf / F] * scale);
+          float* dst = reinterpret_cast<float*>(const_cast<void*>(ld.table)) + lrow;
+          b2_red_add(dst, peers.glogit[p][bf / F] * scale);
+          b2_touch_mark(tch, dst, true);
           if (lazy) {
             const int grow = (int) (lz.grow_lr[f] + lrow);
             if (b2_lazy_claim(lz, grow, tmark)) enq_l = grow;
@@ -242,7 +245,10 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
       }
       v = acc;
     }
-    if (leader && e < dim) b2_red_add_v4(drow + e, v);
+    if (leader && e < dim) {
+      b2_red_add_v4(drow + e, v);
+      b2_touch_mark(tch, drow + e, e == 0);
+    }
   }
 }
 
@@ -471,10 +477,13 @@ extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_fiel
                                        int64_t batch_local, int world, int rank, const float* const* peer_gemb,
                                        const float* const* peer_glogit, float scale, const int32_t* owned,
                                        const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                                       void* stream) {
+                                       const b2_touch* touch, void* stream) {
   int rc = check_shard_args(emb_fields, nfields, world, rank);
   if (rc != B2_OK) return rc;
   rc = check_lazy(lazy);
+  if (rc != B2_OK) return rc;
+  b2_touch tch;
+  rc = b2_touch_arg(touch, tch);
   if (rc != B2_OK) return rc;
   B2_REQUIRE(peer_gemb && (lr_fields == nullptr || peer_glogit != nullptr), "NULL peer pointer array");
   B2_REQUIRE(owned && owned_count && owned_capacity >= 1 && ((uintptr_t) owned % 16) == 0, "bad owned list");
@@ -502,7 +511,7 @@ extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_fiel
   const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
   shard_pull_kernel<<<grid, 256, smem, (cudaStream_t) stream>>>(epack, lpack, pp, lz, lazy ? 1 : 0, dim, lpr_log2,
                                                                has_lr, scale, reinterpret_cast<const int4*>(owned),
-                                                               owned_count, owned_capacity);
+                                                               owned_count, owned_capacity, tch);
   B2_CUDA_LAUNCH_CHECK("b2_shard_pull");
   return B2_OK;
 }
@@ -512,7 +521,7 @@ extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* 
                                     const float* const* peer_glogit, float scale, const int32_t* owned,
                                     const int32_t* owned_count, int32_t owned_capacity, void* stream) {
   return b2_shard_pull_ex(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_gemb, peer_glogit, scale,
-                          owned, owned_count, owned_capacity, nullptr, stream);
+                          owned, owned_count, owned_capacity, nullptr, nullptr, stream);
 }
 
 extern "C" B2_API int b2_peer_bcast_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,

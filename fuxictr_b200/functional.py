@@ -47,7 +47,9 @@ def _f32c(t):
 # parameter is hit in a step; a second hit falls back to a fresh tensor so autograd can
 # accumulate.
 # --------------------------------------------------------------------------------------
-def _grad_buffer(param, zero):
+def _grad_buffer(param, zero, marks=False):
+    """marks: the caller's kernel flags every granule it writes (ParamArena.touched, passed as _touch());
+    any other writer into the arena's table prefix gets the whole slot flagged here."""
     slot = getattr(param, "_b2_slot", None)
     if slot is not None:
         arena = slot.arena
@@ -56,8 +58,22 @@ def _grad_buffer(param, zero):
             view = arena.grad_view(slot)  # a fresh view object, so AccumulateGrad can steal it
             if zero and not arena.grads_are_zero:
                 view.zero_()
+            if not marks:
+                arena.mark_slot(slot)
             return view
+        # the buffer below reaches the arena through AccumulateGrad's in-place add or the step's p.grad copy
+        arena.mark_slot(slot)
     return torch.zeros_like(param) if zero else torch.empty_like(param)
+
+
+def _touch(bufs):
+    """byref(b2_touch) of the arena the gradient buffers `bufs` live in, or None (no flags to set)."""
+    for b in bufs:
+        base = b._base if b is not None else None
+        arena = getattr(base, "_b2_arena", None) if base is not None else None
+        if arena is not None and arena.touch is not None:
+            return ctypes.byref(arena.touch)
+    return None
 
 
 def _is_zeroed(buf):
@@ -176,7 +192,7 @@ class _EmbedGather(torch.autograd.Function):
         grads = [None] * len(tables)
         for slot, t in enumerate(tables):
             if t.requires_grad:
-                grads[slot] = _grad_buffer(t, zero=True)
+                grads[slot] = _grad_buffer(t, zero=True, marks=True)
         live = [(f, idx) for f, idx in zip(plan.fields, idx_list) if grads[f.table_slot] is not None]
         if live and batch > 0:
             descs = (b2_field * len(live))()
@@ -192,8 +208,8 @@ class _EmbedGather(torch.autograd.Function):
                 # mean_count is indexed by the position in the *backward* field list
                 rows = [plan.fields.index(f) for f, _ in live]
                 count = count[rows].contiguous()
-            _lib.call("b2_embed_scatter_bwd", descs, len(live), batch, ctx_code(idx_list), B2_F32,
-                      _ptr(count), _stream())
+            _lib.call("b2_embed_scatter_bwd_ex", descs, len(live), batch, ctx_code(idx_list), B2_F32,
+                      _ptr(count), _touch(grads), _stream())
         return (None, None, None) + tuple(grads)
 
 
@@ -241,7 +257,7 @@ class _LRForward(torch.autograd.Function):
         grads = [None] * len(tables)
         for slot, t in enumerate(tables):
             if t.requires_grad:
-                grads[slot] = _grad_buffer(t, zero=True)
+                grads[slot] = _grad_buffer(t, zero=True, marks=True)
         gbias = None
         if bias is not None and bias.requires_grad:
             gbias = _grad_buffer(bias, zero=True)
@@ -254,8 +270,8 @@ class _LRForward(torch.autograd.Function):
                     d.table, d.vocab = g.data_ptr(), g.shape[0]
                     d.idx, d.idx_stride = idx.data_ptr(), idx.stride(0)
                     d.dim, d.seq_len, d.pool, d.padding_idx = 1, f.seq_len, f.pool, f.padding_idx
-                _lib.call("b2_lr_bwd", descs, len(live), batch, ctx_code(idx_list), _ptr(gout),
-                          _ptr(gbias), _stream())
+                _lib.call("b2_lr_bwd_ex", descs, len(live), batch, ctx_code(idx_list), _ptr(gout),
+                          _ptr(gbias), _touch(grads), _stream())
             else:
                 gbias.copy_(gout.sum().view(1))
         return (None, None, None, gbias) + tuple(grads)
@@ -1173,8 +1189,8 @@ class _Front(torch.autograd.Function):
         garena = torch.zeros_like(arena) if garena is None else _f32c(garena)
         glogit = (torch.zeros((batch,), dtype=torch.float32, device=arena.device) if glogit is None
                   else _f32c(glogit).view(-1))
-        egrads = [(_grad_buffer(t, zero=True) if t.requires_grad else None) for t in ctx.emb_tables]
-        lgrads = [(_grad_buffer(t, zero=True) if t.requires_grad else None) for t in ctx.lr_tables]
+        egrads = [(_grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in ctx.emb_tables]
+        lgrads = [(_grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in ctx.lr_tables]
         bias = ctx.bias
         gbias = _grad_buffer(bias, zero=True) if (bias is not None and bias.requires_grad) else None
         if batch > 0:
@@ -1197,9 +1213,14 @@ class _Front(torch.autograd.Function):
                     d.idx, d.idx_stride = idx.data_ptr(), idx.stride(0)
                     d.dim, d.seq_len, d.pool, d.padding_idx = 1, 1, 0, f.padding_idx
             lz = ctx.lazy_ctx
-            _lib.call("b2_front_bwd", descs, lr_descs, len(plan.fields), batch, ctx_code(idx_list),
-                      1 if ctx.want_fm else 0, _ptr(arena), _ptr(garena), _ptr(sums), _ptr(glogit),
-                      _ptr(gbias), ctypes.byref(lz) if lz is not None else None, _stream())
+            args = [descs, lr_descs, len(plan.fields), batch, ctx_code(idx_list), 1 if ctx.want_fm else 0,
+                    _ptr(arena), _ptr(garena), _ptr(sums), _ptr(glogit), _ptr(gbias),
+                    ctypes.byref(lz) if lz is not None else None]
+            touch = _touch(egrads + lgrads)
+            if touch is None:      # lazy tables, or gradients outside an arena
+                _lib.call("b2_front_bwd", *args, _stream())
+            else:
+                _lib.call("b2_front_bwd_ex", *args, touch, _stream())
         return (None, None, None, None, None, gbias, None) + tuple(egrads) + tuple(lgrads)
 
 

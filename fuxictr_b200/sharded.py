@@ -268,7 +268,8 @@ class ShardedFront(object):
         _lib.call("b2_shard_pull_ex", self._descs(emb_grads, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.gemb_ptrs), _ptr_array(self.glogit_ptrs) if lr is not None else None,
                   self.pull_scale, F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
-                  ctypes.byref(lz) if lz is not None else None, F2._stream())
+                  ctypes.byref(lz) if lz is not None else None, F2._touch(list(emb_grads) + list(lr_grads or ())),
+                  F2._stream())
 
 
 class _ShardedFrontFn(torch.autograd.Function):
@@ -309,8 +310,8 @@ class _ShardedFrontFn(torch.autograd.Function):
             front.on_dense_grads_ready()
         g.barrier()                      # every rank's gradient rows are ready to be pulled
         n = front.F
-        egrads = [(F2._grad_buffer(t, zero=True) if t.requires_grad else None) for t in tables[:n]]
-        lgrads = [(F2._grad_buffer(t, zero=True) if t.requires_grad else None) for t in tables[n:]]
+        egrads = [(F2._grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in tables[:n]]
+        lgrads = [(F2._grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in tables[n:]]
         front.phase_pull(egrads, lgrads if front.lr_tables else None)
         return (None, None, gbias) + tuple(egrads) + tuple(lgrads)
 

@@ -137,6 +137,24 @@ B2_API int b2_embed_scatter_bwd(const b2_field* fields, int nfields, int64_t bat
                          int elem_dtype, const float* mean_count, void* stream);
 
 /*
+ * Touched-granule flags of a gradient arena's table prefix: one byte per 64-byte granule (16 floats)
+ * of [base, base + n).  A backward kernel given a b2_touch sets the byte of every granule it adds a
+ * gradient into (a plain store: idempotent, no atomic); writes outside [base, base + n) mark nothing.
+ * Invariant the optimizer relies on: every nonzero float of [base, base + n) lies in a flagged granule
+ * (b2_sumsq_ex / b2_adam_step_ex skip the others).  Marking more is always safe.
+ * flags == NULL or n == 0: no flags.
+ */
+typedef struct b2_touch {
+  uint8_t* flags;      /* [(n + 15) / 16] */
+  const float* base;   /* first element covered (16-byte aligned) */
+  int64_t n;           /* elements covered */
+} b2_touch;
+/* b2_embed_scatter_bwd, also marking `touch` (NULL = none). */
+B2_API int b2_embed_scatter_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
+                                   int elem_dtype, const float* mean_count, const b2_touch* touch,
+                                   void* stream);
+
+/*
  * LogisticRegression.forward (layers/blocks/logistic_regression.py:55-58):
  * out[b] = sum over features (and sequence positions, MaskedSumPooling,
  * feature_embedding.py:135-138) of table_f[idx] + bias[0].  Tables are
@@ -149,6 +167,9 @@ B2_API int b2_lr_fwd(const b2_field* fields, int nfields, int64_t batch, int idx
  * gbias[0] += sum_b gout[b]. `table` fields point at the (vocab,1) gradient buffers. */
 B2_API int b2_lr_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
               const float* gout, float* gbias, void* stream);
+/* b2_lr_bwd, also marking `touch` (NULL = none). */
+B2_API int b2_lr_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
+                        const float* gout, float* gbias, const b2_touch* touch, void* stream);
 
 
 /*
@@ -211,6 +232,11 @@ B2_API int b2_front_bwd(const b2_field* emb_fields, const b2_field* lr_fields, i
                         int idx_dtype, int want_fm, const float* emb_saved, const float* gx,
                         const float* sums, const float* glogit, float* gbias,
                         const b2_lazy_ctx* lazy /* non-NULL: enqueue every touched row once */, void* stream);
+/* b2_front_bwd, also marking `touch` (NULL = none) for every embedding and LR gradient it writes. */
+B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch,
+                           int idx_dtype, int want_fm, const float* emb_saved, const float* gx,
+                           const float* sums, const float* glogit, float* gbias, const b2_lazy_ctx* lazy,
+                           const b2_touch* touch, void* stream);
 /*
  * Lazy optimizer step over the rows enqueued by b2_front_bwd (tables[i]: parameter pointer, rows, dim,
  * global row base, sorted by base; gradients/moments at the arena deltas):
@@ -269,7 +295,8 @@ B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, 
  * brings every served row with last_step[grow] < *step_dev up to date in registers before the store
  * (nothing is written back), and the pull appends every owned, non-padding row it scatters a gradient
  * into to the worklist, once per step (claimed through mark).  grow = grow_emb[f] / grow_lr[f] + local
- * row.  The caller zeroes lazy->counter before the pull of a step. */
+ * row.  The caller zeroes lazy->counter before the pull of a step.  touch (NULL = none): the pull marks
+ * the granules of every gradient row it scatters into (b2_touch). */
 B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
                             int64_t batch_local, int world, int rank, const void* const* peer_ids,
                             int idx_dtype, int64_t ids_stride, float* const* peer_emb,
@@ -279,7 +306,7 @@ B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_field
                             int64_t batch_local, int world, int rank, const float* const* peer_gemb,
                             const float* const* peer_glogit, float scale, const int32_t* owned,
                             const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                            void* stream);
+                            const b2_touch* touch, void* stream);
 B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream);
 /* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
  * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world. */
@@ -540,6 +567,18 @@ B2_API int b2_sumsq(const float* g, int64_t n, float* out, void* stream);
 B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
                  float max_norm, float lr, float beta1, float beta2, float eps,
                  const int64_t* step_dev, int zero_grad, void* stream);
+/* The same two passes reading G only where a batch wrote it: flags[k] (b2_touch) covers elements
+ * [16k, 16k + 16) of the first n_flagged elements (n_flagged % 4 == 0, <= n); the elements after
+ * n_flagged have no flags and run as above.  An unflagged granule holds only zeros: b2_sumsq_ex skips
+ * it (each thread keeps its elements, so the block partials equal b2_sumsq's), b2_adam_step_ex applies
+ * g = 0 without loading or storing G.  A flagged granule is updated as b2_adam_step does, and with
+ * zero_grad != 0 its flag is cleared together with its gradient.  flags == NULL is the plain form. */
+B2_API int b2_sumsq_ex(const float* g, int64_t n, float* out, const uint8_t* flags, int64_t n_flagged,
+                       void* stream);
+B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
+                           float max_norm, float lr, float beta1, float beta2, float eps,
+                           const int64_t* step_dev, int zero_grad, uint8_t* flags, int64_t n_flagged,
+                           void* stream);
 B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
                          int64_t sched_len, void* stream);
 B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
