@@ -18,15 +18,17 @@
 //     round-to-nearest, so the error does not grow with the length of the contraction.
 //   bf16 operands (elem_dtype B2_BF16): wgmma .bf16, 64-element k-blocks, fp32 accumulation.
 //
-// Structure (one CTA per 128 x BN output tile and K split; 384 threads), one ring of 2-4 stages:
+// Structure (one CTA per 128 x BN output tile and K split; 384 threads), one ring of 2-4 stages whose layout
+// depends on the operand majors (Ring):
 //   K-major operands are loaded by TMA with the 128B swizzle, straight into the layout wgmma reads; wgmma
 //   .tf32 reads an fp32 value as its truncation big(x), so the raw tile is the big part (DESIGN.md §4).
 //   MN-major operands land unswizzled in a staging tile of the same stage; wgmma reads tf32 from shared memory
 //   only K-major, so they are transposed into the swizzled tile in shared memory and stay as they lie in HBM.
 //   warp 0         one thread issues the TMA loads of a stage as soon as the consumers release it.
-//   warps 1-3      converter: MN-major staging -> swizzled tile; 3xTF32: the small parts of A and B, written at
-//                  the offsets of the swizzled tile in their own tiles (no re-layout).
-//   warpgroups 1-2 64 rows each: wgmma m64nBNk8 (tf32) / k16 (bf16), both operands from shared memory.  3xTF32
+//   warps 1-3      converter: MN-major staging -> swizzled tile; 3xTF32: the small parts of B and of an MN-major
+//                  A, written at the offsets of the swizzled tile in their own tiles (no re-layout).
+//   warpgroups 1-2 64 rows each: wgmma m64nBNk8 (tf32) / k16 (bf16), both operands from shared memory, except in
+//                  3xTF32 with a K-major A: each thread loads its A fragment and splits it in registers.  3xTF32
 //                  commits each k-block as two groups, the main product and then the cross terms; the main
 //                  product is folded into the sum while the cross terms still run, and a stage is released
 //                  one k-block later.  The single-pass modes likewise keep one group in flight.  Then the fused
@@ -45,22 +47,45 @@ constexpr int NTHREADS = 384;    // producer / converter warpgroup + two wgmma w
 constexpr int NCONV = 96;        // converter threads (warps 1-3)
 enum Mode { TF32 = 0, BF16 = 1, X3 = 2 };
 
-// Shared memory of one pipeline stage: the swizzled A and B tiles wgmma reads, their small parts (3xTF32), and
-// unswizzled staging tiles where an MN-major operand lands.  Every tile starts 1024-byte aligned.
-template <int BN, int MODE>
+// Shared memory of one pipeline stage, sized per launch from the operand majors: the swizzled A and B tiles
+// wgmma reads, the small parts the converter still makes (B always in 3xTF32; A only when it is MN-major, since a
+// K-major A is split in registers), and unswizzled staging tiles only for an MN-major operand.  Every tile
+// starts 1024-byte aligned.
 struct Ring {
-  static constexpr uint32_t A_BYTES = BM * 128, B_BYTES = BN * 128;
-  static constexpr uint32_t OFF_B = A_BYTES;
-  static constexpr uint32_t OFF_AS = OFF_B + B_BYTES;                               // A small (3xTF32)
-  static constexpr uint32_t OFF_BS = OFF_AS + (MODE == X3 ? A_BYTES : 0);           // B small (3xTF32)
-  static constexpr uint32_t OFF_SA = OFF_BS + (MODE == X3 ? B_BYTES : 0);           // A staging (MN-major)
-  static constexpr uint32_t OFF_SB = OFF_SA + A_BYTES;                              // B staging (MN-major)
-  static constexpr uint32_t STAGE = OFF_SB + B_BYTES;
-  static constexpr uint32_t EXTRA = 1024 + 128;                                     // alignment slack, mbarriers
-  static constexpr int STAGES = (227u * 1024u - EXTRA) / STAGE >= 4 ? 4 : (int) ((227u * 1024u - EXTRA) / STAGE);
-  static constexpr size_t SMEM = (size_t) STAGES * STAGE + EXTRA;
-  static_assert(STAGES >= 2, "ring does not fit shared memory");
+  uint32_t off_b, off_as, off_bs, off_sa, off_sb;   // byte offsets in a stage (A sits at 0)
+  uint32_t stage;                                    // bytes per stage
+  int stages;                                        // 2-4
+  size_t smem;                                       // dynamic shared memory of the launch
 };
+constexpr uint32_t RING_EXTRA = 1024 + 128;          // alignment slack, mbarriers
+constexpr uint32_t SMEM_MAX = 227u * 1024u;
+constexpr Ring ring_layout(int bn, int mode, bool a_mn, bool b_mn) {
+  const uint32_t a = BM * 128, b = (uint32_t) bn * 128;
+  Ring r{};
+  uint32_t o = a;
+  r.off_b = o;  o += b;
+  r.off_as = o; o += (mode == X3 && a_mn) ? a : 0;
+  r.off_bs = o; o += mode == X3 ? b : 0;
+  r.off_sa = o; o += a_mn ? a : 0;
+  r.off_sb = o; o += b_mn ? b : 0;
+  r.stage = o;
+  r.stages = (SMEM_MAX - RING_EXTRA) / o >= 4 ? 4 : (int) ((SMEM_MAX - RING_EXTRA) / o);
+  r.smem = (size_t) r.stages * o + RING_EXTRA;
+  return r;
+}
+// The largest ring an instantiation launches with, over the four operand-major pairs: its shared-memory attribute.
+// (Not always both MN-major: a smaller stage can buy a deeper ring.)
+constexpr size_t ring_smem_max(int bn, int mode) {
+  size_t m = 0;
+  for (int a_mn = 0; a_mn < 2; ++a_mn)
+    for (int b_mn = 0; b_mn < 2; ++b_mn) {
+      const size_t s = ring_layout(bn, mode, a_mn != 0, b_mn != 0).smem;
+      m = s > m ? s : m;
+    }
+  return m;
+}
+static_assert(ring_layout(128, TF32, true, true).stages >= 2 && ring_layout(64, X3, true, true).stages >= 2,
+              "ring does not fit shared memory");
 
 struct Params {
   CUtensorMap map_a;
@@ -79,6 +104,7 @@ struct Params {
   int esz;                // operand element bytes: 4 = fp32 (tf32 passes), 2 = bf16
   int64_t ld_aux;         // leading dimension of c_small
   int tiles_m, tiles_n, splits;
+  Ring ring;              // this launch's stage layout (ring_layout of its tile width, mode and operand majors)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -164,6 +190,22 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a, uint64_t 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a), "l"(b), "r"(scale_d));
 }
+// The same m64nNk8 tf32 with A from registers: a[] is this thread's fragment of the warp's 16 rows x 8 k —
+// a[0] (row l/4, k l%4), a[1] (row l/4 + 8, k l%4), a[2] (row l/4, k l%4 + 4), a[3] (row l/4 + 8, k l%4 + 4).
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}
 __device__ __forceinline__ void wgmma_bf16(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
@@ -221,8 +263,13 @@ __device__ __forceinline__ void transpose_tile(const uint8_t* src, uint8_t* dst,
       }
     }
   } else {
+    // Thread b takes 4 rows from r0 and k-chunk kq.  Each group of 64 covers 8 row quads x 8 chunks: the 8 lanes of a
+    // quarter-warp take 8 consecutive row quads (16-byte loads in 8 different bank groups, whatever the k-row pitch)
+    // and chunks kq = q ^ s; the swizzled stores of row r0 + i then land in chunks kq ^ (r0 + i) % 8 =
+    // q ^ 4 (q & 1) ^ s ^ i, distinct over q: both sides are conflict-free.  rows is a multiple of 32.
     for (int b = ct; b < 2 * rows; b += NCONV) {
-      const int kq = b & 7, r0 = (b >> 3) * 4;
+      const int q = b & 7, s = (b >> 3) & 7;
+      const int kq = q ^ s, r0 = ((b >> 6) * 8 + q) * 4;
       float4 v[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((4 * kq + j) * rows + r0) * 4);
@@ -272,14 +319,14 @@ __device__ __forceinline__ float epilogue_elem(const Params& p, int m, int n, fl
 template <int BN, int MODE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
-  using R = Ring<BN, MODE>;
-  constexpr int S = R::STAGES;
   constexpr int NR = BN / 2;                            // accumulators per thread: 64 x BN per warpgroup
   constexpr int BKE = MODE == BF16 ? 64 : 32;           // k elements per k-block: one 128-byte swizzle row
+  const Ring& R = p.ring;
+  const int S = R.stages;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte aligned bases: align by hand (1 KB of slack is requested).
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * R::STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * R.stage);
   // per stage: TMA landed; converter done; consumers done (the producer may refill it)
   const uint32_t full0 = smem_u32(bars), conv0 = smem_u32(bars + S), empty0 = smem_u32(bars + 2 * S);
 
@@ -313,54 +360,62 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
     // ---------------- warpgroup 0: TMA producer (warp 0) and converter (warps 1-3) ----------------
     if (warp == 0) {
       if (lane == 0) {
+        int s = 0;
+        uint32_t ph = 0;
         for (int i = 0; i < nkb; ++i) {
-          const int s = i % S, kb = kb_begin + i;
-          if (i >= S) mbar_wait(empty0 + 8 * s, ((uint32_t) (i / S) & 1u) ^ 1u);
-          const uint32_t st = smem_u32(smem + s * R::STAGE), bar = full0 + 8 * s;
-          mbar_expect_tx(bar, R::A_BYTES + R::B_BYTES);   // out-of-range parts of a box arrive zero-filled, count in full
-          if (p.a_mn) tma_load_2d(st + R::OFF_SA, &p.map_a, bar, m0, kb * BKE);
+          const int kb = kb_begin + i;
+          if (i >= S) mbar_wait(empty0 + 8 * s, ph ^ 1u);
+          const uint32_t st = smem_u32(smem + s * R.stage), bar = full0 + 8 * s;
+          mbar_expect_tx(bar, (BM + BN) * 128);   // out-of-range parts of a box arrive zero-filled, count in full
+          if (p.a_mn) tma_load_2d(st + R.off_sa, &p.map_a, bar, m0, kb * BKE);
           else tma_load_2d(st, &p.map_a, bar, kb * BKE, m0);
-          if (p.b_mn) tma_load_2d(st + R::OFF_SB, &p.map_b, bar, n0, kb * BKE);
-          else tma_load_2d(st + R::OFF_B, &p.map_b, bar, kb * BKE, n0);
+          if (p.b_mn) tma_load_2d(st + R.off_sb, &p.map_b, bar, n0, kb * BKE);
+          else tma_load_2d(st + R.off_b, &p.map_b, bar, kb * BKE, n0);
+          if (++s == S) { s = 0; ph ^= 1u; }
         }
       }
     } else if (conv) {
       const int ct = threadIdx.x - 32;
+      int s = 0;
+      uint32_t ph = 0;
       for (int i = 0; i < nkb; ++i) {
-        const int s = i % S;
-        mbar_wait(full0 + 8 * s, (uint32_t) (i / S) & 1u);
-        uint8_t* st = smem + s * R::STAGE;
+        mbar_wait(full0 + 8 * s, ph);
+        uint8_t* st = smem + s * R.stage;
         if constexpr (MODE == BF16) {
-          if (p.a_mn) transpose_tile<true, RAW>(st + R::OFF_SA, st, 0, BM, ct);
-          if (p.b_mn) transpose_tile<true, RAW>(st + R::OFF_SB, st + R::OFF_B, 0, BN, ct);
+          if (p.a_mn) transpose_tile<true, RAW>(st + R.off_sa, st, 0, BM, ct);
+          if (p.b_mn) transpose_tile<true, RAW>(st + R.off_sb, st + R.off_b, 0, BN, ct);
         } else if constexpr (MODE == TF32) {
-          if (p.a_mn) transpose_tile<false, BIG>(st + R::OFF_SA, st, 0, BM, ct);
-          if (p.b_mn) transpose_tile<false, BIG>(st + R::OFF_SB, st + R::OFF_B, 0, BN, ct);
+          if (p.a_mn) transpose_tile<false, BIG>(st + R.off_sa, st, 0, BM, ct);
+          if (p.b_mn) transpose_tile<false, BIG>(st + R.off_sb, st + R.off_b, 0, BN, ct);
         } else {
-          if (p.a_mn) transpose_tile<false, BIG_SMALL>(st + R::OFF_SA, st, R::OFF_AS, BM, ct);
-          else small_tile(st, st + R::OFF_AS, BM, ct);
-          if (p.b_mn) transpose_tile<false, BIG_SMALL>(st + R::OFF_SB, st + R::OFF_B, R::OFF_BS - R::OFF_B, BN, ct);
-          else small_tile(st + R::OFF_B, st + R::OFF_BS, BN, ct);
+          // a K-major A is split by the consumers in registers
+          if (p.a_mn) transpose_tile<false, BIG_SMALL>(st + R.off_sa, st, R.off_as, BM, ct);
+          if (p.b_mn) transpose_tile<false, BIG_SMALL>(st + R.off_sb, st + R.off_b, R.off_bs - R.off_b, BN, ct);
+          else small_tile(st + R.off_b, st + R.off_bs, BN, ct);
         }
         // generic-proxy stores -> visible to wgmma (async proxy) before the consumers are told
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         if (lane == 0) mbar_arrive(conv0 + 8 * s);
+        if (++s == S) { s = 0; ph ^= 1u; }
       }
     }
   } else {
     // ---------------- warpgroups 1-2: wgmma on rows 64 g .. 64 g + 63 of the tile, then the epilogue ----------
     const int g = (warp >> 2) - 1;
-    auto ready = [&](int i) -> const uint8_t* {
-      const int s = i % S;
-      const uint32_t ph = (uint32_t) (i / S) & 1u;
-      mbar_wait(full0 + 8 * s, ph);
-      if (conv) mbar_wait(conv0 + 8 * s, ph);
-      return smem + s * R::STAGE;
+    int rs = 0, fs = 0;                // stage of the next k-block to consume / to release
+    uint32_t rph = 0;
+    auto ready = [&]() -> const uint8_t* {
+      mbar_wait(full0 + 8 * rs, rph);
+      if (conv) mbar_wait(conv0 + 8 * rs, rph);
+      const uint8_t* st = smem + rs * R.stage;
+      if (++rs == S) { rs = 0; rph ^= 1u; }
+      return st;
     };
-    auto release = [&](int i) {        // k-block i's wgmma group has completed: its stage may be refilled
+    auto release = [&]() {             // the oldest unreleased k-block's wgmma groups have completed
       __syncwarp();
-      if (lane == 0) mbar_arrive(empty0 + 8 * (i % S));
+      if (lane == 0) mbar_arrive(empty0 + 8 * fs);
+      if (++fs == S) fs = 0;
     };
     float acc[NR];
 #pragma unroll
@@ -369,37 +424,84 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
       float corr[NR], part[NR];
 #pragma unroll
       for (int r = 0; r < NR; ++r) { corr[r] = 0.f; part[r] = 0.f; }
-      for (int i = 0; i < nkb; ++i) {
-        const uint32_t base = smem_u32(ready(i));
-        // one instruction consumes 32 bytes of K per row (8 tf32): +2 in the (addr >> 4) field
-        const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R::OFF_B),
-                       asd = make_smem_desc(base + R::OFF_AS + g * 64 * 128), bsd = make_smem_desc(base + R::OFF_BS);
-        // two groups: the main product A_big.B_big from zero into part, then the cross terms into corr
-        wgmma_fence();
+      // Per k-block two groups: the main product A_big.B_big from zero into part, then the cross terms
+      // A_big.B_small + A_small.B_big into corr.  Once all but the cross group just committed are done, this
+      // k-block's main product is folded (fp32 round-to-nearest) while the cross terms run, and the previous
+      // k-block's stage is released.  One instruction consumes 32 bytes of K per row (8 tf32): +2 in the
+      // (addr >> 4) field of a descriptor.
+      if (p.a_mn) {
+        // A transposed by the converter: both parts of A from shared memory
+        for (int i = 0; i < nkb; ++i) {
+          const uint32_t base = smem_u32(ready());
+          const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R.off_b),
+                         asd = make_smem_desc(base + R.off_as + g * 64 * 128), bsd = make_smem_desc(base + R.off_bs);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_tf32(part, ad + 2 * k, bd + 2 * k, k > 0 ? 1u : 0u);        // A_big . B_big
-        wgmma_commit();
+          for (int k = 0; k < 4; ++k) wgmma_tf32(part, ad + 2 * k, bd + 2 * k, k > 0 ? 1u : 0u);        // A_big . B_big
+          wgmma_commit();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wgmma_tf32(corr, ad + 2 * k, bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                    // A_big . B_small
-          wgmma_tf32(corr, asd + 2 * k, bd + 2 * k, 1u);                                           // A_small . B_big
+          for (int k = 0; k < 4; ++k) {
+            wgmma_tf32(corr, ad + 2 * k, bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                    // A_big . B_small
+            wgmma_tf32(corr, asd + 2 * k, bd + 2 * k, 1u);                                           // A_small . B_big
+          }
+          wgmma_commit();
+          wgmma_wait1();
+#pragma unroll
+          for (int r = 0; r < NR; ++r) acc[r] += part[r];
+          if (i > 0) release();
         }
-        wgmma_commit();
-        // all but the cross group just committed are done: fold this k-block's main product (fp32
-        // round-to-nearest) while the cross terms run, and release the previous k-block's stage
-        wgmma_wait1();
+        wgmma_wait0();
+      } else {
+        // K-major A: each thread loads its wgmma fragment of the swizzled tile (rows l/4 and l/4 + 8 of its warp's
+        // 16, one 4-byte word of 16-byte chunk c: 8 rows x one chunk per load, the chunks distinct under the
+        // swizzle, so conflict-free) and splits it in registers.  One fragment set: it is rewritten only after the
+        // previous k-block's cross group has completed (a second set does not fit the 168-register launch bound,
+        // which ptxas keeps even under setmaxnreg).  Meanwhile the other warpgroup keeps the tensor cores busy.
+        const int ra = g * 64 + (warp & 3) * 16 + (lane >> 2);
+        const uint32_t aoff = (uint32_t) ra * 128 + 4 * (lane & 3);
+        const int rx = ra & 7;
+        uint32_t ab[4][4], as[4][4];
+        for (int i = 0; i < nkb; ++i) {
+          const uint8_t* st = ready();
+          if (i > 0) {
+            wgmma_wait0();
+            release();
+          }
+          const float* tile = reinterpret_cast<const float*>(st);
 #pragma unroll
-        for (int r = 0; r < NR; ++r) acc[r] += part[r];
-        if (i > 0) release(i - 1);
+          for (int k = 0; k < 4; ++k) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {   // j: row + 8 (j & 1), chunk 2k + (j >> 1)
+              const float v = tile[(aoff + 1024 * (j & 1) + (((2 * k + (j >> 1)) ^ rx) << 4)) >> 2];
+              ab[k][j] = __float_as_uint(tf32_big(v));
+              as[k][j] = __float_as_uint(tf32_small(v));
+            }
+          }
+          const uint32_t base = smem_u32(st);
+          const uint64_t bd = make_smem_desc(base + R.off_b), bsd = make_smem_desc(base + R.off_bs);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_tf32_rs(part, ab[k], bd + 2 * k, k > 0 ? 1u : 0u);          // A_big . B_big
+          wgmma_commit();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            wgmma_tf32_rs(corr, ab[k], bsd + 2 * k, (i > 0 || k > 0) ? 1u : 0u);                      // A_big . B_small
+            wgmma_tf32_rs(corr, as[k], bd + 2 * k, 1u);                                             // A_small . B_big
+          }
+          wgmma_commit();
+          wgmma_wait1();
+#pragma unroll
+          for (int r = 0; r < NR; ++r) acc[r] += part[r];
+        }
+        wgmma_wait0();
       }
-      wgmma_wait0();
 #pragma unroll
       for (int r = 0; r < NR; ++r) acc[r] += corr[r];
     } else {
       for (int i = 0; i < nkb; ++i) {
-        const uint32_t base = smem_u32(ready(i));
+        const uint32_t base = smem_u32(ready());
         // one instruction consumes 32 bytes of K per row (8 tf32 / 16 bf16): +2 in the (addr >> 4) field
-        const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R::OFF_B);
+        const uint64_t ad = make_smem_desc(base + g * 64 * 128), bd = make_smem_desc(base + R.off_b);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -408,7 +510,7 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
         }
         wgmma_commit();
         wgmma_wait1();
-        if (i > 0) release(i - 1);
+        if (i > 0) release();
       }
       wgmma_wait0();
     }
@@ -691,35 +793,30 @@ extern "C" B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const fl
 template <int BN, int MODE>
 static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
   void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE>;
-  const size_t smem = tc::Ring<BN, MODE>::SMEM;
-  // opt-in to > 48 KB of dynamic shared memory: an idempotent per-process property of each instantiation
-  // (C++11 guarantees the initialiser runs once, thread-safely)
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+  // opt-in to > 48 KB of dynamic shared memory, for the largest ring this instantiation launches with: an
+  // idempotent per-process property (C++11 guarantees the initialiser runs once, thread-safely)
+  static const cudaError_t attr_rc =
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) tc::ring_smem_max(BN, MODE));
   if (attr_rc != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: smem attribute: %s", cudaGetErrorString(attr_rc));
-  B2_LAUNCH(kern, grid, tc::NTHREADS, smem, st, p);
+  B2_REQUIRE(p.ring.smem <= tc::ring_smem_max(BN, MODE), "ring exceeds the shared-memory attribute");
+  B2_LAUNCH(kern, grid, tc::NTHREADS, p.ring.smem, st, p);
   B2_CUDA_LAUNCH_CHECK("b2_gemm_tc");
   return B2_OK;
 }
 
 // One kernel instantiation per tile width and arithmetic mode (tf32 and bf16 single pass, 3xTF32 up to bn = 64).
-struct GemmInst {
-  int (*launch)(const tc::Params&, int, cudaStream_t);
-  size_t smem;
-  int stages;
-};
-template <int BN, int MODE>
-static GemmInst gemm_inst_of() { return {gemm_launch<BN, MODE>, tc::Ring<BN, MODE>::SMEM, tc::Ring<BN, MODE>::STAGES}; }
-static GemmInst gemm_inst(int bn, int mode) {
+typedef int (*GemmLaunch)(const tc::Params&, int, cudaStream_t);
+static GemmLaunch gemm_inst(int bn, int mode) {
   switch (bn * 4 + mode) {
-    case 32 * 4 + tc::TF32: return gemm_inst_of<32, tc::TF32>();
-    case 64 * 4 + tc::TF32: return gemm_inst_of<64, tc::TF32>();
-    case 128 * 4 + tc::TF32: return gemm_inst_of<128, tc::TF32>();
-    case 32 * 4 + tc::BF16: return gemm_inst_of<32, tc::BF16>();
-    case 64 * 4 + tc::BF16: return gemm_inst_of<64, tc::BF16>();
-    case 128 * 4 + tc::BF16: return gemm_inst_of<128, tc::BF16>();
-    case 32 * 4 + tc::X3: return gemm_inst_of<32, tc::X3>();
-    case 64 * 4 + tc::X3: return gemm_inst_of<64, tc::X3>();
-    default: return {nullptr, 0, 0};
+    case 32 * 4 + tc::TF32: return gemm_launch<32, tc::TF32>;
+    case 64 * 4 + tc::TF32: return gemm_launch<64, tc::TF32>;
+    case 128 * 4 + tc::TF32: return gemm_launch<128, tc::TF32>;
+    case 32 * 4 + tc::BF16: return gemm_launch<32, tc::BF16>;
+    case 64 * 4 + tc::BF16: return gemm_launch<64, tc::BF16>;
+    case 128 * 4 + tc::BF16: return gemm_launch<128, tc::BF16>;
+    case 32 * 4 + tc::X3: return gemm_launch<32, tc::X3>;
+    case 64 * 4 + tc::X3: return gemm_launch<64, tc::X3>;
+    default: return nullptr;
   }
 }
 
@@ -762,16 +859,19 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   double best_cost = 1e300;
   const int bn_max = three_pass ? 64 : 128;
   for (int bn = 32; bn <= bn_max; bn *= 2) {
-    // Cycles per k-block: the larger of the tensor pipe — passes x 4 instructions x bn/2 (m64 per warpgroup, two
-    // in parallel) — and shared memory at 128 B (one tile row) a cycle.  Shared-memory rows: TMA writes A and B;
-    // the converter reads and writes an MN-major tile again, and in 3xTF32 reads each tile and writes its small
-    // part (both in one pass for an MN-major tile); wgmma reads 64 rows of A and B per pass and warpgroup.
+    // Cycles per k-block: the larger of the tensor pipe — passes x 2 warpgroups x 4 instructions x bn/2 (an
+    // m64nBNk8 tf32 takes bn/2 cycles of the SM's tensor cores, which the two warpgroups share) — and shared memory
+    // at 128 B (one tile row) a cycle.  Shared-memory rows: TMA writes A and B; the converter reads and writes an
+    // MN-major tile again, and in 3xTF32 writes the small part of B and of an MN-major A (a K-major B is read
+    // once more for it; a K-major A is split in registers); wgmma reads bn rows of B per pass and warpgroup, and
+    // 64 rows of A — per pass from shared memory, or once into registers for a K-major A in 3xTF32.
     const bool mn_a = d->a_mn_major != 0, mn_b = d->b_mn_major != 0;
+    const double passes = three_pass ? 3.0 : 1.0;
     const double rows_tma = tc::BM + bn;
     const double rows_conv = (mn_a ? 2.0 : 0.0) * tc::BM + (mn_b ? 2.0 : 0.0) * bn +
-                             (three_pass ? (mn_a ? 1.0 : 2.0) * tc::BM + (mn_b ? 1.0 : 2.0) * bn : 0.0);
-    const double rows_mma = (three_pass ? 3.0 : 1.0) * 2.0 * (64 + bn);
-    const double per_kb = fmax((three_pass ? 3.0 : 1.0) * 2.0 * bn, rows_tma + rows_conv + rows_mma);
+                             (three_pass ? (mn_a ? 1.0 : 0.0) * tc::BM + (mn_b ? 1.0 : 2.0) * bn : 0.0);
+    const double rows_mma = passes * 2.0 * bn + (three_pass && !mn_a ? 1.0 : passes) * tc::BM;
+    const double per_kb = fmax(passes * 4.0 * bn, rows_tma + rows_conv + rows_mma);
     const int64_t tiles_n = b2_ceil_div(N, bn);
     for (int split = 1; split <= 32; split *= 2) {
       if (split > 1 && (!linear || num_kb / split < 8)) break;
@@ -802,13 +902,15 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   const int64_t total_tiles = tiles_m * tiles_n * splits;
   B2_REQUIRE(total_tiles < (1ll << 31), "too many tiles");
   p.tiles_m = (int) tiles_m; p.tiles_n = (int) tiles_n; p.splits = splits;
-  const GemmInst inst = gemm_inst(best_bn, three_pass ? tc::X3 : (esz == 2 ? tc::BF16 : tc::TF32));
-  B2_REQUIRE(inst.launch != nullptr, "no GEMM instantiation for bn %d", best_bn);
-  B2_REQUIRE(inst.smem <= (size_t) 227 * 1024, "tile does not fit shared memory");
+  const int mode = three_pass ? tc::X3 : (esz == 2 ? tc::BF16 : tc::TF32);
+  const GemmLaunch launch = gemm_inst(best_bn, mode);
+  B2_REQUIRE(launch != nullptr, "no GEMM instantiation for bn %d", best_bn);
+  p.ring = tc::ring_layout(best_bn, mode, p.a_mn != 0, p.b_mn != 0);
+  B2_REQUIRE(p.ring.stages >= 2 && p.ring.smem <= tc::SMEM_MAX, "tile does not fit shared memory");
   if (plan != nullptr) {
-    plan->bn = best_bn; plan->splits = splits; plan->stages = inst.stages; plan->cstages = inst.stages;
+    plan->bn = best_bn; plan->splits = splits; plan->stages = p.ring.stages; plan->cstages = p.ring.stages;
     plan->grid = (int) total_tiles; plan->threads = tc::NTHREADS; plan->tiles_m = p.tiles_m; plan->tiles_n = p.tiles_n;
-    plan->passes = three_pass ? 3 : 1; plan->kb_per_split = p.kb_per_split; plan->smem_bytes = (int64_t) inst.smem;
+    plan->passes = three_pass ? 3 : 1; plan->kb_per_split = p.kb_per_split; plan->smem_bytes = (int64_t) p.ring.smem;
     return B2_OK;
   }
   if (splits > 1 && !p.beta && !(d->flags & B2_GEMM_C_IS_ZERO)) {
@@ -819,7 +921,7 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
     cudaError_t e = cudaMemsetAsync(d->colsum, 0, sizeof(float) * (size_t) N, st);
     if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
   }
-  return inst.launch(p, (int) total_tiles, st);
+  return launch(p, (int) total_tiles, st);
 }
 
 extern "C" B2_API int b2_gemm_tc_ex(const b2_gemm_desc* d, void* stream) { return gemm_tc_impl(d, stream, nullptr); }
