@@ -32,8 +32,9 @@
 //                  commits each k-block as two groups, the main product and then the cross terms; the main
 //                  product is folded into the sum while the cross terms still run, and a stage is released
 //                  one k-block later.  The single-pass modes likewise keep one group in flight.  Then the fused
-//                  epilogue straight from the accumulator registers (each quad of lanes writes 32 contiguous
-//                  bytes of one output row).
+//                  epilogue: the accumulators are staged as a row-major tile in the dead ring, and each thread walks
+//                  it in 16-byte row segments, a batch at a time, with every global load of a batch issued before
+//                  its first store.
 // Kernels of a step are chained with programmatic dependent launch (prologue under the predecessor's tail).
 // Every mbarrier wait is bounded: a pipeline bug traps with a message instead of hanging the GPU.
 #include "b2_common.cuh"
@@ -86,6 +87,22 @@ constexpr size_t ring_smem_max(int bn, int mode) {
 }
 static_assert(ring_layout(128, TF32, true, true).stages >= 2 && ring_layout(64, X3, true, true).stages >= 2,
               "ring does not fit shared memory");
+// The epilogue stages the accumulators in the dead ring: a row-major fp32 tile of BM x BN with a row pitch of BN + 8
+// floats, then 256 x 4 column partial sums.  A pitch of 8 (mod 32) words makes the float2 fragment stores (8 rows x
+// 32 bytes per instruction) hit 32 distinct banks per 128 bytes; a quarter-warp's float4 row reads are contiguous.
+constexpr int epi_pitch(int bn) { return bn + 8; }
+constexpr uint32_t epi_bytes(int bn) { return (uint32_t) (BM * epi_pitch(bn) + 256 * 4) * 4u; }
+constexpr bool epi_fits(int bn, int mode) {
+  for (int a_mn = 0; a_mn < 2; ++a_mn)
+    for (int b_mn = 0; b_mn < 2; ++b_mn) {
+      const Ring r = ring_layout(bn, mode, a_mn != 0, b_mn != 0);
+      if ((uint32_t) r.stages * r.stage < epi_bytes(bn)) return false;
+    }
+  return true;
+}
+static_assert(epi_fits(32, TF32) && epi_fits(64, TF32) && epi_fits(128, TF32) && epi_fits(32, BF16) &&
+              epi_fits(64, BF16) && epi_fits(128, BF16) && epi_fits(32, X3) && epi_fits(64, X3),
+              "epilogue tile does not fit the ring");
 
 struct Params {
   CUtensorMap map_a;
@@ -103,6 +120,7 @@ struct Params {
   int a_mn, b_mn;         // operand is MN-major (memory (K, rows))
   int esz;                // operand element bytes: 4 = fp32 (tf32 passes), 2 = bf16
   int64_t ld_aux;         // leading dimension of c_small
+  int vec;                // every epilogue pointer and leading dimension allows 16-byte row segments (bf16 c_small: 8)
   int tiles_m, tiles_n, splits;
   Ring ring;              // this launch's stage layout (ring_layout of its tile width, mode and operand majors)
 };
@@ -289,32 +307,61 @@ __device__ __forceinline__ void small_tile(const uint8_t* src, uint8_t* dst, int
   }
 }
 
-// One output element (m, n) of the fused epilogue, t = accumulator + bias; returns what enters the column sum.
-__device__ __forceinline__ float epilogue_elem(const Params& p, int m, int n, float t) {
-  const int64_t o = (int64_t) m * p.ldc + n;
-  if (p.splits > 1) {          // split-K: partial sums of a plain linear output (C was zeroed by the host)
-    b2_red_add(p.c + o, t);
-    return 0.f;
+// A row segment of the epilogue: 4 consecutive fp32 of one row as one 16-byte access when `vec` (whole and aligned),
+// else the first `nv` of them one by one (the rest read as 0).  NC: read-only for the whole kernel.
+template <bool NC>
+__device__ __forceinline__ float4 seg_load(const float* p, bool vec, int nv) {
+  if (vec) return NC ? __ldg(reinterpret_cast<const float4*>(p)) : *reinterpret_cast<const float4*>(p);
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (nv > 0) v.x = NC ? __ldg(p) : p[0];
+  if (nv > 1) v.y = NC ? __ldg(p + 1) : p[1];
+  if (nv > 2) v.z = NC ? __ldg(p + 2) : p[2];
+  if (nv > 3) v.w = NC ? __ldg(p + 3) : p[3];
+  return v;
+}
+__device__ __forceinline__ void seg_store(float* p, const float4& v, bool vec, int nv) {
+  if (vec) { *reinterpret_cast<float4*>(p) = v; return; }
+  if (nv > 0) p[0] = v.x;
+  if (nv > 1) p[1] = v.y;
+  if (nv > 2) p[2] = v.z;
+  if (nv > 3) p[3] = v.w;
+}
+__device__ __forceinline__ void seg_red_add(float* p, const float4& v, bool vec, int nv) {
+  if (vec) { b2_red_add_v4(p, v); return; }
+  if (nv > 0) b2_red_add(p, v.x);
+  if (nv > 1) b2_red_add(p + 1, v.y);
+  if (nv > 2) b2_red_add(p + 2, v.z);
+  if (nv > 3) b2_red_add(p + 3, v.w);
+}
+__device__ __forceinline__ void seg_store_bf16(__nv_bfloat16* p, const float4& v, bool vec, int nv) {
+  const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+  if (vec) {
+    *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
+    return;
   }
-  if (p.c_pre != nullptr) p.c_pre[o] = t;
-  if (p.mul != nullptr) t *= __ldg(p.mul + o);
-  if (p.add != nullptr) t += __ldg(p.add + o);
+  if (nv > 0) p[0] = lo.x;
+  if (nv > 1) p[1] = lo.y;
+  if (nv > 2) p[2] = hi.x;
+  if (nv > 3) p[3] = hi.y;
+}
+
+// The fused epilogue of one element after c_pre: t = accumulator + bias; mv, av, yv, cv are its mul, add, ybwd and
+// (beta) C.  Every operation is rounded on its own (no contraction into fma).
+__device__ __forceinline__ float epilogue_elem(const Params& p, float t, float mv, float av, float yv, float cv) {
+  if (p.mul != nullptr) t = __fmul_rn(t, mv);
+  if (p.add != nullptr) t = __fadd_rn(t, av);
   if (p.act == B2_ACT_RELU) t = fmaxf(t, 0.f);
   else if (p.act == B2_ACT_SIGMOID) t = 1.f / (1.f + expf(-t));
   if (p.ybwd != nullptr) {     // activation backward of the PRODUCER of this gradient, fused
-    const float yv = __ldg(p.ybwd + o);
     if (p.act_bwd == B2_ACT_RELU) t = (yv > 0.f) ? t : 0.f;
-    else if (p.act_bwd == B2_ACT_SIGMOID) t = t * ((1.f - yv) * yv);
+    else if (p.act_bwd == B2_ACT_SIGMOID) t = __fmul_rn(t, __fmul_rn(__fsub_rn(1.f, yv), yv));
   }
-  if (p.beta) t += p.c[o];
-  p.c[o] = t;
-  if (p.c_small != nullptr) {
-    const int64_t oa = (int64_t) m * p.ld_aux + n;
-    if (p.esz == 4) p.c_small[oa] = tf32_small(t);   // the consumer's 3xTF32 small part, produced where C is
-    else reinterpret_cast<__nv_bfloat16*>(p.c_small)[oa] = __float2bfloat16_rn(t);   // bf16 mode operand
-  }
+  if (p.beta) t = __fadd_rn(t, cv);
   return t;
 }
+
+// The two consumer warpgroups (threads 128-383) meet; barrier 0 is __syncthreads.
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 template <int BN, int MODE>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -514,27 +561,94 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
       }
       wgmma_wait0();
     }
+    // ---------------- epilogue ----------------
+    // Once both warpgroups are past the mainloop the ring is dead (warpgroup 0 finished with it before the last
+    // k-block was consumed): the accumulators go through a row-major tile in it.
     // wgmma fragment: d[4j + 2h + e] is row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e of the warpgroup
-    const int row0 = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2);
+    constexpr int P = epi_pitch(BN);
+    float* tile = reinterpret_cast<float*>(smem);
+    consumer_sync();
+    {
+      float* row = tile + (g * 64 + (warp & 3) * 16 + (lane >> 2)) * P + 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
+      for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = n0 + 8 * j + 2 * (lane & 3) + e;
-        const bool n_ok = n < p.N;
-        const float bv = (n_ok && p.bias != nullptr && z == 0) ? __ldg(p.bias + n) : 0.f;
-        float cs = 0.f;
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(row + 8 * h * P + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
+    consumer_sync();
+    // Each thread walks segments of 4 columns x 1 row, in batches: every global load of a batch is issued before its
+    // first store, so a thread waits for one round trip to L2 per batch rather than one per element.  A warp covers
+    // 512 contiguous bytes of output rows.  Whole, aligned segments take 16-byte accesses; the others (the N tail, or
+    // a launch with a misaligned pointer or leading dimension) element by element in the same loop.
+    constexpr int SPR = BN / 4;                        // segments per row; divides 256
+    constexpr int SEG = BM * SPR / 256;                // segments per thread: 4, 8, 16
+    constexpr int BATCH = 4;                           // sized to the 168-register launch bound (worst case 16 / segment)
+    const int et = threadIdx.x - 128;
+    const int c4 = et % SPR, r0 = et / SPR;            // a thread keeps its columns in every segment
+    const int n = n0 + 4 * c4;
+    const int nv = min(4, p.N - n);                    // columns of the segment inside N (<= 0: none)
+    const bool vec_n = p.vec && nv == 4;
+    const float4 bv = (p.bias != nullptr && z == 0 && nv > 0) ? seg_load<true>(p.bias + n, vec_n, nv)
+                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
+    float cs[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+    for (int b0 = 0; b0 < SEG; b0 += BATCH) {
+      float4 mv[BATCH], av[BATCH], yv[BATCH], cv[BATCH];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int m = row0 + 8 * h;
-          if (n_ok && m < p.M) cs += epilogue_elem(p, m, n, acc[4 * j + 2 * h + e] + bv);
+      for (int i = 0; i < BATCH; ++i) {                // loads
+        const int m = m0 + r0 + (256 / SPR) * (b0 + i);
+        const int k = m < p.M ? nv : 0;
+        const bool v = vec_n && m < p.M;
+        const int64_t o = (int64_t) m * p.ldc + n;
+        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+        mv[i] = p.mul != nullptr ? seg_load<true>(p.mul + o, v, k) : zero;
+        av[i] = p.add != nullptr ? seg_load<true>(p.add + o, v, k) : zero;
+        yv[i] = p.ybwd != nullptr ? seg_load<true>(p.ybwd + o, v, k) : zero;
+        cv[i] = (p.beta && p.splits == 1) ? seg_load<false>(p.c + o, v, k) : zero;   // split-K adds with red.add
+      }
+#pragma unroll
+      for (int i = 0; i < BATCH; ++i) {                // arithmetic and stores
+        const int r = r0 + (256 / SPR) * (b0 + i);
+        const int m = m0 + r;
+        const int k = m < p.M ? nv : 0;
+        const bool v = vec_n && m < p.M;
+        const int64_t o = (int64_t) m * p.ldc + n;
+        const float4 a = *reinterpret_cast<const float4*>(tile + r * P + 4 * c4);
+        float4 t = make_float4(__fadd_rn(a.x, bv.x), __fadd_rn(a.y, bv.y), __fadd_rn(a.z, bv.z), __fadd_rn(a.w, bv.w));
+        if (p.splits > 1) {        // split-K: partial sums of a plain linear output (C was zeroed by the host)
+          seg_red_add(p.c + o, t, v, k);
+          continue;
         }
-        if (p.colsum != nullptr) {    // bias gradient: the 8 lanes of one column, then one red.add per warp
-          cs += __shfl_xor_sync(0xffffffffu, cs, 4);
-          cs += __shfl_xor_sync(0xffffffffu, cs, 8);
-          cs += __shfl_xor_sync(0xffffffffu, cs, 16);
-          if (lane < 4 && n_ok) b2_red_add(p.colsum + n, cs);
+        if (p.c_pre != nullptr) seg_store(p.c_pre + o, t, v, k);
+        t.x = epilogue_elem(p, t.x, mv[i].x, av[i].x, yv[i].x, cv[i].x);
+        t.y = epilogue_elem(p, t.y, mv[i].y, av[i].y, yv[i].y, cv[i].y);
+        t.z = epilogue_elem(p, t.z, mv[i].z, av[i].z, yv[i].z, cv[i].z);
+        t.w = epilogue_elem(p, t.w, mv[i].w, av[i].w, yv[i].w, cv[i].w);
+        seg_store(p.c + o, t, v, k);
+        if (p.c_small != nullptr) {
+          const int64_t oa = (int64_t) m * p.ld_aux + n;
+          if (p.esz == 4)          // the consumer's 3xTF32 small part, produced where C is
+            seg_store(p.c_small + oa, make_float4(tf32_small(t.x), tf32_small(t.y), tf32_small(t.z), tf32_small(t.w)), v, k);
+          else                     // bf16 mode operand
+            seg_store_bf16(reinterpret_cast<__nv_bfloat16*>(p.c_small) + oa, t, v, k);
         }
+        if (k > 0) cs[0] += t.x;
+        if (k > 1) cs[1] += t.y;
+        if (k > 2) cs[2] += t.z;
+        if (k > 3) cs[3] += t.w;
+      }
+    }
+    if (p.colsum != nullptr) {
+      // bias gradient: the threads' partial sums meet in shared memory past the tile; one red.add per column and CTA
+      float* part = tile + BM * P;
+      *reinterpret_cast<float4*>(part + 4 * et) = make_float4(cs[0], cs[1], cs[2], cs[3]);
+      consumer_sync();
+      if (et < BN && n0 + et < p.N) {
+        float s = 0.f;
+#pragma unroll
+        for (int u = et >> 2; u < 256; u += SPR) s += part[4 * u + (et & 3)];
+        b2_red_add(p.colsum + n0 + et, s);
       }
     }
   }
@@ -896,6 +1010,12 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   p.M = (int) M; p.N = (int) N; p.K = (int) K; p.act = d->act; p.act_bwd = d->act_bwd; p.esz = esz;
   p.a_mn = d->a_mn_major ? 1 : 0; p.b_mn = d->b_mn_major ? 1 : 0;
   p.beta = d->beta_accumulate ? 1 : 0;
+  {
+    auto al = [](const void* q, uintptr_t b) { return reinterpret_cast<uintptr_t>(q) % b == 0; };
+    p.vec = al(c, 16) && ldc % 4 == 0 && al(d->c_pre, 16) && al(d->bias, 16) && al(d->mul, 16) &&
+            al(d->add, 16) && al(d->ybwd, 16) && al(d->c_small, esz == 4 ? 16 : 8) &&
+            (d->c_small == nullptr || ld_aux % 4 == 0);
+  }
   p.kb_per_split = (int) b2_ceil_div(num_kb, best_split);
   const int splits = (int) b2_ceil_div(num_kb, p.kb_per_split);
   const int64_t tiles_n = b2_ceil_div(N, best_bn);
