@@ -16,7 +16,7 @@ B2_F32, B2_BF16, B2_F64, B2_I64, B2_I32 = 0, 1, 2, 3, 4
 B2_POOL_NONE, B2_POOL_SUM, B2_POOL_MEAN = 0, 1, 2
 B2_ACT_NONE, B2_ACT_RELU, B2_ACT_SIGMOID = 0, 1, 2
 B2_PREP_MUL = 3
-B2_GEMM_C_IS_ZERO, B2_GEMM_COLSUM_IS_ZERO, B2_GEMM_X3_INLINE = 1, 2, 4
+B2_GEMM_C_IS_ZERO, B2_GEMM_COLSUM_IS_ZERO, B2_GEMM_X3_INLINE, B2_GEMM_BACKFILL = 1, 2, 4, 8
 B2_MAX_FIELDS = 128
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 

@@ -73,6 +73,12 @@ class ParamArena(object):
         self.tail_params = uniq[n_first:]      # the dense (non-`first`) parameters, contiguous from tail_offset
         self.step_id = 0
         self.grads_are_zero = True
+        # Weight gradients still being written on a side stream (functional._WgradFork): (event, operands kept
+        # alive) pairs.  A backward leaves them here, instead of joining them itself, only while defer_join is set:
+        # fused_train_step sets it around the backward of its fused-logit path (no regulariser: the MLP chain is the
+        # one reader of its weights), and FusedAdam joins where it first reads the dense tail.
+        self.defer_join = False
+        self.pending = []
         # Touched-granule flags of the table prefix G[:tail_offset] (b2_touch): one byte per 16 floats.  The
         # backward kernels set the byte of every granule they add a table gradient into; FusedAdam's clip
         # and Adam passes read G only there and clear the bytes again.  Invariant: every nonzero float of
@@ -99,10 +105,18 @@ class ParamArena(object):
             end = min(slot.offset + slot.numel, self.tail_offset)
             self.touched[slot.offset // 16:(end + 15) // 16].fill_(1)
 
+    def join_grads(self):
+        """The current stream waits until every pending side-stream gradient is written."""
+        cur = torch.cuda.current_stream() if self.pending else None
+        for ev, _ in self.pending:
+            cur.wait_event(ev)
+        self.pending = []
+
     def begin_step(self, grads_zeroed):
         """Call once per training step before backward. `grads_zeroed`: G is already all-zero
         (e.g. the previous fused Adam step cleared it); otherwise sparse-written grads
         (embedding tables) are zero-filled lazily by the kernels' wrappers."""
+        self.join_grads()
         self.step_id += 1
         self.grads_are_zero = bool(grads_zeroed)
         for p in self.params:
@@ -293,6 +307,8 @@ class FusedAdam(object):
         # Gradients produced by stock autograd ops (parameters our kernels do not own, e.g. Dice's
         # alpha or a Conv1d weight reached through a view) live in p.grad, not in the arena: bring
         # them in.  Kernel-written gradients already alias their arena slot and are skipped.
+        if self.grad_allreduce or self.sharded:
+            a.join_grads()
         g_base = a.G.data_ptr()
         for p in a.params:
             g = p.grad
@@ -356,16 +372,27 @@ class FusedAdam(object):
                 _lib.call("b2_lazy_sumsq", ctypes.c_void_p(lz.tables_dev.data_ptr()), len(lz.tables),
                           ctypes.c_void_p(lz.worklist.data_ptr()), ctypes.c_void_p(lz.counter.data_ptr()),
                           lz.capacity, dg, ctypes.c_void_p(self.sumsq.data_ptr()), st)
+                a.join_grads()
                 if a.numel > a.tail_offset:
                     _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr() + 4 * a.tail_offset),
                               a.numel - a.tail_offset, ctypes.c_void_p(self.sumsq.data_ptr()), st)
+            elif flags is not None and a.pending:
+                # the table prefix depends only on the front's backward: summed while the MLP's weight-gradient
+                # GEMMs still run on their side stream, the dense tail after the join
+                _lib.call("b2_sumsq_ex", ctypes.c_void_p(a.G.data_ptr()), a.tail_offset,
+                          ctypes.c_void_p(self.sumsq.data_ptr()), ctypes.c_void_p(flags.data_ptr()), a.tail_offset, st)
+                a.join_grads()
+                _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr() + 4 * a.tail_offset), a.numel - a.tail_offset,
+                          ctypes.c_void_p(self.sumsq.data_ptr()), st)
             elif flags is not None:
                 _lib.call("b2_sumsq_ex", ctypes.c_void_p(a.G.data_ptr()), a.numel,
                           ctypes.c_void_p(self.sumsq.data_ptr()), ctypes.c_void_p(flags.data_ptr()), a.tail_offset, st)
             else:
+                a.join_grads()
                 _lib.call("b2_sumsq", ctypes.c_void_p(a.G.data_ptr()), a.numel,
                           ctypes.c_void_p(self.sumsq.data_ptr()), st)
             sumsq_ptr = ctypes.c_void_p(self.sumsq.data_ptr())
+        a.join_grads()
         vp = ctypes.c_void_p
         lo = 0
         if flags is not None:

@@ -63,6 +63,8 @@ def _grad_buffer(param, zero, marks=False):
             return view
         # the buffer below reaches the arena through AccumulateGrad's in-place add or the step's p.grad copy
         arena.mark_slot(slot)
+        # ... and that add or copy reads the first gradient, which a deferred side stream may still be writing
+        arena.join_grads()
     return torch.zeros_like(param) if zero else torch.empty_like(param)
 
 
@@ -441,11 +443,12 @@ def transpose_f32(t, want_small):
 
 def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=None, act=B2_ACT_NONE,
             mul=None, add=None, ybwd=None, act_bwd=B2_ACT_NONE, out_small=None, colsum=None, accumulate=False,
-            out_pre=None, out_is_zero=False):
+            out_pre=None, out_is_zero=False, backfill=False):
     """out (M,N) = epi(sum_k A(m,k) B(n,k)) on the wgmma kernel (b2_gemm_tc_ex).  a is (M,K), or (K,M) when
     a_mn (MN-major: the tensor is consumed as it lies, no transpose); b is (N,K), or (K,N) when b_mn.
     a_small / b_small: the operands' 3xTF32 small parts (both or neither).  Epilogue extras: ybwd/act_bwd
-    (activation backward of the gradient's producer), out_small (3xTF32 small part of out), colsum (N)."""
+    (activation backward of the gradient's producer), out_small (3xTF32 small part of out), colsum (N).
+    backfill: the launch runs beside a chain of launches on another stream (B2_GEMM_BACKFILL: short split-K CTAs)."""
     d = _lib.b2_gemm_desc()
     K, M = (a.shape if a_mn else a.shape[::-1])
     K2, N = (b.shape if b_mn else b.shape[::-1])
@@ -483,7 +486,8 @@ def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=
     d.a_mn_major, d.b_mn_major = int(bool(a_mn)), int(bool(b_mn))
     d.act, d.act_bwd = act, (act_bwd if ybwd is not None else B2_ACT_NONE)
     d.beta_accumulate = 1 if accumulate else 0
-    d.flags = (_lib.B2_GEMM_C_IS_ZERO if out_is_zero else 0) | (_lib.B2_GEMM_COLSUM_IS_ZERO if _is_zeroed(colsum) else 0)
+    d.flags = (_lib.B2_GEMM_C_IS_ZERO if out_is_zero else 0) | (_lib.B2_GEMM_COLSUM_IS_ZERO if _is_zeroed(colsum) else 0) \
+        | (_lib.B2_GEMM_BACKFILL if backfill else 0)
     if a_small is None and not bf16 and _MATMUL["mode"] == "tf32x3" and _MATMUL["x3_inline"]:
         d.flags |= _lib.B2_GEMM_X3_INLINE
     _lib.call("b2_gemm_tc_ex", ctypes.byref(d), _stream())
@@ -689,6 +693,64 @@ class _LinearAct(torch.autograd.Function):
         return gx, gw, gb, None
 
 
+_FORK = {"on": True, "side": {}}     # the weight-gradient side stream of each device
+
+
+def set_backward_fork(on):
+    """on (default): an MLP chain's backward runs its weight-gradient GEMMs on a side stream (see _WgradFork);
+    off: every launch on the current stream, one after another (the reference order the fork is tested against)."""
+    _FORK["on"] = bool(on)
+
+
+class _WgradFork(object):
+    """The weight-gradient GEMMs of a chain backward on a side stream.  The data-gradient chain (head backward,
+    then each dgrad) stays on the current stream; a wgrad waits only for the launch that produced its dZ, so it
+    fills the SMs a dgrad's last wave leaves idle.  Launched as backfill (B2_GEMM_BACKFILL): split over K into
+    short CTAs, so that none holds an SM for long when the next dgrad wants it.  (A launch priority does not
+    help: the wgrads already run at the lowest, and raising the dgrads above them made the backward slower.)
+
+    Everything is an event record / wait, so the fork and the join are captured into a CUDA graph as edges.
+    The operands the side stream reads stay referenced until the join, after which the current stream can
+    reuse their memory.  The join: the current stream waits for the side stream at the end of the backward,
+    unless every weight gradient lives in a ParamArena whose fused optimizer defers it (ParamArena.defer_join):
+    then the optimizer joins where it first reads the dense gradients."""
+
+    def __init__(self, dev):
+        side = _FORK["side"].get(dev)
+        if side is None:
+            side = _FORK["side"][dev] = torch.cuda.Stream(device=dev)
+        self.main, self.side = torch.cuda.current_stream(dev), side
+        self.keep, self.arenas = [], set()
+        self.defer = True
+
+    def ready(self):
+        """Record, on the current stream, that dZ (and its auxiliary operand) are written: before the dgrad launch."""
+        ev = torch.cuda.Event()
+        ev.record(self.main)
+        return ev
+
+    def gemm(self, ready, gz, gz_small, h, h_small, gw):
+        self.side.wait_event(ready)
+        with torch.cuda.stream(self.side):
+            gemm_ex(gz, h, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=h_small,
+                    out_is_zero=_is_zeroed(gw), backfill=True)                                       # dW = dZ^T X
+        self.keep += [gz, gz_small, h, h_small]
+        base = gw._base
+        arena = getattr(base, "_b2_arena", None) if base is not None else None
+        if arena is None or not arena.defer_join:
+            self.defer = False
+        else:
+            self.arenas.add(arena)
+
+    def join(self):
+        done = torch.cuda.Event()
+        done.record(self.side)
+        if self.defer and len(self.arenas) == 1:
+            self.arenas.pop().pending.append((done, self.keep))
+        else:
+            self.main.wait_event(done)
+
+
 class _MLPChain(torch.autograd.Function):
     """A whole Linear(+ReLU/Sigmoid) chain of MLP_Block (mlp_block.py:64-85) as ONE autograd node, so that
     work can move across layer boundaries: the forward epilogue of layer i writes the 3xTF32 small part
@@ -752,6 +814,7 @@ class _MLPChain(torch.autograd.Function):
             return _grad_buffer(b, zero=False) if (b is not None and b.requires_grad) else None
 
         g, g_small, g_is_dz = _f32c(gy), None, False     # g: gradient w.r.t. y_i; g_is_dz: already dZ_i (+ db_i done)
+        fork = None                                      # _WgradFork: the wgrads run beside the dgrad chain
         for i in range(L - 1, -1, -1):
             W, act, h, y = Ws[i], acts[i], hs[i], hs[i + 1]
             N, K = W.shape
@@ -792,6 +855,9 @@ class _MLPChain(torch.autograd.Function):
             else:
                 gz, gz_small = g, g_small
             if kinds[i] == "tc":
+                if fork is None and W.requires_grad and _FORK["on"] and gz.is_cuda:
+                    fork = _WgradFork(dev)
+                ready = fork.ready() if (fork is not None and W.requires_grad) else None
                 if gx is not None:
                     prev_act = acts[i - 1] if fuse_prev else B2_ACT_NONE
                     gb_prev = bias_buf(i - 1) if fuse_prev else None
@@ -800,8 +866,11 @@ class _MLPChain(torch.autograd.Function):
                             out_small=gx_small, colsum=gb_prev)                                   # dX (= dZ_{i-1})
                 if W.requires_grad:
                     gw = _grad_buffer(W, zero=False)
-                    gemm_ex(gz, h, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=smalls[i],
-                            out_is_zero=_is_zeroed(gw))                                              # dW = dZ^T X
+                    if ready is not None:
+                        fork.gemm(ready, gz, gz_small, h, smalls[i], gw)
+                    else:
+                        gemm_ex(gz, h, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=smalls[i],
+                                out_is_zero=_is_zeroed(gw))                                          # dW = dZ^T X
                     grads[2 * i] = gw
                 g, g_small, g_is_dz = gx, gx_small, fuse_prev
             else:               # fp32 SIMT layer inside a chain (odd shapes)
@@ -815,6 +884,8 @@ class _MLPChain(torch.autograd.Function):
                 continue
             if fuse_prev:
                 grads[2 * (i - 1) + 1] = gb_prev
+        if fork is not None:
+            fork.join()
         return (g if ctx.needs_input_grad[0] else None, None) + tuple(grads)
 
 

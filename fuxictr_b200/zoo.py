@@ -283,15 +283,24 @@ class RankModel(nn.Module):
         opt = self._fused_optimizer
         opt.zero_grad()
         y_true = self.get_labels(batch_data)
-        if hasattr(self, "forward_logits") and not (self._embedding_regularizer or self._net_regularizer):
+        fused_logit = hasattr(self, "forward_logits") and not (self._embedding_regularizer or self._net_regularizer)
+        if fused_logit:
             loss, _ = F2.logit_bce(y_true, *self.forward_logits(batch_data))
         else:
             loss = self.compute_loss(self.forward(batch_data), y_true)
         seed = getattr(self, "_loss_grad", None)      # 1/world for row-sharded runs (see enable_sharding)
-        if seed is not None:
-            loss.backward(seed)
-        else:
-            loss.backward()
+        # opt.step() joins the MLP's weight-gradient side stream where it first reads the dense gradients.  Only on
+        # the fused-logit path, where the MLP chain is the one reader of its weights: a regulariser gives every weight
+        # a second gradient, which autograd adds to the chain's on this stream, so that backward must join itself.  A
+        # sharded step sums the dense gradients over the ranks from inside the backward, so it joins there too.
+        opt.arena.defer_join = fused_logit and not opt.sharded
+        try:
+            if seed is not None:
+                loss.backward(seed)
+            else:
+                loss.backward()
+        finally:
+            opt.arena.defer_join = False
         opt.step()
         return loss
 

@@ -484,6 +484,8 @@ typedef struct b2_gemm_desc {
 #define B2_GEMM_C_IS_ZERO 1      /* split-K accumulates into C with red.global: C needs no clearing */
 #define B2_GEMM_COLSUM_IS_ZERO 2
 #define B2_GEMM_X3_INLINE 4      /* 3xTF32 from the fp32 operands alone: the small parts are made in shared memory */
+#define B2_GEMM_BACKFILL 8       /* runs beside a chain of launches on another stream (a wgrad next to the dgrads): a
+                                    linear epilogue is split over K into short CTAs (b2_gemm_plan.splits reports it) */
 B2_API int b2_gemm_tc_ex(const b2_gemm_desc* desc, void* stream);
 /* The launch plan b2_gemm_tc_ex would use for `desc` (pure host arithmetic: no device call, no stream): lets a
    host-only test check that every plan fits the SM (<= 227 KB of shared memory).  stages: k-blocks in flight in
