@@ -168,6 +168,11 @@ SIGNATURES = {
     "b2_sumsq_ex": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
     "b2_adam_step_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
                                 c_float, c_float, c_float, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
+    "b2_adam_untouched": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float, c_float, c_float,
+                                  c_void_p, c_int, c_void_p]),
+    "b2_adam_touched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float, c_float,
+                                c_float, c_float, c_void_p, c_void_p, c_void_p]),
+    "b2_table_mark": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p]),
     "b2_logloss_sum": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_auc_workspace_bytes": (c_int, [c_int64, ctypes.POINTER(c_int64)]),
     "b2_auc": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),

@@ -84,6 +84,10 @@ class ParamArena(object):
         # and Adam passes read G only there and clear the bytes again.  Invariant: every nonzero float of
         # G[:tail_offset] lies in a flagged granule.  None: no table prefix, or lazy tables (own worklist).
         self.touched, self.touch = None, None
+        # Set while FusedAdam's untouched-granule pass may run (between start_early_tables and the step): a
+        # granule flagged now may already have had its g = 0 update, so only the front kernels, whose every
+        # granule was flagged from the ids before that pass, may still write table gradients.
+        self.flags_frozen = False
         if self.tail_offset > 0:
             self.touched = torch.zeros((self.tail_offset + self.GRANULE - 1) // self.GRANULE, dtype=torch.uint8,
                                        device=dev)
@@ -102,6 +106,9 @@ class ParamArena(object):
     def mark_slot(self, slot):
         """Flag every granule of `slot` (its gradient is written by something that sets no flags)."""
         if self.touched is not None and slot.offset < self.tail_offset:
+            if self.flags_frozen:
+                raise RuntimeError("a table gradient is written outside the fused front while the untouched table "
+                                   "rows are being updated early; call fuxictr_b200.arena.set_early_table_adam(False)")
             end = min(slot.offset + slot.numel, self.tail_offset)
             self.touched[slot.offset // 16:(end + 15) // 16].fill_(1)
 
@@ -206,6 +213,16 @@ class LazyTables(object):
                   opt.betas[0], opt.betas[1], opt.eps, st)
 
 
+_EARLY = {"on": True, "side": {}}     # the untouched-table-granule side stream of each device
+
+
+def set_early_table_adam(on):
+    """on (default): where FusedAdam.early_tables_ok() holds, a step updates the table granules its batch does not
+    touch on a side stream while its forward and backward run (FusedAdam.start_early_tables); off: the whole
+    table pass after the norm, one launch (the serial order the split is tested against)."""
+    _EARLY["on"] = bool(on)
+
+
 class FusedAdam(object):
     """clip_grad_norm_(max_norm) + Adam over a ParamArena, two kernels per step.
 
@@ -233,6 +250,44 @@ class FusedAdam(object):
         self._side = None            # overlap: side stream + its own communicator for the dense-gradient all-reduce
         self._side_group = None
         self._early_pending = False
+        self._early = None           # (done event, operands kept alive) of this step's untouched-granule pass
+
+    # CTAs (= SMs, one 1024-thread CTA each) of the untouched-granule pass; tools/table_adam_overlap_times.py
+    EARLY_CTAS = 32
+
+    def early_tables_ok(self):
+        """The step's table flags are final once its ids are known: one process, flags cleared by every step,
+        dense (not lazy) tables.  The caller adds what only the model knows: every table gradient comes from the
+        front kernels marked by start_early_tables."""
+        a = self.arena
+        return (_EARLY["on"] and not self.sharded and not self.grad_allreduce and self.zero_grad_in_step
+                and self.lazy is None and a.touched is not None)
+
+    def start_early_tables(self, plan, lr_plan, idx_list, emb_tables, lr_tables):
+        """Fork: on a side stream, flag every table granule this step's front reads (b2_table_mark over the
+        parameter arena, from the ids alone), then give every other table granule its g = 0 update of the coming
+        step (b2_adam_untouched).  step_phases joins before it counts the step and then updates only the flagged
+        granules (b2_adam_touched).  Hazards: the front reads P only in flagged granules and the side pass writes
+        only unflagged ones; the previous step's touched pass cleared every flag before this fork; flags are
+        cleared only after the join; until the join nothing but the front kernels may write a table gradient
+        (ParamArena.flags_frozen)."""
+        a = self.arena
+        dev = a.P.device
+        side = _EARLY["side"].get(dev)
+        if side is None:
+            side = _EARLY["side"][dev] = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        vp = ctypes.c_void_p
+        touch = _lib.b2_touch(a.touched.data_ptr(), a.P.data_ptr(), a.tail_offset)
+        with torch.cuda.stream(side):
+            keep = F2.table_mark(plan, lr_plan, idx_list, emb_tables, lr_tables, touch)
+            _lib.call("b2_adam_untouched", vp(a.P.data_ptr()), vp(self.M.data_ptr()), vp(self.V.data_ptr()),
+                      a.tail_offset, vp(a.touched.data_ptr()), self.lr, self.betas[0], self.betas[1], self.eps,
+                      vp(self.step_dev.data_ptr()), self.EARLY_CTAS, vp(side.cuda_stream))
+            done = torch.cuda.Event()
+            done.record(side)
+        self._early = (done, keep)
+        a.flags_frozen = True
 
     def enable_lazy(self, tables):
         """Evaluate the dense Adam semantics of `tables` (the arena's leading parameters) lazily."""
@@ -303,6 +358,10 @@ class FusedAdam(object):
         if not torch.cuda.is_current_stream_capturing():
             self.count_step()
         F2.bump_weight_epoch()        # parameters change through raw pointers: cached 3xTF32 weight splits are stale
+        early = self._early
+        if early is not None:         # the untouched-granule pass reads step_dev as the step before this one
+            torch.cuda.current_stream().wait_event(early[0])
+            self._early = None
         self.step_dev.add_(1)
         # Gradients produced by stock autograd ops (parameters our kernels do not own, e.g. Dice's
         # alpha or a Conv1d weight reached through a view) live in p.grad, not in the arena: bring
@@ -315,6 +374,7 @@ class FusedAdam(object):
             if g is not None and g.data_ptr() != g_base + p._b2_slot.offset * 4:
                 a.grad_view(p._b2_slot).copy_(g)
                 a.mark_slot(p._b2_slot)
+        a.flags_frozen = False
         if self.grad_allreduce:
             import torch.distributed as dist
             dist.all_reduce(a.G, op=dist.ReduceOp.SUM)   # one NCCL collective over the whole arena
@@ -395,7 +455,13 @@ class FusedAdam(object):
         a.join_grads()
         vp = ctypes.c_void_p
         lo = 0
-        if flags is not None:
+        if flags is not None and early is not None:
+            # tables: the unflagged granules were updated by the side pass; the flagged ones now
+            _lib.call("b2_adam_touched", vp(a.P.data_ptr()), vp(a.G.data_ptr()), vp(self.M.data_ptr()),
+                      vp(self.V.data_ptr()), a.tail_offset, sumsq_ptr, float(self.max_norm or 0.0), self.lr,
+                      self.betas[0], self.betas[1], self.eps, vp(self.step_dev.data_ptr()), vp(flags.data_ptr()), st)
+            lo = a.tail_offset
+        elif flags is not None:
             # tables: G loaded (and zeroed, and its flag cleared) only in the granules a backward wrote
             _lib.call("b2_adam_step_ex", vp(a.P.data_ptr()), vp(a.G.data_ptr()), vp(self.M.data_ptr()),
                       vp(self.V.data_ptr()), a.tail_offset, sumsq_ptr, float(self.max_norm or 0.0), self.lr,

@@ -416,11 +416,33 @@ __global__ void adam_sched_kernel(const int64_t* __restrict__ step_dev, float lr
   sched[t] = make_float2((float) ((double) lr / bc1), (float) (1.0 / sqrt(bc2)));
 }
 
+// The two per-step scalars of step t (1-based): lr / (1 - beta1^t) and 1 / sqrt(1 - beta2^t).  Every dense pass
+// computes them here, so a step split over several launches applies the same two floats everywhere.
+__device__ __forceinline__ void adam_step_scalars(int64_t t, float lr, float beta1, float beta2, float& step_size,
+                                                  float& ibc2) {
+  const double bc1 = 1.0 - pow((double) beta1, (double) t);
+  const double bc2 = 1.0 - pow((double) beta2, (double) t);
+  step_size = (float) ((double) lr / bc1);
+  ibc2 = (float) (1.0 / sqrt(bc2));
+}
+
+__device__ __forceinline__ B2AdamConst adam_const(float beta1, float beta2, float eps) {
+  B2AdamConst c;
+  c.w1 = (float) (1.0 - (double) beta1);
+  c.b2 = beta2;
+  c.w2 = (float) (1.0 - (double) beta2);
+  c.eps = eps;
+  return c;
+}
+
+// touched_only: visit only the flagged granules of the first nf4 float4s (the unflagged ones were updated by
+// adam_untouched_kernel earlier in the step); with touched_only = 0 the unflagged granules get g = 0 here.
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
             float* __restrict__ v, int64_t n, const float* __restrict__ sumsq, float max_norm,
             float lr, float beta1, float beta2, float eps, const int64_t* __restrict__ step_dev,
-            int zero_grad, const B2AdamSched* __restrict__ sched, uint8_t* __restrict__ flags, int64_t nf4) {
+            int zero_grad, const B2AdamSched* __restrict__ sched, uint8_t* __restrict__ flags, int64_t nf4,
+            int touched_only) {
   b2_pdl_wait();
   b2_pdl_trigger();
   __shared__ B2AdamConst sc;
@@ -433,19 +455,13 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
       clip = fminf(max_norm / (total_norm + 1e-6f), 1.f);
     }
     s_clip = clip;
-    sc.w1 = (float) (1.0 - (double) beta1);
-    sc.b2 = beta2;
-    sc.w2 = (float) (1.0 - (double) beta2);
-    sc.eps = eps;
+    sc = adam_const(beta1, beta2, eps);
     if (sched != nullptr) {
       const B2AdamSched e = sched[t];
       s_step = e.x;
       s_ibc2 = e.y;
     } else {
-      const double bc1 = 1.0 - pow((double) beta1, (double) t);
-      const double bc2 = 1.0 - pow((double) beta2, (double) t);
-      s_step = (float) ((double) lr / bc1);
-      s_ibc2 = (float) (1.0 / sqrt(bc2));
+      adam_step_scalars(t, lr, beta1, beta2, s_step, s_ibc2);
     }
   }
   __syncthreads();
@@ -465,7 +481,7 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
     const bool flagged = i < nf4;
     const bool live = !flagged || flags[i >> 2] != 0;   // false: the granule's gradient is known to be zero
     if (i0 < nf4) __syncwarp();
-    if (i >= n4) continue;
+    if (i >= n4 || (touched_only && !live)) continue;
     float4 pp = p4[i], mm = m4[i], vv = v4[i];
     const float4 gg = live ? g4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     b2_adam_apply(pp.x, __fmul_rn(gg.x, clip), mm.x, vv.x, c, step_size, ibc2);   // g.mul_(clip_coef) first
@@ -502,7 +518,7 @@ extern "C" B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, in
   const B2AdamSched* no_sched = nullptr;
   const int64_t nf4 = flags != nullptr ? n_flagged >> 2 : 0;
   B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2,
-            eps, step_dev, zero_grad, no_sched, flags, nf4);
+            eps, step_dev, zero_grad, no_sched, flags, nf4, 0);
   B2_CUDA_LAUNCH_CHECK("b2_adam_step");
   return B2_OK;
 }
@@ -513,6 +529,108 @@ extern "C" B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64
                             void* stream) {
   return b2_adam_step_ex(p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2, eps, step_dev, zero_grad, nullptr, 0,
                          stream);
+}
+
+// ---------------------------------------------------------------------------------
+// The dense table pass split in two (b2_adam_untouched + b2_adam_touched): the granules no sample of the
+// batch touches have g = 0, and g * clip = +0 for every finite clip in [0, 1] (fminf drops a NaN norm), so
+// their update depends on the step number only and can run while the forward and backward do.
+// ---------------------------------------------------------------------------------
+constexpr int UNTOUCHED_THREADS = 1024, UNTOUCHED_UNROLL = 2;
+
+__device__ __forceinline__ float4 ld_no_l1(const float4* p) {   // coherent: the same thread writes it back
+  float4 r;
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w)
+               : "l"(p));
+  return r;
+}
+__device__ __forceinline__ void st_evict_first(float4* p, const float4& v) {
+  asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+               : "memory");
+}
+
+// One 1024-thread CTA fills an SM's register file, so the grid is the number of SMs the pass occupies.
+// UNTOUCHED_UNROLL float4s of P, M and V per thread in flight (96 KB per SM).  Streaming hints keep the
+// 3 x 64 B per granule out of L1 and first in line for eviction from L2, where the GEMM operands live.
+__global__ void __launch_bounds__(UNTOUCHED_THREADS, 1)
+adam_untouched_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v, int64_t n4,
+                      const uint8_t* __restrict__ flags, float lr, float beta1, float beta2, float eps,
+                      const int64_t* __restrict__ step_dev) {
+  b2_pdl_wait();
+  __shared__ B2AdamConst sc;
+  __shared__ float s_step, s_ibc2;
+  if (threadIdx.x == 0) {
+    sc = adam_const(beta1, beta2, eps);
+    adam_step_scalars(*step_dev + 1, lr, beta1, beta2, s_step, s_ibc2);   // the step the optimizer is about to count
+  }
+  __syncthreads();
+  const B2AdamConst c = sc;
+  const float step_size = s_step, ibc2 = s_ibc2;
+  float4* p4 = reinterpret_cast<float4*>(p);
+  float4* m4 = reinterpret_cast<float4*>(m);
+  float4* v4 = reinterpret_cast<float4*>(v);
+  const int64_t stride = (int64_t) gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += UNTOUCHED_UNROLL * stride) {
+    bool on[UNTOUCHED_UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNTOUCHED_UNROLL; ++u) {
+      const int64_t j = i + u * stride;
+      on[u] = j < n4 && flags[j >> 2] == 0;
+    }
+    float4 pp[UNTOUCHED_UNROLL], mm[UNTOUCHED_UNROLL], vv[UNTOUCHED_UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNTOUCHED_UNROLL; ++u) {
+      if (!on[u]) continue;
+      const int64_t j = i + u * stride;
+      pp[u] = ld_no_l1(p4 + j); mm[u] = ld_no_l1(m4 + j); vv[u] = ld_no_l1(v4 + j);
+    }
+#pragma unroll
+    for (int u = 0; u < UNTOUCHED_UNROLL; ++u) {
+      if (!on[u]) continue;
+      const int64_t j = i + u * stride;
+      // adam_kernel's unflagged case: g = __fmul_rn(0, clip) = +0
+      b2_adam_apply(pp[u].x, 0.f, mm[u].x, vv[u].x, c, step_size, ibc2);
+      b2_adam_apply(pp[u].y, 0.f, mm[u].y, vv[u].y, c, step_size, ibc2);
+      b2_adam_apply(pp[u].z, 0.f, mm[u].z, vv[u].z, c, step_size, ibc2);
+      b2_adam_apply(pp[u].w, 0.f, mm[u].w, vv[u].w, c, step_size, ibc2);
+      st_evict_first(p4 + j, pp[u]); st_evict_first(m4 + j, mm[u]); st_evict_first(v4 + j, vv[u]);
+    }
+  }
+}
+
+extern "C" B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, float lr,
+                                        float beta1, float beta2, float eps, const int64_t* step_dev, int max_ctas,
+                                        void* stream) {
+  B2_REQUIRE(p && m && v && flags && step_dev, "NULL pointer");
+  B2_REQUIRE((((uintptr_t) p | (uintptr_t) m | (uintptr_t) v) % 16) == 0, "arenas must be 16-byte aligned");
+  B2_REQUIRE(n >= 0 && n % 4 == 0, "n=%lld must be a multiple of 4", (long long) n);
+  B2_REQUIRE(max_ctas >= 1, "max_ctas=%d must be >= 1", max_ctas);
+  if (n == 0) return B2_OK;
+  const int64_t n4 = n >> 2;
+  int64_t blocks = b2_ceil_div(n4, UNTOUCHED_THREADS * UNTOUCHED_UNROLL);
+  if (blocks > max_ctas) blocks = max_ctas;
+  B2_LAUNCH(adam_untouched_kernel, (int) blocks, UNTOUCHED_THREADS, 0, (cudaStream_t) stream, p, m, v, n4, flags, lr,
+            beta1, beta2, eps, step_dev);
+  B2_CUDA_LAUNCH_CHECK("b2_adam_untouched");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_adam_touched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
+                                      float max_norm, float lr, float beta1, float beta2, float eps,
+                                      const int64_t* step_dev, uint8_t* flags, void* stream) {
+  B2_REQUIRE(p && g && m && v && step_dev && flags, "NULL pointer");
+  B2_REQUIRE((((uintptr_t) p | (uintptr_t) g | (uintptr_t) m | (uintptr_t) v) % 16) == 0,
+             "arenas must be 16-byte aligned");
+  B2_REQUIRE(n >= 0 && n % 4 == 0, "n=%lld must be a multiple of 4", (long long) n);
+  if (n == 0) return B2_OK;
+  int64_t blocks = b2_ceil_div(n >> 2, 256 * 2);
+  if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
+  const B2AdamSched* no_sched = nullptr;
+  B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2,
+            eps, step_dev, 1, no_sched, flags, n >> 2, 1);
+  B2_CUDA_LAUNCH_CHECK("b2_adam_touched");
+  return B2_OK;
 }
 
 extern "C" B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
@@ -537,7 +655,7 @@ extern "C" B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v,
   if (blocks < 1) blocks = 1;
   const B2AdamSched* sched_tab = reinterpret_cast<const B2AdamSched*>(sched);
   B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, 0.f, beta1, beta2,
-            eps, step_dev, zero_grad, sched_tab, (uint8_t*) nullptr, (int64_t) 0);
+            eps, step_dev, zero_grad, sched_tab, (uint8_t*) nullptr, (int64_t) 0, 0);
   B2_CUDA_LAUNCH_CHECK("b2_adam_step_sched");
   return B2_OK;
 }

@@ -242,6 +242,40 @@ front_bwd_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant_
   }
 }
 
+// Flags every granule of [p, p + len) that lies in the touch range.
+__device__ __forceinline__ void touch_mark_span(const b2_touch& t, const float* p, int len) {
+  const int64_t o = ((intptr_t) p - (intptr_t) t.base) >> 2;
+  for (int64_t g = o >> 4; g <= (o + len - 1) >> 4; ++g)
+    if (g >= 0 && (g << 4) < t.n) t.flags[g] = 1;
+}
+
+// One thread per (sample, field): the rows a forward reads for it (in range, padding rows included) and so
+// every row its backward can write.  `table` fields are the parameter tables, `tch.base` the parameter arena.
+template <typename IdxT>
+__global__ void __launch_bounds__(256)
+table_mark_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr, int has_lr,
+                  int64_t batch, const b2_touch tch) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const SmemFields sf = b2_stage_fields(emb, smem_raw);
+  SmemFields lf;
+  lf.f = nullptr;
+  lf.slot_start = nullptr;
+  if (has_lr) lf = b2_stage_fields(lr, smem_raw + ((pack_smem_bytes(emb.nfields) + 15) & ~(size_t) 15));
+  b2_pdl_wait();
+  const int F = emb.nfields;
+  const int64_t nitems = batch * (int64_t) F;
+  for (int64_t it = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; it < nitems;
+       it += (int64_t) gridDim.x * blockDim.x) {
+    const int64_t b = it / F;
+    const int f = (int) (it - b * F);
+    const b2_field& fd = sf.f[f];
+    const int64_t row = b2_load_index<IdxT>(fd.idx, b * fd.idx_stride);
+    if (row < 0 || row >= fd.vocab) continue;      // the front's out-of-range rule: nothing read, nothing written
+    touch_mark_span(tch, reinterpret_cast<const float*>(fd.table) + row * fd.dim, fd.dim);
+    if (has_lr) touch_mark_span(tch, reinterpret_cast<const float*>(lf.f[f].table) + row, 1);
+  }
+}
+
 template <typename IdxT>
 int launch_front_fwd(const B2FieldPack& emb, const B2FieldPack& lr, const b2_lazy_ctx& lz, int lazy,
                      int64_t batch, int dim, int has_lr,
@@ -378,4 +412,41 @@ extern "C" B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field
     case B2_I32: return launch_front_bwd<int32_t>(epack, lpack, lz, lzf, batch, dim, has_lr, want_fm, emb_saved, gx, sums, glogit, gbias, tch, st);
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
+}
+
+extern "C" B2_API int b2_table_mark(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch,
+                                    int idx_dtype, const b2_touch* touch, void* stream) {
+  B2_REQUIRE(emb_fields != nullptr, "emb fields is NULL");
+  B2_REQUIRE(nfields >= 1 && nfields <= B2_MAX_FIELDS, "nfields=%d outside [1,%d]", nfields, B2_MAX_FIELDS);
+  B2_REQUIRE(touch != nullptr && touch->flags != nullptr && touch->n > 0, "touch: no flags to set");
+  b2_touch tch;
+  int rc = b2_touch_arg(touch, tch);
+  if (rc != B2_OK) return rc;
+  for (int i = 0; i < nfields; ++i) {
+    const b2_field& f = emb_fields[i];
+    B2_REQUIRE(f.table != nullptr && f.idx != nullptr, "field %d: NULL table or idx", i);
+    B2_REQUIRE(f.dim >= 1 && f.seq_len == 1, "field %d: marking needs dim >= 1 and no sequences", i);
+    if (lr_fields != nullptr) {
+      B2_REQUIRE(lr_fields[i].table != nullptr, "field %d: NULL LR table", i);
+      B2_REQUIRE(lr_fields[i].idx == f.idx && lr_fields[i].idx_stride == f.idx_stride,
+                 "field %d: LR and embedding must share indices", i);
+    }
+  }
+  B2_REQUIRE(batch >= 0, "negative batch");
+  if (batch == 0) return B2_OK;
+  static thread_local B2FieldPack epack, lpack;
+  fill_pack(epack, emb_fields, nfields);
+  const int has_lr = lr_fields != nullptr;
+  if (has_lr) fill_pack(lpack, lr_fields, nfields); else lpack.nfields = 0;
+  cudaStream_t st = (cudaStream_t) stream;
+  const size_t smem = ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + pack_smem_bytes(nfields) + 16;
+  const int grid = grid_for(batch * (int64_t) nfields, 256);
+  switch (idx_dtype) {
+    case B2_F64: B2_LAUNCH(table_mark_kernel<double>, grid, 256, smem, st, epack, lpack, has_lr, batch, tch); break;
+    case B2_I64: B2_LAUNCH(table_mark_kernel<int64_t>, grid, 256, smem, st, epack, lpack, has_lr, batch, tch); break;
+    case B2_I32: B2_LAUNCH(table_mark_kernel<int32_t>, grid, 256, smem, st, epack, lpack, has_lr, batch, tch); break;
+    default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
+  }
+  B2_CUDA_LAUNCH_CHECK("b2_table_mark");
+  return B2_OK;
 }

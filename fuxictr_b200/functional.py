@@ -1318,3 +1318,26 @@ def front(plan, lr_plan, idx_list, emb_tables, lr_tables, bias, want_fm, status=
     idx_list, _ = _prep_indices(list(idx_list), plan.fields)
     return _Front.apply(plan, lr_plan, idx_list, status, bool(want_fm), bias, len(emb_tables),
                         *(tuple(emb_tables) + tuple(lr_tables)))
+
+
+def table_mark(plan, lr_plan, idx_list, emb_tables, lr_tables, touch):
+    """b2_table_mark on the current stream: flag (b2_touch `touch`, over the parameter arena) every granule of
+    every table row the front (or gather) of `plan` reads for these ids.  Returns the index views the launch
+    reads, which must stay alive until it has run."""
+    _require_cuda(*idx_list)
+    idx_list, code = _prep_indices(list(idx_list), plan.fields)
+    batch = idx_list[0].shape[0]
+    descs = (b2_field * len(plan.fields))()
+    for d, f, idx in zip(descs, plan.fields, idx_list):
+        t = emb_tables[f.table_slot]
+        d.table, d.vocab, d.dim, d.seq_len = t.data_ptr(), t.shape[0], f.dim, 1
+        d.idx, d.idx_stride = idx.data_ptr(), (idx.stride(0) if batch > 0 else 0)
+    lr_descs = None
+    if lr_plan is not None:
+        lr_descs = (b2_field * len(lr_plan.fields))()
+        for d, f, idx in zip(lr_descs, lr_plan.fields, idx_list):
+            t = lr_tables[f.table_slot]
+            d.table, d.vocab, d.dim, d.seq_len = t.data_ptr(), t.shape[0], 1, 1
+            d.idx, d.idx_stride = idx.data_ptr(), (idx.stride(0) if batch > 0 else 0)
+    _lib.call("b2_table_mark", descs, lr_descs, len(plan.fields), batch, code, ctypes.byref(touch), _stream())
+    return idx_list

@@ -311,17 +311,16 @@ class FeatureEmbeddingDict(nn.Module):
         return self.dict2tensor(feature_emb_dict, flatten_emb=flatten_emb)
 
 
-def fused_front(embedding_layer, lr_layer, X, want_fm):
-    """One launch for FeatureEmbedding + (FM product_sum) + (LogisticRegression): returns
-    (feature_emb (B,F,D), logit (B,1)), or None when the configuration needs the general path
-    (sequence / numeric features, mixed dims, dim % 4 != 0)."""
+def front_plan(embedding_layer, lr_layer, X):
+    """(order, plan, tables, lr_plan, lr_tables) of the launch fused_front makes for inputs X, or None when the
+    configuration needs the general path (sequence / numeric features, mixed dims, dim % 4 != 0)."""
     fed = embedding_layer.embedding_layer
     names = fed._active_features(X, [], [])
     order = [f for f in fed._feature_map.features.keys() if f in set(names)]
     if not order or not all(fed._is_fusable(f) for f in order):
         return None
     plan, tables = fed._plan(order, order)
-    lr_plan = lr_tables = bias = None
+    lr_plan = lr_tables = None
     if lr_layer is not None:
         lfed = lr_layer.embedding_layer.embedding_layer
         lnames = lfed._active_features(X, [], [])
@@ -329,9 +328,19 @@ def fused_front(embedding_layer, lr_layer, X, want_fm):
         if lorder != order or not all(lfed._is_fusable(f) for f in lorder):
             return None
         lr_plan, lr_tables = lfed._plan(lorder, lorder)
-        bias = lr_layer.bias
     if not F2.front_supported(plan, lr_plan):
         return None
+    return order, plan, tables, lr_plan, lr_tables
+
+
+def fused_front(embedding_layer, lr_layer, X, want_fm):
+    """One launch for FeatureEmbedding + (FM product_sum) + (LogisticRegression): returns
+    (feature_emb (B,F,D), logit (B,1)), or None when the configuration needs the general path."""
+    fp = front_plan(embedding_layer, lr_layer, X)
+    if fp is None:
+        return None
+    order, plan, tables, lr_plan, lr_tables = fp
+    bias = lr_layer.bias if lr_layer is not None else None
     arena, logit = F2.front(plan, lr_plan, [X[f] for f in order], [t.weight for t in tables],
                             [t.weight for t in lr_tables] if lr_tables else [], bias, want_fm)
     return arena.view(arena.shape[0], len(plan.fields), plan.fields[0].dim), logit

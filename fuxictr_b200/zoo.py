@@ -18,7 +18,7 @@ same RNG consumption) and nothing else.
 import torch
 from torch import nn
 
-from .layers import (fused_front, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
+from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, InnerProductInteraction, DIN_Attention, Dice,
                      CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
@@ -277,13 +277,26 @@ class RankModel(nn.Module):
         self.materialize_tables()
         return super(RankModel, self).state_dict(*args, **kwargs)
 
+    def _table_reads(self, X):
+        """(plan, lr_plan, ids, emb_tables, lr_tables) of the one fused-front launch through which this model's
+        forward reads, and its backward writes, every table row of a step on inputs X; None keeps the serial
+        table pass.  Only DeepFM gives one: xDeepFM and DLRM read their tables the same way, but the side pass
+        made their steps slower on H100 (the CIN kernels and DLRM's 200 M-row tables need every SM; DESIGN.md 4)."""
+        return None
+
     def fused_train_step(self, batch_data):
         """train_step with the arena optimizer and the fused logit+BCE kernel when the model
         exposes its pre-sigmoid logit terms (`forward_logits`)."""
         opt = self._fused_optimizer
         opt.zero_grad()
+        regularised = bool(self._embedding_regularizer or self._net_regularizer)
+        if not regularised and opt.early_tables_ok():
+            # the untouched table granules get this step's update on a side stream while forward and backward run
+            reads = self._table_reads(self.get_inputs(batch_data))
+            if reads is not None:
+                opt.start_early_tables(*reads)
         y_true = self.get_labels(batch_data)
-        fused_logit = hasattr(self, "forward_logits") and not (self._embedding_regularizer or self._net_regularizer)
+        fused_logit = hasattr(self, "forward_logits") and not regularised
         if fused_logit:
             loss, _ = F2.logit_bce(y_true, *self.forward_logits(batch_data))
         else:
@@ -339,6 +352,15 @@ class DeepFM(RankModel):
                              hidden_activations=hidden_activations, output_dim=1, output_activation=None,
                              dropout_rates=net_dropout, batch_norm=batch_norm)
         self._finish(kwargs, learning_rate)
+
+    def _table_reads(self, X):
+        if getattr(self, "_sharded_front", None) is not None:
+            return None
+        fp = front_plan(self.embedding_layer, self.fm.lr_layer, X)
+        if fp is None:
+            return None
+        order, plan, tables, lr_plan, lr_tables = fp
+        return plan, lr_plan, [X[f] for f in order], [t.weight for t in tables], [t.weight for t in lr_tables]
 
     def forward_logits(self, inputs):
         if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull

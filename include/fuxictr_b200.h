@@ -238,6 +238,14 @@ B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field* lr_fields
                            const float* sums, const float* glogit, float* gbias, const b2_lazy_ctx* lazy,
                            const b2_touch* touch, void* stream);
 /*
+ * Flags (b2_touch over the PARAMETER arena) every granule of every row a fused front or fused gather reads
+ * for this batch: emb_fields[i].table / lr_fields[i].table are the parameter tables, idx as in b2_front_fwd
+ * (same id decoding; out-of-range ids mark nothing, padding rows are marked).  That covers every granule the
+ * backward writes, so the marks are final as soon as the ids are (see b2_adam_untouched).
+ */
+B2_API int b2_table_mark(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch,
+                         int idx_dtype, const b2_touch* touch, void* stream);
+/*
  * Lazy optimizer step over the rows enqueued by b2_front_bwd (tables[i]: parameter pointer, rows, dim,
  * global row base, sorted by base; gradients/moments at the arena deltas):
  *   b2_lazy_sumsq      sumsq[0] += sum of g^2 over the enqueued rows
@@ -580,6 +588,19 @@ B2_API int b2_sumsq_ex(const float* g, int64_t n, float* out, const uint8_t* fla
 B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
                            float max_norm, float lr, float beta1, float beta2, float eps,
                            const int64_t* step_dev, int zero_grad, uint8_t* flags, int64_t n_flagged,
+                           void* stream);
+/* The table pass of b2_adam_step_ex (zero_grad = 1, n_flagged = n) split in two launches, for a step whose
+ * flags are final before its gradients exist (every granule the backward will write is flagged first):
+ *   b2_adam_untouched  every UNFLAGGED granule gets the g = 0 update of step *step_dev + 1 (the optimizer
+ *                      counts the step later); P, M, V only, never G or the flags.  At most max_ctas CTAs of
+ *                      1024 threads (one per SM), persistent: it is meant to run beside the forward and backward.
+ *   b2_adam_touched    every FLAGGED granule is updated as b2_adam_step_ex does (step *step_dev), its gradient
+ *                      zeroed and its flag cleared; an unflagged granule costs one flag read.
+ * Together they leave P, M, V, G and the flags bit-identical to b2_adam_step_ex.  n % 4 == 0. */
+B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, float lr, float beta1,
+                             float beta2, float eps, const int64_t* step_dev, int max_ctas, void* stream);
+B2_API int b2_adam_touched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq, float max_norm,
+                           float lr, float beta1, float beta2, float eps, const int64_t* step_dev, uint8_t* flags,
                            void* stream);
 B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
                          int64_t sched_len, void* stream);
