@@ -114,6 +114,11 @@ SIGNATURES = {
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2_shard_pull_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_float,
                                  c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "b2_shard_push_pad": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                  c_void_p]),
+    "b2_shard_publish_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, _FIELD_P, _FIELD_P, c_int, c_int, c_int,
+                                     c_void_p, c_void_p]),
     "b2_peer_bcast": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "b2_peer_bcast_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "b2_front_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,

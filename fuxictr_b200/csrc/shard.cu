@@ -42,25 +42,33 @@ struct BcastDst { void* p[16]; };
 #define B2_OWN_LR (1 << 16)
 
 #define B2_OWN_ZERO (1 << 18)    // out-of-range id: the slot is defined as a zero row, no gradient
+#define B2_OWN_PAD (1 << 19)     // padding id: the requester copies the published padding row, no gradient
 
 constexpr int SERVE_U = 4;       // list entries a lane group serves at once (loads in flight)
 
-// Two phases per 256-item chunk.  SCAN: one thread per (requester, sample, field) candidate reads the id
-// and keeps it only when this rank owns the row — the (world-1)/world candidates that belong to other
-// ranks cost one coalesced 4-byte load each.  SERVE: the block walks the compacted list in shared memory
-// with dim/4 lanes per entry (gather the table row, 16-byte P2P stores into the requester's slot), and
-// appends the entries that will receive a gradient to the rank's owned-row list with ONE global atomic
-// per chunk (a per-warp atomic on the one counter serialises ~1e5 times per launch at 8 ranks).
-// LAZY: the tables are lazily evaluated (b2_lazy_ctx) — a separate instantiation, so that the plain
-// push keeps its register budget (and occupancy).
-template <typename IdxT, bool LAZY>
+// Candidates are (requester, sample, SLOT): a categorical field is one slot, an unpooled sequence of
+// length L is L consecutive slots (slot_start of the pack), S = nslots slots per sample.  Slot s of
+// sample b takes its id from column idx_stride + (s - slot_start[f]) and lands at b*S*D + s*D of the
+// requester's emb; rem = b*S + s is what an owned-list entry keeps in .y.
+// Two phases per 256-item chunk.  SCAN: one thread per candidate reads the id and keeps it only when this
+// rank owns the row — the (world-1)/world candidates that belong to other ranks cost one coalesced 4-byte
+// load each.  With pad_rows, a padding id is served by the REQUESTER itself from the padding rows their
+// owners published before the push (b2_shard_publish_ids): no rank serves other ranks' padding slots.
+// SERVE: the block walks the compacted list in shared memory with dim/4 lanes per entry (gather the table
+// row, 16-byte P2P stores into the requester's slot), and appends the entries that will receive a gradient
+// to the rank's owned-row list with ONE global atomic per chunk (a per-warp atomic on the one counter
+// serialises ~1e5 times per launch at 8 ranks).
+// LAZY: the tables are lazily evaluated (b2_lazy_ctx); ALL_LEN1: every field is one slot (no slot ->
+// field search) — separate instantiations, so that the plain categorical push keeps its register budget
+// (and occupancy).
+template <typename IdxT, bool LAZY, bool ALL_LEN1>
 __global__ void __launch_bounds__(256)
 shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr,
                   const __grid_constant__ PeerPtrs peers, const __grid_constant__ b2_lazy_ctx lz,
                   int64_t batch_local, int64_t ids_stride,
                   int dim, int lpr_log2, int has_lr, int world, int rank,
                   int32_t* __restrict__ status, int4* __restrict__ owned, int32_t* __restrict__ owned_count,
-                  int32_t owned_cap) {
+                  int32_t owned_cap, const float* __restrict__ pad_rows) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(emb, smem_raw);
   SmemFields lf;
@@ -71,11 +79,12 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
   int4* list = reinterpret_cast<int4*>(smem_raw + 2 * pack_bytes);      // 256 entries
   __shared__ int s_front, s_back, s_gbase;
   const int F = emb.nfields;
+  const int S = ALL_LEN1 ? F : emb.nslots;
   const int LPR = 1 << lpr_log2;
   const int lane = threadIdx.x & 31;
   const int sub = threadIdx.x & (LPR - 1);
   const int e = sub * 4;
-  const int64_t per_rank = batch_local * (int64_t) F;
+  const int64_t per_rank = batch_local * (int64_t) S;
   const int64_t nitems = per_rank * world;
   const int done = LAZY ? (int) *lz.step_dev : 0;   // lazy tables: steps completed so far
   const int gstride = 256 >> lpr_log2;               // lane groups per block
@@ -89,15 +98,23 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
     if (item < nitems) {
       const int p = (int) (item / per_rank);           // requesting rank
       const int64_t rem = item - (int64_t) p * per_rank;
-      const int64_t b = rem / F;
-      const int f = (int) (rem - b * F);
+      const int64_t b = rem / S;
+      const int slot = (int) (rem - b * S);
+      const int f = ALL_LEN1 ? slot : b2_slot_field(sf.slot_start, F, slot);
       const b2_field& fd = sf.f[f];
-      // fd.idx_stride carries the COLUMN of this field inside the batch matrix
-      const int64_t row = b2_load_index<IdxT>(peers.ids[p], b * ids_stride + fd.idx_stride);
+      // fd.idx_stride carries the COLUMN of this field inside the batch matrix (a sequence's columns are
+      // consecutive: position k of it is column idx_stride + k)
+      const int64_t col = ALL_LEN1 ? fd.idx_stride : fd.idx_stride + (slot - sf.slot_start[f]);
+      const int64_t row = b2_load_index<IdxT>(peers.ids[p], b * ids_stride + col);
       if (row < 0 || row >= fd.vocab) {
         if (status != nullptr && p == rank) atomicMax(status, f + 1);
         if ((row < 0 ? 0 : (int) (row % world)) == rank) {  // keep the slot defined: zero row
           entry = make_int4(p, (int) rem, 0, f | B2_OWN_ZERO);
+          kind = 2;
+        }
+      } else if (pad_rows != nullptr && row == (int64_t) fd.padding_idx) {   // my own padding slot
+        if (p == rank) {
+          entry = make_int4(p, (int) rem, f, f | B2_OWN_PAD);
           kind = 2;
         }
       } else if ((int) (row % world) == rank) {          // my row
@@ -139,14 +156,22 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
         it[u] = (k < nserve) ? list[k < nfront ? k : 255 - (k - nfront)] : make_int4(-1, 0, 0, B2_OWN_ZERO);
         f[u] = it[u].w & 0xffff;
         lrow[u] = it[u].z;
-        const bool row_ok = !(it[u].w & B2_OWN_ZERO);
+        // a padding entry reads row f of the published padding rows (its .z holds f): bit-exact, any value,
+        // and never replayed (a padding row has no gradient, so Adam leaves it unchanged)
+        const bool pad = (it[u].w & B2_OWN_PAD) != 0;
+        const bool row_ok = !(it[u].w & (B2_OWN_ZERO | B2_OWN_PAD));
         on_e[u] = row_ok && e < dim;
         on_l[u] = row_ok && has_lr && sub == 0;
         v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
         w[u] = 0.f;
-        if (on_e[u])
-          v[u] = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(sf.f[f[u]].table) + lrow[u] * dim + e));
-        if (on_l[u]) w[u] = __ldg(reinterpret_cast<const float*>(lf.f[f[u]].table) + lrow[u]);
+        if ((row_ok || pad) && e < dim) {
+          const float* t = pad ? pad_rows : reinterpret_cast<const float*>(sf.f[f[u]].table);
+          v[u] = __ldg(reinterpret_cast<const float4*>(t + lrow[u] * dim + e));
+        }
+        if ((row_ok || pad) && has_lr && sub == 0) {
+          const float* t = pad ? pad_rows + (int64_t) F * dim : reinterpret_cast<const float*>(lf.f[f[u]].table);
+          w[u] = __ldg(t + lrow[u]);
+        }
       }
       if (LAZY) b2_lazy_replay<SERVE_U>(lz, done, sf, lf, dim, e, f, lrow, on_e, on_l, v, w);
 #pragma unroll
@@ -179,7 +204,7 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
   lf.f = nullptr;
   lf.slot_start = nullptr;
   if (has_lr) lf = b2_stage_fields(lr, smem_raw + ((pack_smem_bytes(emb.nfields) + 15) & ~(size_t) 15));
-  const int F = emb.nfields;
+  const int S = emb.nslots;     // an entry's .y is sample * S + slot
   const int LPR = 1 << lpr_log2;
   const int lane = threadIdx.x & 31;
   const int sub = lane & (LPR - 1);
@@ -217,7 +242,7 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
         const b2_field& ld = lf.f[f];
         if (ld.table != nullptr) {
           float* dst = reinterpret_cast<float*>(const_cast<void*>(ld.table)) + lrow;
-          b2_red_add(dst, peers.glogit[p][bf / F] * scale);
+          b2_red_add(dst, peers.glogit[p][bf / S] * scale);
           b2_touch_mark(tch, dst, true);
           if (lazy) {
             const int grow = (int) (lz.grow_lr[f] + lrow);
@@ -273,8 +298,7 @@ shard_bcast_kernel(const void* __restrict__ src, int64_t nbytes, const __grid_co
 // only need the row numbers — one launch truncates like `.long()`, narrows to int32 (vocabularies < 2^31)
 // and stores the result into this rank's slot on every peer: 4 bytes per id over NVLink instead of 8.
 template <typename IdxT>
-__global__ void __launch_bounds__(256)
-shard_bcast_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world) {
+__device__ __forceinline__ void bcast_ids(const void* __restrict__ src, int64_t n, const BcastDst& dst, int world) {
   const int64_t tid = (int64_t) blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t) gridDim.x * blockDim.x;
   const int64_t n4 = n >> 2;
   for (int64_t i = tid; i < n4; i += nth) {
@@ -288,6 +312,43 @@ shard_bcast_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_con
   for (int64_t i = (n4 << 2) + tid; i < n; i += nth) {
     const int v = (int) b2_load_index<IdxT>(src, i);
     for (int p = 0; p < world; ++p) reinterpret_cast<int32_t*>(dst.p[p])[i] = v;
+  }
+}
+
+template <typename IdxT>
+__global__ void __launch_bounds__(256)
+shard_bcast_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world) {
+  bcast_ids<IdxT>(src, n, dst, world);
+}
+
+// Padding rows this rank owns (NULL: another rank publishes that field's row), and every rank's pad buffer.
+struct PadSrc {
+  const float* e[B2_MAX_FIELDS];
+  const float* l[B2_MAX_FIELDS];
+};
+struct PadDst { float* p[16]; };
+
+// The id exchange, plus the padding rows: the owner of each field's padding row stores it (and its LR weight)
+// into every rank's pad buffer, (F, D) rows then F weights, so that every rank fills its own padding slots in
+// the push.  The push that reads them comes after the barrier that follows this launch.
+template <typename IdxT>
+__global__ void __launch_bounds__(256)
+shard_publish_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world,
+                         const __grid_constant__ PadSrc ps, const __grid_constant__ PadDst pd, int nfields, int dim) {
+  bcast_ids<IdxT>(src, n, dst, world);
+  const int64_t tid = (int64_t) blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t) gridDim.x * blockDim.x;
+  const int64_t nemb = (int64_t) nfields * dim, npad = nemb + nfields;
+  for (int64_t i = tid; i < npad; i += nth) {
+    const float* s;
+    if (i < nemb) {
+      const int f = (int) (i / dim);
+      s = ps.e[f] != nullptr ? ps.e[f] + (i - (int64_t) f * dim) : nullptr;
+    } else {
+      s = ps.l[i - nemb];
+    }
+    if (s == nullptr) continue;
+    const float v = *s;
+    for (int p = 0; p < world; ++p) pd.p[p][i] = v;
   }
 }
 
@@ -376,33 +437,55 @@ front_gprep_kernel(const float* __restrict__ gx, const float* __restrict__ emb,
   }
 }
 
+// One slot per categorical field, seq_len consecutive slots per unpooled sequence (the slots of `fields`,
+// the LR pack takes the embedding pack's layout: LR tables exist only when every field is one slot).
 void fill_pack_cols(B2FieldPack& pack, const b2_field* fields, int nfields) {
+  int slots = 0;
   for (int i = 0; i < nfields; ++i) {
     pack.f[i] = fields[i];
-    pack.slot_start[i] = i;
+    pack.slot_start[i] = slots;
+    slots += fields[i].seq_len;
   }
-  pack.slot_start[nfields] = nfields;
+  pack.slot_start[nfields] = slots;
   pack.nfields = nfields;
-  pack.nslots = nfields;
-  pack.all_len1 = 1;
+  pack.nslots = slots;
+  pack.all_len1 = (slots == nfields) ? 1 : 0;
   pack.pad_ = 0;
 }
 
-int check_shard_args(const b2_field* emb, int nfields, int world, int rank) {
+int64_t count_slots(const b2_field* emb, int nfields) {
+  int64_t s = 0;
+  for (int i = 0; i < nfields; ++i) s += emb[i].seq_len;
+  return s;
+}
+
+int check_shard_args(const b2_field* emb, const b2_field* lr, int nfields, int world, int rank) {
   B2_REQUIRE(emb != nullptr, "emb fields is NULL");
   B2_REQUIRE(nfields >= 1 && nfields <= B2_MAX_FIELDS, "nfields=%d outside [1,%d]", nfields, B2_MAX_FIELDS);
   B2_REQUIRE(world >= 1 && world <= 16 && rank >= 0 && rank < world, "bad world/rank %d/%d", world, rank);
   const int dim = emb[0].dim;
   B2_REQUIRE(dim >= 4 && dim <= 128 && dim % 4 == 0, "sharded front needs emb dim %% 4 == 0 and <= 128 (got %d)", dim);
-  for (int i = 0; i < nfields; ++i)
-    B2_REQUIRE(emb[i].dim == dim && emb[i].seq_len == 1, "field %d: one common dim, no sequences", i);
+  for (int i = 0; i < nfields; ++i) {
+    B2_REQUIRE(emb[i].dim == dim, "field %d: one common dim", i);
+    B2_REQUIRE(emb[i].seq_len >= 1 && (emb[i].seq_len == 1 || emb[i].pool == B2_POOL_NONE),
+               "field %d: a sequence (seq_len %d) needs pool == B2_POOL_NONE (no pooling across owners)", i,
+               emb[i].seq_len);
+    B2_REQUIRE(lr == nullptr || emb[i].seq_len == 1, "field %d: LR tables need one slot per field", i);
+  }
+  B2_REQUIRE(count_slots(emb, nfields) <= (1 << 30), "more than 2^30 slots per sample");
   return B2_OK;
 }
 
+template <typename IdxT, bool LAZY, typename... Args>
+void launch_push_len(bool all_len1, int grid, size_t smem, cudaStream_t st, Args... args) {
+  if (all_len1) shard_push_kernel<IdxT, LAZY, true><<<grid, 256, smem, st>>>(args...);
+  else shard_push_kernel<IdxT, LAZY, false><<<grid, 256, smem, st>>>(args...);
+}
+
 template <typename IdxT, typename... Args>
-int launch_push(bool lazy, int grid, size_t smem, cudaStream_t st, Args... args) {
-  if (lazy) shard_push_kernel<IdxT, true><<<grid, 256, smem, st>>>(args...);
-  else shard_push_kernel<IdxT, false><<<grid, 256, smem, st>>>(args...);
+int launch_push(bool lazy, bool all_len1, int grid, size_t smem, cudaStream_t st, Args... args) {
+  if (lazy) launch_push_len<IdxT, true>(all_len1, grid, smem, st, args...);
+  else launch_push_len<IdxT, false>(all_len1, grid, smem, st, args...);
   return B2_OK;
 }
 
@@ -415,20 +498,26 @@ int check_lazy(const b2_lazy_ctx* lz) {
 }
 }  // namespace
 
-extern "C" B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                       int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                                       int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                                       float* const* peer_lrw, int32_t* status, int32_t* owned,
-                                       int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                                       void* stream) {
-  int rc = check_shard_args(emb_fields, nfields, world, rank);
+extern "C" B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                        int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                                        int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                                        float* const* peer_lrw, int32_t* status, int32_t* owned,
+                                        int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                        const float* pad_rows, void* stream) {
+  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
   if (rc != B2_OK) return rc;
   rc = check_lazy(lazy);
   if (rc != B2_OK) return rc;
   B2_REQUIRE(peer_ids && peer_emb && (lr_fields == nullptr || peer_lrw != nullptr), "NULL peer pointer array");
   B2_REQUIRE(owned == nullptr || (owned_count != nullptr && owned_capacity >= 1), "owned list needs a counter and a capacity");
   B2_REQUIRE(owned == nullptr || ((uintptr_t) owned % 16) == 0, "owned list must be 16-byte aligned");
-  B2_REQUIRE(batch_local * (int64_t) nfields < (1ll << 31), "batch_local * nfields must fit 31 bits");
+  B2_REQUIRE(pad_rows == nullptr || ((uintptr_t) pad_rows % 16) == 0, "pad_rows must be 16-byte aligned");
+  if (pad_rows != nullptr && lr_fields != nullptr)
+    for (int i = 0; i < nfields; ++i)
+      B2_REQUIRE(lr_fields[i].padding_idx == emb_fields[i].padding_idx,
+                 "field %d: the LR and embedding tables need one padding row", i);
+  const int64_t nslots = count_slots(emb_fields, nfields);
+  B2_REQUIRE(batch_local * nslots < (1ll << 31), "batch_local * slots must fit 31 bits");
   cudaStream_t st = (cudaStream_t) stream;
   if (owned != nullptr) {
     cudaError_t e = cudaMemsetAsync(owned_count, 0, sizeof(int32_t), st);
@@ -450,18 +539,29 @@ extern "C" B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_fiel
   const int dim = emb_fields[0].dim;
   const int lpr_log2 = next_pow2_log2((dim + 3) / 4);
   const size_t smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
-  const int grid = grid_for(batch_local * (int64_t) nfields * world, 256);
+  const int grid = grid_for(batch_local * nslots * world, 256);
   int4* ow = reinterpret_cast<int4*>(owned);
   static thread_local b2_lazy_ctx lz_none;
   const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
+  const bool len1 = epack.all_len1 != 0;
   switch (idx_dtype) {
-    case B2_F64: rc = launch_push<double>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
-    case B2_I64: rc = launch_push<int64_t>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
-    case B2_I32: rc = launch_push<int32_t>(lazy != nullptr, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity); break;
+    case B2_F64: rc = launch_push<double>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
+    case B2_I64: rc = launch_push<int64_t>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
+    case B2_I32: rc = launch_push<int32_t>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
   B2_CUDA_LAUNCH_CHECK("b2_shard_push");
   return B2_OK;
+}
+
+extern "C" B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                       int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                                       int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                                       float* const* peer_lrw, int32_t* status, int32_t* owned,
+                                       int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                       void* stream) {
+  return b2_shard_push_pad(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_ids, idx_dtype, ids_stride,
+                           peer_emb, peer_lrw, status, owned, owned_count, owned_capacity, lazy, nullptr, stream);
 }
 
 extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
@@ -478,7 +578,7 @@ extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_fiel
                                        const float* const* peer_glogit, float scale, const int32_t* owned,
                                        const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
                                        const b2_touch* touch, void* stream) {
-  int rc = check_shard_args(emb_fields, nfields, world, rank);
+  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
   if (rc != B2_OK) return rc;
   rc = check_lazy(lazy);
   if (rc != B2_OK) return rc;
@@ -503,8 +603,8 @@ extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_fiel
   const int dim = emb_fields[0].dim;
   const int lpr_log2 = next_pow2_log2((dim + 3) / 4);
   const size_t smem = ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + pack_smem_bytes(nfields) + 16;
-  // the list holds ~batch_local * nfields entries on a balanced batch (this rank's share of the global batch)
-  int64_t expect = batch_local * (int64_t) nfields * 2;
+  // the list holds ~batch_local * slots entries on a balanced batch (this rank's share of the global batch)
+  int64_t expect = batch_local * (int64_t) epack.nslots * 2;
   if (expect > owned_capacity) expect = owned_capacity;
   const int grid = grid_for(expect << lpr_log2, 256);
   static thread_local b2_lazy_ctx lz_none;
@@ -543,6 +643,47 @@ extern "C" B2_API int b2_peer_bcast_ids(const void* src, int idx_dtype, int64_t 
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
   B2_CUDA_LAUNCH_CHECK("b2_peer_bcast_ids");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,
+                                           const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                           int world, int rank, float* const* peer_pad, void* stream) {
+  B2_REQUIRE(src && peer_dst && peer_pad && count >= 0, "bad argument");
+  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
+  if (rc != B2_OK) return rc;
+  BcastDst d;
+  PadDst pd;
+  for (int i = 0; i < 16; ++i) { d.p[i] = nullptr; pd.p[i] = nullptr; }
+  for (int i = 0; i < world; ++i) {
+    B2_REQUIRE(peer_dst[i] != nullptr && ((uintptr_t) peer_dst[i] % 16) == 0, "peer_dst[%d] NULL or misaligned", i);
+    B2_REQUIRE(peer_pad[i] != nullptr && ((uintptr_t) peer_pad[i] % 16) == 0, "peer_pad[%d] NULL or misaligned", i);
+    d.p[i] = peer_dst[i];
+    pd.p[i] = peer_pad[i];
+  }
+  const int dim = emb_fields[0].dim;
+  static thread_local PadSrc ps;
+  for (int f = 0; f < nfields; ++f) {
+    ps.e[f] = nullptr;
+    ps.l[f] = nullptr;
+    const int64_t pad = emb_fields[f].padding_idx;
+    if (pad < 0 || pad >= emb_fields[f].vocab || (int) (pad % world) != rank) continue;     // not mine
+    if (emb_fields[f].table != nullptr) ps.e[f] = reinterpret_cast<const float*>(emb_fields[f].table) + (pad / world) * dim;
+    if (lr_fields != nullptr) {
+      B2_REQUIRE(lr_fields[f].padding_idx == pad, "field %d: the LR and embedding tables need one padding row", f);
+      if (lr_fields[f].table != nullptr) ps.l[f] = reinterpret_cast<const float*>(lr_fields[f].table) + pad / world;
+    }
+  }
+  const int64_t npad = (int64_t) nfields * (dim + 1);
+  const int grid = grid_for((count >> 2) > npad ? (count >> 2) : npad, 256);
+  cudaStream_t st = (cudaStream_t) stream;
+  switch (idx_dtype) {
+    case B2_F64: shard_publish_ids_kernel<double><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim); break;
+    case B2_I64: shard_publish_ids_kernel<int64_t><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim); break;
+    case B2_I32: shard_publish_ids_kernel<int32_t><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim); break;
+    default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
+  }
+  B2_CUDA_LAUNCH_CHECK("b2_shard_publish_ids");
   return B2_OK;
 }
 

@@ -150,27 +150,72 @@ def _ptr_array(ptrs):
     return (ctypes.c_void_p * len(ptrs))(*ptrs)
 
 
+def slot_layout(seq_lens):
+    """(slot_start, S): a one-slot field is one slot, an unpooled sequence of length L is L consecutive slots;
+    slot s of sample b lands at b*S*D + s*D of the requester's (B, S*D) buffer."""
+    starts, s = [], 0
+    for n in seq_lens:
+        starts.append(s)
+        s += int(n)
+    return starts + [s], s
+
+
+def owned_capacity(world, batch_local, seq_lens):
+    """Entries of the owned-row list: every (requester, sample, slot) candidate of the global batch, so the
+    list can never overflow.  Entries and slot offsets are int32: refused (ValueError) past 2^31 - 1."""
+    _, S = slot_layout(seq_lens)
+    if batch_local * S >= 2 ** 31 or world * batch_local * S >= 2 ** 31:
+        raise ValueError("sharded front: world * batch_local * slots = %d * %d * %d does not fit int32"
+                         % (world, batch_local, S))
+    return world * batch_local * S
+
+
+def _distinct(tables):
+    """(distinct tables in first-seen order, index of each entry in that list): a table shared by several
+    fields (share_embedding) is one autograd input with one gradient buffer."""
+    out, where = [], []
+    for t in tables:
+        for i, u in enumerate(out):
+            if u is t:
+                where.append(i)
+                break
+        else:
+            where.append(len(out))
+            out.append(t)
+    return out, where
+
+
 # --------------------------------------------------------------------------------------------
 # The sharded front: FeatureEmbedding (+ FM product_sum) (+ LogisticRegression) over row shards
 # --------------------------------------------------------------------------------------------
 class ShardedFront(object):
     """Holds the peer buffers and launches the phases.
 
-    emb_tables / lr_tables: lists of this rank's SHARD parameters (one per field, fp32 CUDA);
-    vocabs: global vocabulary sizes; columns: column of each field in the batch matrix."""
+    emb_tables / lr_tables: lists of this rank's SHARD parameters (one per field, fp32 CUDA; a shared table
+    appears once per field that reads it); vocabs: global vocabulary sizes; columns: column of each field
+    in the batch matrix (its first column for a sequence); seq_lens: slots of each field (1, or the length
+    of an unpooled sequence)."""
 
     def __init__(self, group, names, emb_tables, lr_tables, vocabs, columns, padding, dim, batch_local,
-                 matrix_width, idx_dtype, bias=None, want_fm=True):
+                 matrix_width, idx_dtype, bias=None, want_fm=True, seq_lens=None):
         self.group, self.names = group, list(names)
         self.emb_tables, self.lr_tables = list(emb_tables), (list(lr_tables) if lr_tables else None)
         self.vocabs, self.columns, self.padding = list(vocabs), list(columns), list(padding)
         self.dim, self.B, self.W = dim, batch_local, matrix_width
         self.F = len(self.names)
+        self.seq_lens = [int(n) for n in seq_lens] if seq_lens is not None else [1] * self.F
+        self.slot_start, self.S = slot_layout(self.seq_lens)
         self.bias, self.want_fm = bias, want_fm
         self.idx_dtype = idx_dtype
         self.idx_code = F2._IDX_CODE[idx_dtype]
         if max(self.vocabs) >= 2 ** 31:
             raise NotImplementedError("the id exchange narrows row numbers to int32 (vocabulary >= 2^31)")
+        if self.S != self.F and (self.lr_tables or want_fm):
+            raise NotImplementedError("sharded front: LR tables and the FM term need one slot per field "
+                                      "(no sequences)")
+        self.owned_cap = owned_capacity(group.world, batch_local, self.seq_lens)
+        self._emb_distinct, self._emb_where = _distinct(self.emb_tables)
+        self._lr_distinct, self._lr_where = _distinct(self.lr_tables or [])
         g = group
         # ids_all[p] = batch matrix of rank p: every rank BROADCASTS its ids into slot `rank` of all
         # peers (one launch of P2P stores), so the push kernel walks local memory only.
@@ -184,12 +229,14 @@ class ShardedFront(object):
         self.ids_ptrs = [self.ids_all.data_ptr() + p * self._slot_bytes for p in range(g.world)]
         self._ids_src = torch.empty((batch_local, matrix_width), dtype=idx_dtype, device="cuda")
         # rows this rank served in the forward (filled by the push, walked by the pull): int32[4] entries
-        self.owned_cap = g.world * batch_local * self.F
         self.owned = torch.empty((self.owned_cap, 4), dtype=torch.int32, device="cuda")
         self.owned_count = torch.zeros(1, dtype=torch.int32, device="cuda")
-        self.emb, self.emb_ptrs, _ = g.alloc("emb", (batch_local, self.F * dim), torch.float32)
+        self.emb, self.emb_ptrs, _ = g.alloc("emb", (batch_local, self.S * dim), torch.float32)
         self.lrw, self.lrw_ptrs, _ = g.alloc("lrw", (batch_local, self.F), torch.float32)
-        self.gemb, self.gemb_ptrs, _ = g.alloc("gemb", (batch_local, self.F * dim), torch.float32)
+        self.gemb, self.gemb_ptrs, _ = g.alloc("gemb", (batch_local, self.S * dim), torch.float32)
+        # the padding row of every field (then its LR weight), published by its owner with the ids: each rank
+        # fills its own padding slots from here, so no rank serves the others' (half of a DIN history)
+        self.pad_rows, self.pad_ptrs, _ = g.alloc("pad_rows", (self.F * dim + self.F,), torch.float32)
         self.glogit, self.glogit_ptrs, _ = g.alloc("glogit", (batch_local,), torch.float32)
         self.status = torch.zeros(1, dtype=torch.int32, device="cuda")
         # mean over the GLOBAL batch (rank_model.py:130): either the pull scales every gradient row by
@@ -198,13 +245,22 @@ class ShardedFront(object):
         self.on_dense_grads_ready = None     # set by RankModel.use_fused_optimizer (overlapped dense all-reduce)
         self._lazy_ctx = None                # b2_lazy_ctx when the shard tables are lazily evaluated (lazy_ctx())
         self._lazy_owner = None
+        self._desc_cache = {}
 
     # -- descriptors --------------------------------------------------------------------------
     def _descs(self, tables, dim):
-        descs = (b2_field * self.F)()
-        for d, t, v, c, pad in zip(descs, tables, self.vocabs, self.columns, self.padding):
+        """The b2_field array of `tables` (one per field), built once per set of table addresses: every launch of
+        a step passes one (the ids launch, the push and the pull each take the tables or their gradients)."""
+        key = (dim,) + tuple(t.data_ptr() if t is not None else 0 for t in tables)
+        descs = self._desc_cache.get(key)
+        if descs is not None:
+            return descs
+        if len(self._desc_cache) >= 16:
+            self._desc_cache.clear()
+        descs = self._desc_cache[key] = (b2_field * self.F)()
+        for d, t, v, c, pad, n in zip(descs, tables, self.vocabs, self.columns, self.padding, self.seq_lens):
             d.table = t.data_ptr() if t is not None else 0
-            d.vocab, d.idx_stride, d.dim, d.seq_len, d.pool = v, c, dim, 1, 0
+            d.vocab, d.idx_stride, d.dim, d.seq_len, d.pool = v, c, dim, n, 0
             d.padding_idx = -1 if pad is None else int(pad)
             d.idx, d.out, d.out_stride = 0, 0, 0
         return descs
@@ -217,7 +273,10 @@ class ShardedFront(object):
             self._ids_src.copy_(batch_matrix)
             src = self._ids_src
         dst = [int(base) + g.rank * self._slot_bytes for base in self._ids_all_ptrs]     # my slot on every rank
-        _lib.call("b2_peer_bcast_ids", F2._ptr(src), self.src_code, self.B * self.W, _ptr_array(dst), g.world,
+        lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
+        # the padding rows this rank owns travel in the same launch (the push reads them after the barrier)
+        _lib.call("b2_shard_publish_ids", F2._ptr(src), self.src_code, self.B * self.W, _ptr_array(dst),
+                  self._descs(self.emb_tables, self.dim), lr, self.F, g.world, g.rank, _ptr_array(self.pad_ptrs),
                   F2._stream())
 
     def lazy_ctx(self):
@@ -234,14 +293,15 @@ class ShardedFront(object):
         g = self.group
         lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
         lz = self.lazy_ctx()
-        _lib.call("b2_shard_push_ex", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
+        _lib.call("b2_shard_push_pad", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.ids_ptrs), self.idx_code, self.W, _ptr_array(self.emb_ptrs),
                   _ptr_array(self.lrw_ptrs) if lr is not None else None, F2._ptr(self.status),
                   F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
-                  ctypes.byref(lz) if lz is not None else None, F2._stream())
+                  ctypes.byref(lz) if lz is not None else None, F2._ptr(self.pad_rows), F2._stream())
 
     def phase_reduce(self):
-        """Local: logit (B,1) and field sums from the landed rows.  Returns (emb copy, logit, sums)."""
+        """Local: logit (B,1) and field sums from the landed rows (one slot per field whenever there is a logit
+        to reduce).  Returns (emb, logit, sums)."""
         # The landed rows are consumed in place: the next overwrite of this peer buffer is the NEXT
         # step's push, which is ordered after this step's backward (and its closing barrier).
         emb = self.emb
@@ -256,12 +316,14 @@ class ShardedFront(object):
 
     # -- backward phases ------------------------------------------------------------------------
     def phase_gprep(self, gx, emb, sums, glogit, gbias=None):
-        _lib.call("b2_front_gprep", F2._ptr(gx), F2._ptr(emb), F2._ptr(sums), F2._ptr(glogit), self.B, self.F,
+        _lib.call("b2_front_gprep", F2._ptr(gx), F2._ptr(emb), F2._ptr(sums), F2._ptr(glogit), self.B, self.S,
                   self.dim, 1 if self.want_fm else 0, F2._ptr(self.gemb),
                   F2._ptr(self.glogit) if glogit is not None else None, F2._ptr(gbias),
                   1 if (gbias is not None and F2._is_zeroed(gbias)) else 0, F2._stream())
 
     def phase_pull(self, emb_grads, lr_grads):
+        """emb_grads / lr_grads: the gradient buffer of each FIELD's table (one buffer, repeated, for a shared
+        table: the pull adds both fields' rows into it)."""
         g = self.group
         lr = self._descs(lr_grads, 1) if lr_grads else None
         lz = self.lazy_ctx()        # lazy tables: the pull enqueues every row it scatters a gradient into
@@ -271,9 +333,21 @@ class ShardedFront(object):
                   ctypes.byref(lz) if lz is not None else None, F2._touch(list(emb_grads) + list(lr_grads or ())),
                   F2._stream())
 
+    def distinct_tables(self):
+        """Every table once (embedding tables, then LR tables): the autograd inputs of sharded_front."""
+        return tuple(self._emb_distinct) + tuple(self._lr_distinct)
+
+    def field_views(self, emb):
+        """(B, S, D) landed rows -> name -> (B, D) for a one-slot field, (B, L, D) for a sequence (views)."""
+        out = {}
+        for name, s0, n in zip(self.names, self.slot_start, self.seq_lens):
+            out[name] = emb[:, s0] if n == 1 else emb[:, s0:s0 + n]
+        return out
+
 
 class _ShardedFrontFn(torch.autograd.Function):
-    """(emb (B,F,D), logit (B,1)) with sharded tables; 2 barriers forward, 1 backward.
+    """(emb (B,S,D), logit (B,1)) with sharded tables; 2 barriers forward, 1 backward.  `tables` are the
+    distinct tables (ShardedFront.distinct_tables): a shared table gets one gradient, the sum over its fields.
 
     No closing barrier: a peer buffer of this step is next written only behind the NEXT step's first
     barrier (ids visible), which no rank passes before every rank has finished this step's backward
@@ -290,7 +364,7 @@ class _ShardedFrontFn(torch.autograd.Function):
         emb, logit, sums = front.phase_reduce()
         ctx.front, ctx.tables, ctx.bias = front, tables, bias
         ctx.save_for_backward(emb, sums)
-        return emb.view(front.B, front.F, front.dim), logit
+        return emb.view(front.B, front.S, front.dim), logit
 
     @staticmethod
     def backward(ctx, gemb, glogit):
@@ -309,13 +383,14 @@ class _ShardedFrontFn(torch.autograd.Function):
         if front.on_dense_grads_ready is not None:      # every dense gradient now exists: start their all-reduce
             front.on_dense_grads_ready()
         g.barrier()                      # every rank's gradient rows are ready to be pulled
-        n = front.F
+        n = len(front._emb_distinct)
         egrads = [(F2._grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in tables[:n]]
         lgrads = [(F2._grad_buffer(t, zero=True, marks=True) if t.requires_grad else None) for t in tables[n:]]
-        front.phase_pull(egrads, lgrads if front.lr_tables else None)
+        front.phase_pull([egrads[i] for i in front._emb_where],
+                         [lgrads[i] for i in front._lr_where] if front.lr_tables else None)
         return (None, None, gbias) + tuple(egrads) + tuple(lgrads)
 
 
 def sharded_front(front, batch_matrix):
-    tables = tuple(front.emb_tables) + tuple(front.lr_tables or ())
-    return _ShardedFrontFn.apply(front, batch_matrix, front.bias, *tables)
+    """(emb (B, S, D), logit (B, 1)) of this rank's samples, read from the row-sharded tables."""
+    return _ShardedFrontFn.apply(front, batch_matrix, front.bias, *front.distinct_tables())

@@ -15,6 +15,8 @@ same RNG consumption) and nothing else.
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
+from collections import OrderedDict
+
 import torch
 from torch import nn
 
@@ -157,26 +159,49 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM) may be sharded: any other forward would keep reading the 1/world row shards
-        with global ids."""
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN) may be sharded: any other forward would keep reading the
+        1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
+        a table shared by several fields is sharded once), one common embedding dim; an LR term needs
+        categorical features only.  Anything else is refused before a table is touched."""
         from . import sharded as SH
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
-                                      "is implemented for DeepFM and DLRM" % type(self).__name__)
-        fed = self.embedding_layer.embedding_layer
+                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM and DIN" % type(self).__name__)
+        fed = self.embedding_layer
+        if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
+            fed = fed.embedding_layer
         lr_layer = self.fm.lr_layer if hasattr(self, "fm") else getattr(self, "lr_layer", None)
-        names = [f for f in self.feature_map.features.keys() if f in fed.embedding_layers]
-        if not all(fed._is_fusable(f) and self.feature_map.features[f]["type"] == "categorical" for f in names):
-            raise NotImplementedError("sharded front needs categorical features only")
+        specs = self.feature_map.features
+        names = [f for f in specs.keys() if f in fed.embedding_layers]
+        for f in names:
+            kind = specs[f]["type"]
+            if kind not in ("categorical", "sequence") or type(fed.embedding_layers[f]) != nn.Embedding:
+                raise NotImplementedError("sharded front needs categorical or sequence features (%s is %s)"
+                                          % (f, kind))
+            if f in fed.feature_encoders:
+                raise NotImplementedError("sharded front: feature %s has an encoder (a pooled sequence's rows come "
+                                          "from several owners)" % f)
+        dims = set(fed.embedding_layers[f].embedding_dim for f in names)
+        if len(dims) != 1:
+            raise NotImplementedError("sharded front needs one common embedding dim (got %s)" % sorted(dims))
+        seq_lens = [int(specs[f]["max_len"]) if specs[f]["type"] == "sequence" else 1 for f in names]
+        if (lr_layer is not None or want_fm) and any(n != 1 for n in seq_lens):
+            raise NotImplementedError("sharded front: an LR or FM term over sequence features is not supported")
         lfed = lr_layer.embedding_layer.embedding_layer if lr_layer is not None else None
+        if lfed is not None and not all(f in lfed.embedding_layers and type(lfed.embedding_layers[f]) == nn.Embedding
+                                        and f not in lfed.feature_encoders for f in names):
+            raise NotImplementedError("sharded front: the LR term needs one plain table per feature")
+        dim = dims.pop()
+        SH.owned_capacity(group.world, batch_local, seq_lens)       # the int32 bound, before any allocation
         vocabs, cols, pads, etabs, ltabs = [], [], [], [], []
         with torch.no_grad():
             for f in names:
                 emb = fed.embedding_layers[f]
                 vocabs.append(emb.num_embeddings)
-                cols.append(self.feature_map.get_column_index(f))
+                col = self.feature_map.get_column_index(f)
+                cols.append(col[0] if isinstance(col, list) else col)    # a sequence's columns are consecutive
                 pads.append(emb.padding_idx)
-                if not getattr(emb, "_b2_sharded", False):
+                if not getattr(emb, "_b2_sharded", False):     # a shared table: sharded once, listed per field
                     emb.weight.data = SH.shard_rows(emb.weight.data, group.rank, group.world)
                     emb._b2_sharded = True
                 etabs.append(emb.weight)
@@ -186,12 +211,11 @@ class RankModel(nn.Module):
                         lemb.weight.data = SH.shard_rows(lemb.weight.data, group.rank, group.world)
                         lemb._b2_sharded = True
                     ltabs.append(lemb.weight)
-        dim = fed.embedding_layers[names[0]].embedding_dim
         self._sharded_front = SH.ShardedFront(group, names, etabs, ltabs or None, vocabs, cols, pads, dim,
                                               batch_local, matrix_width, idx_dtype,
                                               bias=(lr_layer.bias if lr_layer is not None else None),
-                                              want_fm=want_fm)
-        self._sharded_params = etabs + ltabs
+                                              want_fm=want_fm, seq_lens=seq_lens)
+        self._sharded_params = list(self._sharded_front.distinct_tables())
         # fused_train_step seeds backward() with 1/world, so every gradient (dense and rows) is born
         # divided by the world size: the pull and the dense all-reduce then need no scaling pass
         self._sharded_front.pull_scale = 1.0
@@ -201,14 +225,21 @@ class RankModel(nn.Module):
     def _batch_matrix(self, inputs):
         """The (B, W) matrix the collator sliced `inputs` from, rebuilt from one column view's
         storage offset and row stride (the views' `_base` may be a larger tensor)."""
-        name = next(iter(self.feature_map.features.keys()))
-        v = inputs[name]
-        col = self.feature_map.get_column_index(name)
         width = self.feature_map.input_length + len(self.feature_map.labels)
-        if v.dim() != 1 or v.stride(0) < width or v.storage_offset() < col:
-            raise RuntimeError("sharded front needs the batch dict to be column views of one matrix")
-        mat = v.as_strided((v.shape[0], width), (v.stride(0), 1), v.storage_offset() - col)
-        return mat.to(self.device)
+        for name in list(self.feature_map.features.keys()) + list(self.feature_map.labels):
+            v = inputs.get(name)
+            col = self.feature_map.get_column_index(name)
+            if isinstance(col, list):   # a sequence: a column-range view (batch_views), or a copy (batch_dict)
+                col = col[0]
+                if v is None or v.dim() != 2 or v.stride(1) != 1:
+                    continue
+            elif v is None or v.dim() != 1:
+                continue
+            if v.stride(0) < width or v.storage_offset() < col:
+                continue
+            mat = v.as_strided((v.shape[0], width), (v.stride(0), 1), v.storage_offset() - col)
+            return mat.to(self.device)
+        raise RuntimeError("sharded front needs the batch dict to be column views of one matrix")
 
     def _front_tables(self):
         """Embedding + LR tables read ONLY through the fused front kernels (lazy-Adam candidates)."""
@@ -390,6 +421,7 @@ class DCNv2(RankModel):
     """model_zoo/DCNv2/src/DCNv2.py:47-132: CrossNetV2 and DNN towers combined per `model_structure`
     (crossnet_only | stacked | parallel | stacked_parallel), one Linear to the logit."""
     _STRUCTURES = ("crossnet_only", "stacked", "parallel", "stacked_parallel")
+    _routes_sharded_front = True
 
     def __init__(self, feature_map, model_id="DCNv2", gpu=-1, model_structure="parallel",
                  use_low_rank_mixture=False, low_rank=32, num_experts=4, learning_rate=1e-3,
@@ -426,7 +458,11 @@ class DCNv2(RankModel):
 
     def _final_out(self, inputs):
         """DCNv2.py:108-128: what the last Linear sees for each model_structure."""
-        emb = self.embedding_layer(self.get_inputs(inputs), flatten_emb=True)
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull
+            from .sharded import sharded_front
+            emb = sharded_front(self._sharded_front, self._batch_matrix(inputs))[0].flatten(start_dim=1)
+        else:
+            emb = self.embedding_layer(self.get_inputs(inputs), flatten_emb=True)
         cross = self.crossnet(emb)
         left = self.stacked_dnn(cross) if hasattr(self, "stacked_dnn") else cross
         if not hasattr(self, "parallel_dnn"):
@@ -506,6 +542,7 @@ class DLRM(RankModel):
 class DIN(RankModel):
     """model_zoo/DIN/src/DIN.py:50-149: one DIN_Attention per (target, sequence) field pair (tuples of
     fields are concatenated), pooled sequences replace the raw ones, one DNN over all embeddings."""
+    _routes_sharded_front = True
 
     def __init__(self, feature_map, model_id="DIN", gpu=-1, dnn_hidden_units=[512, 128, 64],
                  dnn_activations="ReLU", attention_hidden_units=[64], attention_hidden_activations="Dice",
@@ -549,7 +586,14 @@ class DIN(RankModel):
         """DIN.py:109-142: attention-pool every sequence group against its target, write the pooled
         vectors back under the sequence names, then one DNN over all embeddings in FeatureMap order."""
         X = self.get_inputs(inputs)
-        emb = self.embedding_layer(X)
+        front = getattr(self, "_sharded_front", None)
+        if front is not None:       # row-sharded tables: (B, D) / (B, L, D) views of the landed rows
+            from .sharded import sharded_front
+            landed, _ = sharded_front(front, self._batch_matrix(inputs))
+            views = front.field_views(landed)
+            emb = OrderedDict((name, views[name]) for name in self.feature_map.features.keys() if name in views)
+        else:
+            emb = self.embedding_layer(X)
         for head, target, sequence in zip(self.attention_layers, self.din_target_field, self.din_sequence_field):
             seq_names = list(_flatten([sequence]))
             valid = X[seq_names[0]].long() != 0            # padding id 0 marks the empty history slots
@@ -561,6 +605,7 @@ class DIN(RankModel):
 
 class xDeepFM(RankModel):
     """model_zoo/xDeepFM/src/xDeepFM.py:41-97: y = sigmoid(LR(X) + CIN(E) [+ DNN(flatten(E))])."""
+    _routes_sharded_front = True
     _replays_lazy_tables = True
 
     def __init__(self, feature_map, model_id="xDeepFM", gpu=-1, learning_rate=1e-3, embedding_dim=10,
@@ -581,6 +626,13 @@ class xDeepFM(RankModel):
         self._finish(kwargs, learning_rate)
 
     def forward_logits(self, inputs):
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables (and LR), P2P push/pull
+            from .sharded import sharded_front
+            feature_emb, lr_logit = sharded_front(self._sharded_front, self._batch_matrix(inputs))
+            terms = [lr_logit, self.cin(feature_emb)]
+            if self.dnn is not None:
+                terms.append(self.dnn(feature_emb.flatten(start_dim=1)))
+            return tuple(terms)
         X = self.get_inputs(inputs)
         fused = fused_front(self.embedding_layer, self.lr_layer, X, want_fm=False)
         if fused is not None:     # gather + LR in one launch

@@ -315,6 +315,29 @@ B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_field
                             const float* const* peer_glogit, float scale, const int32_t* owned,
                             const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
                             const b2_touch* touch, void* stream);
+/* Sequence fields: a field with seq_len L > 1 (pool must be B2_POOL_NONE: a pooled sequence's rows come from
+ * several owners) is L consecutive SLOTS, with its ids in columns idx_stride .. idx_stride + L - 1.  With
+ * S = sum of seq_len, slot s of sample b lands at b*S*D + s*D of peer_emb / is read at the same offset of
+ * peer_gemb, and an owned-list entry keeps b*S + s where a one-slot field keeps b*F + f.  Requires
+ * batch_local * S < 2^31; an owned list of world * batch_local * S entries never overflows.  LR tables
+ * (lr_fields != NULL) need seq_len == 1 on every field.
+ * b2_shard_push_pad: b2_shard_push_ex where every rank fills its OWN padding slots (id == padding_idx)
+ * from pad_rows, this rank's (F*D + F)-float buffer that b2_shard_publish_ids filled before the push
+ * (padding row of field f at f*D, its LR weight at F*D + f): no rank serves the padding slots of the
+ * others, and the copy is bit-exact whatever the padding row holds.  Padding slots get no gradient.
+ * pad_rows == NULL is b2_shard_push_ex (the owner of the padding row serves it like any other row). */
+B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                             int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                             int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                             float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
+                             int32_t owned_capacity, const b2_lazy_ctx* lazy, const float* pad_rows,
+                             void* stream);
+/* b2_peer_bcast_ids, and in the same launch the padding rows: for every field whose padding row this rank
+ * owns, the row (emb_fields[f].table = this rank's shard) and its LR weight are stored into peer_pad[p]
+ * (16-byte aligned, F*D + F floats, layout as pad_rows above) for every p < world. */
+B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,
+                                const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int world,
+                                int rank, float* const* peer_pad, void* stream);
 B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream);
 /* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
  * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world. */
