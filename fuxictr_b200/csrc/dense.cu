@@ -290,7 +290,7 @@ extern "C" B2_API int b2_colsum(const float* x, int64_t M, int64_t N, int64_t ld
 // ---------------------------------------------------------------------------------
 // Fused logit sum + sigmoid + binary cross entropy (mean) + dL/dlogit.
 //   p = 1/(1+exp(-z))                                    nn.Sigmoid, rank_model.py:447-448
-//   l = -(y*max(log p,-100) + (1-y)*max(log(1-p),-100))  F.binary_cross_entropy
+//   l = -(y*max(log p,-100) + (1-y)*max(log1p(-p),-100)) F.binary_cross_entropy
 //   dz = (p-y)/max((1-p)*p, 1e-12) * (1-p)*p / B         binary_cross_entropy_backward o sigmoid_backward
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -313,7 +313,9 @@ logit_bce_kernel(const float* __restrict__ t0, const float* __restrict__ t1,
     if (y_pred != nullptr) y_pred[i] = p;
     if (label != nullptr) {
       const float y = __ldg(label + i);
-      const float lp = fmaxf(logf(p), -100.f), lq = fmaxf(logf(1.f - p), -100.f);
+      // log1p(-p), as torch's binary_cross_entropy: log(1 - p) would round 1 - p first and lose every digit
+      // of a loss below ~6e-8
+      const float lp = fmaxf(logf(p), -100.f), lq = fmaxf(log1pf(-p), -100.f);
       part += -(y * lp + (1.f - y) * lq);
       if (glogit != nullptr) {
         const float pq = (1.f - p) * p;

@@ -204,12 +204,12 @@ crossnet_bwd_kernel(const float* __restrict__ x0, const float* __restrict__ w,
       g[c] = (col < d) ? __ldg(gout + b * d + col) : 0.f;
       gx[c] = 0.f;
     }
-    // alpha_l = 1 + sum_{j<l} s_j ; start from alpha_L and peel one s per layer.
-    float alpha = 1.f;
-    for (int l = 0; l < L; ++l) alpha += __ldg(s + b * L + l);
     for (int l = L - 1; l >= 0; --l) {
       const float sl = __ldg(s + b * L + l);
-      alpha -= sl;  // now alpha_l
+      // alpha_l = 1 + sum_{j<l} s_j, summed upward like beta_l: subtracting s_j from a running
+      // total would cancel catastrophically once |s| grows across the layers.
+      float alpha = 1.f;
+      for (int j = 0; j < l; ++j) alpha += __ldg(s + b * L + j);
       float t = 0.f;
 #pragma unroll
       for (int c = 0; c < CH; ++c) t = fmaf(g[c], a0[c], t);

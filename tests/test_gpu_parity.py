@@ -932,14 +932,10 @@ def _taobao_specs():
     return specs
 
 
-@pytest.mark.parametrize("config", ["C3_DCNv2", "C4_DIN", "C5_DLRM_shape", "C2_xDeepFM"])
-def test_baseline_shapes_forward_and_step(config):
-    """BASELINE.json configs[2..4] (and xDeepFM at the C2 shape) at their full batch / field / sequence
-    sizes: predictions and loss against the oracle (1e-5), then one fused training step must run and
-    lower-bound sanity (finite loss, gradient arena consumed).  C5's 200 M-row vocabulary is reduced to
-    26 x 100 k rows so that the CPU oracle can hold it; the shapes that drive the kernels
-    (26 fields, D=16, 325 pair products, top MLP 64-64-64, batch 8192) are the real ones."""
-    from fuxictr_b200 import zoo, functional as F2
+def _baseline_setup(config):
+    """(fm, spec_map, mat, model, pred, state0) of one BASELINE config at full shape: the CPU model with its
+    tables initialised like the C2 test, the oracle's y_pred function and the initial state."""
+    from fuxictr_b200 import zoo
     from fuxictr_b200.schema import FeatureMap
     from oracle import fuxictr_oracle as O
     gen = torch.Generator().manual_seed(5)
@@ -984,6 +980,18 @@ def test_baseline_shapes_forward_and_step(config):
             if isinstance(m, torch.nn.Embedding):
                 m.weight[1:].normal_(0, 0.05)
     state0 = OrderedDict((k, v.detach().clone()) for k, v in model.state_dict().items())
+    return fm, spec_map, mat, model, pred, state0
+
+
+@pytest.mark.parametrize("config", ["C3_DCNv2", "C4_DIN", "C5_DLRM_shape", "C2_xDeepFM"])
+def test_baseline_shapes_forward_and_step(config):
+    """BASELINE.json configs[2..4] (and xDeepFM at the C2 shape) at their full batch / field / sequence
+    sizes: predictions and loss against the oracle (1e-5), then one fused training step must run and
+    lower-bound sanity (finite loss, gradient arena consumed).  C5's 200 M-row vocabulary is reduced to
+    26 x 100 k rows so that the CPU oracle can hold it; the shapes that drive the kernels
+    (26 fields, D=16, 325 pair products, top MLP 64-64-64, batch 8192) are the real ones."""
+    from oracle import fuxictr_oracle as O
+    fm, spec_map, mat, model, pred, state0 = _baseline_setup(config)
     tr = O.OracleTrainer(state0, pred, spec_map, ["label"])
     with torch.no_grad():
         y_ref, y_true = tr.forward(fm.batch_dict(mat))
@@ -1004,6 +1012,106 @@ def test_baseline_shapes_forward_and_step(config):
     assert close(loss, loss_ref, RTOL), (float(loss), float(loss_ref))
     assert float(model._arena.G.abs().sum()) == 0.0
     assert all(torch.isfinite(p).all() for p in model.parameters())
+
+
+@pytest.mark.parametrize("config", ["C3_DCNv2", "C4_DIN", "C5_DLRM_shape", "C2_xDeepFM"])
+def test_baseline_shapes_gradients_and_step_vs_oracle(config):
+    """The configs of test_baseline_shapes_forward_and_step: every parameter gradient, then the loss after
+    one fused Adam step, against the oracle — the bar of test_criteo_shape_deepfm_step_vs_oracle.  The
+    oracle runs in float32 and float64; predictions and loss must satisfy
+        err(ours, fp64) <= max(1e-5, 3 * err(reference fp32, fp64)).
+    All four networks have ReLU layers.  One pre-activation within fp32 rounding of zero takes the other branch
+    than in float64 and moves its sample's whole contribution (see the C2 test), so every gradient is held to
+    1e-2 element-wise (or 3x the fp32 reference's own error, when its kinks land off the float64 side too) and
+    to 1e-4 in total norm.  A dense weight sums that contribution over the batch and always meets the
+    element-wise bound.  A touched table row is mostly one sample's contribution, which such a flip moves by up
+    to ~2 % of the table's largest gradient, so table rows beyond the bound are accepted only when they all
+    belong to at most two samples, each of which has a ReLU pre-activation in the float64 oracle within 1e-5
+    of its layer's RMS of zero: the kink is shown, not assumed."""
+    from fuxictr_b200 import functional as F2
+    from oracle import fuxictr_oracle as O
+    fm, spec_map, mat, model, pred, state0 = _baseline_setup(config)
+    cpu_batch = fm.batch_dict(mat)
+
+    pre = []            # the float64 oracle's ReLU inputs, (batch, units) per layer
+
+    def oracle_run(dtype):
+        st = OrderedDict((k, v.to(dtype) if v.is_floating_point() else v) for k, v in state0.items())
+        tr = O.OracleTrainer(st, pred, spec_map, ["label"])
+        relu = torch.relu
+        if dtype == torch.float64:
+            torch.relu = lambda x: (pre.append(x.detach()), relu(x))[1]
+        try:
+            y_pred, y = tr.forward(cpu_batch)
+        finally:
+            torch.relu = relu
+        loss = O.bce_mean(y_pred, y.to(dtype))
+        loss.backward()
+        return y_pred.detach(), loss.detach(), tr.state
+    y64, l64, s64 = oracle_run(torch.float64)
+    y32, l32, s32 = oracle_run(torch.float32)
+
+    model.device = torch.device("cuda:0")
+    model.model_to_device()
+    model.compile("adam", "binary_crossentropy", 1e-3)
+    model.train()
+    opt = model.use_fused_optimizer()
+    batch = fm.batch_dict(mat.cuda())
+    opt.zero_grad()
+    if hasattr(model, "forward_logits"):
+        loss, y_pred = F2.logit_bce(model.get_labels(batch), *model.forward_logits(batch))
+    else:
+        y_pred = model.forward(batch)["y_pred"]
+        loss = model.compute_loss({"y_pred": y_pred}, model.get_labels(batch))
+    loss.backward()
+
+    def bar(ours, ref32, truth, what):
+        e_ours, e_ref = rel_err(ours, truth), rel_err(ref32, truth)
+        assert e_ours <= max(RTOL, 3 * e_ref), (what, e_ours, e_ref)
+    bar(y_pred, y32, y64, "y_pred")
+    bar(loss, l32, l64, "loss")
+    named = OrderedDict((k, p) for k, p in model.named_parameters() if p.requires_grad)
+    assert len(named) > 0
+    B = mat.shape[0]
+    bad = []            # (table, row) beyond the element-wise bound
+    for k, p in named.items():
+        assert p.grad is not None, k
+        g, g64 = p.grad.double().cpu(), s64[k].grad
+        e_ours, e_ref = rel_err(g, g64), rel_err(s32[k].grad, g64)
+        lim = max(1e-2, 3 * e_ref)
+        if ".embedding_layers." not in k:
+            assert e_ours <= lim, (k, e_ours, e_ref)
+            continue
+        rows = torch.nonzero((g - g64).abs().amax(dim=1) > lim * float(g64.abs().max())).view(-1)
+        bad += [(k, int(r)) for r in rows]
+
+    def samples_of(k, row):
+        """Samples whose ids (of any feature reading table k) include `row`."""
+        feat = k.rsplit(".embedding_layers.", 1)[1][:-len(".weight")]
+        feats = [f for f, sp in spec_map.items()
+                 if f == feat or ("lr_layer." not in k and sp.get("share_embedding") == feat)]
+        return torch.stack([(cpu_batch[f].long().view(B, -1) == row).any(1) for f in feats]).any(0)
+    covers, kinks = [samples_of(k, r) for k, r in bad], []
+    assert all(bool(c.any()) for c in covers), ("gradient in a row no sample reads", bad[:10])
+    while covers:
+        s = int(torch.stack(covers).sum(0).argmax())
+        kinks.append(s)
+        covers = [c for c in covers if not c[s]]
+    assert len(kinks) <= 2, (kinks, bad[:10])
+    for s in kinks:
+        margin = min(float(z[s].abs().min()) / float(z.pow(2).mean().sqrt()) for z in pre)
+        assert margin <= 1e-5, ("table rows off without a ReLU kink", s, margin, bad[:10])
+    ours = torch.cat([p.grad.flatten().double().cpu() for p in named.values()])
+    truth = torch.cat([s64[k].grad.flatten() for k in named])
+    assert float((ours - truth).norm()) <= 1e-4 * float(truth.norm())
+    # one optimiser step, then the next loss (weights feed back through the whole model)
+    tr = O.OracleTrainer(state0, pred, spec_map, ["label"])
+    tr.train_step(cpu_batch)
+    loss_ref2 = float(O.bce_mean(*tr.forward(cpu_batch)))
+    opt.step()
+    with torch.no_grad():
+        loss2 = model.compute_loss(model.forward(batch), model.get_labels(batch))
+    assert abs(float(loss2) - loss_ref2) <= RTOL * abs(loss_ref2), (float(loss2), loss_ref2)
 
 
 # ------------------------------------------------------------------ C5 at its full shape, by properties
