@@ -69,6 +69,7 @@ class b2_gemm_desc(ctypes.Structure):
         ("a_mn_major", c_int32), ("b_mn_major", c_int32), ("act", c_int32), ("act_bwd", c_int32),
         ("beta_accumulate", c_int32), ("elem_dtype", c_int32), ("ld_aux", c_int64),
         ("flags", c_int64),
+        ("drop_rng", c_void_p), ("drop_layer", c_int64), ("drop_thresh", ctypes.c_uint32), ("drop_scale", c_float),
     ]
 
 class b2_gemm_plan(ctypes.Structure):
@@ -157,12 +158,16 @@ SIGNATURES = {
     "b2_split_tf32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "b2_transpose_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_prep_operand": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
-                                c_void_p, c_void_p]),
+                                c_void_p, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p]),
     "b2_head_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "b2_head_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
                             c_void_p, c_void_p]),
     "b2_head_bwd_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
-                               c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+                               c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int64, ctypes.c_uint32, c_float,
+                               c_void_p]),
+    "b2_dropout_rng_take": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
+    "b2_dropout_apply": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, ctypes.c_uint32,
+                                 c_float, c_void_p]),
     "b2_act_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "b2_colsum": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_void_p]),
     "b2_logit_bce_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,

@@ -35,9 +35,14 @@
 //                  epilogue: the accumulators are staged as a row-major tile in the dead ring, and each thread walks
 //                  it in 16-byte row segments, a batch at a time, with every global load of a batch issued before
 //                  its first store.
+// Dropout (MLP_Block's Linear -> act -> Dropout): a launch whose descriptor carries a dropout snapshot runs the
+// DROP instantiation of its kernel, whose epilogue applies the layer's mask keep(seed, offset, m, n) (philox.cuh)
+// after the activation and before the activation backward; launches without one keep the instantiations as
+// they were.
 // Kernels of a step are chained with programmatic dependent launch (prologue under the predecessor's tail).
 // Every mbarrier wait is bounded: a pipeline bug traps with a message instead of hanging the GPU.
 #include "b2_common.cuh"
+#include "philox.cuh"
 #include <string.h>
 #include <cstdlib>
 #include <cuda.h>  // CUtensorMap + enums only; cuTensorMapEncodeTiled is resolved at run time
@@ -124,6 +129,10 @@ struct Params {
   int vec;                // every epilogue pointer and leading dimension allows 16-byte row segments (bf16 c_small: 8)
   int tiles_m, tiles_n, splits;
   Ring ring;              // this launch's stage layout (ring_layout of its tile width, mode and operand majors)
+  const int64_t* drop_rng;  // DROP instantiations only: the forward's {seed, offset} snapshot
+  int64_t drop_layer;       // counter offset of the mask: snapshot offset + drop_layer
+  uint32_t drop_thresh;     // keep iff the element's Philox word < drop_thresh
+  float drop_scale;         // 1 / (1 - p) as fp32
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -348,14 +357,23 @@ __device__ __forceinline__ void seg_store_bf16(__nv_bfloat16* p, const float4& v
 
 // The fused epilogue of one element after c_pre: t = accumulator + bias; mv, av, yv, cv are its mul, add, ybwd and
 // (beta) C.  Every operation is rounded on its own (no contraction into fma).
-__device__ __forceinline__ float epilogue_elem(const Params& p, float t, float mv, float av, float yv, float cv) {
+// DROP: keep is the element's dropout mask bit.  The mask multiplies after the activation (forward: y = act(z) *
+// keep * scale) and before the activation backward (dgrad: dZ = act'(.) * keep * scale * dH), where ybwd holds the
+// dropped output: ReLU's act' is ybwd > 0 as before; sigmoid's s is recovered as ybwd / scale on kept elements.
+template <bool DROP>
+__device__ __forceinline__ float epilogue_elem(const Params& p, float t, float mv, float av, float yv, float cv,
+                                              bool keep) {
   if (p.mul != nullptr) t = __fmul_rn(t, mv);
   if (p.add != nullptr) t = __fadd_rn(t, av);
   if (p.act == B2_ACT_RELU) t = fmaxf(t, 0.f);
   else if (p.act == B2_ACT_SIGMOID) t = 1.f / (1.f + expf(-t));
+  if constexpr (DROP) t = keep ? __fmul_rn(t, p.drop_scale) : 0.f;
   if (p.ybwd != nullptr) {     // activation backward of the PRODUCER of this gradient, fused
     if (p.act_bwd == B2_ACT_RELU) t = (yv > 0.f) ? t : 0.f;
-    else if (p.act_bwd == B2_ACT_SIGMOID) t = __fmul_rn(t, __fmul_rn(__fsub_rn(1.f, yv), yv));
+    else if (p.act_bwd == B2_ACT_SIGMOID) {
+      const float s = DROP ? __fdiv_rn(yv, p.drop_scale) : yv;
+      t = __fmul_rn(t, __fmul_rn(__fsub_rn(1.f, s), s));
+    }
   }
   if (p.beta) t = __fadd_rn(t, cv);
   return t;
@@ -364,7 +382,7 @@ __device__ __forceinline__ float epilogue_elem(const Params& p, float t, float m
 // The two consumer warpgroups (threads 128-383) meet; barrier 0 is __syncthreads.
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-template <int BN, int MODE>
+template <int BN, int MODE, bool DROP>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
   constexpr int NR = BN / 2;                            // accumulators per thread: 64 x BN per warpgroup
@@ -593,6 +611,11 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
     const float4 bv = (p.bias != nullptr && z == 0 && nv > 0) ? seg_load<true>(p.bias + n, vec_n, nv)
                                                              : make_float4(0.f, 0.f, 0.f, 0.f);
     float cs[4] = {0.f, 0.f, 0.f, 0.f};
+    uint64_t dseed = 0, doff = 0;
+    if constexpr (DROP) {
+      dseed = (uint64_t) p.drop_rng[0];
+      doff = (uint64_t) p.drop_rng[1] + (uint64_t) p.drop_layer;
+    }
 #pragma unroll 1
     for (int b0 = 0; b0 < SEG; b0 += BATCH) {
       float4 mv[BATCH], av[BATCH], yv[BATCH], cv[BATCH];
@@ -622,10 +645,14 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
           continue;
         }
         if (p.c_pre != nullptr) seg_store(p.c_pre + o, t, v, k);
-        t.x = epilogue_elem(p, t.x, mv[i].x, av[i].x, yv[i].x, cv[i].x);
-        t.y = epilogue_elem(p, t.y, mv[i].y, av[i].y, yv[i].y, cv[i].y);
-        t.z = epilogue_elem(p, t.z, mv[i].z, av[i].z, yv[i].z, cv[i].z);
-        t.w = epilogue_elem(p, t.w, mv[i].w, av[i].w, yv[i].w, cv[i].w);
+        uint32_t kb = 0;       // keep bits of the segment's elements: one Philox call when it starts on a group
+        if constexpr (DROP) {
+          if (k > 0) kb = b2_drop_keep4(dseed, doff, (uint64_t) m * (uint64_t) p.N + (uint64_t) n, k, p.drop_thresh);
+        }
+        t.x = epilogue_elem<DROP>(p, t.x, mv[i].x, av[i].x, yv[i].x, cv[i].x, kb & 1u);
+        t.y = epilogue_elem<DROP>(p, t.y, mv[i].y, av[i].y, yv[i].y, cv[i].y, kb & 2u);
+        t.z = epilogue_elem<DROP>(p, t.z, mv[i].z, av[i].z, yv[i].z, cv[i].z, kb & 4u);
+        t.w = epilogue_elem<DROP>(p, t.w, mv[i].w, av[i].w, yv[i].w, cv[i].w, kb & 8u);
         seg_store(p.c + o, t, v, k);
         if (p.c_small != nullptr) {
           const int64_t oa = (int64_t) m * p.ld_aux + n;
@@ -698,26 +725,40 @@ transpose_kernel(const float* __restrict__ in, int64_t rows, int64_t cols, int64
 //   outT   = v^T          (C, R)            outT_small = tf32_small(v^T)
 //   colsum[c] += sum_r v[r, c]              (bias gradient)
 // Any output pointer may be NULL.  32 x 32 tiles through padded shared memory.
+// DROP: x is the gradient of a dropout layer's output, y that dropped output: v = act'(y) * keep * scale * x
+// (the mask first; sigmoid's s = y / scale on kept elements).
 // ---------------------------------------------------------------------------------
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 prep_operand_kernel(const float* __restrict__ x, const float* __restrict__ y, int act, int64_t R,
                     int64_t C, int64_t ld_in, float* __restrict__ out, float* __restrict__ out_small,
-                    float* __restrict__ outT, float* __restrict__ outT_small, float* __restrict__ colsum) {
+                    float* __restrict__ outT, float* __restrict__ outT_small, float* __restrict__ colsum,
+                    const int64_t* __restrict__ drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale) {
   b2_pdl_wait();
   b2_pdl_trigger();
   __shared__ float tile[32][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
   const int64_t c0 = (int64_t) blockIdx.x * 32, r0 = (int64_t) blockIdx.y * 32;
+  uint64_t dseed = 0, doff = 0;
+  if constexpr (DROP) {
+    dseed = (uint64_t) drop_rng[0];
+    doff = (uint64_t) drop_rng[1] + (uint64_t) drop_layer;
+  }
 #pragma unroll
   for (int i = 0; i < 32; i += 8) {
     const int64_t r = r0 + ty + i, c = c0 + tx;
     float v = 0.f;
     if (r < R && c < C) {
       v = __ldg(x + r * ld_in + c);
+      if constexpr (DROP)
+        v = b2_drop_keep(dseed, doff, (uint64_t) (r * C + c), drop_thresh) ? __fmul_rn(v, drop_scale) : 0.f;
       if (y != nullptr) {
         const float yv = __ldg(y + r * ld_in + c);
         if (act == B2_ACT_RELU) v = (yv > 0.f) ? v : 0.f;
-        else if (act == B2_ACT_SIGMOID) v = v * ((1.f - yv) * yv);
+        else if (act == B2_ACT_SIGMOID) {
+          const float s = DROP ? __fdiv_rn(yv, drop_scale) : yv;
+          v = v * ((1.f - s) * s);
+        }
         else if (act == B2_PREP_MUL) v = v * yv;
       }
       if (out != nullptr) out[r * C + c] = v;
@@ -756,6 +797,7 @@ prep_operand_kernel(const float* __restrict__ x, const float* __restrict__ y, in
 //   With prev_act != NONE the head's input x IS the previous layer's activation output, so that
 //   layer's activation backward is fused here: gx <- prev_act'(x) * gx (= dZ of the previous layer),
 //   together with its 3xTF32 small part (gx_small) and its bias gradient gb_prev[k] = sum_m gx[m,k].
+//   DROP: the previous layer ends on dropout, x is its dropped output: its mask multiplies gx before prev_act'.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 head_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
@@ -780,13 +822,20 @@ head_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
 }
 
 // CTA = 256 threads = 8 warps; each CTA owns a contiguous block of rows; lane k-strided columns.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ y,
                 const float* __restrict__ gy, int64_t M, int K, int act, int64_t rows_per_cta,
                 float* __restrict__ gx, float* __restrict__ gw, float* __restrict__ gb, int prev_act,
-                float* __restrict__ gx_small, float* __restrict__ gb_prev) {
+                float* __restrict__ gx_small, float* __restrict__ gb_prev,
+                const int64_t* __restrict__ drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale) {
   b2_pdl_wait();
   b2_pdl_trigger();
+  uint64_t dseed = 0, doff = 0;
+  if constexpr (DROP) {
+    dseed = (uint64_t) drop_rng[0];
+    doff = (uint64_t) drop_rng[1] + (uint64_t) drop_layer;
+  }
   extern __shared__ float sgw[];  // K partial sums of gw, then K partial sums of gb_prev
   __shared__ float red[32];
   float* sgp = sgw + K;
@@ -816,8 +865,14 @@ head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
           const float xv = __ldg(x + m * K + k);
           if (gx != nullptr) {
             float val = gz * __ldg(w + k);
+            if constexpr (DROP)
+              val = b2_drop_keep(dseed, doff, (uint64_t) m * (uint64_t) K + (uint64_t) k, drop_thresh)
+                        ? __fmul_rn(val, drop_scale) : 0.f;
             if (prev_act == B2_ACT_RELU) val = (xv > 0.f) ? val : 0.f;
-            else if (prev_act == B2_ACT_SIGMOID) val = val * ((1.f - xv) * xv);
+            else if (prev_act == B2_ACT_SIGMOID) {
+              const float s = DROP ? __fdiv_rn(xv, drop_scale) : xv;
+              val = val * ((1.f - s) * s);
+            }
             gx[m * K + k] = val;
             if (gx_small != nullptr) gx_small[m * K + k] = tf32_small(val);
             cs[j] += val;
@@ -843,6 +898,40 @@ head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
   if (gb != nullptr) {
     const float t = b2_block_sum(gb_acc, red);
     if (threadIdx.x == 0 && t != 0.f) b2_red_add(gb, t);
+  }
+}
+
+// ---------------------------------------------------------------------------------
+// Dropout RNG state and the elementwise mask (philox.cuh).
+//   rng_take: snapshot = state; state.offset += n_layers   (one thread: one per chain forward with dropout)
+//   apply:    y[m, n] = keep(m, n) ? x[m, n] * scale : 0   (one Philox call per element group of 4)
+// ---------------------------------------------------------------------------------
+__global__ void dropout_rng_take_kernel(int64_t* __restrict__ state, int64_t* __restrict__ snapshot, int n_layers) {
+  b2_pdl_wait();
+  b2_pdl_trigger();
+  const int64_t seed = state[0], off = state[1];
+  snapshot[0] = seed;
+  snapshot[1] = off;
+  state[1] = (int64_t) ((uint64_t) off + (uint64_t) n_layers);
+}
+
+__global__ void __launch_bounds__(256)
+dropout_apply_kernel(const float* x, float* y, int64_t M, int64_t N, int64_t ld,     // y may be x (in place)
+                     const int64_t* __restrict__ drop_rng, int64_t drop_layer, uint32_t thresh, float scale) {
+  b2_pdl_wait();
+  b2_pdl_trigger();
+  const uint64_t seed = (uint64_t) drop_rng[0], off = (uint64_t) drop_rng[1] + (uint64_t) drop_layer;
+  const int64_t n_el = M * N, groups = (n_el + 3) >> 2;
+  for (int64_t g = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += (int64_t) gridDim.x * blockDim.x) {
+    const b2_u32x4 r = b2_drop_group(seed, off, (uint64_t) g);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int64_t i = 4 * g + e;
+      if (i < n_el) {
+        const int64_t m = i / N, o = m * ld + (i - m * N);
+        y[o] = r.v[e] < thresh ? __fmul_rn(x[o], scale) : 0.f;
+      }
+    }
   }
 }
 }  // namespace tc
@@ -905,9 +994,9 @@ extern "C" B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const fl
 
 // plan != NULL: fill in the launch plan (tile shape, ring depths, shared memory) and return without
 // touching the device — pure host arithmetic, so the CPU test-suite can sweep it (tests/test_abi.py).
-template <int BN, int MODE>
+template <int BN, int MODE, bool DROP>
 static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
-  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE>;
+  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE, DROP>;
   // opt-in to > 48 KB of dynamic shared memory, for the largest ring this instantiation launches with: an
   // idempotent per-process property (C++11 guarantees the initialiser runs once, thread-safely)
   static const cudaError_t attr_rc =
@@ -919,20 +1008,25 @@ static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
   return B2_OK;
 }
 
-// One kernel instantiation per tile width and arithmetic mode (tf32 and bf16 single pass, 3xTF32 up to bn = 64).
+// One kernel instantiation per tile width and arithmetic mode (tf32 and bf16 single pass, 3xTF32 up to bn = 64),
+// and per dropout: a launch with a dropout mask in its epilogue runs the DROP twin of its instantiation.
 typedef int (*GemmLaunch)(const tc::Params&, int, cudaStream_t);
-static GemmLaunch gemm_inst(int bn, int mode) {
+template <bool DROP>
+static GemmLaunch gemm_inst_t(int bn, int mode) {
   switch (bn * 4 + mode) {
-    case 32 * 4 + tc::TF32: return gemm_launch<32, tc::TF32>;
-    case 64 * 4 + tc::TF32: return gemm_launch<64, tc::TF32>;
-    case 128 * 4 + tc::TF32: return gemm_launch<128, tc::TF32>;
-    case 32 * 4 + tc::BF16: return gemm_launch<32, tc::BF16>;
-    case 64 * 4 + tc::BF16: return gemm_launch<64, tc::BF16>;
-    case 128 * 4 + tc::BF16: return gemm_launch<128, tc::BF16>;
-    case 32 * 4 + tc::X3: return gemm_launch<32, tc::X3>;
-    case 64 * 4 + tc::X3: return gemm_launch<64, tc::X3>;
+    case 32 * 4 + tc::TF32: return gemm_launch<32, tc::TF32, DROP>;
+    case 64 * 4 + tc::TF32: return gemm_launch<64, tc::TF32, DROP>;
+    case 128 * 4 + tc::TF32: return gemm_launch<128, tc::TF32, DROP>;
+    case 32 * 4 + tc::BF16: return gemm_launch<32, tc::BF16, DROP>;
+    case 64 * 4 + tc::BF16: return gemm_launch<64, tc::BF16, DROP>;
+    case 128 * 4 + tc::BF16: return gemm_launch<128, tc::BF16, DROP>;
+    case 32 * 4 + tc::X3: return gemm_launch<32, tc::X3, DROP>;
+    case 64 * 4 + tc::X3: return gemm_launch<64, tc::X3, DROP>;
     default: return nullptr;
   }
+}
+static GemmLaunch gemm_inst(int bn, int mode, bool drop) {
+  return drop ? gemm_inst_t<true>(bn, mode) : gemm_inst_t<false>(bn, mode);
 }
 
 static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan) {
@@ -957,6 +1051,9 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   const bool three_pass = inline_split || d->a_small != nullptr;
   const int64_t ld_aux = d->ld_aux > 0 ? d->ld_aux : ldc;
   B2_REQUIRE(d->c_small == nullptr || ld_aux >= N, "ld_aux too small");
+  const bool drop = d->drop_rng != nullptr;
+  B2_REQUIRE(!drop || (d->drop_scale > 0.f && d->drop_scale < 3.0e38f && d->drop_layer >= 0),
+             "dropout needs a positive finite scale and a layer index >= 0");
   if (!tma_ok_e(a, lda, esz) || !tma_ok_e(b, ldb, esz) ||
       (d->a_small != nullptr && !(tma_ok(d->a_small, lda) && tma_ok(d->b_small, ldb))))
     return b2_fail(B2_E_UNSUPPORTED, "operands are not TMA-addressable (16-byte base, 16-byte row pitch)");
@@ -969,7 +1066,7 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   const int64_t num_kb = b2_ceil_div(K, bke);
   // split-K adds partial tiles with red.global: only for a plain linear epilogue
   const bool linear = (d->act == B2_ACT_NONE && d->mul == nullptr && d->add == nullptr && d->ybwd == nullptr &&
-                       d->c_small == nullptr && d->c_pre == nullptr && d->colsum == nullptr);
+                       d->c_small == nullptr && d->c_pre == nullptr && d->colsum == nullptr && !drop);
   const bool backfill = (d->flags & B2_GEMM_BACKFILL) != 0;
   int best_bn = 0, best_split = 1;
   double best_cost = 1e300;
@@ -1020,6 +1117,7 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   p.M = (int) M; p.N = (int) N; p.K = (int) K; p.act = d->act; p.act_bwd = d->act_bwd; p.esz = esz;
   p.a_mn = d->a_mn_major ? 1 : 0; p.b_mn = d->b_mn_major ? 1 : 0;
   p.beta = d->beta_accumulate ? 1 : 0;
+  p.drop_rng = d->drop_rng; p.drop_layer = d->drop_layer; p.drop_thresh = d->drop_thresh; p.drop_scale = d->drop_scale;
   {
     auto al = [](const void* q, uintptr_t b) { return reinterpret_cast<uintptr_t>(q) % b == 0; };
     p.vec = al(c, 16) && ldc % 4 == 0 && al(d->c_pre, 16) && al(d->bias, 16) && al(d->mul, 16) &&
@@ -1033,7 +1131,7 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   B2_REQUIRE(total_tiles < (1ll << 31), "too many tiles");
   p.tiles_m = (int) tiles_m; p.tiles_n = (int) tiles_n; p.splits = splits;
   const int mode = three_pass ? tc::X3 : (esz == 2 ? tc::BF16 : tc::TF32);
-  const GemmLaunch launch = gemm_inst(best_bn, mode);
+  const GemmLaunch launch = gemm_inst(best_bn, mode, drop);
   B2_REQUIRE(launch != nullptr, "no GEMM instantiation for bn %d", best_bn);
   p.ring = tc::ring_layout(best_bn, mode, p.a_mn != 0, p.b_mn != 0);
   B2_REQUIRE(p.ring.stages >= 2 && p.ring.smem <= tc::SMEM_MAX, "tile does not fit shared memory");
@@ -1122,12 +1220,23 @@ extern "C" B2_API int b2_transpose_f32(const float* in, int64_t rows, int64_t co
   return B2_OK;
 }
 
+// The dropout arguments shared by the entry points that apply a mask: drop_rng == NULL means no dropout.
+static int check_drop(const int64_t* drop_rng, int64_t drop_layer, float drop_scale) {
+  B2_REQUIRE(drop_rng == nullptr || (drop_scale > 0.f && drop_scale < 3.0e38f && drop_layer >= 0),
+             "dropout needs a positive finite scale and a layer index >= 0");
+  return B2_OK;
+}
+
 extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, int64_t R, int64_t C,
                                       float* out, float* out_small, float* outT, float* outT_small,
-                                      float* colsum, void* stream) {
+                                      float* colsum, const int64_t* drop_rng, int64_t drop_layer,
+                                      uint32_t drop_thresh, float drop_scale, void* stream) {
   B2_REQUIRE(x != nullptr, "NULL input");
   B2_REQUIRE(R >= 0 && C >= 0, "bad shape");
   B2_REQUIRE((act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID) || act == B2_PREP_MUL, "bad activation code %d", act);
+  B2_REQUIRE(drop_rng == nullptr || act != B2_PREP_MUL, "B2_PREP_MUL takes no dropout mask");
+  const int rc = check_drop(drop_rng, drop_layer, drop_scale);
+  if (rc != B2_OK) return rc;
   cudaStream_t st = (cudaStream_t) stream;
   if (colsum != nullptr) {
     cudaError_t e = cudaMemsetAsync(colsum, 0, sizeof(float) * (size_t) C, st);
@@ -1136,7 +1245,12 @@ extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, i
   if (R == 0 || C == 0) return B2_OK;
   dim3 grid((unsigned) b2_ceil_div(C, 32), (unsigned) b2_ceil_div(R, 32));
   B2_REQUIRE(grid.y <= 65535, "too many rows for this launch geometry");
-  B2_LAUNCH(tc::prep_operand_kernel, grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT, outT_small, colsum);
+  if (drop_rng != nullptr)
+    B2_LAUNCH(tc::prep_operand_kernel<true>, grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT, outT_small,
+              colsum, drop_rng, drop_layer, drop_thresh, drop_scale);
+  else
+    B2_LAUNCH(tc::prep_operand_kernel<false>, grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT, outT_small,
+              colsum, drop_rng, drop_layer, drop_thresh, drop_scale);
   B2_CUDA_LAUNCH_CHECK("b2_prep_operand");
   return B2_OK;
 }
@@ -1155,18 +1269,24 @@ extern "C" B2_API int b2_head_fwd(const float* x, const float* w, const float* b
 
 extern "C" B2_API int b2_head_bwd(const float* x, const float* w, const float* y, const float* gy, int64_t M,
                                   int K, int act, float* gx, float* gw, float* gb, void* stream) {
-  return b2_head_bwd_ex(x, w, y, gy, M, K, act, gx, gw, gb, B2_ACT_NONE, nullptr, nullptr, 0, stream);
+  return b2_head_bwd_ex(x, w, y, gy, M, K, act, gx, gw, gb, B2_ACT_NONE, nullptr, nullptr, 0, nullptr, 0, 0, 0.f,
+                        stream);
 }
 
 extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float* y, const float* gy, int64_t M,
                                      int K, int act, float* gx, float* gw, float* gb, int prev_act,
-                                     float* gx_small, float* gb_prev, int grads_zeroed, void* stream) {
+                                     float* gx_small, float* gb_prev, int grads_zeroed, const int64_t* prev_drop_rng,
+                                     int64_t prev_drop_layer, uint32_t prev_drop_thresh, float prev_drop_scale,
+                                     void* stream) {
   B2_REQUIRE(x && w && gy && gw, "NULL pointer");
   B2_REQUIRE(K >= 1 && K <= 6144 && act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad K/act");
   B2_REQUIRE(prev_act >= B2_ACT_NONE && prev_act <= B2_ACT_SIGMOID, "bad prev_act");
   B2_REQUIRE(act == B2_ACT_NONE || y != nullptr, "activation backward needs y");
-  B2_REQUIRE(gx != nullptr || (gx_small == nullptr && gb_prev == nullptr && prev_act == B2_ACT_NONE),
-             "prev_act / gx_small / gb_prev need gx");
+  B2_REQUIRE(gx != nullptr || (gx_small == nullptr && gb_prev == nullptr && prev_act == B2_ACT_NONE &&
+                               prev_drop_rng == nullptr),
+             "prev_act / gx_small / gb_prev / a dropout mask need gx");
+  const int rc = check_drop(prev_drop_rng, prev_drop_layer, prev_drop_scale);
+  if (rc != B2_OK) return rc;
   cudaStream_t st = (cudaStream_t) stream;
   cudaError_t e = cudaSuccess;
   if (!grads_zeroed) {    // the caller vouches that gw / gb / gb_prev are all-zero (a gradient arena cleared by Adam)
@@ -1181,8 +1301,38 @@ extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float
   const int64_t rows_per_cta = b2_ceil_div(M, ctas);
   ctas = b2_ceil_div(M, rows_per_cta);
   const float* y_arg = (act == B2_ACT_NONE) ? nullptr : y;
-  B2_LAUNCH(tc::head_bwd_kernel, (int) ctas, 256, 2 * sizeof(float) * (size_t) K, st,
-            x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev);
+  if (prev_drop_rng != nullptr)
+    B2_LAUNCH(tc::head_bwd_kernel<true>, (int) ctas, 256, 2 * sizeof(float) * (size_t) K, st,
+              x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
+              prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
+  else
+    B2_LAUNCH(tc::head_bwd_kernel<false>, (int) ctas, 256, 2 * sizeof(float) * (size_t) K, st,
+              x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
+              prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
   B2_CUDA_LAUNCH_CHECK("b2_head_bwd");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_dropout_rng_take(int64_t* state, int64_t* snapshot, int n_layers, void* stream) {
+  B2_REQUIRE(state && snapshot, "NULL pointer");
+  B2_REQUIRE(n_layers >= 1, "n_layers must be >= 1");
+  B2_LAUNCH(tc::dropout_rng_take_kernel, 1, 1, 0, (cudaStream_t) stream, state, snapshot, n_layers);
+  B2_CUDA_LAUNCH_CHECK("b2_dropout_rng_take");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_dropout_apply(const float* x, float* y, int64_t M, int64_t N, int64_t ld,
+                                       const int64_t* snapshot, int64_t layer, uint32_t thresh, float scale,
+                                       void* stream) {
+  B2_REQUIRE(x && y && snapshot, "NULL pointer");
+  B2_REQUIRE(M >= 0 && N >= 0 && ld >= N, "bad shape");
+  const int rc = check_drop(snapshot, layer, scale);
+  if (rc != B2_OK) return rc;
+  if (M == 0 || N == 0) return B2_OK;
+  int64_t blocks = b2_ceil_div(b2_ceil_div(M * N, 4), 256);
+  if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
+  B2_LAUNCH(tc::dropout_apply_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, x, y, M, N, ld, snapshot, layer,
+            thresh, scale);
+  B2_CUDA_LAUNCH_CHECK("b2_dropout_apply");
   return B2_OK;
 }

@@ -443,12 +443,13 @@ def transpose_f32(t, want_small):
 
 def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=None, act=B2_ACT_NONE,
             mul=None, add=None, ybwd=None, act_bwd=B2_ACT_NONE, out_small=None, colsum=None, accumulate=False,
-            out_pre=None, out_is_zero=False, backfill=False):
+            out_pre=None, out_is_zero=False, backfill=False, drop=None):
     """out (M,N) = epi(sum_k A(m,k) B(n,k)) on the wgmma kernel (b2_gemm_tc_ex).  a is (M,K), or (K,M) when
     a_mn (MN-major: the tensor is consumed as it lies, no transpose); b is (N,K), or (K,N) when b_mn.
     a_small / b_small: the operands' 3xTF32 small parts (both or neither).  Epilogue extras: ybwd/act_bwd
     (activation backward of the gradient's producer), out_small (3xTF32 small part of out), colsum (N).
-    backfill: the launch runs beside a chain of launches on another stream (B2_GEMM_BACKFILL: short split-K CTAs)."""
+    backfill: the launch runs beside a chain of launches on another stream (B2_GEMM_BACKFILL: short split-K CTAs).
+    drop: (snapshot, layer, thresh, scale), the dropout mask of out's (M, N) elements (see dropout_snapshot)."""
     d = _lib.b2_gemm_desc()
     K, M = (a.shape if a_mn else a.shape[::-1])
     K2, N = (b.shape if b_mn else b.shape[::-1])
@@ -490,6 +491,8 @@ def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=
         | (_lib.B2_GEMM_BACKFILL if backfill else 0)
     if a_small is None and not bf16 and _MATMUL["mode"] == "tf32x3" and _MATMUL["x3_inline"]:
         d.flags |= _lib.B2_GEMM_X3_INLINE
+    if drop is not None:
+        d.drop_rng, d.drop_layer, d.drop_thresh, d.drop_scale = drop[0].data_ptr(), drop[1], drop[2], drop[3]
     _lib.call("b2_gemm_tc_ex", ctypes.byref(d), _stream())
     return out
 
@@ -590,17 +593,74 @@ def weight_aux(w):
 
 
 def prep_operand(x, y=None, act=B2_ACT_NONE, want_out=False, want_small=False, want_t=False,
-                 want_t_small=False, colsum=None):
-    """One pass over x (R, C): [act-backward with y] -> out / out_small / out^T / out^T_small / column sums."""
+                 want_t_small=False, colsum=None, drop=None):
+    """One pass over x (R, C): [dropout mask (drop = (snapshot, layer, thresh, scale)), act-backward with y]
+    -> out / out_small / out^T / out^T_small / column sums."""
     R, C = x.shape
     dev = x.device
     out = torch.empty((R, C), dtype=torch.float32, device=dev) if want_out else None
     small = torch.empty((R, C), dtype=torch.float32, device=dev) if want_small else None
     out_t = torch.empty((C, R), dtype=torch.float32, device=dev) if want_t else None
     t_small = torch.empty((C, R), dtype=torch.float32, device=dev) if want_t_small else None
+    snap, layer, thresh, scale = drop if drop is not None else (None, 0, 0, 0.0)
     _lib.call("b2_prep_operand", _ptr(x), _ptr(y), act, R, C, _ptr(out), _ptr(small), _ptr(out_t), _ptr(t_small),
-              _ptr(colsum), _stream())
+              _ptr(colsum), _ptr(snap), layer, thresh, scale, _stream())
     return out, small, out_t, t_small
+
+
+# ---- dropout masks of MLP chains (include/fuxictr_b200.h "Dropout masks", csrc/philox.cuh) -------------------
+# One {seed, offset} int64 pair per device.  Its seed is drawn from torch's generator of that device on first eager
+# use, and drawn again on the first eager use after torch.manual_seed (so seed_everything governs the masks as it
+# governs nn.Dropout).  Every chain forward with dropout snapshots it on the device and advances its offset, so a
+# CUDA graph replay reads and advances the device state: fresh masks every replay, no host value in the graph.
+_DROPOUT = {}       # device -> [state tensor, torch.initial_seed() it was drawn under]
+
+
+def dropout_consts(p):
+    """(thresh, scale) of a dropout probability 0 < p < 1: keep iff the Philox word < thresh; kept x -> x * scale."""
+    if not 0.0 < p < 1.0:
+        raise ValueError("dropout probability must lie in (0, 1), got %r" % (p,))
+    thresh = min(int(round((1.0 - p) * 4294967296.0)), 4294967295)
+    return thresh, float(ctypes.c_float(1.0 / (1.0 - p)).value)
+
+
+def dropout_state(dev):
+    """The device's {seed, offset} state (int64[2]), drawn when absent or torch.manual_seed changed it.  Never
+    drawn inside a CUDA graph capture: an eager forward (TrainPipeline's warm-up steps) must create it first."""
+    dev = torch.device(dev)
+    capturing = dev.type == "cuda" and torch.cuda.is_current_stream_capturing()
+    ent = _DROPOUT.get(dev)
+    seed_now = torch.initial_seed()
+    if ent is not None and (ent[1] == seed_now or capturing):
+        return ent[0]
+    if capturing:
+        raise RuntimeError("the dropout RNG state of %s is created by an eager forward; run one before capturing "
+                           "a CUDA graph" % dev)
+    seed = torch.randint(0, 1 << 62, (1,), dtype=torch.int64, device=dev)
+    state = torch.cat([seed, torch.zeros(1, dtype=torch.int64, device=dev)])
+    _DROPOUT[dev] = [state, seed_now]
+    return state
+
+
+def dropout_snapshot(dev, n_layers):
+    """Snapshot the device's dropout state and advance its offset by n_layers (one launch); layer l of the
+    forward draws its mask at offset snapshot.offset + l."""
+    state = dropout_state(dev)
+    snap = torch.empty(2, dtype=torch.int64, device=state.device)
+    _lib.call("b2_dropout_rng_take", _ptr(state), _ptr(snap), n_layers, _stream())
+    return snap
+
+
+def dropout_apply(x, snap, layer, p, out=None):
+    """out (M, N) = keep ? x * scale : 0 with the mask of layer `layer` of snapshot `snap` (out may be x)."""
+    thresh, scale = dropout_consts(p)
+    M, N = x.shape
+    if out is None:
+        out = torch.empty_like(x)
+    if x.stride(1) != 1 or out.stride() != x.stride():
+        raise ValueError("dropout_apply: x and out must share one row-major layout")
+    _lib.call("b2_dropout_apply", _ptr(x), _ptr(out), M, N, x.stride(0), _ptr(snap), layer, thresh, scale, _stream())
+    return out
 
 
 def _tc_layer_ok(weight):
@@ -756,15 +816,27 @@ class _MLPChain(torch.autograd.Function):
     work can move across layer boundaries: the forward epilogue of layer i writes the 3xTF32 small part
     layer i+1 consumes; the dgrad GEMM of layer i+1 applies layer i's activation backward in its
     epilogue and emits dZ_i, its small part and layer i's bias gradient directly (the N = 1 head does
-    the same in its fused backward).  Launches per 3-hidden-layer MLP step: 15 (was 26)."""
+    the same in its fused backward).  Launches per 3-hidden-layer MLP step: 15 (was 26).
+
+    Dropout (drops: per-layer p, or None): layer i's output is act(z_i) * keep_i * scale_i, the mask applied by
+    whichever launch writes it (the forward epilogue; b2_dropout_apply after a head or SIMT layer), so h_{i+1} holds
+    the dropped value.  The forward takes one snapshot of the dropout state (dropout_snapshot) and keeps it for
+    the backward, which regenerates each mask where it folds that layer's activation backward: the next layer's
+    dgrad epilogue, the head backward, or the explicit pass (b2_prep_operand) at the top or below a SIMT layer."""
 
     @staticmethod
-    def forward(ctx, x, acts, *params):
+    def forward(ctx, x, acts, drops, *params):
         x = _f32c(x)
         M = x.shape[0]
         L = len(acts)
         Ws, bs = params[0::2], params[1::2]
         x3 = _x3_aux()
+        dl = [None] * L                 # per layer: (snapshot, ordinal, thresh, scale) of its dropout, or None
+        n_drop = sum(1 for p in (drops or ()) if p > 0)
+        snap = dropout_snapshot(x.device, n_drop) if n_drop else None
+        for i, p in enumerate(drops or ()):
+            if p > 0:
+                dl[i] = (snap, sum(1 for q in drops[:i] if q > 0)) + dropout_consts(p)
         kinds = []
         for W in Ws:
             if W.shape[0] == 1 and W.is_contiguous():
@@ -786,22 +858,25 @@ class _MLPChain(torch.autograd.Function):
                 _lib.call("b2_head_fwd", _ptr(h), _ptr(W), _ptr(b), M, K, act, _ptr(y), _stream())
             elif kinds[i] == "tc" and h.data_ptr() % 16 == 0:
                 y_small = empty_aux(M, N, x.device) if want_small else None
-                gemm_ex(h, W, y, a_small=smalls[-1], b_small=weight_aux(W), bias=b, act=act, out_small=y_small)
+                gemm_ex(h, W, y, a_small=smalls[-1], b_small=weight_aux(W), bias=b, act=act, out_small=y_small,
+                        drop=dl[i])
             else:
                 kinds[i] = "simt"
                 gemm_f32(h, W, y, b_t=True, bias=b, act=act)
+            if dl[i] is not None and kinds[i] != "tc":
+                dropout_apply(y, snap, dl[i][1], drops[i], out=y)
             if want_small and y_small is None:
                 y_small = make_aux(y)
             hs.append(y)
             smalls.append(y_small)
-        ctx.acts, ctx.kinds, ctx.smalls, ctx.params = acts, kinds, smalls, params
+        ctx.acts, ctx.kinds, ctx.smalls, ctx.params, ctx.dl = acts, kinds, smalls, params, dl
         ctx.save_for_backward(*hs)
         return hs[-1]
 
     @staticmethod
     def backward(ctx, gy):
         hs = ctx.saved_tensors
-        acts, kinds, smalls, params = ctx.acts, ctx.kinds, ctx.smalls, ctx.params
+        acts, kinds, smalls, params, dl = ctx.acts, ctx.kinds, ctx.smalls, ctx.params, ctx.dl
         Ws, bs = params[0::2], params[1::2]
         L = len(acts)
         M = hs[0].shape[0]
@@ -825,15 +900,24 @@ class _MLPChain(torch.autograd.Function):
             gx_small = empty_aux(M, K, dev) if (prev_small and gx is not None) else None
             gb_prev = None
             if kinds[i] == "head":
+                if dl[i] is not None and not g_is_dz:   # a width-1 dropout layer: its mask in the explicit pass
+                    gb = bias_buf(i)
+                    g, _, _, _ = prep_operand(g, y if act != B2_ACT_NONE else None, act, want_out=True, colsum=gb,
+                                              drop=dl[i])
+                    grads[2 * i + 1] = gb
+                    g_is_dz = True
                 gw = _grad_buffer(W, zero=False)
                 gb = None if g_is_dz else bias_buf(i)          # g already dZ_i: activation backward and db_i are done
                 gb_prev = bias_buf(i - 1) if fuse_prev else None
                 fp32_small = gx_small if (gx_small is not None and gx_small.dtype == torch.float32) else None
+                pdrop = dl[i - 1] if fuse_prev else None
                 _lib.call("b2_head_bwd_ex", _ptr(h), _ptr(W), None if g_is_dz else _ptr(y), _ptr(g), M, K,
                           B2_ACT_NONE if g_is_dz else act, _ptr(gx), _ptr(gw), _ptr(gb),
                           acts[i - 1] if fuse_prev else B2_ACT_NONE, _ptr(fp32_small), _ptr(gb_prev),
                           1 if (_is_zeroed(gw) and (gb is None or _is_zeroed(gb))
-                                and (gb_prev is None or _is_zeroed(gb_prev))) else 0, _stream())
+                                and (gb_prev is None or _is_zeroed(gb_prev))) else 0,
+                          *((_ptr(pdrop[0]),) + pdrop[1:] if pdrop is not None else (_ptr(None), 0, 0, 0.0)),
+                          _stream())
                 if gx_small is not None and fp32_small is None:     # bf16 mode: the head kernel emits fp32 only
                     gx_small = make_aux(gx)
                 grads[2 * i] = gw
@@ -846,9 +930,9 @@ class _MLPChain(torch.autograd.Function):
             if not g_is_dz:     # top of the chain (or below a non-fusing layer): one explicit pass over dY
                 gb = bias_buf(i)
                 fused = act != B2_ACT_NONE
-                out, sm, _, _ = prep_operand(g, y if fused else None, act, want_out=fused,
-                                             want_small=x3 and kinds[i] == "tc", colsum=gb)
-                gz, gz_small = (out if fused else g), sm
+                out, sm, _, _ = prep_operand(g, y if fused else None, act, want_out=fused or dl[i] is not None,
+                                             want_small=x3 and kinds[i] == "tc", colsum=gb, drop=dl[i])
+                gz, gz_small = (out if (fused or dl[i] is not None) else g), sm
                 if gz_small is None and kinds[i] == "tc":
                     gz_small = make_aux(gz)          # bf16 mode (None for single-pass TF32)
                 grads[2 * i + 1] = gb
@@ -863,7 +947,8 @@ class _MLPChain(torch.autograd.Function):
                     gb_prev = bias_buf(i - 1) if fuse_prev else None
                     gemm_ex(gz, W, gx, b_mn=True, a_small=gz_small, b_small=weight_aux(W),
                             ybwd=hs[i] if (fuse_prev and prev_act != B2_ACT_NONE) else None, act_bwd=prev_act,
-                            out_small=gx_small, colsum=gb_prev)                                   # dX (= dZ_{i-1})
+                            out_small=gx_small, colsum=gb_prev,
+                            drop=dl[i - 1] if fuse_prev else None)                                # dX (= dZ_{i-1})
                 if W.requires_grad:
                     gw = _grad_buffer(W, zero=False)
                     if ready is not None:
@@ -886,7 +971,7 @@ class _MLPChain(torch.autograd.Function):
                 grads[2 * (i - 1) + 1] = gb_prev
         if fork is not None:
             fork.join()
-        return (g if ctx.needs_input_grad[0] else None, None) + tuple(grads)
+        return (g if ctx.needs_input_grad[0] else None, None, None) + tuple(grads)
 
 
 class _CrossV2Layer(torch.autograd.Function):
@@ -950,17 +1035,25 @@ def mlp_chain_supported():
 
 
 def mlp_chain(x, layers):
-    """layers: list of (weight, bias or None, act code).  Returns act_L(...act_0(x W_0^T + b_0)...)."""
+    """layers: list of (weight, bias or None, act code[, dropout p]).  Returns h_L with
+    h_{i+1} = dropout_{p_i}(act_i(h_i W_i^T + b_i)), h_0 = x; p = 0 (or absent) is no dropout, else 0 < p < 1
+    (training-mode nn.Dropout: a fresh mask every forward, see dropout_state)."""
     _require_cuda(x)
-    acts = tuple(a for _, _, a in layers)
+    acts = tuple(layer[2] for layer in layers)
+    drops = tuple(float(layer[3]) if len(layer) > 3 and layer[3] else 0.0 for layer in layers)
+    for p in drops:
+        if p:
+            dropout_consts(p)           # raises outside (0, 1)
+    drops = drops if any(drops) else None
     flat = []
-    for w, b, _ in layers:
+    for layer in layers:
+        w, b = layer[0], layer[1]
         _require_cuda(w, b)
         flat += [w, b]
     if x.dim() != 2:
         lead = x.shape[:-1]
-        return _MLPChain.apply(x.reshape(-1, x.shape[-1]), acts, *flat).view(*lead, -1)
-    return _MLPChain.apply(x, acts, *flat)
+        return _MLPChain.apply(x.reshape(-1, x.shape[-1]), acts, drops, *flat).view(*lead, -1)
+    return _MLPChain.apply(x, acts, drops, *flat)
 
 
 def linear_act(x, weight, bias=None, act=B2_ACT_NONE):

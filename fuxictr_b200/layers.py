@@ -556,24 +556,38 @@ class MLP_Block(nn.Module):
             stack.append(get_activation(output_activation))
         self.mlp = nn.Sequential(*stack)
 
+    def chain_layers(self):
+        """The stack as F2.mlp_chain layers when it is Linear -> [ReLU|Sigmoid] -> [Dropout(0 < p < 1)] throughout,
+        else None.  A Dropout in training mode passes its p to the chain (the mask of the chain's epilogues); in
+        eval mode it is the identity and the plain chain runs."""
+        mods = list(self.mlp)
+        layers, i = [], 0
+        while i < len(mods):
+            if type(mods[i]) != nn.Linear:
+                return None
+            act = B2_ACT_NONE
+            if i + 1 < len(mods) and type(mods[i + 1]) == nn.ReLU:
+                act = B2_ACT_RELU
+            elif i + 1 < len(mods) and type(mods[i + 1]) == nn.Sigmoid:
+                act = B2_ACT_SIGMOID
+            layer = (mods[i].weight, mods[i].bias, act)
+            i += 2 if act != B2_ACT_NONE else 1
+            if i < len(mods) and type(mods[i]) == nn.Dropout:
+                if not 0.0 < mods[i].p < 1.0:
+                    return None
+                if mods[i].training:
+                    layer += (mods[i].p,)
+                i += 1
+            layers.append(layer)
+        return layers or None
+
     def forward(self, inputs):
         mods = list(self.mlp)
         x = inputs
         if F2.mlp_chain_supported() and inputs.is_cuda:
-            # a pure Linear(+ReLU/Sigmoid) stack runs as ONE autograd node (cross-layer epilogue fusion)
-            layers, i, pure = [], 0, len(mods) > 0
-            while i < len(mods):
-                if type(mods[i]) != nn.Linear:
-                    pure = False
-                    break
-                act = B2_ACT_NONE
-                if i + 1 < len(mods) and type(mods[i + 1]) == nn.ReLU:
-                    act = B2_ACT_RELU
-                elif i + 1 < len(mods) and type(mods[i + 1]) == nn.Sigmoid:
-                    act = B2_ACT_SIGMOID
-                layers.append((mods[i].weight, mods[i].bias, act))
-                i += 2 if act != B2_ACT_NONE else 1
-            if pure:
+            # such a stack runs as ONE autograd node (cross-layer epilogue fusion)
+            layers = self.chain_layers()
+            if layers is not None:
                 return F2.mlp_chain(x, layers)
         i = 0
         while i < len(mods):

@@ -511,6 +511,15 @@ typedef struct b2_gemm_desc {
   int32_t elem_dtype;     /* B2_F32 (wgmma .tf32 passes on fp32) or B2_BF16 (wgmma .bf16, fp32 accumulation) */
   int64_t ld_aux;         /* leading dimension of c_small (0 = ldc) */
   int64_t flags;          /* B2_GEMM_*: the caller vouches an output is already all-zero (skips its memset) */
+  /* Dropout (see "Dropout masks" below); drop_rng == NULL (a zeroed descriptor): no mask.  The mask of the
+   * (M, N) output is applied after act and before act_bwd:  v = act(v) * keep * drop_scale  in a forward,
+   * v = act_bwd'(ybwd) * keep * drop_scale * v  in a dgrad that folds a dropout layer's backward (ybwd is then
+   * that layer's DROPPED output; sigmoid's s is recovered as ybwd / drop_scale).  c_small and colsum see the
+   * masked value.  A launch with a mask is never split over K. */
+  const int64_t* drop_rng; /* device {seed, offset} snapshot of the forward (b2_dropout_rng_take) */
+  int64_t drop_layer;     /* the mask's counter offset: snapshot offset + drop_layer */
+  uint32_t drop_thresh;   /* keep iff the element's Philox word < drop_thresh */
+  float drop_scale;       /* 1 / (1 - p) */
 } b2_gemm_desc;
 #define B2_GEMM_C_IS_ZERO 1      /* split-K accumulates into C with red.global: C needs no clearing */
 #define B2_GEMM_COLSUM_IS_ZERO 2
@@ -542,9 +551,14 @@ B2_API int b2_transpose_f32(const float* in, int64_t rows, int64_t cols, int64_t
  *   act == B2_PREP_MUL: v = x * y
  *   out (R,C) = v, out_small = 3xTF32 small part, outT (C,R) = v^T, outT_small, colsum[c] = sum_r v[r,c]
  * Every output may be NULL.  Replaces b2_act_bwd + b2_transpose_f32 + b2_split_tf32 + b2_colsum.
+ * drop_rng != NULL: x is the gradient of a dropout layer's output and y (if any) that DROPPED output:
+ *   v = act'(y) * keep * drop_scale * x  with the mask of (R, C) at counter offset snapshot offset + drop_layer
+ *   (not with B2_PREP_MUL).  drop_rng == NULL: no mask, the other drop arguments are ignored.
  */
 B2_API int b2_prep_operand(const float* x, const float* y, int act, int64_t R, int64_t C, float* out,
-                           float* out_small, float* outT, float* outT_small, float* colsum, void* stream);
+                           float* out_small, float* outT, float* outT_small, float* colsum,
+                           const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale,
+                           void* stream);
 /*
  * The N = 1 output head of MLP_Block (Linear(K, 1), mlp_block.py:82): warp-per-row GEMV forward,
  * y[m] = act(<x[m,:], w> + b); and one fused backward: gz = act'(y)*gy, gx[m,:] = gz[m]*w (gx may
@@ -557,10 +571,29 @@ B2_API int b2_head_bwd(const float* x, const float* w, const float* y, const flo
 /* Same, fused with the activation backward of the layer that PRODUCED x (x is that layer's
  * activation output, mlp_block.py:78-80): gx <- prev_act'(x) * gx, gx_small = its 3xTF32 small part
  * (or NULL), gb_prev (K) = sum_m gx[m,:] = that layer's bias gradient (or NULL).  grads_zeroed != 0: the
- * caller vouches gw, gb and gb_prev are already all-zero (a gradient arena cleared by the optimizer pass). */
+ * caller vouches gw, gb and gb_prev are already all-zero (a gradient arena cleared by the optimizer pass).
+ * prev_drop_rng != NULL: that layer ends on dropout and x is its dropped output; its (M, K) mask multiplies gx
+ * before prev_act' (gx <- prev_act'(x) * keep * prev_drop_scale * gx), as in b2_gemm_desc. */
 B2_API int b2_head_bwd_ex(const float* x, const float* w, const float* y, const float* gy, int64_t M, int K,
                           int act, float* gx, float* gw, float* gb, int prev_act, float* gx_small,
-                          float* gb_prev, int grads_zeroed, void* stream);
+                          float* gb_prev, int grads_zeroed, const int64_t* prev_drop_rng, int64_t prev_drop_layer,
+                          uint32_t prev_drop_thresh, float prev_drop_scale, void* stream);
+
+/*
+ * Dropout masks (nn.Dropout of MLP_Block, mlp_block.py:80: y = x * keep / (1 - p), keep ~ Bernoulli(1 - p)).
+ * The mask is a pure function of a device {seed, offset} pair (int64 each) and the element:
+ *   i = m * N + n  (the element of the (M, N) layer output, 64-bit);  off = snapshot offset + layer;
+ *   r = Philox4x32-10(counter = {lo32(i >> 2), hi32(i >> 2), lo32(off), hi32(off)}, key = {lo32(seed), hi32(seed)});
+ *   keep  <=>  r[i & 3] < thresh,  thresh = min(round((1 - p) * 2^32), 2^32 - 1);  scale = fp32(1 / (1 - p)).
+ * A kept element is x * scale (one fp32 multiply), a dropped one is 0.
+ * b2_dropout_rng_take: snapshot = state, then state.offset += n_layers (one single-thread launch per forward of
+ *   a chain with n_layers dropout layers, which use offsets snapshot.offset + 0 .. n_layers - 1): no two
+ *   (forward, layer, element group) share a counter, and a CUDA graph replay draws fresh masks.
+ * b2_dropout_apply: y = keep ? x * scale : 0 over (M, N) with leading dimension ld (x and y; y may be x).
+ */
+B2_API int b2_dropout_rng_take(int64_t* state, int64_t* snapshot, int n_layers, void* stream);
+B2_API int b2_dropout_apply(const float* x, float* y, int64_t M, int64_t N, int64_t ld, const int64_t* snapshot,
+                            int64_t layer, uint32_t thresh, float scale, void* stream);
 /* Elementwise helpers used by the dense backward.
  * b2_act_bwd: gx = gy * act'(y) where y is the activation OUTPUT (relu, sigmoid). */
 B2_API int b2_act_bwd(const float* y, const float* gy, float* gx, int64_t n, int act, void* stream);
