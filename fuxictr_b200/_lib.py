@@ -120,6 +120,10 @@ SIGNATURES = {
                                   c_void_p]),
     "b2_shard_publish_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, _FIELD_P, _FIELD_P, c_int, c_int, c_int,
                                      c_void_p, c_void_p]),
+    "b2_shard_publish_rows": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p, _FIELD_P, _FIELD_P, c_int,
+                                      c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_shard_lookup": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_peer_bcast": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "b2_peer_bcast_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "b2_front_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,

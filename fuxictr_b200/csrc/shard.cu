@@ -61,14 +61,17 @@ constexpr int SERVE_U = 4;       // list entries a lane group serves at once (lo
 // LAZY: the tables are lazily evaluated (b2_lazy_ctx); ALL_LEN1: every field is one slot (no slot ->
 // field search) — separate instantiations, so that the plain categorical push keeps its register budget
 // (and occupancy).
-template <typename IdxT, bool LAZY, bool ALL_LEN1>
+// RAGGED (the evaluation lookup, b2_shard_lookup): requester p has rows_all[p] <= batch_local samples this
+// round, so the candidates of samples b >= rows_all[p] are skipped; it runs without an owned list and lazy
+// context, and the training instantiations (RAGGED = false) never read rows_all.
+template <typename IdxT, bool LAZY, bool ALL_LEN1, bool RAGGED>
 __global__ void __launch_bounds__(256)
 shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant__ B2FieldPack lr,
                   const __grid_constant__ PeerPtrs peers, const __grid_constant__ b2_lazy_ctx lz,
                   int64_t batch_local, int64_t ids_stride,
                   int dim, int lpr_log2, int has_lr, int world, int rank,
                   int32_t* __restrict__ status, int4* __restrict__ owned, int32_t* __restrict__ owned_count,
-                  int32_t owned_cap, const float* __restrict__ pad_rows) {
+                  int32_t owned_cap, const float* __restrict__ pad_rows, const int32_t* __restrict__ rows_all) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const SmemFields sf = b2_stage_fields(emb, smem_raw);
   SmemFields lf;
@@ -95,7 +98,7 @@ shard_push_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
     const int64_t item = base + threadIdx.x;
     int4 entry = make_int4(0, 0, 0, 0);
     int kind = 0;                       // 1: goes on the owned list (front), 2: served only (back)
-    if (item < nitems) {
+    if (item < nitems && (!RAGGED || (item % per_rank) / S < (int64_t) __ldg(rows_all + item / per_rank))) {
       const int p = (int) (item / per_rank);           // requesting rank
       const int64_t rem = item - (int64_t) p * per_rank;
       const int64_t b = rem / S;
@@ -332,9 +335,8 @@ struct PadDst { float* p[16]; };
 // into every rank's pad buffer, (F, D) rows then F weights, so that every rank fills its own padding slots in
 // the push.  The push that reads them comes after the barrier that follows this launch.
 template <typename IdxT>
-__global__ void __launch_bounds__(256)
-shard_publish_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world,
-                         const __grid_constant__ PadSrc ps, const __grid_constant__ PadDst pd, int nfields, int dim) {
+__device__ __forceinline__ void publish_ids_pad(const void* __restrict__ src, int64_t n, const BcastDst& dst,
+                                                int world, const PadSrc& ps, const PadDst& pd, int nfields, int dim) {
   bcast_ids<IdxT>(src, n, dst, world);
   const int64_t tid = (int64_t) blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t) gridDim.x * blockDim.x;
   const int64_t nemb = (int64_t) nfields * dim, npad = nemb + nfields;
@@ -350,6 +352,27 @@ shard_publish_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_c
     const float v = *s;
     for (int p = 0; p < world; ++p) pd.p[p][i] = v;
   }
+}
+
+template <typename IdxT>
+__global__ void __launch_bounds__(256)
+shard_publish_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world,
+                         const __grid_constant__ PadSrc ps, const __grid_constant__ PadDst pd, int nfields, int dim) {
+  publish_ids_pad<IdxT>(src, n, dst, world, ps, pd, nfields, dim);
+}
+
+struct RowsDst { int32_t* p[16]; };
+
+// The evaluation round's exchange: the first `rows` rows of the batch matrix (n = rows * width ids), the padding
+// rows, and the row count itself into word `rank` of every peer's rows_all — the bound of the lookup that follows
+// the barrier.
+template <typename IdxT>
+__global__ void __launch_bounds__(256)
+shard_publish_rows_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world,
+                          const __grid_constant__ PadSrc ps, const __grid_constant__ PadDst pd, int nfields, int dim,
+                          const __grid_constant__ RowsDst rd, int rank, int32_t rows) {
+  publish_ids_pad<IdxT>(src, n, dst, world, ps, pd, nfields, dim);
+  if (blockIdx.x == 0 && (int) threadIdx.x < world) rd.p[threadIdx.x][rank] = rows;
 }
 
 // After the push: logit[b] = [0.5*sum_d((sum_f e)^2 - sum_f e^2)] + [sum_f lrw[b,f] + bias]; sums[b,:] = sum_f e.
@@ -476,16 +499,44 @@ int check_shard_args(const b2_field* emb, const b2_field* lr, int nfields, int w
   return B2_OK;
 }
 
-template <typename IdxT, bool LAZY, typename... Args>
+template <typename IdxT, bool LAZY, bool RAGGED, typename... Args>
 void launch_push_len(bool all_len1, int grid, size_t smem, cudaStream_t st, Args... args) {
-  if (all_len1) shard_push_kernel<IdxT, LAZY, true><<<grid, 256, smem, st>>>(args...);
-  else shard_push_kernel<IdxT, LAZY, false><<<grid, 256, smem, st>>>(args...);
+  if (all_len1) shard_push_kernel<IdxT, LAZY, true, RAGGED><<<grid, 256, smem, st>>>(args...);
+  else shard_push_kernel<IdxT, LAZY, false, RAGGED><<<grid, 256, smem, st>>>(args...);
 }
 
 template <typename IdxT, typename... Args>
 int launch_push(bool lazy, bool all_len1, int grid, size_t smem, cudaStream_t st, Args... args) {
-  if (lazy) launch_push_len<IdxT, true>(all_len1, grid, smem, st, args...);
-  else launch_push_len<IdxT, false>(all_len1, grid, smem, st, args...);
+  const int32_t* no_rows = nullptr;      // the training push serves full batches
+  if (lazy) launch_push_len<IdxT, true, false>(all_len1, grid, smem, st, args..., no_rows);
+  else launch_push_len<IdxT, false, false>(all_len1, grid, smem, st, args..., no_rows);
+  return B2_OK;
+}
+
+// The publish launches' destinations and the padding rows this rank owns (both publish entry points).
+int publish_setup(int32_t* const* peer_dst, const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                  int world, int rank, float* const* peer_pad, BcastDst& d, PadDst& pd, PadSrc& ps) {
+  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
+  if (rc != B2_OK) return rc;
+  for (int i = 0; i < 16; ++i) { d.p[i] = nullptr; pd.p[i] = nullptr; }
+  for (int i = 0; i < world; ++i) {
+    B2_REQUIRE(peer_dst[i] != nullptr && ((uintptr_t) peer_dst[i] % 16) == 0, "peer_dst[%d] NULL or misaligned", i);
+    B2_REQUIRE(peer_pad[i] != nullptr && ((uintptr_t) peer_pad[i] % 16) == 0, "peer_pad[%d] NULL or misaligned", i);
+    d.p[i] = peer_dst[i];
+    pd.p[i] = peer_pad[i];
+  }
+  const int dim = emb_fields[0].dim;
+  for (int f = 0; f < nfields; ++f) {
+    ps.e[f] = nullptr;
+    ps.l[f] = nullptr;
+    const int64_t pad = emb_fields[f].padding_idx;
+    if (pad < 0 || pad >= emb_fields[f].vocab || (int) (pad % world) != rank) continue;     // not mine
+    if (emb_fields[f].table != nullptr) ps.e[f] = reinterpret_cast<const float*>(emb_fields[f].table) + (pad / world) * dim;
+    if (lr_fields != nullptr) {
+      B2_REQUIRE(lr_fields[f].padding_idx == pad, "field %d: the LR and embedding tables need one padding row", f);
+      if (lr_fields[f].table != nullptr) ps.l[f] = reinterpret_cast<const float*>(lr_fields[f].table) + pad / world;
+    }
+  }
   return B2_OK;
 }
 
@@ -650,30 +701,12 @@ extern "C" B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64
                                            const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
                                            int world, int rank, float* const* peer_pad, void* stream) {
   B2_REQUIRE(src && peer_dst && peer_pad && count >= 0, "bad argument");
-  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
-  if (rc != B2_OK) return rc;
   BcastDst d;
   PadDst pd;
-  for (int i = 0; i < 16; ++i) { d.p[i] = nullptr; pd.p[i] = nullptr; }
-  for (int i = 0; i < world; ++i) {
-    B2_REQUIRE(peer_dst[i] != nullptr && ((uintptr_t) peer_dst[i] % 16) == 0, "peer_dst[%d] NULL or misaligned", i);
-    B2_REQUIRE(peer_pad[i] != nullptr && ((uintptr_t) peer_pad[i] % 16) == 0, "peer_pad[%d] NULL or misaligned", i);
-    d.p[i] = peer_dst[i];
-    pd.p[i] = peer_pad[i];
-  }
-  const int dim = emb_fields[0].dim;
   static thread_local PadSrc ps;
-  for (int f = 0; f < nfields; ++f) {
-    ps.e[f] = nullptr;
-    ps.l[f] = nullptr;
-    const int64_t pad = emb_fields[f].padding_idx;
-    if (pad < 0 || pad >= emb_fields[f].vocab || (int) (pad % world) != rank) continue;     // not mine
-    if (emb_fields[f].table != nullptr) ps.e[f] = reinterpret_cast<const float*>(emb_fields[f].table) + (pad / world) * dim;
-    if (lr_fields != nullptr) {
-      B2_REQUIRE(lr_fields[f].padding_idx == pad, "field %d: the LR and embedding tables need one padding row", f);
-      if (lr_fields[f].table != nullptr) ps.l[f] = reinterpret_cast<const float*>(lr_fields[f].table) + pad / world;
-    }
-  }
+  int rc = publish_setup(peer_dst, emb_fields, lr_fields, nfields, world, rank, peer_pad, d, pd, ps);
+  if (rc != B2_OK) return rc;
+  const int dim = emb_fields[0].dim;
   const int64_t npad = (int64_t) nfields * (dim + 1);
   const int grid = grid_for((count >> 2) > npad ? (count >> 2) : npad, 256);
   cudaStream_t st = (cudaStream_t) stream;
@@ -684,6 +717,90 @@ extern "C" B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
   B2_CUDA_LAUNCH_CHECK("b2_shard_publish_ids");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_shard_publish_rows(const void* src, int idx_dtype, int64_t rows, int64_t width,
+                                            int64_t capacity_rows, int32_t* const* peer_dst,
+                                            const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                            int world, int rank, float* const* peer_pad, int32_t* const* peer_rows,
+                                            void* stream) {
+  B2_REQUIRE(peer_dst && peer_pad && peer_rows, "NULL peer pointer array");
+  B2_REQUIRE(capacity_rows >= 0 && capacity_rows < (1ll << 31), "capacity_rows %lld outside [0, 2^31)",
+             (long long) capacity_rows);
+  B2_REQUIRE(rows >= 0 && rows <= capacity_rows, "rows %lld outside [0, capacity_rows = %lld]", (long long) rows,
+             (long long) capacity_rows);
+  B2_REQUIRE(width >= 1, "width %lld < 1", (long long) width);
+  B2_REQUIRE(src != nullptr || rows == 0, "src is NULL");
+  BcastDst d;
+  PadDst pd;
+  RowsDst rd;
+  static thread_local PadSrc ps;
+  int rc = publish_setup(peer_dst, emb_fields, lr_fields, nfields, world, rank, peer_pad, d, pd, ps);
+  if (rc != B2_OK) return rc;
+  for (int i = 0; i < 16; ++i) rd.p[i] = nullptr;
+  for (int i = 0; i < world; ++i) {
+    B2_REQUIRE(peer_rows[i] != nullptr && ((uintptr_t) peer_rows[i] % 4) == 0, "peer_rows[%d] NULL or misaligned", i);
+    rd.p[i] = peer_rows[i];
+  }
+  const int dim = emb_fields[0].dim;
+  const int64_t count = rows * width;
+  const int64_t npad = (int64_t) nfields * (dim + 1);
+  const int grid = grid_for((count >> 2) > npad ? (count >> 2) : npad, 256);
+  cudaStream_t st = (cudaStream_t) stream;
+  const int32_t r32 = (int32_t) rows;
+  switch (idx_dtype) {
+    case B2_F64: shard_publish_rows_kernel<double><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim, rd, rank, r32); break;
+    case B2_I64: shard_publish_rows_kernel<int64_t><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim, rd, rank, r32); break;
+    case B2_I32: shard_publish_rows_kernel<int32_t><<<grid, 256, 0, st>>>(src, count, d, world, ps, pd, nfields, dim, rd, rank, r32); break;
+    default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
+  }
+  B2_CUDA_LAUNCH_CHECK("b2_shard_publish_rows");
+  return B2_OK;
+}
+
+extern "C" B2_API int b2_shard_lookup(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                      int64_t batch_local, int world, int rank, const int32_t* const* peer_ids,
+                                      int64_t ids_stride, float* const* peer_emb, float* const* peer_lrw,
+                                      const int32_t* rows_all, int32_t* status, const float* pad_rows, void* stream) {
+  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
+  if (rc != B2_OK) return rc;
+  B2_REQUIRE(peer_ids && peer_emb && (lr_fields == nullptr || peer_lrw != nullptr), "NULL peer pointer array");
+  B2_REQUIRE(rows_all != nullptr, "rows_all is NULL");
+  B2_REQUIRE(batch_local >= 0, "batch_local %lld < 0", (long long) batch_local);
+  B2_REQUIRE(ids_stride >= 1, "ids_stride %lld < 1", (long long) ids_stride);
+  B2_REQUIRE(pad_rows == nullptr || ((uintptr_t) pad_rows % 16) == 0, "pad_rows must be 16-byte aligned");
+  if (pad_rows != nullptr && lr_fields != nullptr)
+    for (int i = 0; i < nfields; ++i)
+      B2_REQUIRE(lr_fields[i].padding_idx == emb_fields[i].padding_idx,
+                 "field %d: the LR and embedding tables need one padding row", i);
+  for (int i = 0; i < world; ++i)
+    B2_REQUIRE(peer_ids[i] && peer_emb[i] && (lr_fields == nullptr || peer_lrw[i]), "peer %d: NULL buffer", i);
+  const int64_t nslots = count_slots(emb_fields, nfields);
+  B2_REQUIRE(batch_local * nslots < (1ll << 31), "batch_local * slots must fit 31 bits");
+  if (batch_local == 0) return B2_OK;
+  static thread_local B2FieldPack epack, lpack;
+  fill_pack_cols(epack, emb_fields, nfields);
+  const int has_lr = lr_fields != nullptr;
+  if (has_lr) fill_pack_cols(lpack, lr_fields, nfields); else lpack.nfields = 0;
+  PeerPtrs pp;
+  for (int i = 0; i < world; ++i) {
+    pp.ids[i] = peer_ids[i];
+    pp.emb[i] = peer_emb[i];
+    pp.lrw[i] = has_lr ? peer_lrw[i] : nullptr;
+    pp.gemb[i] = nullptr;
+    pp.glogit[i] = nullptr;
+  }
+  const int dim = emb_fields[0].dim;
+  const int lpr_log2 = next_pow2_log2((dim + 3) / 4);
+  const size_t smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
+  // the grid covers every candidate of a full round; the samples past rows_all[p] drop out in the scan
+  const int grid = grid_for(batch_local * nslots * world, 256);
+  static thread_local b2_lazy_ctx lz_none;
+  launch_push_len<int32_t, false, true>(epack.all_len1 != 0, grid, smem, (cudaStream_t) stream, epack, lpack, pp,
+                                        lz_none, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status,
+                                        (int4*) nullptr, (int32_t*) nullptr, (int32_t) 0, pad_rows, rows_all);
+  B2_CUDA_LAUNCH_CHECK("b2_shard_lookup");
   return B2_OK;
 }
 

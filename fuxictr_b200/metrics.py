@@ -19,7 +19,7 @@ from . import functional as F2
 _DEVICE_METRICS = ("logloss", "binary_crossentropy", "AUC")
 
 
-def _check_metrics(metrics):
+def check_metrics(metrics):
     for m in metrics:
         if m in _DEVICE_METRICS:
             continue
@@ -31,7 +31,14 @@ def _check_metrics(metrics):
 
 def evaluate_metrics(y_true, y_pred, metrics, group_id=None):
     """Same signature and return type as fuxictr.metrics.evaluate_metrics, on fp32 CUDA tensors."""
-    _check_metrics(metrics)
+    check_metrics(metrics)
+    words = metric_words(y_true, y_pred, metrics)
+    return metrics_from_words(words.cpu(), y_pred.numel(), metrics)     # the one D2H of the evaluation
+
+
+def metric_words(y_true, y_pred, metrics):
+    """The 48-byte result of the metric kernels, on the device: int64 [0:5] the b2_auc words (n_neg, n_pos,
+    n_nan, n_bad, 2U), [5] the fp64 logloss sum's bits.  Small enough to hand to other ranks as it is."""
     F2._require_cuda(y_pred, y_true)
     y_pred = F2._f32c(y_pred.detach().reshape(-1))
     y_true = F2._f32c(y_true.detach().reshape(-1))
@@ -53,7 +60,11 @@ def evaluate_metrics(y_true, y_pred, metrics, group_id=None):
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=y_pred.device)   # caching allocator: 512-byte aligned
         _lib.call("b2_auc", F2._ptr(y_pred), F2._ptr(y_true), n, F2._ptr(ws), nbytes.value, F2._ptr(out),
                   F2._stream())
-    host = out.cpu()                                                   # the one D2H of the evaluation
+    return out
+
+
+def metrics_from_words(host, n, metrics):
+    """metric_words (copied to the host) of n predictions -> the reference's OrderedDict of metrics."""
     n_neg, n_pos, n_nan, n_bad, twice_u = (int(v) for v in host[:5])
     result = OrderedDict()
     for m in metrics:

@@ -61,6 +61,11 @@ class PeerGroup(object):
         """buf <- sum over the ranks of buf (in place, on the current stream)."""
         raise NotImplementedError
 
+    def gather(self, tensors):
+        """Every rank's 1-D CUDA tensors, in rank order: [[rank 0's tensors[i], rank 1's, ...] for each i].  The
+        tensors of one rank are equally long; the length may differ between ranks (a rank may have none)."""
+        raise NotImplementedError
+
 
 class SymmPeerGroup(PeerGroup):
     """One process per GPU; buffers come from torch.distributed symmetric memory (NVLink P2P)."""
@@ -87,6 +92,27 @@ class SymmPeerGroup(PeerGroup):
     def all_reduce_sum(self, buf):
         self._dist.all_reduce(buf, op=self._dist.ReduceOp.SUM, group=self.group)
 
+    def gather(self, tensors):
+        """NCCL: the lengths first, then one all_gather per tensor of buffers padded to the longest."""
+        dist = self._dist
+        dev = tensors[0].device
+        counts = torch.empty(self.world, dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(counts, torch.tensor([tensors[0].numel()], dtype=torch.int64, device=dev),
+                                    group=self.group)
+        counts = [int(c) for c in counts.cpu()]
+        width = max(counts)
+        out = []
+        for t in tensors:
+            if width == 0:
+                out.append([t.new_empty(0) for _ in range(self.world)])
+                continue
+            mine = t.new_zeros(width)
+            mine[:t.numel()] = t
+            every = t.new_empty(self.world * width)
+            dist.all_gather_into_tensor(every, mine, group=self.group)
+            out.append([every[r * width:r * width + counts[r]] for r in range(self.world)])
+        return out
+
 
 class VirtualPeerGroup(PeerGroup):
     """`world` virtual ranks in one process: buffers are ordinary tensors shared through a dict;
@@ -109,6 +135,13 @@ class VirtualPeerGroup(PeerGroup):
         if self.world != 1:
             raise RuntimeError("virtual ranks sum over ranks in lock step: drive their optimizer steps with "
                                "fuxictr_b200.sharded.lockstep_steps")
+
+    def gather(self, tensors):
+        """One virtual rank is its own gather; more need every rank's tensors at once: lockstep_evaluate does it."""
+        if self.world != 1:
+            raise RuntimeError("virtual ranks evaluate in lock step: use fuxictr_b200.sharded.lockstep_evaluate / "
+                               "lockstep_predict")
+        return [[t] for t in tensors]
 
 
 def lockstep_steps(optimizers, combine=None):
@@ -238,6 +271,10 @@ class ShardedFront(object):
         # fills its own padding slots from here, so no rank serves the others' (half of a DIN history)
         self.pad_rows, self.pad_ptrs, _ = g.alloc("pad_rows", (self.F * dim + self.F,), torch.float32)
         self.glogit, self.glogit_ptrs, _ = g.alloc("glogit", (batch_local,), torch.float32)
+        # the evaluation round's row counts: word p = rows of rank p's batch, stored by p's publish (eval_phase_ids)
+        self.rows_all, self.rows_ptrs, _ = g.alloc("rows_all", (g.world,), torch.int32)
+        self._eval_rows = 0
+        self._landed = None                  # (emb, logit) of an evaluation round, taken by the next sharded_front
         self.status = torch.zeros(1, dtype=torch.int32, device="cuda")
         # mean over the GLOBAL batch (rank_model.py:130): either the pull scales every gradient row by
         # 1/world (default), or the caller seeds backward() with 1/world and sets pull_scale = 1
@@ -267,6 +304,9 @@ class ShardedFront(object):
 
     # -- forward phases -------------------------------------------------------------------------
     def phase_ids(self, batch_matrix):
+        if tuple(batch_matrix.shape) != (self.B, self.W):
+            raise ValueError("sharded front: a training batch matrix must be (batch_local, matrix_width) = (%d, %d), "
+                             "got %s" % (self.B, self.W, tuple(batch_matrix.shape)))
         g = self.group
         src = batch_matrix
         if (not src.is_contiguous()) or src.data_ptr() % 16 != 0:
@@ -313,6 +353,73 @@ class ShardedFront(object):
                   F2._ptr(self.bias), self.B, self.F, self.dim, 1 if self.want_fm else 0, F2._ptr(logit),
                   F2._ptr(sums), F2._stream())
         return emb, logit, sums
+
+    # -- evaluation round (forward only, ragged) --------------------------------------------------
+    # publish ids, rows and padding rows -> barrier -> lookup -> barrier -> reduce over `rows`.  The lookup keeps
+    # no owned list (nothing is pulled) and takes no lazy context (evaluate() materialises lazy tables first), so
+    # neither the owned list nor the lazy bookkeeping of the next training step is touched.  Every buffer the
+    # round writes (ids_all, pad_rows, emb, lrw) is rewritten in full by the next training step's own publish
+    # and push, inside a captured TrainPipeline graph too.
+    def eval_rows(self, batch_matrix):
+        """Rows of an evaluation batch matrix; refuses (ValueError) a batch the round cannot serve."""
+        shape = tuple(batch_matrix.shape)
+        if len(shape) != 2 or shape[1] != self.W:
+            raise ValueError("sharded evaluation: the batch matrix is %s, the front was built for %d columns "
+                             "(matrix_width)" % (shape, self.W))
+        if shape[0] > self.B:
+            raise ValueError("sharded evaluation: a batch of %d rows is more than batch_local = %d; build the "
+                             "validation loader with batch_size <= batch_local" % (shape[0], self.B))
+        return shape[0]
+
+    def eval_phase_ids(self, batch_matrix):
+        """Before the first barrier: this rank's ids, its row count and the padding rows it owns, to every rank.
+        Returns the row count."""
+        rows = self.eval_rows(batch_matrix)
+        g = self.group
+        src = batch_matrix if rows else None
+        if rows and (src.dtype != self._ids_src.dtype or not src.is_contiguous() or src.data_ptr() % 16 != 0):
+            src = self._ids_src[:rows]
+            src.copy_(batch_matrix)
+        dst = [int(base) + g.rank * self._slot_bytes for base in self._ids_all_ptrs]
+        lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
+        _lib.call("b2_shard_publish_rows", F2._ptr(src), self.src_code, rows, self.W, self.B, _ptr_array(dst),
+                  self._descs(self.emb_tables, self.dim), lr, self.F, g.world, g.rank, _ptr_array(self.pad_ptrs),
+                  _ptr_array(self.rows_ptrs), F2._stream())
+        self._eval_rows = rows
+        self._landed = None
+        return rows
+
+    def eval_phase_lookup(self):
+        """Between the barriers: the rows this rank owns, to every rank's first rows_all[p] samples."""
+        g = self.group
+        lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
+        _lib.call("b2_shard_lookup", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
+                  _ptr_array(self.ids_ptrs), self.W, _ptr_array(self.emb_ptrs),
+                  _ptr_array(self.lrw_ptrs) if lr is not None else None, F2._ptr(self.rows_all), F2._ptr(self.status),
+                  F2._ptr(self.pad_rows), F2._stream())
+
+    def eval_phase_reduce(self):
+        """After the second barrier: the logit of this rank's rows; leaves (emb (rows, S, D), logit (rows, 1)),
+        views of the landed rows, for the model's forward (sharded_front takes them).  Nothing for 0 rows."""
+        n = self._eval_rows
+        if n == 0:
+            self._landed = None
+            return None
+        emb = self.emb[:n]
+        if not self.lr_tables and not self.want_fm:
+            logit = torch.zeros((n, 1), dtype=torch.float32, device="cuda")
+        else:
+            logit = torch.empty((n, 1), dtype=torch.float32, device="cuda")
+            sums = torch.empty((n, self.dim), dtype=torch.float32, device="cuda") if self.want_fm else None
+            _lib.call("b2_front_reduce", F2._ptr(emb), F2._ptr(self.lrw) if self.lr_tables else None,
+                      F2._ptr(self.bias), n, self.F, self.dim, 1 if self.want_fm else 0, F2._ptr(logit),
+                      F2._ptr(sums), F2._stream())
+        self._landed = (emb.view(n, self.S, self.dim), logit)
+        return self._landed
+
+    def take_landed(self):
+        landed, self._landed = self._landed, None
+        return landed
 
     # -- backward phases ------------------------------------------------------------------------
     def phase_gprep(self, gx, emb, sums, glogit, gbias=None):
@@ -392,5 +499,187 @@ class _ShardedFrontFn(torch.autograd.Function):
 
 
 def sharded_front(front, batch_matrix):
-    """(emb (B, S, D), logit (B, 1)) of this rank's samples, read from the row-sharded tables."""
+    """(emb (B, S, D), logit (B, 1)) of this rank's samples, read from the row-sharded tables.  Inside an
+    evaluation round the rows have already landed (ShardedFront.eval_phase_reduce): they are taken instead."""
+    landed = front.take_landed()
+    if landed is not None:
+        if landed[0].shape[0] != batch_matrix.shape[0]:
+            raise RuntimeError("sharded evaluation: %d landed rows for a batch of %d"
+                               % (landed[0].shape[0], batch_matrix.shape[0]))
+        return landed
     return _ShardedFrontFn.apply(front, batch_matrix, front.bias, *front.distinct_tables())
+
+
+# --------------------------------------------------------------------------------------------
+# Evaluation over row shards: every rank feeds its own shard of the split, the metrics cover all of them
+# --------------------------------------------------------------------------------------------
+def _loader_plan(generator):
+    """(len(), batch_size) of an evaluation generator; None for what it does not tell."""
+    try:
+        n = len(generator)
+    except TypeError:
+        n = None
+    bs = getattr(generator, "batch_size", None)
+    return n, (int(bs) if isinstance(bs, int) else None)
+
+
+def check_rounds(plans, names, batch_local):
+    """Refuses (ValueError, alike on every rank) what would leave the ranks out of step.  Every rank must run the
+    same number of evaluation rounds, each of them two barriers on every rank, so the lengths must agree.
+    Batches must fit batch_local: a loader that declares a larger batch_size is refused up front, since a
+    refusal inside a round would leave the other ranks at its barrier.  plans[r]: (len() or None, batch_size
+    or None) of rank r's generator; names[r] describes that loader."""
+    missing = [r for r, (n, _) in enumerate(plans) if n is None]
+    if missing:
+        raise ValueError("sharded evaluation needs generators with len() (every rank runs the same number of "
+                         "rounds); %s has none" % ", ".join("rank %d's %s" % (r, names[r]) for r in missing))
+    lengths = [n for n, _ in plans]
+    if len(set(lengths)) != 1:
+        raise ValueError("sharded evaluation: the ranks' generators have different lengths %s; every rank must run "
+                         "the same number of rounds (MatrixDataLoader(shard=(rank, world), drop_last=False) does)"
+                         % lengths)
+    wide = [r for r, (_, bs) in enumerate(plans) if bs is not None and bs > batch_local]
+    if wide:
+        raise ValueError("sharded evaluation: rank %d's %s has batch_size %d, more than batch_local = %d; build the "
+                         "validation loader with batch_size <= batch_local"
+                         % (wide[0], names[wide[0]], plans[wide[0]][1], batch_local))
+
+
+def _check_rounds_collective(group, generator, batch_local):
+    """check_rounds over real ranks: one small gather of every rank's (len(), batch_size) (-1: none)."""
+    n, bs = _loader_plan(generator)
+    mine = torch.tensor([-1 if n is None else n, -1 if bs is None else bs], dtype=torch.int64, device="cuda")
+    plans = [tuple(None if int(v) < 0 else int(v) for v in t.cpu()) for t in group.gather([mine])[0]]
+    names = ["loader" if r != group.rank else type(generator).__name__ for r in range(group.world)]
+    check_rounds(plans, names, batch_local)
+
+
+def eval_rank_rounds(model, generator, acc, with_labels=True):
+    """One rank's evaluation, as phases: yields at each of the two cross-rank barriers of a round, which the
+    caller runs (real ranks) or fills with the same phase of every other virtual rank (lockstep_evaluate).
+    Each round: publish this rank's ids and row count, lookup, reduce over its rows, then the model's own
+    forward on the landed rows (a rank with 0 rows serves its peers and skips it); the predictions (and
+    labels) are appended to `acc` (metrics.DeviceMetrics), in HBM.  Run under torch.no_grad() in eval()."""
+    front = model._sharded_front
+    try:
+        for batch in generator:
+            rows = front.eval_phase_ids(model._batch_matrix(batch))
+            yield
+            front.eval_phase_lookup()
+            yield
+            front.eval_phase_reduce()
+            if rows:
+                acc.append(model.forward(batch)["y_pred"], model.get_labels(batch) if with_labels else None)
+    finally:
+        front._landed = None
+
+
+def _run_rounds(group, phases):
+    for _ in phases:
+        group.barrier()
+
+
+def _lockstep_rounds(phase_lists):
+    """Every virtual rank's phases in lock step: each rank runs up to its next barrier, in rank order."""
+    end = object()
+    try:
+        while True:
+            done = [next(ph, end) is end for ph in phase_lists]
+            if all(done):
+                return
+            if any(done):
+                raise RuntimeError("virtual ranks disagree on the number of evaluation rounds")
+    finally:
+        for ph in phase_lists:
+            ph.close()
+
+
+def _rank_check(models):
+    for r, m in enumerate(models):
+        front = getattr(m, "_sharded_front", None)
+        if front is None:
+            raise ValueError("model %d is not sharded (enable_sharding)" % r)
+        if front.group.rank != r or front.group.world != len(models):
+            raise ValueError("models must be virtual ranks 0..%d in rank order" % (len(models) - 1))
+
+
+def _union_metrics(preds, labels, metrics):
+    """The metric words (metrics.metric_words) of every rank's predictions, concatenated in rank order."""
+    from .metrics import metric_words
+    return metric_words(torch.cat(list(labels)), torch.cat(list(preds)), metrics)
+
+
+def evaluate_sharded(model, generator, metrics):
+    """RankModel.evaluate of a row-sharded model: a collective call.  Each rank feeds its own shard of the split
+    (same len() on every rank, checked first); logloss / AUC cover the union of all ranks' rows, computed on
+    rank 0 over the rank-ordered union and handed to every rank, so every rank returns the same dict, bit for bit."""
+    from .metrics import DeviceMetrics, check_metrics, metrics_from_words
+    check_metrics(metrics)
+    group = model._sharded_front.group
+    if isinstance(group, VirtualPeerGroup) and group.world != 1:
+        raise RuntimeError("virtual ranks evaluate in lock step: use fuxictr_b200.sharded.lockstep_evaluate")
+    _check_rounds_collective(group, generator, model._sharded_front.B)
+    acc = DeviceMetrics(model.device)
+    model.eval()
+    with torch.no_grad():
+        _run_rounds(group, eval_rank_rounds(model, generator, acc))
+        preds, labels = group.gather([acc.predictions(), acc.labels()])
+        n = sum(p.numel() for p in preds)
+        if n == 0 and "AUC" in metrics:                # every rank knows n: they all raise
+            raise ValueError("AUC of an empty prediction set is undefined")
+        if group.rank == 0:
+            words = _union_metrics(preds, labels, metrics)
+        else:
+            words = torch.zeros(6, dtype=torch.int64, device=model.device)
+        words = group.gather([words])[0][0]           # rank 0's words, on every rank
+    return metrics_from_words(words.cpu(), n, metrics)
+
+
+def predict_sharded(model, generator):
+    """RankModel.predict of a row-sharded model: a collective call (every rank runs the same rounds) that returns
+    THIS rank's predictions, in its generator's order, as a float64 numpy array — the data-parallel meaning."""
+    from .metrics import DeviceMetrics
+    group = model._sharded_front.group
+    if isinstance(group, VirtualPeerGroup) and group.world != 1:
+        raise RuntimeError("virtual ranks predict in lock step: use fuxictr_b200.sharded.lockstep_predict")
+    _check_rounds_collective(group, generator, model._sharded_front.B)
+    acc = DeviceMetrics(model.device)
+    model.eval()
+    with torch.no_grad():
+        _run_rounds(group, eval_rank_rounds(model, generator, acc, with_labels=False))
+    return acc.predictions().cpu().numpy().astype("float64")
+
+
+def _lockstep_accumulate(models, generators, with_labels):
+    from .metrics import DeviceMetrics
+    _rank_check(models)
+    if len(generators) != len(models):
+        raise ValueError("one generator per virtual rank (%d models, %d generators)" % (len(models), len(generators)))
+    check_rounds([_loader_plan(g) for g in generators], [type(g).__name__ for g in generators],
+                 models[0]._sharded_front.B)
+    accs = [DeviceMetrics(m.device) for m in models]
+    for m in models:
+        m.materialize_tables()
+        m.eval()
+    with torch.no_grad():
+        _lockstep_rounds([eval_rank_rounds(m, g, a, with_labels) for m, g, a in zip(models, generators, accs)])
+    return accs
+
+
+def lockstep_evaluate(models, generators, metrics=None):
+    """evaluate() of every virtual rank (models[r] is rank r, generators[r] its shard of the split), each round's
+    phases driven for all ranks in order; the same per-rank code as evaluate_sharded.  Returns one dict per
+    rank — the same metrics over the rank-ordered union of every rank's rows."""
+    from .metrics import check_metrics, metrics_from_words
+    names = metrics if metrics is not None else ["logloss", "AUC"]
+    check_metrics(names)
+    accs = _lockstep_accumulate(models, generators, True)
+    with torch.no_grad():
+        words = _union_metrics([a.predictions() for a in accs], [a.labels() for a in accs], names)
+    result = metrics_from_words(words.cpu(), sum(a.n for a in accs), names)
+    return [result.copy() for _ in models]
+
+
+def lockstep_predict(models, generators):
+    """predict() of every virtual rank in lock step: each rank's own predictions (float64 numpy), in rank order."""
+    return [a.predictions().cpu().numpy().astype("float64") for a in _lockstep_accumulate(models, generators, False)]

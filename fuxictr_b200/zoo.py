@@ -142,16 +142,27 @@ class RankModel(nn.Module):
     # -- rank_model.py:350-398, device-resident (SURVEY.md 8f row 3) ---------------------------
     def evaluate(self, data_generator, metrics=None):
         """Same contract as BaseModel.evaluate; predictions and labels stay in HBM (no per-batch
-        `.cpu().numpy()`), logloss / AUC come from csrc/metrics.cu, one small D2H at the end."""
+        `.cpu().numpy()`), logloss / AUC come from csrc/metrics.cu, one small D2H at the end.
+        After enable_sharding() this is a collective call: every rank feeds its own shard of the split (generators
+        of equal len(), batches of at most batch_local rows) and gets the metrics over the union of all ranks'
+        rows, the same on every rank (fuxictr_b200.sharded.evaluate_sharded)."""
         from .metrics import evaluate_generator
         self.materialize_tables()
         names = metrics if metrics is not None else getattr(self, "validation_metrics", ["logloss", "AUC"])
+        if getattr(self, "_sharded_front", None) is not None:
+            from .sharded import evaluate_sharded
+            return evaluate_sharded(self, data_generator, names)
         return evaluate_generator(self, data_generator, names)
 
     def predict(self, data_generator):
-        """BaseModel.predict: flattened float64 numpy array; one D2H for the whole generator."""
+        """BaseModel.predict: flattened float64 numpy array; one D2H for the whole generator.  After
+        enable_sharding(): a collective call that returns THIS rank's predictions, in its generator's order
+        (the data-parallel meaning; fuxictr_b200.sharded.predict_sharded)."""
         from .metrics import predict_generator
         self.materialize_tables()
+        if getattr(self, "_sharded_front", None) is not None:
+            from .sharded import predict_sharded
+            return predict_sharded(self, data_generator)
         return predict_generator(self, data_generator)
 
     # -- H100 extension: flat arenas + 2-kernel clip/Adam -------------------------------------

@@ -338,6 +338,29 @@ B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_field* lr_fiel
 B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,
                                 const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int world,
                                 int rank, float* const* peer_pad, void* stream);
+/*
+ * The evaluation round: a forward-only lookup of a ragged batch (0 <= rows <= batch_local samples on each rank,
+ * which may differ between ranks and between rounds).
+ * b2_shard_publish_rows: b2_shard_publish_ids of the first `rows` rows of a (rows, width) batch matrix — only
+ * rows * width ids are read and stored into peer_dst[p] — and, in the same launch, the row count into word
+ * `rank` of peer_rows[p] (int32[world] on every rank, 4-byte aligned) for every p < world.  Refused: rows
+ * outside [0, capacity_rows] (capacity_rows = the batch_local of the peer buffers), NULL src with rows > 0.
+ * b2_shard_lookup: b2_shard_push_pad over the candidates (requester p, sample b < rows_all[p], slot), where
+ * rows_all is this rank's int32[world] buffer that every rank's publish filled before the barrier: the bound
+ * comes from device memory, so no rank needs its peers' counts on the host, and a rank with 0 rows still
+ * serves the others.  peer_ids hold the int32 ids the publish stored (row pitch ids_stride).  It keeps no
+ * owned-row list and takes no lazy context: it reads the tables as they are (materialise lazy tables first),
+ * and leaves the owned list and the lazy bookkeeping of the next training step untouched.  Out-of-range ids
+ * set *status (if not NULL) and land as zero rows, as in the push.  Follow it with b2_front_reduce over
+ * `rows` samples. */
+B2_API int b2_shard_publish_rows(const void* src, int idx_dtype, int64_t rows, int64_t width, int64_t capacity_rows,
+                                 int32_t* const* peer_dst, const b2_field* emb_fields, const b2_field* lr_fields,
+                                 int nfields, int world, int rank, float* const* peer_pad, int32_t* const* peer_rows,
+                                 void* stream);
+B2_API int b2_shard_lookup(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch_local,
+                           int world, int rank, const int32_t* const* peer_ids, int64_t ids_stride,
+                           float* const* peer_emb, float* const* peer_lrw, const int32_t* rows_all, int32_t* status,
+                           const float* pad_rows, void* stream);
 B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream);
 /* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
  * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world. */
