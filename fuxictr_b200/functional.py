@@ -1030,6 +1030,127 @@ def cross_v2_layer(x0, xi, weight, bias):
     return _CrossV2Layer.apply(x0, xi, weight, bias)
 
 
+def crossnet_mix_bound(low_rank, num_experts):
+    """None when the CrossNetMix kernels cover (low_rank, num_experts), else the bound it breaks."""
+    if not 1 <= low_rank <= _lib.B2_CROSSMIX_MAX_RANK:
+        return "low_rank must lie in [1, %d], got %d" % (_lib.B2_CROSSMIX_MAX_RANK, low_rank)
+    if num_experts < 1 or num_experts * low_rank > _lib.B2_CROSSMIX_MAX_COLS:
+        return "num_experts * low_rank must lie in [1, %d], got %d" % (_lib.B2_CROSSMIX_MAX_COLS,
+                                                                     num_experts * low_rank)
+    return None
+
+
+def _aux_args(aux):
+    """(pointer, dtype code, row pitch) of an auxiliary operand written by a row kernel (see empty_aux)."""
+    if aux is None:
+        return _ptr(None), B2_F32, 0
+    return _ptr(aux), (B2_BF16 if aux.dtype == torch.bfloat16 else B2_F32), aux.stride(0)
+
+
+class _CrossMixLayer(torch.autograd.Function):
+    """One CrossNetMix layer (cross_net.py:168-198) as two GEMMs around a per-row expert kernel
+    (include/fuxictr_b200.h "CrossNetMix"): P = x_l W1^T (the E rank-r projections and the E gate logits in
+    one GEMM), A2 = [p_e tanh(tanh(h_e) C_e^T)] (b2_crossmix_fwd), x_next = x_l + x_0 * (A2 W2^T + b) (the
+    CrossNetV2 epilogue, lin kept).  W1, W2 are packed from U, V and the gating weights each forward.
+    Backward: dlin = g * x_0 (+ bias gradient), dA2 = dlin W2, dW2 = dlin^T A2, the row kernel back to
+    dA1 = dP (+ dC), dx_l = g + dA1 W1, dW1 = dA1^T x_l, and one unpack of dW1, dW2 into U, V, gating."""
+
+    @staticmethod
+    def forward(ctx, x0, xl, U, V, C, G, bias):
+        x0, xl = _f32c(x0), _f32c(xl)
+        U, V, C, G = _f32c(U), _f32c(V), _f32c(C), _f32c(G)
+        B, d = xl.shape
+        E, _, r = U.shape
+        n1, k2 = (E * r + E + 3) // 4 * 4, (E * r + 3) // 4 * 4
+        dev = xl.device
+        W1 = torch.empty((n1, d), dtype=torch.float32, device=dev)
+        W2 = torch.empty((d, k2), dtype=torch.float32, device=dev)
+        _lib.call("b2_crossmix_pack", _ptr(U), _ptr(V), _ptr(G), d, r, E, _ptr(W1), _ptr(W2), _stream())
+        tc = _tc_layer_ok(W1) and _tc_layer_ok(W2) and xl.data_ptr() % 16 == 0 and x0.data_ptr() % 16 == 0
+        P = torch.empty((B, n1), dtype=torch.float32, device=dev)
+        A2 = torch.empty((B, k2), dtype=torch.float32, device=dev)
+        out = torch.empty_like(xl)
+        lin = torch.empty_like(xl)
+        b = bias.view(-1)
+        xl_aux = a2_aux = w1_aux = w2_aux = None
+        if tc:
+            xl_aux, w1_aux, w2_aux = make_aux(xl), make_aux(W1), make_aux(W2)
+            a2_aux = empty_aux(B, k2, dev)
+            gemm_ex(xl, W1, P, a_small=xl_aux, b_small=w1_aux)
+        else:
+            gemm_f32(xl, W1, P, b_t=True)
+        _lib.call("b2_crossmix_fwd", _ptr(P), _ptr(C), B, r, E, _ptr(A2), *_aux_args(a2_aux), _stream())
+        if tc:
+            gemm_ex(A2, W2, out, a_small=a2_aux, b_small=w2_aux, bias=b, mul=x0, add=xl, out_pre=lin)
+        else:
+            gemm_f32(A2, W2, lin, b_t=True, bias=b)
+            torch.addcmul(xl, x0, lin, out=out)
+        ctx.save_for_backward(x0, xl, lin, P, A2, W1, W2, C)
+        ctx.tc, ctx.aux, ctx.r, ctx.bias = tc, (xl_aux, a2_aux, w1_aux, w2_aux), r, bias
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x0, xl, lin, P, A2, W1, W2, C = ctx.saved_tensors
+        g = _f32c(g)
+        xl_aux, a2_aux, w1_aux, w2_aux = ctx.aux
+        tc, r, bias = ctx.tc, ctx.r, ctx.bias
+        B, d = xl.shape
+        E = C.shape[0]
+        n1, k2 = W1.shape[0], W2.shape[1]
+        dev = xl.device
+        gb = _grad_buffer(bias, zero=False) if bias.requires_grad else None
+        dlin, dlin_small, _, _ = prep_operand(g, x0, B2_PREP_MUL, want_out=True, want_small=_x3_aux() and tc,
+                                              colsum=gb)
+        if tc and dlin_small is None:
+            dlin_small = make_aux(dlin)          # bf16 mode (None for single-pass TF32)
+        dA2 = torch.empty((B, k2), dtype=torch.float32, device=dev)
+        dW2 = torch.empty((d, k2), dtype=torch.float32, device=dev)
+        dA1 = torch.empty((B, n1), dtype=torch.float32, device=dev)
+        dW1 = torch.empty((n1, d), dtype=torch.float32, device=dev)
+        gxl = torch.empty_like(xl)
+        gC = torch.zeros_like(C)
+        da1_aux = empty_aux(B, n1, dev) if tc else None
+        if tc:
+            gemm_ex(dlin, W2, dA2, b_mn=True, a_small=dlin_small, b_small=w2_aux)                   # dA2 = dlin W2
+            gemm_ex(dlin, A2, dW2, a_mn=True, b_mn=True, a_small=dlin_small, b_small=a2_aux)      # dW2 = dlin^T A2
+        else:
+            gemm_f32(dlin, W2, dA2)
+            gemm_f32(dlin, A2, dW2, a_t=True)
+        _lib.call("b2_crossmix_bwd", _ptr(P), _ptr(C), _ptr(dA2), B, r, E, _ptr(dA1), *_aux_args(da1_aux),
+                  _ptr(gC), _stream())
+        if tc:
+            gemm_ex(dA1, W1, gxl, b_mn=True, a_small=da1_aux, b_small=w1_aux, add=g)               # dx_l = g + dA1 W1
+            gemm_ex(dA1, xl, dW1, a_mn=True, b_mn=True, a_small=da1_aux, b_small=xl_aux)          # dW1 = dA1^T x_l
+        else:
+            gemm_f32(dA1, W1, gxl, add=g)
+            gemm_f32(dA1, xl, dW1, a_t=True)
+        gU = torch.empty((E, d, r), dtype=torch.float32, device=dev)
+        gV = torch.empty_like(gU)
+        gG = torch.empty((E, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_crossmix_unpack", _ptr(dW1), _ptr(dW2), d, r, E, _ptr(gU), _ptr(gV), _ptr(gG), _stream())
+        gx0 = g * lin if ctx.needs_input_grad[0] else None
+        return gx0, gxl, gU, gV, gC, gG, gb
+
+
+def crossnet_mix_layer(x0, xl, U, V, C, gating_weights, bias):
+    """x_next of one CrossNetMix layer: U, V (E, d, r), C (E, r, r) and bias (d, 1) are the layer's
+    U_list[i], V_list[i], C_list[i], bias[i]; gating_weights the (E, d) rows of every gating[e].weight
+    (a tensor, or the E (1, d) weights, which are concatenated)."""
+    if isinstance(gating_weights, (list, tuple)):
+        gating_weights = torch.cat([w.reshape(1, -1) for w in gating_weights], dim=0)
+    _require_cuda(x0, xl, U, V, C, gating_weights, bias)
+    E, d, r = U.shape
+    if xl.dim() != 2 or xl.shape[1] != d or tuple(V.shape) != (E, d, r) or tuple(C.shape) != (E, r, r) \
+            or tuple(gating_weights.shape) != (E, d) or bias.numel() != d:
+        raise ValueError("crossnet_mix_layer: shapes x%s U%s V%s C%s gating%s bias%s do not match"
+                         % tuple(tuple(t.shape) for t in (xl, U, V, C, gating_weights, bias)))
+    bound = crossnet_mix_bound(r, E)
+    if bound is not None:
+        raise NotImplementedError("CrossNetMix kernels: " + bound)
+    return _CrossMixLayer.apply(x0, xl, U, V, C, gating_weights, bias)
+
+
 def mlp_chain_supported():
     return _MATMUL["mode"] != "fp32"
 

@@ -488,6 +488,40 @@ class CrossNetV2(nn.Module):
         return X_i
 
 
+class CrossNetMix(nn.Module):
+    """cross_net.py:132-201 (DCN-Mix): per layer a softmax-gated mixture of E low-rank experts,
+    x_{l+1} = x_l + sum_e p_e x_0 * (U_e tanh(C_e tanh(V_e^T x_l)) + b).  Each layer is one autograd node:
+    two GEMMs around the per-row expert kernel (functional._CrossMixLayer).  Parameters, their names,
+    registration order and initialisation draws are the reference's; the output is squeezed like its
+    `x_l.squeeze()`."""
+
+    def __init__(self, in_features, layer_num=2, low_rank=32, num_experts=4):
+        super(CrossNetMix, self).__init__()
+        bound = F2.crossnet_mix_bound(low_rank, num_experts)
+        if bound is not None:
+            raise NotImplementedError("CrossNetMix kernels: " + bound)
+        self.layer_num = layer_num
+        self.num_experts = num_experts
+        self.U_list = torch.nn.ParameterList([nn.Parameter(nn.init.xavier_normal_(
+            torch.empty(num_experts, in_features, low_rank))) for i in range(self.layer_num)])
+        self.V_list = torch.nn.ParameterList([nn.Parameter(nn.init.xavier_normal_(
+            torch.empty(num_experts, in_features, low_rank))) for i in range(self.layer_num)])
+        self.C_list = torch.nn.ParameterList([nn.Parameter(nn.init.xavier_normal_(
+            torch.empty(num_experts, low_rank, low_rank))) for i in range(self.layer_num)])
+        self.gating = nn.ModuleList([nn.Linear(in_features, 1, bias=False) for i in range(self.num_experts)])
+        self.bias = torch.nn.ParameterList([nn.Parameter(nn.init.zeros_(
+            torch.empty(in_features, 1))) for i in range(self.layer_num)])
+
+    def forward(self, inputs):
+        x_l = inputs
+        if self.layer_num > 0:
+            gates = torch.cat([g.weight for g in self.gating], dim=0)        # (E, d), shared by every layer
+            for i in range(self.layer_num):
+                x_l = F2.crossnet_mix_layer(inputs, x_l, self.U_list[i], self.V_list[i], self.C_list[i], gates,
+                                            self.bias[i])
+        return x_l.squeeze()
+
+
 # --------------------------------------------------------------------------------------
 # CIN
 # --------------------------------------------------------------------------------------

@@ -443,7 +443,10 @@ class DCNv2(RankModel):
                                     embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
                                     **kwargs)
         if use_low_rank_mixture:
-            raise NotImplementedError("CrossNetMix is outside the H100 hot path (SURVEY.md section 2 row 6)")
+            raise NotImplementedError(
+                "zoo.DCNv2 has no low-rank mixture (arena, fused Adam, graph capture and sharding do not cover "
+                "CrossNetMix); the reference DCNv2 with use_low_rank_mixture=True runs its CrossNetMix on the "
+                "kernels under fuxictr_b200.patch.enable(), or build a model from layers.CrossNetMix")
         if model_structure not in self._STRUCTURES:
             raise AssertionError("model_structure={} not supported!".format(model_structure))
         self.model_structure = model_structure

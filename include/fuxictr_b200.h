@@ -404,6 +404,40 @@ B2_API int b2_crossnet_bwd(const float* x0, const float* w, const float* b, cons
                     float* gb, void* stream);
 
 /*
+ * CrossNetMix (layers/interactions/cross_net.py:132-201), one layer of the low-rank mixture of experts:
+ *   h_e = tanh(x_l V_e), v_e = tanh(h_e C_e^T), p = softmax_e(x_l g_e^T),
+ *   x_{l+1} = x_l + x0 * (A2 @ W2^T + b),  A2 = [p_1 v_1 | ... | p_E v_E]   (exact because sum_e p_e = 1)
+ * as GEMM1 P = x_l @ W1^T, the row kernel P -> A2, and GEMM2 with the CrossNetV2 epilogue.
+ * U, V (E, d, r) and C (E, r, r) are the layer's U_list[i], V_list[i], C_list[i]; G (E, d) the rows
+ * gating[e].weight.  With R = E*r, N1 = round_up(R + E, 4), K2 = round_up(R, 4), all row-major fp32:
+ *   W1 (N1, d) K-major:  W1[e*r + j, :] = V[e, :, j];  W1[R + e, :] = G[e, :];  rows R+E .. N1-1 zero
+ *   W2 (d, K2) K-major:  W2[n, e*r + j] = U[e, n, j];  columns R .. K2-1 zero
+ *   P  (B, N1) = x_l W1^T: columns 0..R-1 the pre-tanh h, R..R+E-1 the gate logits
+ *   A2 (B, K2), dA2 (B, K2): columns R .. K2-1 of A2 are written zero, those of dA2 are not read
+ *   dA1 (B, N1) = [dP | dlogit | 0]: the gradient of P
+ * Supported range: 1 <= r <= B2_CROSSMIX_MAX_RANK and E*r <= B2_CROSSMIX_MAX_COLS (all experts' C in one
+ * CTA's shared memory); outside it every entry point returns B2_E_INVALID.
+ * Saved for the backward: x_l, P, A2 and the packed W1, W2 of the forward; the backward recomputes h, v, p
+ * from P and C.
+ * b2_crossmix_pack: W1, W2 ("=") from U, V, G; one launch.
+ * b2_crossmix_fwd:  A2 "=" from P and C; a2_aux (optional, row pitch ld_aux) receives A2's GEMM operand
+ *   copy: its bf16 rounding (aux_dtype B2_BF16) or its 3xTF32 small part (B2_F32).
+ * b2_crossmix_bwd:  dA1 "=" (+ da1_aux as above) from P, C, dA2; dC (E, r, r) "+=" (caller zeroes): a
+ *   per-CTA sum in shared memory, then one float atomic per element and CTA.
+ * b2_crossmix_unpack: gU, gV (E, d, r) and gG (E, d) "=" from dW1 (N1, d) and dW2 (d, K2).
+ */
+#define B2_CROSSMIX_MAX_RANK 64
+#define B2_CROSSMIX_MAX_COLS 256
+B2_API int b2_crossmix_pack(const float* U, const float* V, const float* G, int d, int r, int E, float* W1,
+                            float* W2, void* stream);
+B2_API int b2_crossmix_fwd(const float* P, const float* C, int64_t batch, int r, int E, float* A2, void* a2_aux,
+                           int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_crossmix_bwd(const float* P, const float* C, const float* dA2, int64_t batch, int r, int E,
+                           float* dA1, void* da1_aux, int aux_dtype, int64_t ld_aux, float* dC, void* stream);
+B2_API int b2_crossmix_unpack(const float* dW1, const float* dW2, int d, int r, int E, float* gU, float* gV,
+                              float* gG, void* stream);
+
+/*
  * One CompressedInteractionNet layer (layers/interactions/compressed_interaction_net.py:70-73)
  * without the (B, F*H, D) Hadamard tensor:
  *   out[b,h',d] = bias[h'] + sum_{f,m} w[h', f*H + m] * x0[b,f,d] * xk[b,m,d]
