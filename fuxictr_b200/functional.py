@@ -608,6 +608,22 @@ def prep_operand(x, y=None, act=B2_ACT_NONE, want_out=False, want_small=False, w
     return out, small, out_t, t_small
 
 
+def _grad_operand(g, y, act, tc, colsum=None, drop=None):
+    """The gradient g of a layer's output as the dZ operand of its dgrad and wgrad, in one pass over g
+    (prep_operand): the dropout mask `drop` regenerated, the backward of `act` with the output y (B2_PREP_MUL:
+    g * y), the column sums (bias gradient) added to `colsum`.  Returns (dZ, its auxiliary operand): dZ is g
+    itself when the pass changes no value; the auxiliary operand is what the matmul precision wants of a
+    tensor-core operand (see empty_aux, None without `tc`), written by the same pass where the kernel can."""
+    if act == B2_ACT_NONE:
+        y = None
+    keep = y is not None or drop is not None
+    out, aux, _, _ = prep_operand(g, y, act, want_out=keep, want_small=tc and _x3_aux(), colsum=colsum, drop=drop)
+    gz = out if keep else g
+    if tc and aux is None:
+        aux = make_aux(gz)          # bf16 mode (None for single-pass TF32 and in-kernel 3xTF32)
+    return gz, aux
+
+
 # ---- dropout masks of MLP chains (include/fuxictr_b200.h "Dropout masks", csrc/philox.cuh) -------------------
 # One {seed, offset} int64 pair per device.  Its seed is drawn from torch's generator of that device on first eager
 # use, and drawn again on the first eager use after torch.manual_seed (so seed_everything governs the masks as it
@@ -671,6 +687,34 @@ def _tc_layer_ok(weight):
             and weight.is_contiguous() and weight.data_ptr() % 16 == 0)
 
 
+def _linear_fwd(tc, a, a_aux, W, out, w_aux=None, **epilogue):
+    """out = epi(a W^T), W (N, K) as nn.Linear keeps it: on the tensor cores (a_aux, w_aux: the operands' auxiliary
+    ones; w_aux None: weight_aux(W), a parameter's cached one, itself None in a precision that has none) or,
+    without tc, on the SIMT GEMM.  The epilogue keywords are gemm_ex's or gemm_f32's."""
+    if tc:
+        return gemm_ex(a, W, out, a_small=a_aux, b_small=weight_aux(W) if w_aux is None else w_aux, **epilogue)
+    return gemm_f32(a, W, out, b_t=True, **epilogue)
+
+
+def _linear_dgrad(tc, gz, gz_aux, W, gx, w_aux=None, **epilogue):
+    """dX = epi(dZ W): W is consumed as it lies in memory (MN-major), no transpose in HBM."""
+    if tc:
+        return gemm_ex(gz, W, gx, b_mn=True, a_small=gz_aux, b_small=weight_aux(W) if w_aux is None else w_aux,
+                       **epilogue)
+    return gemm_f32(gz, W, gx, **epilogue)
+
+
+def _linear_wgrad(tc, gz, gz_aux, a, a_aux, gw, fork=None, ready=None, backfill=False):
+    """dW = dZ^T X, dZ and X (the forward's `a`, with the auxiliary operand the forward made) both MN-major.
+    ready: fork.ready() recorded before the dgrad was launched; the GEMM then runs on the fork's side stream."""
+    if ready is not None:
+        return fork.gemm(ready, gz, gz_aux, a, a_aux, gw)
+    if tc:
+        return gemm_ex(gz, a, gw, a_mn=True, b_mn=True, a_small=gz_aux, b_small=a_aux, out_is_zero=_is_zeroed(gw),
+                       backfill=backfill)
+    return gemm_f32(gz, a, gw, a_t=True)
+
+
 class _LinearAct(torch.autograd.Function):
     """y = act(x W^T + b): nn.Linear (+ReLU/Sigmoid) of MLP_Block (mlp_block.py:74-80).
 
@@ -684,23 +728,16 @@ class _LinearAct(torch.autograd.Function):
         x = _f32c(x)
         M, K = x.shape
         N = weight.shape[0]
-        mode = _MATMUL["mode"]
         y = torch.empty((M, N), dtype=torch.float32, device=x.device)
         ctx.act, ctx.bias, ctx.has_bias = act, bias, bias is not None
         if N == 1 and weight.is_contiguous():
             ctx.kind = "head"
             _lib.call("b2_head_fwd", _ptr(x), _ptr(weight), _ptr(bias), M, K, act, _ptr(y), _stream())
-            ctx.save_for_backward(x, weight, y if act != B2_ACT_NONE else None)
-            return y
-        if _tc_layer_ok(weight) and x.data_ptr() % 16 == 0:
-            ctx.kind = "tc"
-            x_small = make_aux(x)
-            gemm_ex(x, weight, y, a_small=x_small, b_small=weight_aux(weight), bias=bias, act=act)
-            ctx.x_small = x_small
-            ctx.save_for_backward(x, weight, y if act != B2_ACT_NONE else None)
-            return y
-        ctx.kind = "simt"
-        gemm_f32(x, weight, y, b_t=True, bias=bias, act=act)
+        else:
+            tc = _tc_layer_ok(weight) and x.data_ptr() % 16 == 0
+            ctx.kind = "tc" if tc else "simt"
+            ctx.x_small = make_aux(x) if tc else None
+            _linear_fwd(tc, x, ctx.x_small, weight, y, bias=bias, act=act)
         ctx.save_for_backward(x, weight, y if act != B2_ACT_NONE else None)
         return y
 
@@ -721,35 +758,16 @@ class _LinearAct(torch.autograd.Function):
                       _ptr(gb), _stream())
             return gx, gw, gb, None
         gb = _grad_buffer(ctx.bias, zero=False) if need_b else None
-        fused = act != B2_ACT_NONE
-        if ctx.kind == "tc":
-            x3 = _x3_aux()
-            # dZ = act'(Y) * dY, its 3xTF32 small part and the bias gradient: one pass over dY
-            gz, gz_small, _, _ = prep_operand(gy, y if fused else None, act, want_out=fused, want_small=x3, colsum=gb)
-            if not fused:
-                gz = gy
-            if not x3:
-                gz_small = make_aux(gz)          # bf16 mode: the bf16 operand of dZ (None for single-pass TF32)
-            if need_x:
-                gx = torch.empty((M, K), dtype=torch.float32, device=x.device)
-                gemm_ex(gz, weight, gx, b_mn=True, a_small=gz_small, b_small=weight_aux(weight))   # dX = dZ W
-            if need_w:
-                gw = _grad_buffer(weight, zero=False)
-                gemm_ex(gz, x, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=ctx.x_small,
-                        out_is_zero=_is_zeroed(gw))                                                # dW = dZ^T X
-            return gx, gw, gb, None
-        # fp32 SIMT path
-        gz = gy
-        if fused or gb is not None:
-            out, _, _, _ = prep_operand(gy, y if fused else None, act, want_out=fused, colsum=gb)
-            if fused:
-                gz = out
+        tc = ctx.kind == "tc"
+        gz, gz_aux = gy, None
+        if tc or act != B2_ACT_NONE or gb is not None:      # a SIMT layer with nothing to undo or to sum takes dY as it is
+            gz, gz_aux = _grad_operand(gy, y, act, tc, colsum=gb)
         if need_x:
             gx = torch.empty((M, K), dtype=torch.float32, device=x.device)
-            gemm_f32(gz, weight, gx)
+            _linear_dgrad(tc, gz, gz_aux, weight, gx)
         if need_w:
             gw = _grad_buffer(weight, zero=False)
-            gemm_f32(gz, x, gw, a_t=True)
+            _linear_wgrad(tc, gz, gz_aux, x, ctx.x_small, gw)
         return gx, gw, gb, None
 
 
@@ -792,8 +810,7 @@ class _WgradFork(object):
     def gemm(self, ready, gz, gz_small, h, h_small, gw):
         self.side.wait_event(ready)
         with torch.cuda.stream(self.side):
-            gemm_ex(gz, h, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=h_small,
-                    out_is_zero=_is_zeroed(gw), backfill=True)                                       # dW = dZ^T X
+            _linear_wgrad(True, gz, gz_small, h, h_small, gw, backfill=True)
         self.keep += [gz, gz_small, h, h_small]
         base = gw._base
         arena = getattr(base, "_b2_arena", None) if base is not None else None
@@ -830,7 +847,6 @@ class _MLPChain(torch.autograd.Function):
         M = x.shape[0]
         L = len(acts)
         Ws, bs = params[0::2], params[1::2]
-        x3 = _x3_aux()
         dl = [None] * L                 # per layer: (snapshot, ordinal, thresh, scale) of its dropout, or None
         n_drop = sum(1 for p in (drops or ()) if p > 0)
         snap = dropout_snapshot(x.device, n_drop) if n_drop else None
@@ -858,11 +874,10 @@ class _MLPChain(torch.autograd.Function):
                 _lib.call("b2_head_fwd", _ptr(h), _ptr(W), _ptr(b), M, K, act, _ptr(y), _stream())
             elif kinds[i] == "tc" and h.data_ptr() % 16 == 0:
                 y_small = empty_aux(M, N, x.device) if want_small else None
-                gemm_ex(h, W, y, a_small=smalls[-1], b_small=weight_aux(W), bias=b, act=act, out_small=y_small,
-                        drop=dl[i])
+                _linear_fwd(True, h, smalls[-1], W, y, bias=b, act=act, out_small=y_small, drop=dl[i])
             else:
                 kinds[i] = "simt"
-                gemm_f32(h, W, y, b_t=True, bias=b, act=act)
+                _linear_fwd(False, h, None, W, y, bias=b, act=act)
             if dl[i] is not None and kinds[i] != "tc":
                 dropout_apply(y, snap, dl[i][1], drops[i], out=y)
             if want_small and y_small is None:
@@ -881,7 +896,6 @@ class _MLPChain(torch.autograd.Function):
         L = len(acts)
         M = hs[0].shape[0]
         dev = hs[0].device
-        x3 = _x3_aux()
         grads = [None] * len(params)
 
         def bias_buf(i):
@@ -902,8 +916,7 @@ class _MLPChain(torch.autograd.Function):
             if kinds[i] == "head":
                 if dl[i] is not None and not g_is_dz:   # a width-1 dropout layer: its mask in the explicit pass
                     gb = bias_buf(i)
-                    g, _, _, _ = prep_operand(g, y if act != B2_ACT_NONE else None, act, want_out=True, colsum=gb,
-                                              drop=dl[i])
+                    g, _ = _grad_operand(g, y, act, False, colsum=gb, drop=dl[i])
                     grads[2 * i + 1] = gb
                     g_is_dz = True
                 gw = _grad_buffer(W, zero=False)
@@ -927,51 +940,64 @@ class _MLPChain(torch.autograd.Function):
                     grads[2 * (i - 1) + 1] = gb_prev
                 g, g_small, g_is_dz = gx, gx_small, fuse_prev
                 continue
+            tc = kinds[i] == "tc"       # else an fp32 SIMT layer inside a chain (odd shapes)
             if not g_is_dz:     # top of the chain (or below a non-fusing layer): one explicit pass over dY
                 gb = bias_buf(i)
-                fused = act != B2_ACT_NONE
-                out, sm, _, _ = prep_operand(g, y if fused else None, act, want_out=fused or dl[i] is not None,
-                                             want_small=x3 and kinds[i] == "tc", colsum=gb, drop=dl[i])
-                gz, gz_small = (out if (fused or dl[i] is not None) else g), sm
-                if gz_small is None and kinds[i] == "tc":
-                    gz_small = make_aux(gz)          # bf16 mode (None for single-pass TF32)
+                gz, gz_small = _grad_operand(g, y, act, tc, colsum=gb, drop=dl[i])
                 grads[2 * i + 1] = gb
             else:
                 gz, gz_small = g, g_small
-            if kinds[i] == "tc":
+            ready = None
+            if tc:
                 if fork is None and W.requires_grad and _FORK["on"] and gz.is_cuda:
                     fork = _WgradFork(dev)
-                ready = fork.ready() if (fork is not None and W.requires_grad) else None
+                if fork is not None and W.requires_grad:
+                    ready = fork.ready()
                 if gx is not None:
                     prev_act = acts[i - 1] if fuse_prev else B2_ACT_NONE
                     gb_prev = bias_buf(i - 1) if fuse_prev else None
-                    gemm_ex(gz, W, gx, b_mn=True, a_small=gz_small, b_small=weight_aux(W),
-                            ybwd=hs[i] if (fuse_prev and prev_act != B2_ACT_NONE) else None, act_bwd=prev_act,
-                            out_small=gx_small, colsum=gb_prev,
-                            drop=dl[i - 1] if fuse_prev else None)                                # dX (= dZ_{i-1})
-                if W.requires_grad:
-                    gw = _grad_buffer(W, zero=False)
-                    if ready is not None:
-                        fork.gemm(ready, gz, gz_small, h, smalls[i], gw)
-                    else:
-                        gemm_ex(gz, h, gw, a_mn=True, b_mn=True, a_small=gz_small, b_small=smalls[i],
-                                out_is_zero=_is_zeroed(gw))                                          # dW = dZ^T X
-                    grads[2 * i] = gw
-                g, g_small, g_is_dz = gx, gx_small, fuse_prev
-            else:               # fp32 SIMT layer inside a chain (odd shapes)
-                if gx is not None:
-                    gemm_f32(gz, W, gx)
-                if W.requires_grad:
-                    gw = _grad_buffer(W, zero=False)
-                    gemm_f32(gz, h, gw, a_t=True)
-                    grads[2 * i] = gw
-                g, g_small, g_is_dz = gx, None, False    # layer i-1 takes the explicit pass (its own db)
-                continue
-            if fuse_prev:
-                grads[2 * (i - 1) + 1] = gb_prev
+                    _linear_dgrad(True, gz, gz_small, W, gx,
+                                  ybwd=hs[i] if (fuse_prev and prev_act != B2_ACT_NONE) else None, act_bwd=prev_act,
+                                  out_small=gx_small, colsum=gb_prev,
+                                  drop=dl[i - 1] if fuse_prev else None)                          # dX (= dZ_{i-1})
+                if fuse_prev:
+                    grads[2 * (i - 1) + 1] = gb_prev
+            elif gx is not None:
+                _linear_dgrad(False, gz, None, W, gx)
+            if W.requires_grad:
+                gw = _grad_buffer(W, zero=False)
+                _linear_wgrad(tc, gz, gz_small, h, smalls[i], gw, fork, ready)
+                grads[2 * i] = gw
+            # below a SIMT layer, layer i-1 takes the explicit pass (its own db)
+            g, g_small, g_is_dz = (gx, gx_small, fuse_prev) if tc else (gx, None, False)
         if fork is not None:
             fork.join()
         return (g if ctx.needs_input_grad[0] else None, None, None) + tuple(grads)
+
+
+def _cross_step_fwd(a, a_aux, W, w_aux, bias, x0, add, tc):
+    """The CrossNetV2 step out = add + x0 * lin, lin = a W^T + bias: returns (out, lin).  On the tensor cores the
+    GEMM epilogue applies `add + mul * (acc + bias)` and keeps lin for the backward — no elementwise pass."""
+    out, lin = torch.empty_like(add), torch.empty_like(add)
+    if tc:
+        _linear_fwd(True, a, a_aux, W, out, w_aux, bias=bias, mul=x0, add=add, out_pre=lin)
+    else:
+        _linear_fwd(False, a, None, W, lin, bias=bias)
+        torch.addcmul(add, x0, lin, out=out)
+    return out, lin
+
+
+def _cross_step_bwd(g, x0, a, a_aux, W, w_aux, bias, gw, tc, add_g):
+    """Backward of _cross_step_fwd but for dx_0 = g * lin, which the caller takes: dlin = g * x_0 (one pass: value,
+    auxiliary operand, bias gradient), d_a = dlin W (+ g in the GEMM's epilogue when add_g: `a` was also `add`),
+    dW = dlin^T a into gw (None: not wanted).  Returns (d_a, the bias gradient or None)."""
+    gb = _grad_buffer(bias, zero=False) if (bias is not None and bias.requires_grad) else None
+    dlin, dlin_aux = _grad_operand(g, x0, B2_PREP_MUL, tc, colsum=gb)
+    d_a = torch.empty_like(a)
+    _linear_dgrad(tc, dlin, dlin_aux, W, d_a, w_aux, add=g if add_g else None)
+    if gw is not None:
+        _linear_wgrad(tc, dlin, dlin_aux, a, a_aux, gw)
+    return d_a, gb
 
 
 class _CrossV2Layer(torch.autograd.Function):
@@ -983,19 +1009,10 @@ class _CrossV2Layer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x0, xi, weight, bias):
         x0, xi = _f32c(x0), _f32c(xi)
-        M, d = xi.shape
-        out = torch.empty_like(xi)
-        lin = torch.empty_like(xi)
-        ctx.tc = (_tc_layer_ok(weight) and weight.shape[0] == weight.shape[1] == d
+        ctx.tc = (_tc_layer_ok(weight) and weight.shape[0] == weight.shape[1] == xi.shape[1]
                   and xi.data_ptr() % 16 == 0 and x0.data_ptr() % 16 == 0)
-        ctx.xi_small = None
-        if ctx.tc:
-            ctx.xi_small = make_aux(xi)
-            gemm_ex(xi, weight, out, a_small=ctx.xi_small, b_small=weight_aux(weight), bias=bias,
-                    mul=x0, add=xi, out_pre=lin)
-        else:
-            gemm_f32(xi, weight, lin, b_t=True, bias=bias)
-            torch.addcmul(xi, x0, lin, out=out)
+        ctx.xi_small = make_aux(xi) if ctx.tc else None
+        out, lin = _cross_step_fwd(xi, ctx.xi_small, weight, None, bias, x0, xi, ctx.tc)
         ctx.save_for_backward(x0, xi, lin, weight)
         ctx.bias = bias
         return out
@@ -1004,23 +1021,8 @@ class _CrossV2Layer(torch.autograd.Function):
     def backward(ctx, g):
         x0, xi, lin, weight = ctx.saved_tensors
         g = _f32c(g)
-        bias = ctx.bias
-        gb = _grad_buffer(bias, zero=False) if (bias is not None and bias.requires_grad) else None
-        x3 = _x3_aux()
-        dlin, dlin_small, _, _ = prep_operand(g, x0, B2_PREP_MUL, want_out=True, want_small=x3 and ctx.tc, colsum=gb)
-        if ctx.tc and dlin_small is None:
-            dlin_small = make_aux(dlin)          # bf16 mode (None for single-pass TF32)
-        gxi = torch.empty_like(xi)
         gw = _grad_buffer(weight, zero=False) if weight.requires_grad else None
-        if ctx.tc:
-            gemm_ex(dlin, weight, gxi, b_mn=True, a_small=dlin_small, b_small=weight_aux(weight),
-                    add=g)                                                                   # dx_i = g + dlin W
-            if gw is not None:
-                gemm_ex(dlin, xi, gw, a_mn=True, b_mn=True, a_small=dlin_small, b_small=ctx.xi_small, out_is_zero=_is_zeroed(gw))
-        else:
-            gemm_f32(dlin, weight, gxi, add=g)
-            if gw is not None:
-                gemm_f32(dlin, xi, gw, a_t=True)
+        gxi, gb = _cross_step_bwd(g, x0, xi, ctx.xi_small, weight, None, ctx.bias, gw, ctx.tc, add_g=True)
         gx0 = g * lin if ctx.needs_input_grad[0] else None
         return gx0, gxi, gw, gb
 
@@ -1069,22 +1071,13 @@ class _CrossMixLayer(torch.autograd.Function):
         tc = _tc_layer_ok(W1) and _tc_layer_ok(W2) and xl.data_ptr() % 16 == 0 and x0.data_ptr() % 16 == 0
         P = torch.empty((B, n1), dtype=torch.float32, device=dev)
         A2 = torch.empty((B, k2), dtype=torch.float32, device=dev)
-        out = torch.empty_like(xl)
-        lin = torch.empty_like(xl)
-        b = bias.view(-1)
         xl_aux = a2_aux = w1_aux = w2_aux = None
         if tc:
             xl_aux, w1_aux, w2_aux = make_aux(xl), make_aux(W1), make_aux(W2)
             a2_aux = empty_aux(B, k2, dev)
-            gemm_ex(xl, W1, P, a_small=xl_aux, b_small=w1_aux)
-        else:
-            gemm_f32(xl, W1, P, b_t=True)
+        _linear_fwd(tc, xl, xl_aux, W1, P, w1_aux)
         _lib.call("b2_crossmix_fwd", _ptr(P), _ptr(C), B, r, E, _ptr(A2), *_aux_args(a2_aux), _stream())
-        if tc:
-            gemm_ex(A2, W2, out, a_small=a2_aux, b_small=w2_aux, bias=b, mul=x0, add=xl, out_pre=lin)
-        else:
-            gemm_f32(A2, W2, lin, b_t=True, bias=b)
-            torch.addcmul(xl, x0, lin, out=out)
+        out, lin = _cross_step_fwd(A2, a2_aux, W2, w2_aux, bias.view(-1), x0, xl, tc)
         ctx.save_for_backward(x0, xl, lin, P, A2, W1, W2, C)
         ctx.tc, ctx.aux, ctx.r, ctx.bias = tc, (xl_aux, a2_aux, w1_aux, w2_aux), r, bias
         return out
@@ -1099,32 +1092,17 @@ class _CrossMixLayer(torch.autograd.Function):
         E = C.shape[0]
         n1, k2 = W1.shape[0], W2.shape[1]
         dev = xl.device
-        gb = _grad_buffer(bias, zero=False) if bias.requires_grad else None
-        dlin, dlin_small, _, _ = prep_operand(g, x0, B2_PREP_MUL, want_out=True, want_small=_x3_aux() and tc,
-                                              colsum=gb)
-        if tc and dlin_small is None:
-            dlin_small = make_aux(dlin)          # bf16 mode (None for single-pass TF32)
-        dA2 = torch.empty((B, k2), dtype=torch.float32, device=dev)
         dW2 = torch.empty((d, k2), dtype=torch.float32, device=dev)
         dA1 = torch.empty((B, n1), dtype=torch.float32, device=dev)
         dW1 = torch.empty((n1, d), dtype=torch.float32, device=dev)
         gxl = torch.empty_like(xl)
         gC = torch.zeros_like(C)
         da1_aux = empty_aux(B, n1, dev) if tc else None
-        if tc:
-            gemm_ex(dlin, W2, dA2, b_mn=True, a_small=dlin_small, b_small=w2_aux)                   # dA2 = dlin W2
-            gemm_ex(dlin, A2, dW2, a_mn=True, b_mn=True, a_small=dlin_small, b_small=a2_aux)      # dW2 = dlin^T A2
-        else:
-            gemm_f32(dlin, W2, dA2)
-            gemm_f32(dlin, A2, dW2, a_t=True)
+        dA2, gb = _cross_step_bwd(g, x0, A2, a2_aux, W2, w2_aux, bias, dW2, tc, add_g=False)
         _lib.call("b2_crossmix_bwd", _ptr(P), _ptr(C), _ptr(dA2), B, r, E, _ptr(dA1), *_aux_args(da1_aux),
                   _ptr(gC), _stream())
-        if tc:
-            gemm_ex(dA1, W1, gxl, b_mn=True, a_small=da1_aux, b_small=w1_aux, add=g)               # dx_l = g + dA1 W1
-            gemm_ex(dA1, xl, dW1, a_mn=True, b_mn=True, a_small=da1_aux, b_small=xl_aux)          # dW1 = dA1^T x_l
-        else:
-            gemm_f32(dA1, W1, gxl, add=g)
-            gemm_f32(dA1, xl, dW1, a_t=True)
+        _linear_dgrad(tc, dA1, da1_aux, W1, gxl, w1_aux, add=g)                                    # dx_l = g + dA1 W1
+        _linear_wgrad(tc, dA1, da1_aux, xl, xl_aux, dW1)                                           # dW1 = dA1^T x_l
         gU = torch.empty((E, d, r), dtype=torch.float32, device=dev)
         gV = torch.empty_like(gU)
         gG = torch.empty((E, d), dtype=torch.float32, device=dev)
