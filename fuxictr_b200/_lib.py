@@ -87,19 +87,14 @@ SIGNATURES = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_device_cc": (c_int, [c_int]),
     "b2_set_l2_fetch_granularity": (c_int, [c_int]),
-    "b2_embed_gather_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    "b2_embed_gather_hot_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
-    "b2_embed_scatter_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p]),
-    "b2_embed_scatter_bwd_ex": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_embed_gather_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    "b2_embed_scatter_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_lr_fwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "b2_lr_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
-    "b2_lr_bwd_ex": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_lr_bwd": (c_int, [_FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_front_fwd": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_front_bwd": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                             c_void_p, c_void_p, c_void_p, c_void_p]),
-    "b2_front_bwd_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_lazy_sumsq": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "b2_lazy_adam_step": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_void_p]),
@@ -109,24 +104,16 @@ SIGNATURES = {
     "b2_adam_step_sched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
                                    c_float, c_float, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_shard_push": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
-                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p]),
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                              c_void_p]),
     "b2_shard_pull": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_float,
-                              c_void_p, c_void_p, c_int32, c_void_p]),
-    "b2_shard_push_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
-                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
-    "b2_shard_pull_ex": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_float,
-                                 c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
-    "b2_shard_push_pad": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
-                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
-                                  c_void_p]),
+                              c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
     "b2_shard_publish_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, _FIELD_P, _FIELD_P, c_int, c_int, c_int,
                                      c_void_p, c_void_p]),
     "b2_shard_publish_rows": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p, _FIELD_P, _FIELD_P, c_int,
                                       c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_shard_lookup": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
-    "b2_peer_bcast": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p]),
-    "b2_peer_bcast_ids": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "b2_front_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
                                 c_void_p]),
     "b2_front_gprep": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p,
@@ -161,14 +148,10 @@ SIGNATURES = {
     "b2_din_softmax_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "b2_gemm_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64,
                             c_int64, c_int64, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
-    "b2_gemm_tc_supported": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64]),
-    "b2_gemm_tc": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
-                           c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_gemm_tc_ex": (c_int, [c_void_p, c_void_p]),
     "b2_gemm_tc_plan": (c_int, [c_void_p, c_void_p]),
     "b2_to_bf16": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p]),
     "b2_split_tf32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
-    "b2_transpose_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_prep_operand": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p]),
     "b2_head_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
@@ -180,8 +163,6 @@ SIGNATURES = {
     "b2_dropout_rng_take": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "b2_dropout_apply": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, ctypes.c_uint32,
                                  c_float, c_void_p]),
-    "b2_act_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
-    "b2_colsum": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_void_p]),
     "b2_logit_bce_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_sumsq": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),

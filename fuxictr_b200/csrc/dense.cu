@@ -213,81 +213,6 @@ extern "C" B2_API int b2_gemm_f32(const float* a, int64_t a_rs, int64_t a_cs, co
 }
 
 // ---------------------------------------------------------------------------------
-// Elementwise backward of an activation given its OUTPUT y.
-// ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-act_bwd_kernel(const float* __restrict__ y, const float* __restrict__ gy, float* __restrict__ gx,
-               int64_t n, int act) {
-  for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t) gridDim.x * blockDim.x) {
-    const float yv = __ldg(y + i), g = __ldg(gy + i);
-    float r;
-    if (act == B2_ACT_RELU) r = (yv > 0.f) ? g : 0.f;             // threshold_backward
-    else if (act == B2_ACT_SIGMOID) r = g * ((1.f - yv) * yv);   // sigmoid_backward
-    else r = g;
-    gx[i] = r;
-  }
-}
-
-extern "C" B2_API int b2_act_bwd(const float* y, const float* gy, float* gx, int64_t n, int act,
-                          void* stream) {
-  B2_REQUIRE(y && gy && gx, "NULL pointer");
-  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad activation code %d", act);
-  if (n == 0) return B2_OK;
-  int64_t blocks = b2_ceil_div(n, 256);
-  if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
-  act_bwd_kernel<<<(int) blocks, 256, 0, (cudaStream_t) stream>>>(y, gy, gx, n, act);
-  B2_CUDA_LAUNCH_CHECK("b2_act_bwd");
-  return B2_OK;
-}
-
-// ---------------------------------------------------------------------------------
-// Column sums (bias gradients): out[n] (+)= sum_m x[m, n].
-// CTA = 32 columns x 8 row-lanes; grid.y splits the rows; partials meet with `red`.
-// ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-colsum_kernel(const float* __restrict__ x, int64_t M, int64_t N, int64_t ld,
-              float* __restrict__ out, int64_t rows_per_cta) {
-  __shared__ float sm[8][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int64_t n = (int64_t) blockIdx.x * 32 + tx;
-  const int64_t r0 = (int64_t) blockIdx.y * rows_per_cta;
-  const int64_t r1 = min(M, r0 + rows_per_cta);
-  float acc = 0.f;
-  if (n < N)
-    for (int64_t m = r0 + ty; m < r1; m += 8) acc += __ldg(x + m * ld + n);
-  sm[ty][tx] = acc;
-  __syncthreads();
-  if (ty == 0 && n < N) {
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += sm[i][tx];
-    b2_red_add(out + n, t);
-  }
-}
-
-extern "C" B2_API int b2_colsum(const float* x, int64_t M, int64_t N, int64_t ld, float* out,
-                         int accumulate, void* stream) {
-  B2_REQUIRE(x && out, "NULL pointer");
-  B2_REQUIRE(M >= 0 && N >= 1 && ld >= N, "bad shape");
-  cudaStream_t st = (cudaStream_t) stream;
-  if (!accumulate) {
-    cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float) * N, st);
-    if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_colsum: memset: %s", cudaGetErrorString(e));
-  }
-  if (M == 0) return B2_OK;
-  const int64_t col_blocks = b2_ceil_div(N, 32);
-  int64_t row_splits = b2_ceil_div(2 * B2_NUM_SMS, col_blocks);
-  if (row_splits > b2_ceil_div(M, 64)) row_splits = b2_ceil_div(M, 64);
-  if (row_splits < 1) row_splits = 1;
-  const int64_t rows_per_cta = b2_ceil_div(M, row_splits);
-  dim3 grid((unsigned) col_blocks, (unsigned) b2_ceil_div(M, rows_per_cta));
-  colsum_kernel<<<grid, 256, 0, st>>>(x, M, N, ld, out, rows_per_cta);
-  B2_CUDA_LAUNCH_CHECK("b2_colsum");
-  return B2_OK;
-}
-
-// ---------------------------------------------------------------------------------
 // Fused logit sum + sigmoid + binary cross entropy (mean) + dL/dlogit.
 //   p = 1/(1+exp(-z))                                    nn.Sigmoid, rank_model.py:447-448
 //   l = -(y*max(log p,-100) + (1-y)*max(log1p(-p),-100)) F.binary_cross_entropy

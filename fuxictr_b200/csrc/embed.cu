@@ -445,14 +445,8 @@ static int launch_scatter(const B2FieldPack& pack, int64_t batch, int vec, int m
 }
 
 extern "C" B2_API int b2_embed_gather_fwd(const b2_field* fields, int nfields, int64_t batch,
-                                   int idx_dtype, int elem_dtype, float* mean_count,
-                                   int32_t* status, void* stream) {
-  return b2_embed_gather_hot_fwd(fields, nfields, batch, idx_dtype, elem_dtype, mean_count, status, 0, stream);
-}
-
-extern "C" B2_API int b2_embed_gather_hot_fwd(const b2_field* fields, int nfields, int64_t batch,
-                                       int idx_dtype, int elem_dtype, float* mean_count,
-                                       int32_t* status, int hot_rows, void* stream) {
+                                          int idx_dtype, int elem_dtype, float* mean_count,
+                                          int32_t* status, int hot_rows, void* stream) {
   B2_REQUIRE(hot_rows >= 0, "negative hot_rows");
   B2_REQUIRE(elem_dtype == B2_F32, "elem_dtype %d unsupported (only B2_F32)", elem_dtype);
   B2_REQUIRE(batch >= 0, "negative batch");
@@ -475,14 +469,8 @@ extern "C" B2_API int b2_embed_gather_hot_fwd(const b2_field* fields, int nfield
 }
 
 extern "C" B2_API int b2_embed_scatter_bwd(const b2_field* fields, int nfields, int64_t batch,
-                                    int idx_dtype, int elem_dtype, const float* mean_count,
-                                    void* stream) {
-  return b2_embed_scatter_bwd_ex(fields, nfields, batch, idx_dtype, elem_dtype, mean_count, nullptr, stream);
-}
-
-extern "C" B2_API int b2_embed_scatter_bwd_ex(const b2_field* fields, int nfields, int64_t batch,
-                                              int idx_dtype, int elem_dtype, const float* mean_count,
-                                              const b2_touch* touch, void* stream) {
+                                           int idx_dtype, int elem_dtype, const float* mean_count,
+                                           const b2_touch* touch, void* stream) {
   b2_touch tch;
   int rc = b2_touch_arg(touch, tch);
   if (rc != B2_OK) return rc;
@@ -543,12 +531,7 @@ extern "C" B2_API int b2_lr_fwd(const b2_field* fields, int nfields, int64_t bat
 }
 
 extern "C" B2_API int b2_lr_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                         const float* gout, float* gbias, void* stream) {
-  return b2_lr_bwd_ex(fields, nfields, batch, idx_dtype, gout, gbias, nullptr, stream);
-}
-
-extern "C" B2_API int b2_lr_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                                   const float* gout, float* gbias, const b2_touch* touch, void* stream) {
+                                const float* gout, float* gbias, const b2_touch* touch, void* stream) {
   b2_touch tch;
   int rc = b2_touch_arg(touch, tch);
   if (rc != B2_OK) return rc;

@@ -378,15 +378,7 @@ extern "C" B2_API int b2_front_fwd(const b2_field* emb_fields, const b2_field* l
 extern "C" B2_API int b2_front_bwd(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
                                    int64_t batch, int idx_dtype, int want_fm, const float* emb_saved,
                                    const float* gx, const float* sums, const float* glogit, float* gbias,
-                                   const b2_lazy_ctx* lazy, void* stream) {
-  return b2_front_bwd_ex(emb_fields, lr_fields, nfields, batch, idx_dtype, want_fm, emb_saved, gx, sums, glogit,
-                         gbias, lazy, nullptr, stream);
-}
-
-extern "C" B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                      int64_t batch, int idx_dtype, int want_fm, const float* emb_saved,
-                                      const float* gx, const float* sums, const float* glogit, float* gbias,
-                                      const b2_lazy_ctx* lazy, const b2_touch* touch, void* stream) {
+                                   const b2_lazy_ctx* lazy, const b2_touch* touch, void* stream) {
   int rc = check_front(emb_fields, lr_fields, nfields, true);
   if (rc != B2_OK) return rc;
   b2_touch tch;

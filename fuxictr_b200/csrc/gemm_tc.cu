@@ -692,32 +692,6 @@ split_tf32_kernel(const float* __restrict__ x, float* __restrict__ small, int64_
   }
 }
 
-// out (cols, rows) = in (rows, cols)^T through a padded shared tile; optionally also the
-// small() part of the transposed values (for the 3xTF32 operands of dgrad / wgrad).
-__global__ void __launch_bounds__(256)
-transpose_kernel(const float* __restrict__ in, int64_t rows, int64_t cols, int64_t ld_in,
-                 float* __restrict__ out, int64_t ld_out, float* __restrict__ out_small) {
-  __shared__ float tile[32][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
-  const int64_t c0 = (int64_t) blockIdx.x * 32, r0 = (int64_t) blockIdx.y * 32;
-#pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    const int64_t r = r0 + ty + i, c = c0 + tx;
-    tile[ty + i][tx] = (r < rows && c < cols) ? __ldg(in + r * ld_in + c) : 0.f;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    const int64_t c = c0 + ty + i, r = r0 + tx;  // out[c, r]
-    if (c < cols && r < rows) {
-      const float v = tile[tx][ty + i];
-      out[c * ld_out + r] = v;
-      if (out_small != nullptr)
-        out_small[c * ld_out + r] = tf32_small(v);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------
 // Operand preparation for the K-major tensor-core GEMMs, one pass over a (R, C) matrix:
 //   v      = act'(y) * x          (act-backward fused when y != NULL; y is the activation OUTPUT)
@@ -986,12 +960,6 @@ static bool tma_ok_e(const void* p, int64_t ld, int esz) {
 }
 static bool tma_ok(const float* p, int64_t ld) { return tma_ok_e(p, ld, 4); }
 
-extern "C" B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const float* b, int64_t ldb,
-                                           int64_t M, int64_t N, int64_t K) {
-  return (tma_ok(a, lda) && tma_ok(b, ldb) && M >= 1 && N >= 1 && K >= 1 && M < (1ll << 31) &&
-          N < (1ll << 31) && K < (1ll << 31)) ? 1 : 0;
-}
-
 // plan != NULL: fill in the launch plan (tile shape, ring depths, shared memory) and return without
 // touching the device — pure host arithmetic, so the CPU test-suite can sweep it (tests/test_abi.py).
 template <int BN, int MODE, bool DROP>
@@ -1001,10 +969,10 @@ static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
   // idempotent per-process property (C++11 guarantees the initialiser runs once, thread-safely)
   static const cudaError_t attr_rc =
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) tc::ring_smem_max(BN, MODE));
-  if (attr_rc != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: smem attribute: %s", cudaGetErrorString(attr_rc));
+  if (attr_rc != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc_ex: smem attribute: %s", cudaGetErrorString(attr_rc));
   B2_REQUIRE(p.ring.smem <= tc::ring_smem_max(BN, MODE), "ring exceeds the shared-memory attribute");
   B2_LAUNCH(kern, grid, tc::NTHREADS, p.ring.smem, st, p);
-  B2_CUDA_LAUNCH_CHECK("b2_gemm_tc");
+  B2_CUDA_LAUNCH_CHECK("b2_gemm_tc_ex");
   return B2_OK;
 }
 
@@ -1143,11 +1111,11 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   }
   if (splits > 1 && !p.beta && !(d->flags & B2_GEMM_C_IS_ZERO)) {
     cudaError_t e = cudaMemset2DAsync(c, (size_t) ldc * 4, 0, (size_t) N * 4, (size_t) M, st);
-    if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc_ex: memset: %s", cudaGetErrorString(e));
   }
   if (d->colsum != nullptr && !(d->flags & B2_GEMM_COLSUM_IS_ZERO)) {
     cudaError_t e = cudaMemsetAsync(d->colsum, 0, sizeof(float) * (size_t) N, st);
-    if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc: memset: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_gemm_tc_ex: memset: %s", cudaGetErrorString(e));
   }
   return launch(p, (int) total_tiles, st);
 }
@@ -1185,19 +1153,6 @@ extern "C" B2_API int b2_to_bf16(const float* x, int64_t rows, int64_t cols, int
   return B2_OK;
 }
 
-extern "C" B2_API int b2_gemm_tc(const float* a, int64_t lda, const float* b, int64_t ldb, float* c,
-                                 int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int act,
-                                 const float* mul, const float* add, int beta_accumulate,
-                                 const float* a_small, const float* b_small, void* stream) {
-  b2_gemm_desc d;
-  memset(&d, 0, sizeof(d));
-  d.a = a; d.b = b; d.a_small = a_small; d.b_small = b_small; d.c = c;
-  d.bias = bias; d.mul = mul; d.add = add;
-  d.lda = lda; d.ldb = ldb; d.ldc = ldc; d.M = M; d.N = N; d.K = K;
-  d.act = act; d.beta_accumulate = beta_accumulate;
-  return b2_gemm_tc_ex(&d, stream);
-}
-
 extern "C" B2_API int b2_split_tf32(const float* x, float* small, int64_t n, void* stream) {
   B2_REQUIRE(x && small, "NULL pointer");
   if (n <= 0) return B2_OK;
@@ -1205,18 +1160,6 @@ extern "C" B2_API int b2_split_tf32(const float* x, float* small, int64_t n, voi
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
   B2_LAUNCH(tc::split_tf32_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, x, small, n);
   B2_CUDA_LAUNCH_CHECK("b2_split_tf32");
-  return B2_OK;
-}
-
-extern "C" B2_API int b2_transpose_f32(const float* in, int64_t rows, int64_t cols, int64_t ld_in,
-                                       float* out, int64_t ld_out, float* out_small, void* stream) {
-  B2_REQUIRE(in && out, "NULL pointer");
-  B2_REQUIRE(rows >= 0 && cols >= 0 && ld_in >= cols && ld_out >= rows, "bad shape");
-  if (rows == 0 || cols == 0) return B2_OK;
-  dim3 grid((unsigned) b2_ceil_div(cols, 32), (unsigned) b2_ceil_div(rows, 32));
-  B2_REQUIRE(grid.y <= 65535, "too many rows for this launch geometry");
-  tc::transpose_kernel<<<grid, 256, 0, (cudaStream_t) stream>>>(in, rows, cols, ld_in, out, ld_out, out_small);
-  B2_CUDA_LAUNCH_CHECK("b2_transpose_f32");
   return B2_OK;
 }
 

@@ -18,7 +18,8 @@
 //   pass over the peers' id matrices), pulls each gradient row from the requesting rank's `gemb`
 //   (P2P loads) and scatter-adds it (warp-aggregated `red.global.add.v4.f32`) into its local
 //   dense-gradient shard.
-// `shard_bcast_kernel`: one launch stores this rank's batch matrix into its slot on every peer.
+// `shard_publish_ids_kernel`: one launch stores this rank's ids, narrowed to int32, and the padding rows it owns
+//   into its slot on every peer.
 // Replaces, for sharded tables, FeatureEmbedding/LogisticRegression lookups and their autograd
 // (fuxictr/pytorch/layers/embeddings/feature_embedding.py:261-297,
 //  fuxictr/pytorch/layers/blocks/logistic_regression.py:55-58); the reference has no multi-GPU path.
@@ -280,23 +281,6 @@ shard_pull_kernel(const __grid_constant__ B2FieldPack emb, const __grid_constant
   }
 }
 
-// One launch: this rank's buffer -> the same slot on every peer (P2P stores, 16 B per thread-iteration).
-__global__ void __launch_bounds__(256)
-shard_bcast_kernel(const void* __restrict__ src, int64_t nbytes, const __grid_constant__ BcastDst dst, int world) {
-  const int64_t tid = (int64_t) blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t) gridDim.x * blockDim.x;
-  const int64_t n16 = nbytes >> 4;
-  const int4* s16 = reinterpret_cast<const int4*>(src);
-  for (int64_t i = tid; i < n16; i += nth) {
-    const int4 v = __ldg(s16 + i);
-    for (int p = 0; p < world; ++p) reinterpret_cast<int4*>(dst.p[p])[i] = v;
-  }
-  const int64_t tail0 = n16 << 4;
-  for (int64_t i = tail0 + tid * 4; i + 4 <= nbytes; i += nth * 4) {
-    const int32_t v = *reinterpret_cast<const int32_t*>(reinterpret_cast<const char*>(src) + i);
-    for (int p = 0; p < world; ++p) *reinterpret_cast<int32_t*>(reinterpret_cast<char*>(dst.p[p]) + i) = v;
-  }
-}
-
 // The id exchange, compressed: the batch matrix arrives as float64 (the reference's collator), the owners
 // only need the row numbers — one launch truncates like `.long()`, narrows to int32 (vocabularies < 2^31)
 // and stores the result into this rank's slot on every peer: 4 bytes per id over NVLink instead of 8.
@@ -316,12 +300,6 @@ __device__ __forceinline__ void bcast_ids(const void* __restrict__ src, int64_t 
     const int v = (int) b2_load_index<IdxT>(src, i);
     for (int p = 0; p < world; ++p) reinterpret_cast<int32_t*>(dst.p[p])[i] = v;
   }
-}
-
-template <typename IdxT>
-__global__ void __launch_bounds__(256)
-shard_bcast_ids_kernel(const void* __restrict__ src, int64_t n, const __grid_constant__ BcastDst dst, int world) {
-  bcast_ids<IdxT>(src, n, dst, world);
 }
 
 // Padding rows this rank owns (NULL: another rank publishes that field's row), and every rank's pad buffer.
@@ -547,21 +525,25 @@ int check_lazy(const b2_lazy_ctx* lz) {
   B2_REQUIRE(lz->worklist_capacity >= 1, "lazy context: worklist_capacity %d", lz->worklist_capacity);
   return B2_OK;
 }
-}  // namespace
 
-extern "C" B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                        int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                                        int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                                        float* const* peer_lrw, int32_t* status, int32_t* owned,
-                                        int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                                        const float* pad_rows, void* stream) {
+// What a shard_push_kernel launch needs beyond the caller's own arguments.
+struct PushLaunch {
+  const B2FieldPack* epack;
+  const B2FieldPack* lpack;
+  PeerPtrs pp;
+  int dim, lpr_log2, has_lr, grid;
+  size_t smem;
+};
+
+// The host side shared by the training push and the evaluation lookup (both launch shard_push_kernel): the
+// checks of the fields, the peer pointer arrays and the padding rows, then the field packs, the peer buffers, the
+// shared memory (both packs and the 256-entry list) and a grid over every candidate of a full batch.
+int push_setup(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch_local, int world,
+               int rank, const void* const* peer_ids, float* const* peer_emb, float* const* peer_lrw,
+               const float* pad_rows, PushLaunch& pl) {
   int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
   if (rc != B2_OK) return rc;
-  rc = check_lazy(lazy);
-  if (rc != B2_OK) return rc;
   B2_REQUIRE(peer_ids && peer_emb && (lr_fields == nullptr || peer_lrw != nullptr), "NULL peer pointer array");
-  B2_REQUIRE(owned == nullptr || (owned_count != nullptr && owned_capacity >= 1), "owned list needs a counter and a capacity");
-  B2_REQUIRE(owned == nullptr || ((uintptr_t) owned % 16) == 0, "owned list must be 16-byte aligned");
   B2_REQUIRE(pad_rows == nullptr || ((uintptr_t) pad_rows % 16) == 0, "pad_rows must be 16-byte aligned");
   if (pad_rows != nullptr && lr_fields != nullptr)
     for (int i = 0; i < nfields; ++i)
@@ -569,66 +551,66 @@ extern "C" B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_fie
                  "field %d: the LR and embedding tables need one padding row", i);
   const int64_t nslots = count_slots(emb_fields, nfields);
   B2_REQUIRE(batch_local * nslots < (1ll << 31), "batch_local * slots must fit 31 bits");
+  static thread_local B2FieldPack epack, lpack;
+  fill_pack_cols(epack, emb_fields, nfields);
+  pl.has_lr = lr_fields != nullptr;
+  if (pl.has_lr) fill_pack_cols(lpack, lr_fields, nfields); else lpack.nfields = 0;
+  pl.epack = &epack;
+  pl.lpack = &lpack;
+  for (int i = 0; i < world; ++i) {
+    pl.pp.ids[i] = peer_ids[i];
+    pl.pp.emb[i] = peer_emb[i];
+    pl.pp.lrw[i] = pl.has_lr ? peer_lrw[i] : nullptr;
+    pl.pp.gemb[i] = nullptr;
+    pl.pp.glogit[i] = nullptr;
+  }
+  pl.dim = emb_fields[0].dim;
+  pl.lpr_log2 = next_pow2_log2((pl.dim + 3) / 4);
+  pl.smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
+  pl.grid = grid_for(batch_local * nslots * world, 256);
+  return B2_OK;
+}
+}  // namespace
+
+extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                    int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                                    int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                                    float* const* peer_lrw, int32_t* status, int32_t* owned,
+                                    int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                    const float* pad_rows, void* stream) {
+  PushLaunch pl;
+  int rc = push_setup(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_ids, peer_emb, peer_lrw,
+                      pad_rows, pl);
+  if (rc != B2_OK) return rc;
+  rc = check_lazy(lazy);
+  if (rc != B2_OK) return rc;
+  B2_REQUIRE(owned == nullptr || (owned_count != nullptr && owned_capacity >= 1), "owned list needs a counter and a capacity");
+  B2_REQUIRE(owned == nullptr || ((uintptr_t) owned % 16) == 0, "owned list must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t) stream;
   if (owned != nullptr) {
     cudaError_t e = cudaMemsetAsync(owned_count, 0, sizeof(int32_t), st);
     if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_shard_push: memset: %s", cudaGetErrorString(e));
   }
   if (batch_local <= 0) return B2_OK;
-  static thread_local B2FieldPack epack, lpack;
-  fill_pack_cols(epack, emb_fields, nfields);
-  const int has_lr = lr_fields != nullptr;
-  if (has_lr) fill_pack_cols(lpack, lr_fields, nfields); else lpack.nfields = 0;
-  PeerPtrs pp;
-  for (int i = 0; i < world; ++i) {
-    pp.ids[i] = peer_ids[i];
-    pp.emb[i] = peer_emb[i];
-    pp.lrw[i] = has_lr ? peer_lrw[i] : nullptr;
-    pp.gemb[i] = nullptr;
-    pp.glogit[i] = nullptr;
-  }
-  const int dim = emb_fields[0].dim;
-  const int lpr_log2 = next_pow2_log2((dim + 3) / 4);
-  const size_t smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
-  const int grid = grid_for(batch_local * nslots * world, 256);
   int4* ow = reinterpret_cast<int4*>(owned);
   static thread_local b2_lazy_ctx lz_none;
   const b2_lazy_ctx& lz = lazy ? *lazy : lz_none;
-  const bool len1 = epack.all_len1 != 0;
+  const bool len1 = pl.epack->all_len1 != 0;
   switch (idx_dtype) {
-    case B2_F64: rc = launch_push<double>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
-    case B2_I64: rc = launch_push<int64_t>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
-    case B2_I32: rc = launch_push<int32_t>(lazy != nullptr, len1, grid, smem, st, epack, lpack, pp, lz, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
+    case B2_F64: rc = launch_push<double>(lazy != nullptr, len1, pl.grid, pl.smem, st, *pl.epack, *pl.lpack, pl.pp, lz, batch_local, ids_stride, pl.dim, pl.lpr_log2, pl.has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
+    case B2_I64: rc = launch_push<int64_t>(lazy != nullptr, len1, pl.grid, pl.smem, st, *pl.epack, *pl.lpack, pl.pp, lz, batch_local, ids_stride, pl.dim, pl.lpr_log2, pl.has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
+    case B2_I32: rc = launch_push<int32_t>(lazy != nullptr, len1, pl.grid, pl.smem, st, *pl.epack, *pl.lpack, pl.pp, lz, batch_local, ids_stride, pl.dim, pl.lpr_log2, pl.has_lr, world, rank, status, ow, owned_count, owned_capacity, pad_rows); break;
     default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
   }
   B2_CUDA_LAUNCH_CHECK("b2_shard_push");
   return B2_OK;
 }
 
-extern "C" B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                       int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                                       int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                                       float* const* peer_lrw, int32_t* status, int32_t* owned,
-                                       int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                                       void* stream) {
-  return b2_shard_push_pad(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_ids, idx_dtype, ids_stride,
-                           peer_emb, peer_lrw, status, owned, owned_count, owned_capacity, lazy, nullptr, stream);
-}
-
-extern "C" B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                    int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                                    int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                                    float* const* peer_lrw, int32_t* status, int32_t* owned,
-                                    int32_t* owned_count, int32_t owned_capacity, void* stream) {
-  return b2_shard_push_ex(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_ids, idx_dtype, ids_stride,
-                          peer_emb, peer_lrw, status, owned, owned_count, owned_capacity, nullptr, stream);
-}
-
-extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                       int64_t batch_local, int world, int rank, const float* const* peer_gemb,
-                                       const float* const* peer_glogit, float scale, const int32_t* owned,
-                                       const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                                       const b2_touch* touch, void* stream) {
+extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                                    int64_t batch_local, int world, int rank, const float* const* peer_gemb,
+                                    const float* const* peer_glogit, float scale, const int32_t* owned,
+                                    const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                                    const b2_touch* touch, void* stream) {
   int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
   if (rc != B2_OK) return rc;
   rc = check_lazy(lazy);
@@ -664,36 +646,6 @@ extern "C" B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_fiel
                                                                has_lr, scale, reinterpret_cast<const int4*>(owned),
                                                                owned_count, owned_capacity, tch);
   B2_CUDA_LAUNCH_CHECK("b2_shard_pull");
-  return B2_OK;
-}
-
-extern "C" B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                                    int64_t batch_local, int world, int rank, const float* const* peer_gemb,
-                                    const float* const* peer_glogit, float scale, const int32_t* owned,
-                                    const int32_t* owned_count, int32_t owned_capacity, void* stream) {
-  return b2_shard_pull_ex(emb_fields, lr_fields, nfields, batch_local, world, rank, peer_gemb, peer_glogit, scale,
-                          owned, owned_count, owned_capacity, nullptr, nullptr, stream);
-}
-
-extern "C" B2_API int b2_peer_bcast_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,
-                                        int world, void* stream) {
-  B2_REQUIRE(src && peer_dst && world >= 1 && world <= 16 && count >= 0, "bad argument");
-  if (count == 0) return B2_OK;
-  BcastDst d;
-  for (int i = 0; i < 16; ++i) d.p[i] = nullptr;
-  for (int i = 0; i < world; ++i) {
-    B2_REQUIRE(peer_dst[i] != nullptr && ((uintptr_t) peer_dst[i] % 16) == 0, "peer_dst[%d] NULL or misaligned", i);
-    d.p[i] = peer_dst[i];
-  }
-  const int grid = grid_for(count >> 2, 256);
-  cudaStream_t st = (cudaStream_t) stream;
-  switch (idx_dtype) {
-    case B2_F64: shard_bcast_ids_kernel<double><<<grid, 256, 0, st>>>(src, count, d, world); break;
-    case B2_I64: shard_bcast_ids_kernel<int64_t><<<grid, 256, 0, st>>>(src, count, d, world); break;
-    case B2_I32: shard_bcast_ids_kernel<int32_t><<<grid, 256, 0, st>>>(src, count, d, world); break;
-    default: return b2_fail(B2_E_INVALID, "idx_dtype %d unsupported", idx_dtype);
-  }
-  B2_CUDA_LAUNCH_CHECK("b2_peer_bcast_ids");
   return B2_OK;
 }
 
@@ -763,60 +715,23 @@ extern "C" B2_API int b2_shard_lookup(const b2_field* emb_fields, const b2_field
                                       int64_t batch_local, int world, int rank, const int32_t* const* peer_ids,
                                       int64_t ids_stride, float* const* peer_emb, float* const* peer_lrw,
                                       const int32_t* rows_all, int32_t* status, const float* pad_rows, void* stream) {
-  int rc = check_shard_args(emb_fields, lr_fields, nfields, world, rank);
-  if (rc != B2_OK) return rc;
-  B2_REQUIRE(peer_ids && peer_emb && (lr_fields == nullptr || peer_lrw != nullptr), "NULL peer pointer array");
   B2_REQUIRE(rows_all != nullptr, "rows_all is NULL");
   B2_REQUIRE(batch_local >= 0, "batch_local %lld < 0", (long long) batch_local);
   B2_REQUIRE(ids_stride >= 1, "ids_stride %lld < 1", (long long) ids_stride);
-  B2_REQUIRE(pad_rows == nullptr || ((uintptr_t) pad_rows % 16) == 0, "pad_rows must be 16-byte aligned");
-  if (pad_rows != nullptr && lr_fields != nullptr)
-    for (int i = 0; i < nfields; ++i)
-      B2_REQUIRE(lr_fields[i].padding_idx == emb_fields[i].padding_idx,
-                 "field %d: the LR and embedding tables need one padding row", i);
+  PushLaunch pl;
+  int rc = push_setup(emb_fields, lr_fields, nfields, batch_local, world, rank,
+                      reinterpret_cast<const void* const*>(peer_ids), peer_emb, peer_lrw, pad_rows, pl);
+  if (rc != B2_OK) return rc;
   for (int i = 0; i < world; ++i)
     B2_REQUIRE(peer_ids[i] && peer_emb[i] && (lr_fields == nullptr || peer_lrw[i]), "peer %d: NULL buffer", i);
-  const int64_t nslots = count_slots(emb_fields, nfields);
-  B2_REQUIRE(batch_local * nslots < (1ll << 31), "batch_local * slots must fit 31 bits");
   if (batch_local == 0) return B2_OK;
-  static thread_local B2FieldPack epack, lpack;
-  fill_pack_cols(epack, emb_fields, nfields);
-  const int has_lr = lr_fields != nullptr;
-  if (has_lr) fill_pack_cols(lpack, lr_fields, nfields); else lpack.nfields = 0;
-  PeerPtrs pp;
-  for (int i = 0; i < world; ++i) {
-    pp.ids[i] = peer_ids[i];
-    pp.emb[i] = peer_emb[i];
-    pp.lrw[i] = has_lr ? peer_lrw[i] : nullptr;
-    pp.gemb[i] = nullptr;
-    pp.glogit[i] = nullptr;
-  }
-  const int dim = emb_fields[0].dim;
-  const int lpr_log2 = next_pow2_log2((dim + 3) / 4);
-  const size_t smem = 2 * ((pack_smem_bytes(nfields) + 15) & ~(size_t) 15) + 256 * sizeof(int4);
   // the grid covers every candidate of a full round; the samples past rows_all[p] drop out in the scan
-  const int grid = grid_for(batch_local * nslots * world, 256);
   static thread_local b2_lazy_ctx lz_none;
-  launch_push_len<int32_t, false, true>(epack.all_len1 != 0, grid, smem, (cudaStream_t) stream, epack, lpack, pp,
-                                        lz_none, batch_local, ids_stride, dim, lpr_log2, has_lr, world, rank, status,
-                                        (int4*) nullptr, (int32_t*) nullptr, (int32_t) 0, pad_rows, rows_all);
+  launch_push_len<int32_t, false, true>(pl.epack->all_len1 != 0, pl.grid, pl.smem, (cudaStream_t) stream, *pl.epack,
+                                        *pl.lpack, pl.pp, lz_none, batch_local, ids_stride, pl.dim, pl.lpr_log2,
+                                        pl.has_lr, world, rank, status, (int4*) nullptr, (int32_t*) nullptr,
+                                        (int32_t) 0, pad_rows, rows_all);
   B2_CUDA_LAUNCH_CHECK("b2_shard_lookup");
-  return B2_OK;
-}
-
-extern "C" B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream) {
-  B2_REQUIRE(src && peer_dst && world >= 1 && world <= 16, "bad argument");
-  B2_REQUIRE(nbytes >= 0 && nbytes % 4 == 0 && ((uintptr_t) src % 16) == 0, "buffer must be 16-byte aligned, a multiple of 4 bytes");
-  if (nbytes == 0) return B2_OK;
-  BcastDst d;
-  for (int i = 0; i < 16; ++i) d.p[i] = nullptr;
-  for (int i = 0; i < world; ++i) {
-    B2_REQUIRE(peer_dst[i] != nullptr && ((uintptr_t) peer_dst[i] % 16) == 0, "peer_dst[%d] NULL or misaligned", i);
-    d.p[i] = peer_dst[i];
-  }
-  const int grid = grid_for(nbytes >> 4, 256);
-  shard_bcast_kernel<<<grid, 256, 0, (cudaStream_t) stream>>>(src, nbytes, d, world);
-  B2_CUDA_LAUNCH_CHECK("b2_peer_bcast");
   return B2_OK;
 }
 

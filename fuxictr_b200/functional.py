@@ -181,7 +181,7 @@ class _EmbedGather(torch.autograd.Function):
         count = (torch.empty((len(plan.fields), max(batch, 1)), dtype=torch.float32, device=dev)
                  if plan.needs_count else None)
         descs = plan.fill(tables, idx_list, arena, batch)
-        _lib.call("b2_embed_gather_hot_fwd", descs, len(plan.fields), batch, ctx_code(idx_list),
+        _lib.call("b2_embed_gather_fwd", descs, len(plan.fields), batch, ctx_code(idx_list),
                   B2_F32, _ptr(count), _ptr(status), int(plan.hot_rows), _stream())
         ctx.plan, ctx.idx_list, ctx.count, ctx.tables = plan, idx_list, count, tables
         return arena
@@ -210,7 +210,7 @@ class _EmbedGather(torch.autograd.Function):
                 # mean_count is indexed by the position in the *backward* field list
                 rows = [plan.fields.index(f) for f, _ in live]
                 count = count[rows].contiguous()
-            _lib.call("b2_embed_scatter_bwd_ex", descs, len(live), batch, ctx_code(idx_list), B2_F32,
+            _lib.call("b2_embed_scatter_bwd", descs, len(live), batch, ctx_code(idx_list), B2_F32,
                       _ptr(count), _touch(grads), _stream())
         return (None, None, None) + tuple(grads)
 
@@ -272,7 +272,7 @@ class _LRForward(torch.autograd.Function):
                     d.table, d.vocab = g.data_ptr(), g.shape[0]
                     d.idx, d.idx_stride = idx.data_ptr(), idx.stride(0)
                     d.dim, d.seq_len, d.pool, d.padding_idx = 1, f.seq_len, f.pool, f.padding_idx
-                _lib.call("b2_lr_bwd_ex", descs, len(live), batch, ctx_code(idx_list), _ptr(gout),
+                _lib.call("b2_lr_bwd", descs, len(live), batch, ctx_code(idx_list), _ptr(gout),
                           _ptr(gbias), _touch(grads), _stream())
             else:
                 gbias.copy_(gout.sum().view(1))
@@ -430,15 +430,6 @@ def split_tf32(t):
     small = torch.empty_like(t)
     _lib.call("b2_split_tf32", _ptr(t), _ptr(small), t.numel(), _stream())
     return small
-
-
-def transpose_f32(t, want_small):
-    """(rows, cols) -> contiguous (cols, rows) [+ its 3xTF32 small part]."""
-    rows, cols = t.shape
-    out = torch.empty((cols, rows), dtype=torch.float32, device=t.device)
-    small = torch.empty_like(out) if want_small else None
-    _lib.call("b2_transpose_f32", _ptr(t), rows, cols, t.stride(0), _ptr(out), rows, _ptr(small), _stream())
-    return out, small
 
 
 def gemm_ex(a, b, out, a_mn=False, b_mn=False, a_small=None, b_small=None, bias=None, act=B2_ACT_NONE,
@@ -1476,14 +1467,9 @@ class _Front(torch.autograd.Function):
                     d.idx, d.idx_stride = idx.data_ptr(), idx.stride(0)
                     d.dim, d.seq_len, d.pool, d.padding_idx = 1, 1, 0, f.padding_idx
             lz = ctx.lazy_ctx
-            args = [descs, lr_descs, len(plan.fields), batch, ctx_code(idx_list), 1 if ctx.want_fm else 0,
-                    _ptr(arena), _ptr(garena), _ptr(sums), _ptr(glogit), _ptr(gbias),
-                    ctypes.byref(lz) if lz is not None else None]
-            touch = _touch(egrads + lgrads)
-            if touch is None:      # lazy tables, or gradients outside an arena
-                _lib.call("b2_front_bwd", *args, _stream())
-            else:
-                _lib.call("b2_front_bwd_ex", *args, touch, _stream())
+            _lib.call("b2_front_bwd", descs, lr_descs, len(plan.fields), batch, ctx_code(idx_list),
+                      1 if ctx.want_fm else 0, _ptr(arena), _ptr(garena), _ptr(sums), _ptr(glogit), _ptr(gbias),
+                      ctypes.byref(lz) if lz is not None else None, _touch(egrads + lgrads), _stream())
         return (None, None, None, None, None, gbias, None) + tuple(egrads) + tuple(lgrads)
 
 

@@ -333,7 +333,7 @@ class ShardedFront(object):
         g = self.group
         lr = self._descs(self.lr_tables, 1) if self.lr_tables else None
         lz = self.lazy_ctx()
-        _lib.call("b2_shard_push_pad", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
+        _lib.call("b2_shard_push", self._descs(self.emb_tables, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.ids_ptrs), self.idx_code, self.W, _ptr_array(self.emb_ptrs),
                   _ptr_array(self.lrw_ptrs) if lr is not None else None, F2._ptr(self.status),
                   F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
@@ -434,7 +434,7 @@ class ShardedFront(object):
         g = self.group
         lr = self._descs(lr_grads, 1) if lr_grads else None
         lz = self.lazy_ctx()        # lazy tables: the pull enqueues every row it scatters a gradient into
-        _lib.call("b2_shard_pull_ex", self._descs(emb_grads, self.dim), lr, self.F, self.B, g.world, g.rank,
+        _lib.call("b2_shard_pull", self._descs(emb_grads, self.dim), lr, self.F, self.B, g.world, g.rank,
                   _ptr_array(self.gemb_ptrs), _ptr_array(self.glogit_ptrs) if lr is not None else None,
                   self.pull_scale, F2._ptr(self.owned), F2._ptr(self.owned_count), self.owned_cap,
                   ctypes.byref(lz) if lz is not None else None, F2._touch(list(emb_grads) + list(lr_grads or ())),

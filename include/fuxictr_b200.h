@@ -111,30 +111,15 @@ typedef struct b2_field {
  *              pooling.py:46-47) for the backward.
  *   status     device int32[1], or NULL.  Set (atomicMax) to 1+field if an index is
  *              outside [0, vocab) (the reference raises IndexError); the row is zero-filled.
+ *   hot_rows   >= 0; 0 = no staging.  The first `hot_rows` rows of every table are staged once per CTA
+ *              in shared memory and served from there (north_star "shared-memory staging of hot rows"):
+ *              FuxiCTR's tokenizer numbers ids by descending frequency, so the small ids are the hot
+ *              ones.  Applies when every field is one slot of one common dim (% 4) and the staging area
+ *              fits 44 KB per CTA; otherwise ignored.  The result is bit-identical either way.
  */
 B2_API int b2_embed_gather_fwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                        int elem_dtype, float* mean_count, int32_t* status, void* stream);
-/* Same, with the first `hot_rows` rows of every table staged once per CTA in shared memory and served
- * from there (north_star "shared-memory staging of hot rows"): FuxiCTR's tokenizer numbers ids by
- * descending frequency, so the small ids are the hot ones.  Applies when every field is one slot of one
- * common dim (% 4) and the staging area fits 44 KB per CTA; otherwise identical to b2_embed_gather_fwd.
- * The result is bit-identical either way. */
-B2_API int b2_embed_gather_hot_fwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                                   int elem_dtype, float* mean_count, int32_t* status, int hot_rows,
-                                   void* stream);
-
-/*
- * Backward of the fused gather: dense-gradient scatter-add with warp-level
- * aggregation of duplicate rows.  Replaces F x aten::embedding_dense_backward
- * (autograd of feature_embedding.py:285,288).  In each descriptor `table` is the
- * (vocab, dim) f32 GRADIENT buffer (accumulated into: the caller zeroes it when it
- * wants "=" semantics), `out` is the incoming gradient laid out exactly like the
- * forward output; rows whose index equals padding_idx receive no gradient
- * (nn.Embedding(padding_idx)).  mean_count is the buffer the forward filled
- * (NULL when no field uses B2_POOL_MEAN).
- */
-B2_API int b2_embed_scatter_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                         int elem_dtype, const float* mean_count, void* stream);
+                               int elem_dtype, float* mean_count, int32_t* status, int hot_rows,
+                               void* stream);
 
 /*
  * Touched-granule flags of a gradient arena's table prefix: one byte per 64-byte granule (16 floats)
@@ -149,10 +134,21 @@ typedef struct b2_touch {
   const float* base;   /* first element covered (16-byte aligned) */
   int64_t n;           /* elements covered */
 } b2_touch;
-/* b2_embed_scatter_bwd, also marking `touch` (NULL = none). */
-B2_API int b2_embed_scatter_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                                   int elem_dtype, const float* mean_count, const b2_touch* touch,
-                                   void* stream);
+
+/*
+ * Backward of the fused gather: dense-gradient scatter-add with warp-level
+ * aggregation of duplicate rows.  Replaces F x aten::embedding_dense_backward
+ * (autograd of feature_embedding.py:285,288).  In each descriptor `table` is the
+ * (vocab, dim) f32 GRADIENT buffer (accumulated into: the caller zeroes it when it
+ * wants "=" semantics), `out` is the incoming gradient laid out exactly like the
+ * forward output; rows whose index equals padding_idx receive no gradient
+ * (nn.Embedding(padding_idx)).  mean_count is the buffer the forward filled
+ * (NULL when no field uses B2_POOL_MEAN).  touch (NULL = none): marks the granules
+ * of every gradient row it adds into (b2_touch).
+ */
+B2_API int b2_embed_scatter_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
+                                int elem_dtype, const float* mean_count, const b2_touch* touch,
+                                void* stream);
 
 /*
  * LogisticRegression.forward (layers/blocks/logistic_regression.py:55-58):
@@ -164,12 +160,10 @@ B2_API int b2_embed_scatter_bwd_ex(const b2_field* fields, int nfields, int64_t 
 B2_API int b2_lr_fwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype, const float* bias,
               float* out, int32_t* status, void* stream);
 /* Backward: table_f[idx] += gout[b] (skipping padding_idx); if gbias != NULL,
- * gbias[0] += sum_b gout[b]. `table` fields point at the (vocab,1) gradient buffers. */
+ * gbias[0] += sum_b gout[b]. `table` fields point at the (vocab,1) gradient buffers.
+ * touch (NULL = none): marks the granules of every gradient row it adds into (b2_touch). */
 B2_API int b2_lr_bwd(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-              const float* gout, float* gbias, void* stream);
-/* b2_lr_bwd, also marking `touch` (NULL = none). */
-B2_API int b2_lr_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int idx_dtype,
-                        const float* gout, float* gbias, const b2_touch* touch, void* stream);
+                     const float* gout, float* gbias, const b2_touch* touch, void* stream);
 
 
 /*
@@ -183,7 +177,7 @@ B2_API int b2_lr_bwd_ex(const b2_field* fields, int nfields, int64_t batch, int 
  * scalars (sched[t], written by b2_adam_sched) and the same explicitly rounded arithmetic as the
  * dense pass, so the result is BIT-IDENTICAL to dense Adam (tests/test_gpu_parity.py).
  * Rows are numbered globally: table i owns rows [grow_base[i], grow_base[i] + vocab_i).
- * Row-sharded tables (b2_shard_push_ex / b2_shard_pull_ex): the same protocol over the rows THIS rank
+ * Row-sharded tables (b2_shard_push / b2_shard_pull): the same protocol over the rows THIS rank
  * owns.  The push replays a stale row before it stores it into the requester's buffer; the pull, where
  * several requesters may send gradients for one row, enqueues the row once.  grow_emb / grow_lr and
  * the worklist then count this rank's LOCAL rows (shard row r of table i is row grow_base[i] + r);
@@ -227,16 +221,13 @@ B2_API int b2_front_fwd(const b2_field* emb_fields, const b2_field* lr_fields, i
  *   g = gx[b,f,:] + glogit[b] * (sums[b,:] - emb_saved[b,f,:])      (second term only if want_fm)
  * is scatter-added (warp-aggregated) into the gradient table, rows equal to padding_idx skipped;
  * lr_fields[i].table (vocab,1) += glogit[b]; gbias[0] += sum_b glogit[b].
+ * touch (NULL = none): marks (b2_touch) every embedding and LR gradient it writes.
  */
 B2_API int b2_front_bwd(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch,
                         int idx_dtype, int want_fm, const float* emb_saved, const float* gx,
                         const float* sums, const float* glogit, float* gbias,
-                        const b2_lazy_ctx* lazy /* non-NULL: enqueue every touched row once */, void* stream);
-/* b2_front_bwd, also marking `touch` (NULL = none) for every embedding and LR gradient it writes. */
-B2_API int b2_front_bwd_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int64_t batch,
-                           int idx_dtype, int want_fm, const float* emb_saved, const float* gx,
-                           const float* sums, const float* glogit, float* gbias, const b2_lazy_ctx* lazy,
-                           const b2_touch* touch, void* stream);
+                        const b2_lazy_ctx* lazy /* non-NULL: enqueue every touched row once */,
+                        const b2_touch* touch, void* stream);
 /*
  * Flags (b2_touch over the PARAMETER arena) every granule of every row a fused front or fused gather reads
  * for this batch: emb_fields[i].table / lr_fields[i].table are the parameter tables, idx as in b2_front_fwd
@@ -287,54 +278,40 @@ B2_API int b2_lazy_materialize(const b2_lazy_table* tables_dev, int ntables, int
  * (B_local, F*D) / peer_glogit[p] (B_local) and scatter-adds `scale *` them into the local gradient
  * shards — ~B_local*F entries instead of world*B_local*F candidates, and no second pass over the
  * peers' ids.  Cross-rank ordering is the caller's barrier.  world <= 16.
- * b2_peer_bcast: one launch copies `nbytes` (multiple of 4, 16-byte aligned buffers) from src into
- * peer_dst[p] for every p < world (P2P stores): the batch-matrix exchange.
- */
-B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                         int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                         int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                         float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
-                         int32_t owned_capacity, void* stream);
-B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                         int64_t batch_local, int world, int rank, const float* const* peer_gemb,
-                         const float* const* peer_glogit, float scale, const int32_t* owned,
-                         const int32_t* owned_count, int32_t owned_capacity, void* stream);
-/* Lazy tables (see b2_lazy_ctx): lazy == NULL is b2_shard_push / b2_shard_pull.  Otherwise the push
+ * Lazy tables (see b2_lazy_ctx): lazy == NULL means the tables are up to date.  Otherwise the push
  * brings every served row with last_step[grow] < *step_dev up to date in registers before the store
  * (nothing is written back), and the pull appends every owned, non-padding row it scatters a gradient
  * into to the worklist, once per step (claimed through mark).  grow = grow_emb[f] / grow_lr[f] + local
  * row.  The caller zeroes lazy->counter before the pull of a step.  touch (NULL = none): the pull marks
- * the granules of every gradient row it scatters into (b2_touch). */
-B2_API int b2_shard_push_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                            int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                            int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                            float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
-                            int32_t owned_capacity, const b2_lazy_ctx* lazy, void* stream);
-B2_API int b2_shard_pull_ex(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                            int64_t batch_local, int world, int rank, const float* const* peer_gemb,
-                            const float* const* peer_glogit, float scale, const int32_t* owned,
-                            const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
-                            const b2_touch* touch, void* stream);
-/* Sequence fields: a field with seq_len L > 1 (pool must be B2_POOL_NONE: a pooled sequence's rows come from
+ * the granules of every gradient row it scatters into (b2_touch).
+ * Padding rows: with pad_rows != NULL every rank fills its OWN padding slots (id == padding_idx) from
+ * pad_rows, this rank's (F*D + F)-float buffer (16-byte aligned) that b2_shard_publish_ids filled before
+ * the push (padding row of field f at f*D, its LR weight at F*D + f): no rank serves the padding slots of
+ * the others, and the copy is bit-exact whatever the padding row holds.  Padding slots get no gradient.
+ * pad_rows == NULL: the owner of the padding row serves it like any other row.
+ * Sequence fields: a field with seq_len L > 1 (pool must be B2_POOL_NONE: a pooled sequence's rows come from
  * several owners) is L consecutive SLOTS, with its ids in columns idx_stride .. idx_stride + L - 1.  With
  * S = sum of seq_len, slot s of sample b lands at b*S*D + s*D of peer_emb / is read at the same offset of
  * peer_gemb, and an owned-list entry keeps b*S + s where a one-slot field keeps b*F + f.  Requires
  * batch_local * S < 2^31; an owned list of world * batch_local * S entries never overflows.  LR tables
  * (lr_fields != NULL) need seq_len == 1 on every field.
- * b2_shard_push_pad: b2_shard_push_ex where every rank fills its OWN padding slots (id == padding_idx)
- * from pad_rows, this rank's (F*D + F)-float buffer that b2_shard_publish_ids filled before the push
- * (padding row of field f at f*D, its LR weight at F*D + f): no rank serves the padding slots of the
- * others, and the copy is bit-exact whatever the padding row holds.  Padding slots get no gradient.
- * pad_rows == NULL is b2_shard_push_ex (the owner of the padding row serves it like any other row). */
-B2_API int b2_shard_push_pad(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
-                             int64_t batch_local, int world, int rank, const void* const* peer_ids,
-                             int idx_dtype, int64_t ids_stride, float* const* peer_emb,
-                             float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
-                             int32_t owned_capacity, const b2_lazy_ctx* lazy, const float* pad_rows,
-                             void* stream);
-/* b2_peer_bcast_ids, and in the same launch the padding rows: for every field whose padding row this rank
- * owns, the row (emb_fields[f].table = this rank's shard) and its LR weight are stored into peer_pad[p]
- * (16-byte aligned, F*D + F floats, layout as pad_rows above) for every p < world. */
+ */
+B2_API int b2_shard_push(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                         int64_t batch_local, int world, int rank, const void* const* peer_ids,
+                         int idx_dtype, int64_t ids_stride, float* const* peer_emb,
+                         float* const* peer_lrw, int32_t* status, int32_t* owned, int32_t* owned_count,
+                         int32_t owned_capacity, const b2_lazy_ctx* lazy, const float* pad_rows,
+                         void* stream);
+B2_API int b2_shard_pull(const b2_field* emb_fields, const b2_field* lr_fields, int nfields,
+                         int64_t batch_local, int world, int rank, const float* const* peer_gemb,
+                         const float* const* peer_glogit, float scale, const int32_t* owned,
+                         const int32_t* owned_count, int32_t owned_capacity, const b2_lazy_ctx* lazy,
+                         const b2_touch* touch, void* stream);
+/* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
+ * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world.  In the same
+ * launch the padding rows: for every field whose padding row this rank owns, the row (emb_fields[f].table =
+ * this rank's shard) and its LR weight are stored into peer_pad[p] (16-byte aligned, F*D + F floats, layout
+ * as pad_rows above) for every p < world. */
 B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst,
                                 const b2_field* emb_fields, const b2_field* lr_fields, int nfields, int world,
                                 int rank, float* const* peer_pad, void* stream);
@@ -345,7 +322,7 @@ B2_API int b2_shard_publish_ids(const void* src, int idx_dtype, int64_t count, i
  * rows * width ids are read and stored into peer_dst[p] — and, in the same launch, the row count into word
  * `rank` of peer_rows[p] (int32[world] on every rank, 4-byte aligned) for every p < world.  Refused: rows
  * outside [0, capacity_rows] (capacity_rows = the batch_local of the peer buffers), NULL src with rows > 0.
- * b2_shard_lookup: b2_shard_push_pad over the candidates (requester p, sample b < rows_all[p], slot), where
+ * b2_shard_lookup: b2_shard_push over the candidates (requester p, sample b < rows_all[p], slot), where
  * rows_all is this rank's int32[world] buffer that every rank's publish filled before the barrier: the bound
  * comes from device memory, so no rank needs its peers' counts on the host, and a rank with 0 rows still
  * serves the others.  peer_ids hold the int32 ids the publish stored (row pitch ids_stride).  It keeps no
@@ -361,11 +338,6 @@ B2_API int b2_shard_lookup(const b2_field* emb_fields, const b2_field* lr_fields
                            int world, int rank, const int32_t* const* peer_ids, int64_t ids_stride,
                            float* const* peer_emb, float* const* peer_lrw, const int32_t* rows_all, int32_t* status,
                            const float* pad_rows, void* stream);
-B2_API int b2_peer_bcast(const void* src, int64_t nbytes, void* const* peer_dst, int world, void* stream);
-/* The id exchange, compressed: `count` contiguous ids of dtype idx_dtype (B2_F64 truncates like .long())
- * are narrowed to int32 and stored into peer_dst[p] (16-byte aligned) for every p < world. */
-B2_API int b2_peer_bcast_ids(const void* src, int idx_dtype, int64_t count, int32_t* const* peer_dst, int world,
-                             void* stream);
 /* After the push: logit[b] = [FM product_sum of emb[b]] (if want_fm) + sum_f lrw[b,f] + bias;
  * sums[b,:] = sum_f emb[b,f,:] (saved for the backward). */
 B2_API int b2_front_reduce(const float* emb, const float* lrw, const float* bias, int64_t batch,
@@ -506,25 +478,8 @@ B2_API int b2_gemm_f32(const float* a, int64_t a_rs, int64_t a_cs, const float* 
                 int beta_accumulate, void* stream);
 
 /*
- * Tensor-core dense layer: same contract as b2_gemm_f32 for the K-major case
- *   C[m,n] = epi( sum_k A[m,k] * B[n,k] + bias[n] ),  A (M,K) ld=lda, B (N,K) ld=ldb, fp32,
- * computed by a TMA-fed wgmma .tf32 kernel with the accumulators in registers.
- *   a_small == b_small == NULL : single-pass TF32 (operand mantissas truncated to 10 bits).
- *   a_small, b_small given      : error-compensated 3xTF32 (fp32-class accuracy).  The pointers act as a
- *                                 mode flag: their contents are NOT read (the kernel derives the small
- *                                 parts of A and B itself); only their TMA alignment is checked.
- * Operands must be TMA-addressable (16-byte aligned base, ld % 4 == 0): b2_gemm_tc_supported()
- * says whether they are; otherwise B2_E_UNSUPPORTED is returned and the caller uses b2_gemm_f32.
- */
-B2_API int b2_gemm_tc_supported(const float* a, int64_t lda, const float* b, int64_t ldb, int64_t M,
-                                int64_t N, int64_t K);
-B2_API int b2_gemm_tc(const float* a, int64_t lda, const float* b, int64_t ldb, float* c, int64_t ldc,
-                      int64_t M, int64_t N, int64_t K, const float* bias, int act, const float* mul,
-                      const float* add, int beta_accumulate, const float* a_small,
-                      const float* b_small, void* stream);
-
-/*
- * The general tensor-core contraction:  C[m,n] = epi( sum_k A(m,k) * B(n,k) ).
+ * The tensor-core contraction:  C[m,n] = epi( sum_k A(m,k) * B(n,k) ), computed by a TMA-fed wgmma
+ * kernel with the accumulators in registers.
  * Operand layouts (TMA loads either as it lies and the kernel re-lays it out in shared memory, so
  * no transpose pass in global memory is ever needed):
  *   a_mn_major == 0:  A in memory (M, K), k contiguous, leading dimension lda   ("K-major")
@@ -540,8 +495,13 @@ B2_API int b2_gemm_tc(const float* a, int64_t lda, const float* b, int64_t ldb, 
  *                                  sigmoid_backward of the reference's autograd);
  *   C = v (+ C if beta_accumulate);  c_small = v - tf32_trunc(v) (the consumer's 3xTF32 operand);
  *   colsum[n] = sum_m v  (bias gradient; the call zeroes colsum first).
- * mul, add, ybwd, c_small share C's leading dimension.  a_small/b_small: both non-NULL selects 3xTF32
- * (contents not read, see b2_gemm_tc; B2_GEMM_X3_INLINE selects it without them), both NULL single-pass TF32.
+ * mul, add, ybwd, c_small share C's leading dimension.
+ * fp32 operands: a_small == b_small == NULL is single-pass TF32 (operand mantissas truncated to 10 bits);
+ * both non-NULL is error-compensated 3xTF32 (fp32-class accuracy).  The pointers act as a mode flag: their
+ * contents are NOT read (the kernel derives the small parts of A and B itself); only their TMA alignment is
+ * checked.  B2_GEMM_X3_INLINE selects 3xTF32 without them.
+ * Operands must be TMA-addressable (16-byte aligned base, 16-byte row pitch); otherwise B2_E_UNSUPPORTED
+ * is returned and the caller uses b2_gemm_f32.
  * elem_dtype == B2_BF16 (BASELINE configs[1] "bf16"): a and b hold bf16 (row pitch a multiple of 16
  * bytes, i.e. leading dimensions % 8 == 0), one pass of wgmma .bf16 with fp32 accumulation;
  * C stays fp32 and c_small, if given, receives C rounded to bf16 (leading dimension ld_aux) — the
@@ -597,17 +557,14 @@ B2_API int b2_to_bf16(const float* x, int64_t rows, int64_t cols, int64_t ld_in,
                       void* stream);
 /* small[i] = x[i] - (x[i] with the 13 low mantissa bits cleared). */
 B2_API int b2_split_tf32(const float* x, float* small, int64_t n, void* stream);
-/* out (cols, rows; ld_out) = in (rows, cols; ld_in)^T; if out_small != NULL it also receives the
- * 3xTF32 small part of the transposed values. */
-B2_API int b2_transpose_f32(const float* in, int64_t rows, int64_t cols, int64_t ld_in, float* out,
-                            int64_t ld_out, float* out_small, void* stream);
 
 /*
  * One-pass operand preparation for the K-major tensor-core GEMMs over x (R, C):
  *   v = act'(y) * x when y != NULL (y = activation OUTPUT; fuses the activation backward);
  *   act == B2_PREP_MUL: v = x * y
  *   out (R,C) = v, out_small = 3xTF32 small part, outT (C,R) = v^T, outT_small, colsum[c] = sum_r v[r,c]
- * Every output may be NULL.  Replaces b2_act_bwd + b2_transpose_f32 + b2_split_tf32 + b2_colsum.
+ * Every output may be NULL.  One pass where an activation backward, a transpose, a 3xTF32 split and a
+ * column sum would each read x again.
  * drop_rng != NULL: x is the gradient of a dropout layer's output and y (if any) that DROPPED output:
  *   v = act'(y) * keep * drop_scale * x  with the mask of (R, C) at counter offset snapshot offset + drop_layer
  *   (not with B2_PREP_MUL).  drop_rng == NULL: no mask, the other drop arguments are ignored.
@@ -651,12 +608,6 @@ B2_API int b2_head_bwd_ex(const float* x, const float* w, const float* y, const 
 B2_API int b2_dropout_rng_take(int64_t* state, int64_t* snapshot, int n_layers, void* stream);
 B2_API int b2_dropout_apply(const float* x, float* y, int64_t M, int64_t N, int64_t ld, const int64_t* snapshot,
                             int64_t layer, uint32_t thresh, float scale, void* stream);
-/* Elementwise helpers used by the dense backward.
- * b2_act_bwd: gx = gy * act'(y) where y is the activation OUTPUT (relu, sigmoid). */
-B2_API int b2_act_bwd(const float* y, const float* gy, float* gx, int64_t n, int act, void* stream);
-/* b2_colsum: out[n] (+)= sum_m x[m*ld + n]  (bias gradients). */
-B2_API int b2_colsum(const float* x, int64_t M, int64_t N, int64_t ld, float* out, int accumulate,
-              void* stream);
 
 /*
  * Final glue of DeepFM.forward + BaseModel.add_loss (model_zoo/DeepFM/DeepFM_torch/

@@ -51,7 +51,7 @@ def test_field_struct_layout(lib):
     assert lib.b2_field.vocab.offset == 24 and lib.b2_field.dim.offset == 48
 
 
-def test_argument_validation_needs_no_gpu(lib):
+def test_entry_points_reject_bad_arguments_without_a_gpu(lib):
     L = lib.load()
     null = ctypes.c_void_p(0)
     rc = L.b2_gemm_f32(null, 1, 1, null, 1, 1, null, 1, 4, 4, 4, null, 0, null, null, 0, null)
@@ -59,12 +59,12 @@ def test_argument_validation_needs_no_gpu(lib):
     rc = L.b2_fm_fwd(ctypes.c_void_p(16), 4, 3, 8, 7, ctypes.c_void_p(16), null)
     assert rc == -1 and b"mode" in L.b2_last_error()
     fields = (lib.b2_field * 1)()
-    rc = L.b2_embed_gather_fwd(fields, 0, 4, lib.B2_F64, lib.B2_F32, null, null, null)
+    rc = L.b2_embed_gather_fwd(fields, 0, 4, lib.B2_F64, lib.B2_F32, null, null, 0, null)
     assert rc == -1 and b"nfields" in L.b2_last_error()
-    rc = L.b2_embed_gather_fwd(fields, 1, 4, lib.B2_F64, lib.B2_BF16, null, null, null)
+    rc = L.b2_embed_gather_fwd(fields, 1, 4, lib.B2_F64, lib.B2_BF16, null, null, 0, null)
     assert rc == -1
-    with pytest.raises(lib.B2Error):
-        lib.call("b2_act_bwd", null, null, null, 8, 0, null)
+    with pytest.raises(lib.B2Error, match="NULL"):
+        lib.call("b2_split_tf32", null, null, 8, null)
 
 
 def test_missing_library_is_a_hard_error(lib, monkeypatch):
