@@ -19,6 +19,7 @@ B2_PREP_MUL = 3
 B2_GEMM_C_IS_ZERO, B2_GEMM_COLSUM_IS_ZERO, B2_GEMM_X3_INLINE, B2_GEMM_BACKFILL = 1, 2, 4, 8
 B2_MAX_FIELDS = 128
 B2_CROSSMIX_MAX_RANK, B2_CROSSMIX_MAX_COLS = 64, 256
+B2_MHTA_MAX_WIDTH, B2_MHTA_MAX_HEADS = 1024, 32
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
 c_void_p, c_int, c_int32, c_int64, c_float = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,
@@ -130,6 +131,14 @@ SIGNATURES = {
                                 c_int64, c_void_p, c_void_p]),
     "b2_crossmix_unpack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p]),
+    "b2_mhta_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
+                             c_void_p, c_void_p]),
+    "b2_mhta_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float,
+                            c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
+    "b2_mhta_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int,
+                            c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
+    "b2_mhta_unpack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                               c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_cin_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p,
                            c_void_p]),
     "b2_cin_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p,

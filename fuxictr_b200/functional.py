@@ -1120,6 +1120,127 @@ def crossnet_mix_layer(x0, xl, U, V, C, gating_weights, bias):
     return _CrossMixLayer.apply(x0, xl, U, V, C, gating_weights, bias)
 
 
+# --------------------------------------------------------------------------------------
+# MultiHeadTargetAttention
+# --------------------------------------------------------------------------------------
+def target_attention_bound(width, heads):
+    """None when the MultiHeadTargetAttention kernels cover a row of `width` columns split into `heads` heads,
+    else the bound it breaks.  width is the row of q' and p: heads * input_dim with the projections (use_qkvo),
+    input_dim without."""
+    if not 1 <= heads <= _lib.B2_MHTA_MAX_HEADS:
+        return "num_heads must lie in [1, %d], got %d" % (_lib.B2_MHTA_MAX_HEADS, heads)
+    if not 1 <= width <= _lib.B2_MHTA_MAX_WIDTH:
+        return "the attention row width (num_heads * input_dim with use_qkvo, else input_dim) must lie in " \
+               "[1, %d], got %d" % (_lib.B2_MHTA_MAX_WIDTH, width)
+    return None
+
+
+class _TargetAttention(torch.autograd.Function):
+    """MultiHeadTargetAttention.forward (target_attention.py:150-172) on the kernels (include/fuxictr_b200.h
+    "MultiHeadTargetAttention").  With the projections: W_M, W_N packed from W_q, W_k, W_v, W_o (b2_mhta_pack),
+    q' = t W_M^T (GEMM1), the row kernel's masked online softmax and pooled p (b2_mhta_fwd), out = p W_N^T
+    (GEMM2).  Backward: dp = g W_N, dW_N = g^T p, the row kernel back to dq' and dx (b2_mhta_bwd),
+    dt = dq' W_M, dW_M = dq'^T t, and one unpack of dW_M, dW_N into the four weights.  Without them the row
+    kernels alone, sliced by head: q = t, out = p.  The GEMMs follow the matmul precision (SIMT below 16 or
+    off-by-4 shapes); the row kernels run in fp32."""
+
+    @staticmethod
+    def forward(ctx, t, x, mask_u8, heads, scale, Wq, Wk, Wv, Wo):
+        t, x = _f32c(t), _f32c(x)
+        B, L, d = x.shape
+        H, dev = heads, x.device
+        qkvo = Wq is not None
+        tc, aux, packed = False, (None, None, None, None), (None, None)
+        if qkvo:
+            Wq, Wk, Wv, Wo = _f32c(Wq), _f32c(Wk), _f32c(Wv), _f32c(Wo)
+            hd = Wq.shape[0] // H
+            WM = torch.empty((H * d, d), dtype=torch.float32, device=dev)
+            WN = torch.empty((d, H * d), dtype=torch.float32, device=dev)
+            _lib.call("b2_mhta_pack", _ptr(Wq), _ptr(Wk), _ptr(Wv), _ptr(Wo), d, H, hd, scale, _ptr(WM), _ptr(WN),
+                      _stream())
+            tc = _tc_layer_ok(WM) and _tc_layer_ok(WN) and t.data_ptr() % 16 == 0
+            if tc:
+                aux = (make_aux(t), make_aux(WM), make_aux(WN), empty_aux(B, H * d, dev))
+            q = torch.empty((B, H * d), dtype=torch.float32, device=dev)
+            _linear_fwd(tc, t, aux[0], WM, q, aux[1])
+            width, x_step, row_scale, packed = d, 0, 1.0, (WM, WN)
+        else:
+            q, width, x_step, row_scale = t, d // H, d // H, scale
+        p = torch.empty((B, H * width), dtype=torch.float32, device=dev)
+        stats = torch.empty((B, H, 2), dtype=torch.float32, device=dev)
+        _lib.call("b2_mhta_fwd", _ptr(q), _ptr(x), _ptr(mask_u8), B, L, d, H, width, x_step, row_scale, _ptr(p),
+                  _ptr(stats), *_aux_args(aux[3]), _stream())
+        out = p
+        if qkvo:
+            out = torch.empty((B, d), dtype=torch.float32, device=dev)
+            _linear_fwd(tc, p, aux[3], packed[1], out, aux[2])
+        ctx.save_for_backward(t, x, q, p, stats, *packed, Wq, Wk, Wv, Wo)
+        ctx.mask, ctx.tc, ctx.aux, ctx.geom = mask_u8, tc, aux, (H, width, x_step, row_scale, scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        t, x, q, p, stats, WM, WN, Wq, Wk, Wv, Wo = ctx.saved_tensors
+        g = _f32c(g)
+        t_aux, wm_aux, wn_aux, p_aux = ctx.aux
+        H, width, x_step, row_scale, scale = ctx.geom
+        tc, qkvo = ctx.tc, Wq is not None
+        B, L, d = x.shape
+        dev = x.device
+        dp = g
+        if qkvo:
+            g_aux = make_aux(g) if tc else None
+            dp = torch.empty((B, H * d), dtype=torch.float32, device=dev)
+            dWN = torch.empty((d, H * d), dtype=torch.float32, device=dev)
+            _linear_dgrad(tc, g, g_aux, WN, dp, wn_aux)                        # dp = g W_N
+            _linear_wgrad(tc, g, g_aux, p, p_aux, dWN)                        # dW_N = g^T p
+        dq = torch.empty((B, H * width), dtype=torch.float32, device=dev)
+        dx = torch.empty_like(x)
+        dq_aux = empty_aux(B, H * width, dev) if tc else None
+        _lib.call("b2_mhta_bwd", _ptr(q), _ptr(x), _ptr(ctx.mask), _ptr(p), _ptr(stats), _ptr(dp), B, L, d, H, width,
+                  x_step, row_scale, _ptr(dq), _ptr(dx), *_aux_args(dq_aux), _stream())
+        if not qkvo:
+            return dq, dx, None, None, None, None, None, None, None
+        dt = torch.empty_like(t)
+        dWM = torch.empty((H * d, d), dtype=torch.float32, device=dev)
+        _linear_dgrad(tc, dq, dq_aux, WM, dt, wm_aux)                          # dt = dq' W_M
+        _linear_wgrad(tc, dq, dq_aux, t, t_aux, dWM)                          # dW_M = dq'^T t
+        gWq, gWk, gWv, gWo = (torch.empty_like(w) for w in (Wq, Wk, Wv, Wo))
+        _lib.call("b2_mhta_unpack", _ptr(Wq), _ptr(Wk), _ptr(Wv), _ptr(Wo), _ptr(dWM), _ptr(dWN), d, H,
+                  Wq.shape[0] // H, scale, _ptr(gWq), _ptr(gWk), _ptr(gWv), _ptr(gWo), _stream())
+        return dt, dx, None, None, None, gWq, gWk, gWv, gWo
+
+
+def target_attention(target_item, history_sequence, mask=None, num_heads=1, use_scale=True, W_q=None, W_k=None,
+                     W_v=None, W_o=None):
+    """MultiHeadTargetAttention with ScaledDotProductAttention (no attention dropout): target_item (B, d),
+    history_sequence (B, L, d), mask any B*L elements (nonzero = valid) or None; W_q, W_k, W_v (A, d) and
+    W_o (d, A), all four or none (use_qkvo False: A = d, heads slice the columns).  Returns (B, d)."""
+    _require_cuda(target_item, history_sequence, mask, W_q, W_k, W_v, W_o)
+    if history_sequence.dim() != 3 or target_item.dim() != 2:
+        raise ValueError("target_attention: target%s history%s must be (B, d) and (B, L, d)"
+                         % (tuple(target_item.shape), tuple(history_sequence.shape)))
+    B, L, d = history_sequence.shape
+    weights = (W_q, W_k, W_v, W_o)
+    qkvo = W_q is not None
+    if tuple(target_item.shape) != (B, d) or (mask is not None and mask.numel() != B * L) \
+            or any((w is None) == qkvo for w in weights):
+        raise ValueError("target_attention: target%s history%s mask%s or the weights do not match"
+                         % (tuple(target_item.shape), tuple(history_sequence.shape),
+                            None if mask is None else tuple(mask.shape)))
+    A = W_q.shape[0] if qkvo else d
+    if A % num_heads != 0 or (qkvo and (tuple(W_k.shape) != (A, d) or tuple(W_v.shape) != (A, d)
+                                        or tuple(W_q.shape) != (A, d) or tuple(W_o.shape) != (d, A))):
+        raise ValueError("target_attention: attention_dim %d, num_heads %d and the weights do not match"
+                         % (A, num_heads))
+    bound = target_attention_bound(num_heads * d if qkvo else d, num_heads)
+    if bound is not None:
+        raise NotImplementedError("MultiHeadTargetAttention kernels: " + bound)
+    scale = 1.0 / (A // num_heads) ** 0.5 if use_scale else 1.0
+    mask_u8 = None if mask is None else torch.ne(mask.reshape(B, L), 0).view(torch.uint8)
+    return _TargetAttention.apply(target_item, history_sequence, mask_u8, num_heads, scale, *weights)
+
+
 def mlp_chain_supported():
     return _MATMUL["mode"] != "fp32"
 

@@ -15,6 +15,8 @@ Reference files (relative to the reference root):
   CrossInteraction / CrossNet / CrossNetV2 fuxictr/pytorch/layers/interactions/cross_net.py:24-129
   CompressedInteractionNet                 fuxictr/pytorch/layers/interactions/compressed_interaction_net.py:23-76
   DIN_Attention                            fuxictr/pytorch/layers/attentions/target_attention.py:26-92
+  MultiHeadTargetAttention                 fuxictr/pytorch/layers/attentions/target_attention.py:95-172
+  ScaledDotProductAttention                fuxictr/pytorch/layers/attentions/dot_product_attention.py:24-58
   Dice                                     fuxictr/pytorch/layers/activations.py:24-51
   MLP_Block                                fuxictr/pytorch/layers/blocks/mlp_block.py:24-96
 """
@@ -659,3 +661,53 @@ class DIN_Attention(nn.Module):
 
     def forward(self, target_item, history_sequence, mask=None):
         return F2.din_attention(self, target_item, history_sequence, mask)
+
+
+class ScaledDotProductAttention(nn.Module):
+    """dot_product_attention.py:24-58, as a child of MultiHeadTargetAttention: the same constructor and
+    `dropout` child.  Its arithmetic runs inside MultiHeadTargetAttention's kernels, which fold the
+    projections around it; on its own it has no kernel and raises."""
+
+    def __init__(self, dropout_rate=0.):
+        super(ScaledDotProductAttention, self).__init__()
+        self.dropout = nn.Dropout(dropout_rate) if dropout_rate > 0 else None
+
+    def forward(self, Q, K, V, scale=None, mask=None):
+        raise NotImplementedError("ScaledDotProductAttention runs on the kernels only inside "
+                                  "MultiHeadTargetAttention")
+
+
+class MultiHeadTargetAttention(nn.Module):
+    """target_attention.py:95-172: the target item attends over its history, per head, with optional Q, K, V, O
+    projections.  One autograd node (functional._TargetAttention): with the projections, two GEMMs on weights
+    folded per head around the row kernel, so the history is never projected; without them, the row kernel
+    alone.  Parameters, child names, registration order and initialisation draws are the reference's.
+    Attention dropout in training mode has no kernel and raises."""
+
+    def __init__(self, input_dim=64, attention_dim=64, num_heads=1, dropout_rate=0, use_scale=True, use_qkvo=True):
+        super(MultiHeadTargetAttention, self).__init__()
+        if not use_qkvo:
+            attention_dim = input_dim
+        assert attention_dim % num_heads == 0, \
+            "attention_dim={} is not divisible by num_heads={}".format(attention_dim, num_heads)
+        bound = F2.target_attention_bound(num_heads * input_dim if use_qkvo else input_dim, num_heads)
+        if bound is not None:
+            raise NotImplementedError("MultiHeadTargetAttention kernels: " + bound)
+        self.num_heads = num_heads
+        self.head_dim = attention_dim // num_heads
+        self.scale = self.head_dim ** 0.5 if use_scale else None
+        self.use_qkvo = use_qkvo
+        if use_qkvo:
+            self.W_q = nn.Linear(input_dim, attention_dim, bias=False)
+            self.W_k = nn.Linear(input_dim, attention_dim, bias=False)
+            self.W_v = nn.Linear(input_dim, attention_dim, bias=False)
+            self.W_o = nn.Linear(attention_dim, input_dim, bias=False)
+        self.dot_attention = ScaledDotProductAttention(dropout_rate)
+
+    def forward(self, target_item, history_sequence, mask=None):
+        if self.dot_attention.dropout is not None and self.training:
+            raise NotImplementedError("MultiHeadTargetAttention kernels: attention dropout in training mode "
+                                      "has no kernel")
+        weights = (self.W_q.weight, self.W_k.weight, self.W_v.weight, self.W_o.weight) if self.use_qkvo else ()
+        return F2.target_attention(target_item, history_sequence, mask, self.num_heads, self.scale is not None,
+                                   *weights)

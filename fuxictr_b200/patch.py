@@ -9,7 +9,8 @@ when its tensors are CUDA tensors and the configuration is one the kernels cover
 calls the reference's original forward (the reference's own code, not a fallback of ours).
 
 Patched: FeatureEmbedding, FeatureEmbeddingDict, LogisticRegression, InnerProductInteraction,
-CrossNet, CrossNetV2, CrossNetMix, CompressedInteractionNet, DIN_Attention, Dice, MLP_Block
+CrossNet, CrossNetV2, CrossNetMix, CompressedInteractionNet, DIN_Attention, MultiHeadTargetAttention,
+Dice, MLP_Block
 (fuxictr/pytorch/layers/**, SURVEY.md 8a); and BaseModel.evaluate / BaseModel.predict
 (fuxictr/pytorch/models/rank_model.py:350-398, SURVEY.md 8f row 3): for a model on a CUDA device
 whose metrics are logloss / AUC (no group metrics) the predictions stay in HBM and
@@ -78,6 +79,16 @@ def _crossnet_mix_supported(self):
     return F2.crossnet_mix_bound(self.U_list[0].shape[2], self.num_experts) is None
 
 
+def _target_attention_supported(self):
+    """The kernels' row width and head count (include/fuxictr_b200.h "MultiHeadTargetAttention"), and no
+    attention dropout in training mode."""
+    from . import functional as F2
+    if self.dot_attention.dropout is not None and self.training:
+        return False
+    width = self.num_heads * self.W_q.in_features if self.use_qkvo else self.num_heads * self.head_dim
+    return F2.target_attention_bound(width, self.num_heads) is None
+
+
 def _wrap_base_model(base_cls):
     from . import metrics as DM
     orig_evaluate, orig_predict = base_cls.evaluate, base_cls.predict
@@ -131,6 +142,7 @@ def enable():
     _wrap(R.CrossNetMix, M.CrossNetMix.forward, _crossnet_mix_supported)
     _wrap(R.CompressedInteractionNet, M.CompressedInteractionNet.forward)
     _wrap(R.DIN_Attention, M.DIN_Attention.forward)
+    _wrap(R.MultiHeadTargetAttention, M.MultiHeadTargetAttention.forward, _target_attention_supported)
     _wrap(R.Dice, M.Dice.forward)
     _graft_methods(R.MLP_Block, M.MLP_Block, ["chain_layers"])     # the tensor-core modes' one-node chain
     _wrap(R.MLP_Block, M.MLP_Block.forward, _mlp_supported)

@@ -410,6 +410,59 @@ B2_API int b2_crossmix_unpack(const float* dW1, const float* dW2, int d, int r, 
                               float* gG, void* stream);
 
 /*
+ * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
+ * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
+ * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
+ * W_o,h head h's hd columns of W_o, and s = 1/sqrt(hd) (1 without use_scale).  The layer is linear in x but
+ * for the softmax, so the projections fold into the query and output GEMMs and x is never projected:
+ *   score_hl = q'_h . x_l,  q' = t W_M^T,  M_h = s W_q,h^T W_k,h (d x d)
+ *   out = p W_N^T,  p_h = sum_l a_hl x_l,  N_h = W_v,h^T W_o,h^T (d x d)
+ * All row-major fp32:
+ *   W_M (H*d, d) K-major, the GEMM1 weight:  W_M[h*d + j, i] = M_h[i, j]
+ *   W_N (d, H*d) K-major, the GEMM2 weight:  W_N[j, h*d + i] = N_h[i, j]
+ *   q' (B, H*d), p (B, H*d): head h at columns h*d .. h*d + d - 1
+ *   stats (B, H, 2): {m_h, l_h}, the softmax's max score and sum of exp(score - m_h) over the L positions.
+ *     Not the log-sum-exp m_h + log l_h: with every position masked, m_h = -1e9 and fp32 spacing there (64)
+ *     swallows log L.
+ * Sliced form (use_qkvo False; no weights, no GEMMs): q = t, head h reads columns [h*hd, (h+1)*hd) of t and
+ * x, score_hl = scale * q_h . x_l, and p (B, d) is the layer's output.
+ * The row kernels take the per-head width `width` (d folded, hd sliced), `x_step`, head h's first column of
+ * x (0 folded, hd sliced) and `scale` (1 folded: s is in W_M).  q and p have row pitch heads*width.
+ * Masking: mask (B, L) bytes, 0 = masked, or NULL (no masking).  A masked score is exactly -1e9 after the
+ * scale (masked_fill(mask == 0, -1e9)); the softmax runs over all L positions, so a row with every position
+ * masked gets a_hl = 1/L: p is the mean of all L history rows and each of them receives dp_h / L.
+ * Range: heads <= B2_MHTA_MAX_HEADS; heads*width <= B2_MHTA_MAX_WIDTH (one row's q', p, dp, dq' in one
+ * warp's registers and shared memory); d <= B2_MHTA_MAX_WIDTH; batch*L within int32.  The pack and unpack
+ * need heads*d <= B2_MHTA_MAX_WIDTH.  Outside the range every entry point returns B2_E_INVALID.
+ * Saved for the backward: t, x, the mask, q', p, stats and the packed W_M, W_N of the forward; the backward
+ * recomputes a_hl = exp(score_hl - m_h) / l_h and uses sum_l a_hl (dp_h . x_l) = dp_h . p_h, so it reads x
+ * once and writes dx once:
+ *   ds_hl = a_hl (dp_h . x_l - dp_h . p_h) (0 where masked),  dx_l = sum_h (a_hl dp_h + scale ds_hl q_h),
+ *   dq_h = scale sum_l ds_hl x_l
+ * (the sums over h and the columns of q_h, dp_h as they map onto x: all heads onto all d folded, head h onto
+ * its own hd sliced).
+ * b2_mhta_pack:   W_M, W_N "=" from W_q, W_k, W_v, W_o; one launch.
+ * b2_mhta_fwd:    p, stats "=" from q, x, mask; p_aux (optional, row pitch ld_aux) receives p's GEMM operand
+ *   copy: its bf16 rounding (aux_dtype B2_BF16) or its 3xTF32 small part (B2_F32).
+ * b2_mhta_bwd:    dq "=" (+ dq_aux as above), dx (B, L, d) "=" from q, x, mask, p, stats and dp.
+ * b2_mhta_unpack: gWq, gWk, gWv (A, d) and gWo (d, A) "=" from dW_M (H*d, d) and dW_N (d, H*d):
+ *   gW_q,h = s W_k,h dM_h^T,  gW_k,h = s W_q,h dM_h,  gW_v,h = W_o,h^T dN_h^T,  gW_o,h = dN_h^T W_v,h^T.
+ */
+#define B2_MHTA_MAX_WIDTH 1024
+#define B2_MHTA_MAX_HEADS 32
+B2_API int b2_mhta_pack(const float* Wq, const float* Wk, const float* Wv, const float* Wo, int d, int heads,
+                        int head_dim, float scale, float* WM, float* WN, void* stream);
+B2_API int b2_mhta_fwd(const float* q, const float* x, const uint8_t* mask, int64_t batch, int L, int d, int heads,
+                       int width, int x_step, float scale, float* p, float* stats, void* p_aux, int aux_dtype,
+                       int64_t ld_aux, void* stream);
+B2_API int b2_mhta_bwd(const float* q, const float* x, const uint8_t* mask, const float* p, const float* stats,
+                       const float* dp, int64_t batch, int L, int d, int heads, int width, int x_step, float scale,
+                       float* dq, float* dx, void* dq_aux, int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_mhta_unpack(const float* Wq, const float* Wk, const float* Wv, const float* Wo, const float* dWM,
+                          const float* dWN, int d, int heads, int head_dim, float scale, float* gWq, float* gWk,
+                          float* gWv, float* gWo, void* stream);
+
+/*
  * One CompressedInteractionNet layer (layers/interactions/compressed_interaction_net.py:70-73)
  * without the (B, F*H, D) Hadamard tensor:
  *   out[b,h',d] = bias[h'] + sum_{f,m} w[h', f*H + m] * x0[b,f,d] * xk[b,m,d]
