@@ -22,8 +22,8 @@ B2_CROSSMIX_MAX_RANK, B2_CROSSMIX_MAX_COLS = 64, 256
 B2_MHTA_MAX_WIDTH, B2_MHTA_MAX_HEADS = 1024, 32
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
-c_void_p, c_int, c_int32, c_int64, c_float = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,
-                                              ctypes.c_int64, ctypes.c_float)
+c_void_p, c_int, c_int32, c_int64, c_float, c_double = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,
+                                                        ctypes.c_int64, ctypes.c_float, ctypes.c_double)
 
 
 class b2_lazy_ctx(ctypes.Structure):
@@ -98,12 +98,12 @@ SIGNATURES = {
                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_lazy_sumsq": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "b2_lazy_adam_step": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p,
-                                  c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_void_p]),
+                                  c_void_p, c_void_p, c_void_p, c_float, c_double, c_double, c_float, c_void_p]),
     "b2_lazy_materialize": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
-                                    c_float, c_float, c_float, c_void_p]),
-    "b2_adam_sched": (c_int, [c_void_p, c_float, c_float, c_float, c_void_p, c_int64, c_void_p]),
-    "b2_adam_step_sched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
-                                   c_float, c_float, c_void_p, c_void_p, c_int, c_void_p]),
+                                    c_double, c_double, c_float, c_void_p]),
+    "b2_adam_sched": (c_int, [c_void_p, c_double, c_double, c_double, c_void_p, c_int64, c_void_p]),
+    "b2_adam_step_sched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_double,
+                                   c_double, c_float, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_shard_push": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_int, c_void_p, c_int, c_int64,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
                               c_void_p]),
@@ -175,15 +175,15 @@ SIGNATURES = {
     "b2_logit_bce_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_sumsq": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
-    "b2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
-                             c_float, c_float, c_float, c_void_p, c_int, c_void_p]),
+    "b2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_double,
+                             c_double, c_double, c_float, c_void_p, c_int, c_void_p]),
     "b2_sumsq_ex": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
-    "b2_adam_step_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float,
-                                c_float, c_float, c_float, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
-    "b2_adam_untouched": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float, c_float, c_float,
-                                  c_void_p, c_int, c_void_p]),
-    "b2_adam_touched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float, c_float,
-                                c_float, c_float, c_void_p, c_void_p, c_void_p]),
+    "b2_adam_step_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_double,
+                                c_double, c_double, c_float, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
+    "b2_adam_untouched": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_double, c_double, c_double,
+                                  c_float, c_void_p, c_int, c_void_p]),
+    "b2_adam_touched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_double,
+                                c_double, c_double, c_float, c_void_p, c_void_p, c_void_p]),
     "b2_table_mark": (c_int, [_FIELD_P, _FIELD_P, c_int, c_int64, c_int, c_void_p, c_void_p]),
     "b2_logloss_sum": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "b2_auc_workspace_bytes": (c_int, [c_int64, ctypes.POINTER(c_int64)]),

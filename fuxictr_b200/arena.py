@@ -133,6 +133,14 @@ class ParamArena(object):
         self.G.zero_()
 
 
+def adam_consts(betas):
+    """(fl32(1 - beta1), fl32(beta2), fl32(1 - beta2)): adam_const() in csrc/dense.cu and make_const() in
+    csrc/lazy_adam.cu.  1 - beta is taken in double and rounded once, as torch.optim.Adam passes the Python float
+    1 - beta2 to addcmul_; rounding beta to fp32 first would leave V 1e-5 (relative) off torch's."""
+    b1, b2 = float(betas[0]), float(betas[1])
+    return float(np.float32(1.0 - b1)), float(np.float32(b2)), float(np.float32(1.0 - b2))
+
+
 class LazyTables(object):
     """Bookkeeping of the lazily evaluated tables (see b2_lazy_ctx in include/fuxictr_b200.h):
     per-row `last_step`, the per-step worklist, the schedule table shared with the dense pass."""
@@ -177,11 +185,8 @@ class LazyTables(object):
         ctx.worklist, ctx.counter = self.worklist.data_ptr(), self.counter.data_ptr()
         ctx.delta_m = (opt.M.data_ptr() - a.P.data_ptr()) // 4
         ctx.delta_v = (opt.V.data_ptr() - a.P.data_ptr()) // 4
-        # the same float32 roundings as make_const() in csrc/lazy_adam.cu / adam_kernel in dense.cu:
-        # beta is rounded to fp32 FIRST, then 1 - beta is taken in double and rounded again
-        b1, b2 = float(np.float32(opt.betas[0])), float(np.float32(opt.betas[1]))
-        ctx.w1, ctx.beta2 = float(np.float32(1.0 - b1)), b2
-        ctx.w2, ctx.eps = float(np.float32(1.0 - b2)), opt.eps
+        ctx.w1, ctx.beta2, ctx.w2 = adam_consts(opt.betas)
+        ctx.eps = opt.eps
         ctx.worklist_capacity = self.capacity
         for i, t in enumerate(emb_tables):
             ctx.grow_emb[i] = t._b2_grow_base

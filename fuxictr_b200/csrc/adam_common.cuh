@@ -10,10 +10,13 @@
 #pragma once
 #include <cuda_runtime.h>
 
+// 1 - beta is taken in double from the caller's double beta and rounded to fp32 once, as torch rounds the
+// Python float 1 - beta2 it passes to addcmul_ (adam_const in dense.cu, make_const in lazy_adam.cu and
+// LazyTables._new_ctx in arena.py form the same three floats).
 struct B2AdamConst {
-  float w1;    // 1 - beta1
-  float b2;    // beta2
-  float w2;    // 1 - beta2
+  float w1;    // fl32(1 - beta1)
+  float b2;    // fl32(beta2)
+  float w2;    // fl32(1 - beta2)
   float eps;
 };
 

@@ -334,30 +334,33 @@ extern "C" B2_API int b2_sumsq(const float* g, int64_t n, float* out, void* stre
 
 // sched[step] is written first so that the dense pass and every later lazy catch-up of the same
 // step read the SAME two scalars.
-__global__ void adam_sched_kernel(const int64_t* __restrict__ step_dev, float lr, float beta1, float beta2,
+__global__ void adam_sched_kernel(const int64_t* __restrict__ step_dev, double lr, double beta1, double beta2,
                                   B2AdamSched* __restrict__ sched, int64_t sched_len) {
   const int64_t t = *step_dev;
   if (t < 1 || t >= sched_len) return;
-  const double bc1 = 1.0 - pow((double) beta1, (double) t);
-  const double bc2 = 1.0 - pow((double) beta2, (double) t);
-  sched[t] = make_float2((float) ((double) lr / bc1), (float) (1.0 / sqrt(bc2)));
+  const double bc1 = 1.0 - pow(beta1, (double) t);
+  const double bc2 = 1.0 - pow(beta2, (double) t);
+  sched[t] = make_float2((float) (lr / bc1), (float) (1.0 / sqrt(bc2)));
 }
 
 // The two per-step scalars of step t (1-based): lr / (1 - beta1^t) and 1 / sqrt(1 - beta2^t).  Every dense pass
-// computes them here, so a step split over several launches applies the same two floats everywhere.
-__device__ __forceinline__ void adam_step_scalars(int64_t t, float lr, float beta1, float beta2, float& step_size,
+// computes them here, so a step split over several launches applies the same two floats everywhere.  lr and the
+// betas are the caller's doubles, as torch.optim.Adam forms lr / (1 - beta1^t) from Python floats.
+__device__ __forceinline__ void adam_step_scalars(int64_t t, double lr, double beta1, double beta2, float& step_size,
                                                   float& ibc2) {
-  const double bc1 = 1.0 - pow((double) beta1, (double) t);
-  const double bc2 = 1.0 - pow((double) beta2, (double) t);
-  step_size = (float) ((double) lr / bc1);
+  const double bc1 = 1.0 - pow(beta1, (double) t);
+  const double bc2 = 1.0 - pow(beta2, (double) t);
+  step_size = (float) (lr / bc1);
   ibc2 = (float) (1.0 / sqrt(bc2));
 }
 
-__device__ __forceinline__ B2AdamConst adam_const(float beta1, float beta2, float eps) {
+// 1 - beta in double, rounded once (torch passes 1 - beta2 to addcmul_ as a Python float): rounding beta to fp32
+// first would move fl32(1 - 0.999) from 1.00000005e-3 to 0.999987e-3 and leave V 1e-5 off torch's.
+__device__ __forceinline__ B2AdamConst adam_const(double beta1, double beta2, float eps) {
   B2AdamConst c;
-  c.w1 = (float) (1.0 - (double) beta1);
-  c.b2 = beta2;
-  c.w2 = (float) (1.0 - (double) beta2);
+  c.w1 = (float) (1.0 - beta1);
+  c.b2 = (float) beta2;
+  c.w2 = (float) (1.0 - beta2);
   c.eps = eps;
   return c;
 }
@@ -367,7 +370,7 @@ __device__ __forceinline__ B2AdamConst adam_const(float beta1, float beta2, floa
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
             float* __restrict__ v, int64_t n, const float* __restrict__ sumsq, float max_norm,
-            float lr, float beta1, float beta2, float eps, const int64_t* __restrict__ step_dev,
+            double lr, double beta1, double beta2, float eps, const int64_t* __restrict__ step_dev,
             int zero_grad, const B2AdamSched* __restrict__ sched, uint8_t* __restrict__ flags, int64_t nf4,
             int touched_only) {
   b2_pdl_wait();
@@ -430,8 +433,8 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
 }
 
 extern "C" B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n,
-                                      const float* sumsq, float max_norm, float lr, float beta1,
-                                      float beta2, float eps, const int64_t* step_dev, int zero_grad,
+                                      const float* sumsq, float max_norm, double lr, double beta1,
+                                      double beta2, float eps, const int64_t* step_dev, int zero_grad,
                                       uint8_t* flags, int64_t n_flagged, void* stream) {
   B2_REQUIRE(p && g && m && v && step_dev, "NULL pointer");
   B2_REQUIRE((((uintptr_t) p | (uintptr_t) g | (uintptr_t) m | (uintptr_t) v) % 16) == 0,
@@ -451,8 +454,8 @@ extern "C" B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, in
 }
 
 extern "C" B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n,
-                            const float* sumsq, float max_norm, float lr, float beta1,
-                            float beta2, float eps, const int64_t* step_dev, int zero_grad,
+                            const float* sumsq, float max_norm, double lr, double beta1,
+                            double beta2, float eps, const int64_t* step_dev, int zero_grad,
                             void* stream) {
   return b2_adam_step_ex(p, g, m, v, n, sumsq, max_norm, lr, beta1, beta2, eps, step_dev, zero_grad, nullptr, 0,
                          stream);
@@ -482,7 +485,7 @@ __device__ __forceinline__ void st_evict_first(float4* p, const float4& v) {
 // 3 x 64 B per granule out of L1 and first in line for eviction from L2, where the GEMM operands live.
 __global__ void __launch_bounds__(UNTOUCHED_THREADS, 1)
 adam_untouched_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v, int64_t n4,
-                      const uint8_t* __restrict__ flags, float lr, float beta1, float beta2, float eps,
+                      const uint8_t* __restrict__ flags, double lr, double beta1, double beta2, float eps,
                       const int64_t* __restrict__ step_dev) {
   b2_pdl_wait();
   __shared__ B2AdamConst sc;
@@ -526,8 +529,8 @@ adam_untouched_kernel(float* __restrict__ p, float* __restrict__ m, float* __res
   }
 }
 
-extern "C" B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, float lr,
-                                        float beta1, float beta2, float eps, const int64_t* step_dev, int max_ctas,
+extern "C" B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, double lr,
+                                        double beta1, double beta2, float eps, const int64_t* step_dev, int max_ctas,
                                         void* stream) {
   B2_REQUIRE(p && m && v && flags && step_dev, "NULL pointer");
   B2_REQUIRE((((uintptr_t) p | (uintptr_t) m | (uintptr_t) v) % 16) == 0, "arenas must be 16-byte aligned");
@@ -544,7 +547,7 @@ extern "C" B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n,
 }
 
 extern "C" B2_API int b2_adam_touched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
-                                      float max_norm, float lr, float beta1, float beta2, float eps,
+                                      float max_norm, double lr, double beta1, double beta2, float eps,
                                       const int64_t* step_dev, uint8_t* flags, void* stream) {
   B2_REQUIRE(p && g && m && v && step_dev && flags, "NULL pointer");
   B2_REQUIRE((((uintptr_t) p | (uintptr_t) g | (uintptr_t) m | (uintptr_t) v) % 16) == 0,
@@ -560,7 +563,7 @@ extern "C" B2_API int b2_adam_touched(float* p, float* g, float* m, float* v, in
   return B2_OK;
 }
 
-extern "C" B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
+extern "C" B2_API int b2_adam_sched(const int64_t* step_dev, double lr, double beta1, double beta2, float* sched,
                                     int64_t sched_len, void* stream) {
   B2_REQUIRE(step_dev && sched && sched_len >= 2, "NULL pointer / empty schedule table");
   adam_sched_kernel<<<1, 1, 0, (cudaStream_t) stream>>>(step_dev, lr, beta1, beta2,
@@ -570,7 +573,7 @@ extern "C" B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float bet
 }
 
 extern "C" B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
-                                         float max_norm, float beta1, float beta2, float eps,
+                                         float max_norm, double beta1, double beta2, float eps,
                                          const int64_t* step_dev, const float* sched, int zero_grad,
                                          void* stream) {
   B2_REQUIRE(p && g && m && v && step_dev && sched, "NULL pointer");
@@ -581,7 +584,7 @@ extern "C" B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v,
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
   const B2AdamSched* sched_tab = reinterpret_cast<const B2AdamSched*>(sched);
-  B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, 0.f, beta1, beta2,
+  B2_LAUNCH(adam_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, p, g, m, v, n, sumsq, max_norm, 0.0, beta1, beta2,
             eps, step_dev, zero_grad, sched_tab, (uint8_t*) nullptr, (int64_t) 0, 0);
   B2_CUDA_LAUNCH_CHECK("b2_adam_step_sched");
   return B2_OK;

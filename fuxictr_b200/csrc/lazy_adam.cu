@@ -137,11 +137,12 @@ int grid_rows(int64_t rows) {
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
   return (int) (blocks < 1 ? 1 : blocks);
 }
-B2AdamConst make_const(float beta1, float beta2, float eps) {
+// the constants of adam_const() in dense.cu: 1 - beta formed in double and rounded once
+B2AdamConst make_const(double beta1, double beta2, float eps) {
   B2AdamConst c;
-  c.w1 = (float) (1.0 - (double) beta1);
-  c.b2 = beta2;
-  c.w2 = (float) (1.0 - (double) beta2);
+  c.w1 = (float) (1.0 - beta1);
+  c.b2 = (float) beta2;
+  c.w2 = (float) (1.0 - beta2);
   c.eps = eps;
   return c;
 }
@@ -161,7 +162,7 @@ extern "C" B2_API int b2_lazy_adam_step(const b2_lazy_table* tables_dev, int nta
                                         const int32_t* counter, int capacity, int64_t delta_g, int64_t delta_m,
                                         int64_t delta_v, int32_t* last_step, const float* sched,
                                         const int64_t* step_dev, const float* sumsq, float max_norm,
-                                        float beta1, float beta2, float eps, void* stream) {
+                                        double beta1, double beta2, float eps, void* stream) {
   B2_REQUIRE(tables_dev && worklist && counter && last_step && sched && step_dev && ntables >= 1 && capacity >= 1,
              "bad argument");
   lazy_adam_kernel<<<grid_rows(capacity), 256, sizeof(b2_lazy_table) * ntables, (cudaStream_t) stream>>>(
@@ -173,7 +174,7 @@ extern "C" B2_API int b2_lazy_adam_step(const b2_lazy_table* tables_dev, int nta
 
 extern "C" B2_API int b2_lazy_materialize(const b2_lazy_table* tables_dev, int ntables, int64_t total_rows,
                                           int64_t delta_m, int64_t delta_v, int32_t* last_step,
-                                          const float* sched, const int64_t* step_dev, float beta1, float beta2,
+                                          const float* sched, const int64_t* step_dev, double beta1, double beta2,
                                           float eps, void* stream) {
   B2_REQUIRE(tables_dev && last_step && sched && step_dev && ntables >= 1 && total_rows >= 1, "bad argument");
   lazy_materialize_kernel<<<grid_rows(total_rows), 256, 0, (cudaStream_t) stream>>>(

@@ -193,7 +193,7 @@ typedef struct b2_lazy_ctx {
   int32_t* worklist;        /* [capacity] global row ids touched this step */
   int32_t* counter;         /* device scalar: worklist length */
   int64_t delta_m, delta_v; /* element offsets from a parameter to its Adam moments (arena layout) */
-  float w1, beta2, w2, eps; /* 1-beta1, beta2, 1-beta2, eps */
+  float w1, beta2, w2, eps; /* fl32(1-beta1), fl32(beta2), fl32(1-beta2) from the double betas; eps */
   int32_t worklist_capacity, pad_;
   int64_t grow_emb[B2_MAX_FIELDS]; /* global row base of the embedding table of each field */
   int64_t grow_lr[B2_MAX_FIELDS];  /* ... and of its LR table */
@@ -255,11 +255,11 @@ B2_API int b2_lazy_sumsq(const b2_lazy_table* tables_dev, int ntables, const int
 B2_API int b2_lazy_adam_step(const b2_lazy_table* tables_dev, int ntables, const int32_t* worklist,
                              const int32_t* counter, int capacity, int64_t delta_g, int64_t delta_m,
                              int64_t delta_v, int32_t* last_step, const float* sched,
-                             const int64_t* step_dev, const float* sumsq, float max_norm, float beta1,
-                             float beta2, float eps, void* stream);
+                             const int64_t* step_dev, const float* sumsq, float max_norm, double beta1,
+                             double beta2, float eps, void* stream);
 B2_API int b2_lazy_materialize(const b2_lazy_table* tables_dev, int ntables, int64_t total_rows,
                                int64_t delta_m, int64_t delta_v, int32_t* last_step, const float* sched,
-                               const int64_t* step_dev, float beta1, float beta2, float eps, void* stream);
+                               const int64_t* step_dev, double beta1, double beta2, float eps, void* stream);
 
 /*
  * Row-sharded tables across the GPUs of one NVSwitch box (SURVEY.md 8e): row r of every table
@@ -689,10 +689,18 @@ B2_API int b2_logit_bce_fwd(const float* t0, const float* t1, const float* t2, c
  *   If zero_grad != 0 the gradient arena is zeroed in the same pass.
  *   b2_adam_sched writes sched[step] = {lr/(1-b1^step), 1/sqrt(1-b2^step)}; b2_adam_step_sched is
  *   b2_adam_step reading those two scalars from the table (shared with the lazy row-wise kernels).
+ * Constants, as torch forms them from Python floats: every Adam entry point (and b2_lazy_adam_step,
+ * b2_lazy_materialize) takes lr, beta1 and beta2 as double; 1-b1, b2 and 1-b2 are computed in double and
+ * rounded to fp32 once, bc1 and bc2 come from pow of the double betas, and the step size is fl32(lr/bc1).
+ * eps and max_norm are fp32, as torch applies them.
+ * A NaN norm (a NaN gradient) is where these kernels leave torch: torch's clip coefficient is then NaN and
+ * every parameter becomes NaN, here fminf(NaN, 1) = 1 and the step runs unclipped.  b2_adam_untouched runs
+ * before the norm exists, so no pass could follow torch there.  An infinite norm gives clip_coef = 0, as in
+ * torch.
  */
 B2_API int b2_sumsq(const float* g, int64_t n, float* out, void* stream);
 B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
-                 float max_norm, float lr, float beta1, float beta2, float eps,
+                 float max_norm, double lr, double beta1, double beta2, float eps,
                  const int64_t* step_dev, int zero_grad, void* stream);
 /* The same two passes reading G only where a batch wrote it: flags[k] (b2_touch) covers elements
  * [16k, 16k + 16) of the first n_flagged elements (n_flagged % 4 == 0, <= n); the elements after
@@ -703,7 +711,7 @@ B2_API int b2_adam_step(float* p, float* g, float* m, float* v, int64_t n, const
 B2_API int b2_sumsq_ex(const float* g, int64_t n, float* out, const uint8_t* flags, int64_t n_flagged,
                        void* stream);
 B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
-                           float max_norm, float lr, float beta1, float beta2, float eps,
+                           float max_norm, double lr, double beta1, double beta2, float eps,
                            const int64_t* step_dev, int zero_grad, uint8_t* flags, int64_t n_flagged,
                            void* stream);
 /* The table pass of b2_adam_step_ex (zero_grad = 1, n_flagged = n) split in two launches, for a step whose
@@ -714,15 +722,15 @@ B2_API int b2_adam_step_ex(float* p, float* g, float* m, float* v, int64_t n, co
  *   b2_adam_touched    every FLAGGED granule is updated as b2_adam_step_ex does (step *step_dev), its gradient
  *                      zeroed and its flag cleared; an unflagged granule costs one flag read.
  * Together they leave P, M, V, G and the flags bit-identical to b2_adam_step_ex.  n % 4 == 0. */
-B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, float lr, float beta1,
-                             float beta2, float eps, const int64_t* step_dev, int max_ctas, void* stream);
+B2_API int b2_adam_untouched(float* p, float* m, float* v, int64_t n, const uint8_t* flags, double lr, double beta1,
+                             double beta2, float eps, const int64_t* step_dev, int max_ctas, void* stream);
 B2_API int b2_adam_touched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq, float max_norm,
-                           float lr, float beta1, float beta2, float eps, const int64_t* step_dev, uint8_t* flags,
+                           double lr, double beta1, double beta2, float eps, const int64_t* step_dev, uint8_t* flags,
                            void* stream);
-B2_API int b2_adam_sched(const int64_t* step_dev, float lr, float beta1, float beta2, float* sched,
+B2_API int b2_adam_sched(const int64_t* step_dev, double lr, double beta1, double beta2, float* sched,
                          int64_t sched_len, void* stream);
 B2_API int b2_adam_step_sched(float* p, float* g, float* m, float* v, int64_t n, const float* sumsq,
-                              float max_norm, float beta1, float beta2, float eps, const int64_t* step_dev,
+                              float max_norm, double beta1, double beta2, float eps, const int64_t* step_dev,
                               const float* sched, int zero_grad, void* stream);
 
 /*
