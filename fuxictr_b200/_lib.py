@@ -131,7 +131,13 @@ SIGNATURES = {
                                 c_int64, c_void_p, c_void_p]),
     "b2_crossmix_unpack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p]),
-    "b2_mhta_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
+    "b2_gdcn_pack": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2_gdcn_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int,
+                            c_int64, c_void_p]),
+    "b2_gdcn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int,
+                            c_int64, c_void_p, c_void_p, c_void_p]),
+    "b2_gdcn_unpack": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_mhta_pack":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                              c_void_p, c_void_p]),
     "b2_mhta_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float,
                             c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),

@@ -1120,6 +1120,77 @@ def crossnet_mix_layer(x0, xl, U, V, C, gating_weights, bias):
     return _CrossMixLayer.apply(x0, xl, U, V, C, gating_weights, bias)
 
 
+class _GatedCrossLayer(torch.autograd.Function):
+    """One GDCN gated cross layer, x_next = x_0 * (x_i W^T + b) * sigmoid(x_i Wg^T) + x_i (GDCN.py,
+    GateCorssLayer.forward), as one GEMM and one row kernel (include/fuxictr_b200.h "GDCN"): Wp = [W; Wg]
+    (b2_gdcn_pack), P = x_i Wp^T, x_next from P (b2_gdcn_fwd, which also writes x_next's auxiliary operand for the
+    next layer's GEMM).  Backward: dP, dx_0 and the bias gradient from P (b2_gdcn_bwd), dx_i = g + dP Wp (one
+    dgrad, K = 2d, epilogue add), dWp = dP^T x_i (one wgrad) and one b2_gdcn_unpack into the gradients of W, Wg."""
+
+    @staticmethod
+    def forward(ctx, x0, xi, w, wg, b):
+        ctx.w, ctx.wg, ctx.b = w, wg, b             # the parameters: their gradients may live in an arena
+        x0, xi, w, wg, b = _f32c(x0), _f32c(xi), _f32c(w), _f32c(wg), _f32c(b)
+        B, d = xi.shape
+        dev = xi.device
+        Wp = torch.empty((2 * d, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_gdcn_pack", _ptr(w), _ptr(wg), d, _ptr(Wp), _stream())
+        tc = _tc_layer_ok(Wp) and xi.data_ptr() % 16 == 0 and x0.data_ptr() % 16 == 0
+        xi_aux = make_aux(xi) if tc else None
+        wp_aux = make_aux(Wp) if tc else None
+        P = torch.empty((B, 2 * d), dtype=torch.float32, device=dev)
+        _linear_fwd(tc, xi, xi_aux, Wp, P, wp_aux)
+        out = torch.empty_like(xi)
+        out_aux = empty_aux(B, d, dev) if tc else None
+        _lib.call("b2_gdcn_fwd", _ptr(P), _ptr(b), _ptr(x0), _ptr(xi), B, d, _ptr(out), *_aux_args(out_aux),
+                  _stream())
+        if out_aux is not None:         # the next layer's (or the MLP's) make_aux finds it
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        ctx.save_for_backward(x0, xi, P, Wp, b)
+        ctx.tc, ctx.aux = tc, (xi_aux, wp_aux)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x0, xi, P, Wp, b = ctx.saved_tensors
+        g = _f32c(g)
+        xi_aux, wp_aux = ctx.aux
+        tc = ctx.tc
+        B, d = xi.shape
+        dev = xi.device
+        _, _, w_grad, wg_grad, b_grad = ctx.needs_input_grad
+        dP = torch.empty((B, 2 * d), dtype=torch.float32, device=dev)
+        dp_aux = empty_aux(B, 2 * d, dev) if tc else None
+        gx0 = torch.empty_like(x0)
+        gb = _grad_buffer(ctx.b, zero=True) if b_grad else torch.zeros_like(b)
+        _lib.call("b2_gdcn_bwd", _ptr(P), _ptr(b), _ptr(x0), _ptr(g), B, d, _ptr(dP), *_aux_args(dp_aux), _ptr(gx0),
+                  _ptr(gb), _stream())
+        gxi = torch.empty_like(xi)
+        _linear_dgrad(tc, dP, dp_aux, Wp, gxi, wp_aux, add=g)                               # dx_i = g + dP Wp
+        gw = gwg = None
+        if w_grad or wg_grad:
+            dWp = torch.empty_like(Wp)
+            _linear_wgrad(tc, dP, dp_aux, xi, xi_aux, dWp)                                 # dWp = dP^T x_i
+            gw = _grad_buffer(ctx.w, zero=False) if w_grad else torch.empty_like(ctx.w)
+            gwg = _grad_buffer(ctx.wg, zero=False) if wg_grad else torch.empty_like(ctx.wg)
+            _lib.call("b2_gdcn_unpack", _ptr(dWp), d, _ptr(gw), _ptr(gwg), _stream())
+        return (gx0 if ctx.needs_input_grad[0] else None, gxi, gw if w_grad else None, gwg if wg_grad else None,
+                gb if b_grad else None)
+
+
+def gated_cross_layer(x0, xi, w, wg, b):
+    """x_next of one GDCN gated cross layer: w, wg (d, d) are the layer's w[i].weight and wg[i].weight, b (d,) its
+    b[i]; x0 and xi (B, d)."""
+    _require_cuda(x0, xi, w, wg, b)
+    if xi.dim() != 2 or tuple(x0.shape) != tuple(xi.shape):
+        raise ValueError("gated_cross_layer: x0%s and xi%s must be the same (B, d)" % (tuple(x0.shape), tuple(xi.shape)))
+    d = xi.shape[1]
+    if tuple(w.shape) != (d, d) or tuple(wg.shape) != (d, d) or tuple(b.shape) != (d,):
+        raise ValueError("gated_cross_layer: shapes x%s w%s wg%s b%s do not match"
+                         % tuple(tuple(t.shape) for t in (xi, w, wg, b)))
+    return _GatedCrossLayer.apply(x0, xi, w, wg, b)
+
+
 # --------------------------------------------------------------------------------------
 # MultiHeadTargetAttention
 # --------------------------------------------------------------------------------------

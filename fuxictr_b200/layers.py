@@ -524,6 +524,29 @@ class CrossNetMix(nn.Module):
         return x_l.squeeze()
 
 
+class GateCorssLayer(nn.Module):
+    """GDCN's gated cross network (model_zoo/GDCN/src/GDCN.py, GateCorssLayer; the reference's spelling),
+    x_{i+1} = x_0 * (W_i x_i + b_i) * sigmoid(Wg_i x_i) + x_i.  Each layer is one autograd node: one GEMM on the
+    stacked [W_i; Wg_i] and one row kernel (functional._GatedCrossLayer).  Children `w`, `wg` (bias-free Linears),
+    `b` (uniform in [0, 1)) and `activation`, registered and drawn in the reference's order."""
+
+    def __init__(self, input_dim, cn_layers=3):
+        super(GateCorssLayer, self).__init__()
+        self.cn_layers = cn_layers
+        self.w = nn.ModuleList([nn.Linear(input_dim, input_dim, bias=False) for _ in range(cn_layers)])
+        self.wg = nn.ModuleList([nn.Linear(input_dim, input_dim, bias=False) for _ in range(cn_layers)])
+        self.b = nn.ParameterList([nn.Parameter(torch.zeros(input_dim)) for _ in range(cn_layers)])
+        for p in self.b:
+            nn.init.uniform_(p.data)
+        self.activation = nn.Sigmoid()
+
+    def forward(self, x):
+        x0 = x
+        for i in range(self.cn_layers):
+            x = F2.gated_cross_layer(x0, x, self.w[i].weight, self.wg[i].weight, self.b[i])
+        return x
+
+
 # --------------------------------------------------------------------------------------
 # CIN
 # --------------------------------------------------------------------------------------

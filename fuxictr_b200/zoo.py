@@ -12,6 +12,7 @@ same RNG consumption) and nothing else.
   DLRM     model_zoo/DLRM/src/DLRM.py:43-123
   DIN      model_zoo/DIN/src/DIN.py:50-149
   xDeepFM  model_zoo/xDeepFM/src/xDeepFM.py:41-97
+  GDCN, GDCNP  model_zoo/GDCN/src/GDCN.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -21,7 +22,7 @@ import torch
 from torch import nn
 
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
-                     CrossNetV2, InnerProductInteraction, DIN_Attention, Dice,
+                     CrossNetV2, GateCorssLayer, InnerProductInteraction, DIN_Attention, Dice,
                      CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -170,14 +171,14 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN) may be sharded: any other forward would keep reading the
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP) may be sharded: any other forward would keep reading the
         1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
         from . import sharded as SH
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
-                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM and DIN" % type(self).__name__)
+                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN and GDCNP" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -251,6 +252,13 @@ class RankModel(nn.Module):
             mat = v.as_strided((v.shape[0], width), (v.stride(0), 1), v.storage_offset() - col)
             return mat.to(self.device)
         raise RuntimeError("sharded front needs the batch dict to be column views of one matrix")
+
+    def _flat_embedding(self, inputs):
+        """embedding_layer(X, flatten_emb=True), or the same rows from the row-sharded front after enable_sharding()."""
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull
+            from .sharded import sharded_front
+            return sharded_front(self._sharded_front, self._batch_matrix(inputs))[0].flatten(start_dim=1)
+        return self.embedding_layer(self.get_inputs(inputs), flatten_emb=True)
 
     def _front_tables(self):
         """Embedding + LR tables read ONLY through the fused front kernels (lazy-Adam candidates)."""
@@ -472,11 +480,7 @@ class DCNv2(RankModel):
 
     def _final_out(self, inputs):
         """DCNv2.py:108-128: what the last Linear sees for each model_structure."""
-        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull
-            from .sharded import sharded_front
-            emb = sharded_front(self._sharded_front, self._batch_matrix(inputs))[0].flatten(start_dim=1)
-        else:
-            emb = self.embedding_layer(self.get_inputs(inputs), flatten_emb=True)
+        emb = self._flat_embedding(inputs)
         cross = self.crossnet(emb)
         left = self.stacked_dnn(cross) if hasattr(self, "stacked_dnn") else cross
         if not hasattr(self, "parallel_dnn"):
@@ -490,6 +494,71 @@ class DCNv2(RankModel):
     def forward(self, inputs):
         y_pred = F2.linear_act(self._final_out(inputs), self.fc.weight, self.fc.bias)
         return {"y_pred": self.output_activation(y_pred)}
+
+
+def _gdcn_dnn_units(name, dnn_hidden_units):
+    """GDCN and GDCNP need a DNN tower: the reference builds none for empty dnn_hidden_units and then fails (GDCNP
+    at construction, GDCN at its first forward); refuse before anything is built."""
+    if not dnn_hidden_units:
+        raise ValueError("%s needs a non-empty dnn_hidden_units (its DNN tower %s)"
+                         % (name, "gives the logit" if name == "GDCN" else "feeds fc"))
+    return list(dnn_hidden_units)
+
+
+class GDCN(RankModel):
+    """model_zoo/GDCN/src/GDCN.py, GDCN: the gated cross network stacked under a DNN that ends in the logit,
+    y = sigmoid(dnn(cross_net(flatten(E)))).  Unknown keyword arguments (the GDCN_test YAML's `crossing_layers`)
+    are accepted and ignored, as the reference's **kwargs do."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="GDCN", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 dnn_hidden_units=[], dnn_activations="ReLU", num_cross_layers=3, net_dropout=0, batch_norm=False,
+                 embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(GDCN, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                   embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                   **kwargs)
+        units = _gdcn_dnn_units("GDCN", dnn_hidden_units)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        width = feature_map.sum_emb_out_dim()
+        self.dnn = MLP_Block(width, hidden_units=units, hidden_activations=dnn_activations, output_dim=1,
+                             output_activation=None, dropout_rates=net_dropout, batch_norm=batch_norm)
+        self.cross_net = GateCorssLayer(width, num_cross_layers)
+        self._finish(kwargs, learning_rate)
+
+    def forward_logits(self, inputs):
+        return (self.dnn(self.cross_net(self._flat_embedding(inputs))),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class GDCNP(RankModel):
+    """model_zoo/GDCN/src/GDCN.py, GDCNP: the gated cross network beside a DNN tower, one Linear over
+    [cross_net(E) | dnn(E)] to the logit.  Unknown keyword arguments are ignored as in GDCN."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="GDCNP", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 dnn_hidden_units=[], dnn_activations="ReLU", num_cross_layers=3, net_dropout=0, batch_norm=False,
+                 embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(GDCNP, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                    embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                    **kwargs)
+        units = _gdcn_dnn_units("GDCNP", dnn_hidden_units)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        width = feature_map.sum_emb_out_dim()
+        self.dnn = MLP_Block(width, hidden_units=units, hidden_activations=dnn_activations, output_dim=None,
+                             output_activation=None, dropout_rates=net_dropout, batch_norm=batch_norm)
+        self.cross_net = GateCorssLayer(width, num_cross_layers)
+        self.fc = nn.Linear(units[-1] + width, 1)
+        self._finish(kwargs, learning_rate)
+
+    def forward_logits(self, inputs):
+        emb = self._flat_embedding(inputs)
+        cross = self.cross_net(emb)
+        return (F2.linear_act(torch.cat([cross, self.dnn(emb)], dim=1), self.fc.weight, self.fc.bias),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
 
 
 class DLRM(RankModel):

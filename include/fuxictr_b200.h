@@ -410,6 +410,34 @@ B2_API int b2_crossmix_unpack(const float* dW1, const float* dW2, int d, int r, 
                               float* gG, void* stream);
 
 /*
+ * GDCN's gated cross layer (model_zoo/GDCN/src/GDCN.py, GateCorssLayer), one layer:
+ *   x_{i+1} = x_0 * (x_i W^T + b) * sigmoid(x_i Wg^T) + x_i
+ * as one GEMM P = x_i Wp^T on the stacked weight and one row kernel.  W, Wg (d, d) are the layer's
+ * w[i].weight and wg[i].weight, b (d) its b[i].  All row-major fp32:
+ *   Wp (2d, d) K-major: rows 0 .. d-1 are W, rows d .. 2d-1 are Wg
+ *   P  (B, 2d) = x_i Wp^T: columns 0 .. d-1 u = x_i W^T, columns d .. 2d-1 z = x_i Wg^T
+ *   dP (B, 2d): the gradient of P, [g x_0 s | g x_0 lin s (1 - s)] with lin = u + b, s = sigmoid(z)
+ *   dWp (2d, d) = dP^T x_i: rows 0 .. d-1 the gradient of W, rows d .. 2d-1 that of Wg
+ * Saved for the backward: x_0, x_i, P and the forward's Wp; the backward recomputes lin and s from P and b.
+ * Range: any d >= 1 and batch >= 0 with batch * 2d < 2^31; d % 4 == 0 with 16-byte aligned rows takes a float4
+ * path, anything else a scalar one.  Outside the range, or given a NULL pointer, every entry point returns
+ * B2_E_INVALID.
+ * b2_gdcn_pack:   Wp "=" from W, Wg; one launch.
+ * b2_gdcn_fwd:    out (B, d) "=" from P, b, x_0, x_i; out_aux (optional, row pitch ld_aux) receives out's GEMM
+ *   operand copy for the next layer: its bf16 rounding (aux_dtype B2_BF16) or its 3xTF32 small part (B2_F32).
+ * b2_gdcn_bwd:    dP "=" (+ dp_aux as above, row width 2d) and gx0 (B, d) "=" g lin s from P, b, x_0 and the
+ *   output gradient g; db (d) "+=" (caller zeroes) the column sums of dP's first half: a per-CTA sum, then one
+ *   float atomic per column and CTA.
+ * b2_gdcn_unpack: gW, gWg (d, d) "=" from dWp.
+ */
+B2_API int b2_gdcn_pack(const float* W, const float* Wg, int d, float* Wp, void* stream);
+B2_API int b2_gdcn_fwd(const float* P, const float* b, const float* x0, const float* xi, int64_t batch, int d,
+                       float* out, void* out_aux, int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_gdcn_bwd(const float* P, const float* b, const float* x0, const float* g, int64_t batch, int d,
+                       float* dP, void* dp_aux, int aux_dtype, int64_t ld_aux, float* gx0, float* db, void* stream);
+B2_API int b2_gdcn_unpack(const float* dWp, int d, float* gW, float* gWg, void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
