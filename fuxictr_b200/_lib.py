@@ -137,6 +137,15 @@ SIGNATURES = {
     "b2_gdcn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int,
                             c_int64, c_void_p, c_void_p, c_void_p]),
     "b2_gdcn_unpack": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_fs_gate_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_void_p, c_void_p,
+                               c_void_p, c_void_p, c_int, c_int64, c_void_p]),
+    "b2_fs_gate_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_int,
+                               c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_agg_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_agg_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
+    "b2_agg_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                           c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_agg_unpack": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_mhta_pack":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                              c_void_p, c_void_p]),
     "b2_mhta_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float,

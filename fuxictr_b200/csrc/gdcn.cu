@@ -5,58 +5,16 @@
 // holds what lies around it: the pack of Wp, the row kernel that gates P into x_{i+1} (and back), and the split
 // of the stacked weight gradient.  Layouts: include/fuxictr_b200.h "GDCN".
 //
-// Row kernels: a CTA is ty_n rows of tx_n column slots (see gd_plan); a slot owns VW consecutive columns (4 on
-// the float4 path, 1 on the scalar one) and walks the batch rows with a grid stride.  The backward sums dlin over
-// its rows per slot in registers, then over the ty_n rows of the CTA in shared memory, and adds that into db with
+// Row kernels: row_common.cuh's layout.  The backward sums dlin per column (rk_cta_colsum) and adds that into db with
 // one float atomic per column and CTA (at most 4 CTAs per SM, so few atomics meet on one column).
 // sigmoid is 1 / (1 + expf(-z)) as torch evaluates it in fp32 (not __expf: its error shows at the 1e-5 bar).
-#include "b2_common.cuh"
-
-#define GD_THREADS 256
+#include "row_common.cuh"
 
 __device__ __forceinline__ float gd_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
 
-template <int VW>
-__device__ __forceinline__ void gd_load(const float* p, float (&v)[VW]) {
-  if constexpr (VW == 4) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(p));
-    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
-  } else {
-    v[0] = __ldg(p);
-  }
-}
-
-template <int VW>
-__device__ __forceinline__ void gd_store(float* p, const float (&v)[VW]) {
-  if constexpr (VW == 4) *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-  else p[0] = v[0];
-}
-
-// The GEMM-operand copy of VW values at aux + off: bf16 rounding or 3xTF32 small part (as b2_crossmix_fwd).
-template <int VW>
-__device__ __forceinline__ void gd_store_aux(void* aux, int aux_dtype, int64_t off, const float (&v)[VW]) {
-  if (aux_dtype == B2_BF16) {
-    __nv_bfloat16* a = reinterpret_cast<__nv_bfloat16*>(aux) + off;
-    if constexpr (VW == 4) {
-      __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
-      uint2 w;
-      w.x = *reinterpret_cast<uint32_t*>(&lo);
-      w.y = *reinterpret_cast<uint32_t*>(&hi);
-      *reinterpret_cast<uint2*>(a) = w;
-    } else {
-      a[0] = __float2bfloat16_rn(v[0]);
-    }
-  } else {
-    float s[VW];
-#pragma unroll
-    for (int k = 0; k < VW; ++k) s[k] = b2_tf32_small(v[k]);
-    gd_store<VW>(reinterpret_cast<float*>(aux) + off, s);
-  }
-}
-
 // out = x0 * (u + b) * sigmoid(z) + xi, u = P[:, :d], z = P[:, d:]
 template <int VW>
-__global__ void __launch_bounds__(GD_THREADS)
+__global__ void __launch_bounds__(RK_THREADS)
 gdcn_fwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const float* __restrict__ x0,
                 const float* __restrict__ xi, int64_t batch, int d, int tx_n, float* __restrict__ out,
                 void* out_aux, int aux_dtype, int64_t ld_aux) {
@@ -65,17 +23,17 @@ gdcn_fwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const 
   b2_pdl_wait();
   if (c < d) {
     float bb[VW];
-    gd_load<VW>(b + c, bb);
+    rk_load<VW>(b + c, bb);
     for (int64_t row = (int64_t) blockIdx.x * ty_n + ty; row < batch; row += (int64_t) gridDim.x * ty_n) {
       float u[VW], z[VW], a[VW], x[VW], o[VW];
-      gd_load<VW>(P + row * 2 * d + c, u);
-      gd_load<VW>(P + row * 2 * d + d + c, z);
-      gd_load<VW>(x0 + row * d + c, a);
-      gd_load<VW>(xi + row * d + c, x);
+      rk_load<VW>(P + row * 2 * d + c, u);
+      rk_load<VW>(P + row * 2 * d + d + c, z);
+      rk_load<VW>(x0 + row * d + c, a);
+      rk_load<VW>(xi + row * d + c, x);
 #pragma unroll
       for (int k = 0; k < VW; ++k) o[k] = a[k] * (u[k] + bb[k]) * gd_sigmoid(z[k]) + x[k];
-      gd_store<VW>(out + row * d + c, o);
-      if (out_aux) gd_store_aux<VW>(out_aux, aux_dtype, row * ld_aux + c, o);
+      rk_store<VW>(out + row * d + c, o);
+      if (out_aux) rk_store_aux<VW>(out_aux, aux_dtype, row * ld_aux + c, o);
     }
   }
   b2_pdl_trigger();
@@ -83,11 +41,11 @@ gdcn_fwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const 
 
 // dP = [g x0 s | g x0 lin s (1 - s)], gx0 = g lin s, db += sum_rows g x0 s    (lin = u + b, s = sigmoid(z))
 template <int VW>
-__global__ void __launch_bounds__(GD_THREADS)
+__global__ void __launch_bounds__(RK_THREADS)
 gdcn_bwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const float* __restrict__ x0,
                 const float* __restrict__ g, int64_t batch, int d, int tx_n, float* __restrict__ dP, void* dp_aux,
                 int aux_dtype, int64_t ld_aux, float* __restrict__ gx0, float* __restrict__ db) {
-  __shared__ float red[GD_THREADS * VW];
+  __shared__ float red[RK_THREADS * VW];
   const int tx = threadIdx.x % tx_n, ty = threadIdx.x / tx_n, ty_n = blockDim.x / tx_n;
   const int c = (blockIdx.y * tx_n + tx) * VW;
   float acc[VW];
@@ -96,13 +54,13 @@ gdcn_bwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const 
   b2_pdl_wait();
   if (c < d) {
     float bb[VW];
-    gd_load<VW>(b + c, bb);
+    rk_load<VW>(b + c, bb);
     for (int64_t row = (int64_t) blockIdx.x * ty_n + ty; row < batch; row += (int64_t) gridDim.x * ty_n) {
       float u[VW], z[VW], a[VW], gg[VW], du[VW], dz[VW], ga[VW];
-      gd_load<VW>(P + row * 2 * d + c, u);
-      gd_load<VW>(P + row * 2 * d + d + c, z);
-      gd_load<VW>(x0 + row * d + c, a);
-      gd_load<VW>(g + row * d + c, gg);
+      rk_load<VW>(P + row * 2 * d + c, u);
+      rk_load<VW>(P + row * 2 * d + d + c, z);
+      rk_load<VW>(x0 + row * d + c, a);
+      rk_load<VW>(g + row * d + c, gg);
 #pragma unroll
       for (int k = 0; k < VW; ++k) {
         const float lin = u[k] + bb[k], s = gd_sigmoid(z[k]), ga_s = gg[k] * a[k] * s;
@@ -111,26 +69,21 @@ gdcn_bwd_kernel(const float* __restrict__ P, const float* __restrict__ b, const 
         ga[k] = gg[k] * lin * s;
         acc[k] += ga_s;
       }
-      gd_store<VW>(dP + row * 2 * d + c, du);
-      gd_store<VW>(dP + row * 2 * d + d + c, dz);
-      gd_store<VW>(gx0 + row * d + c, ga);
+      rk_store<VW>(dP + row * 2 * d + c, du);
+      rk_store<VW>(dP + row * 2 * d + d + c, dz);
+      rk_store<VW>(gx0 + row * d + c, ga);
       if (dp_aux) {
-        gd_store_aux<VW>(dp_aux, aux_dtype, row * ld_aux + c, du);
-        gd_store_aux<VW>(dp_aux, aux_dtype, row * ld_aux + d + c, dz);
+        rk_store_aux<VW>(dp_aux, aux_dtype, row * ld_aux + c, du);
+        rk_store_aux<VW>(dp_aux, aux_dtype, row * ld_aux + d + c, dz);
       }
     }
   }
   b2_pdl_trigger();
-#pragma unroll
-  for (int k = 0; k < VW; ++k) red[threadIdx.x * VW + k] = acc[k];
-  __syncthreads();
+  rk_cta_colsum<VW>(red, tx, tx_n, ty_n, acc);
   if (ty == 0 && c < d) {
 #pragma unroll
-    for (int k = 0; k < VW; ++k) {
-      float s = 0.f;
-      for (int y = 0; y < ty_n; ++y) s += red[(y * tx_n + tx) * VW + k];
-      if (s != 0.f) b2_red_add(db + c + k, s);
-    }
+    for (int k = 0; k < VW; ++k)
+      if (acc[k] != 0.f) b2_red_add(db + c + k, acc[k]);
   }
 }
 
@@ -166,43 +119,6 @@ static int gd_check(int64_t batch, int d) {
   return B2_OK;
 }
 
-static int gd_check_aux(const void* aux, int aux_dtype, int64_t ld_aux, int width) {
-  if (aux == nullptr) return B2_OK;
-  B2_REQUIRE(aux_dtype == B2_F32 || aux_dtype == B2_BF16, "aux_dtype must be B2_F32 or B2_BF16");
-  B2_REQUIRE(ld_aux >= width, "ld_aux %lld < row width %d", (long long) ld_aux, width);
-  return B2_OK;
-}
-
-static bool gd_al16(const void* p) { return p == nullptr || ((uintptr_t) p & 15) == 0; }
-
-// float4 path: d % 4 == 0, every row 16-byte aligned, the auxiliary rows 16 (fp32) / 8 (bf16) bytes
-static bool gd_vec(int d, const void* const* ptrs, int n, const void* aux, int aux_dtype, int64_t ld_aux) {
-  if (d % 4 != 0) return false;
-  for (int i = 0; i < n; ++i)
-    if (!gd_al16(ptrs[i])) return false;
-  if (aux == nullptr) return true;
-  const uintptr_t align = aux_dtype == B2_BF16 ? 8 : 16;
-  return ld_aux % 4 == 0 && ((uintptr_t) aux & (align - 1)) == 0;
-}
-
-// The columns split into gy chunks of at most GD_THREADS slots; a CTA is ty_n rows of tx_n slots (tx_n: a chunk
-// rounded up to a warp), at most per_sm CTAs per SM over the batch.
-struct gd_grid {
-  dim3 grid;
-  int threads, tx_n;
-};
-
-static gd_grid gd_plan(int64_t batch, int d, int vw, int per_sm) {
-  const int cols = (d + vw - 1) / vw;
-  const int gy = (cols + GD_THREADS - 1) / GD_THREADS;
-  const int tx_n = ((cols + gy - 1) / gy + 31) / 32 * 32;
-  const int ty_n = GD_THREADS / tx_n;
-  int64_t cap = (int64_t) B2_NUM_SMS * per_sm / gy, gx = b2_ceil_div(batch, ty_n);
-  cap = cap < 1 ? 1 : cap;
-  gx = gx < 1 ? 1 : (gx > cap ? cap : gx);
-  return {dim3((unsigned) gx, (unsigned) gy), tx_n * ty_n, tx_n};
-}
-
 extern "C" B2_API int b2_gdcn_pack(const float* W, const float* Wg, int d, float* Wp, void* stream) {
   B2_REQUIRE(W && Wg && Wp, "NULL pointer");
   if (int rc = gd_check(0, d)) return rc;
@@ -217,15 +133,15 @@ extern "C" B2_API int b2_gdcn_fwd(const float* P, const float* b, const float* x
                                   int d, float* out, void* out_aux, int aux_dtype, int64_t ld_aux, void* stream) {
   B2_REQUIRE(P && b && x0 && xi && out, "NULL pointer");
   if (int rc = gd_check(batch, d)) return rc;
-  if (int rc = gd_check_aux(out_aux, aux_dtype, ld_aux, d)) return rc;
+  if (int rc = rk_check_aux(out_aux, aux_dtype, ld_aux, d)) return rc;
   if (batch == 0) return B2_OK;
   const void* ptrs[] = {P, b, x0, xi, out};
-  if (gd_vec(d, ptrs, 5, out_aux, aux_dtype, ld_aux)) {
-    const gd_grid g = gd_plan(batch, d, 4, 8);
+  if (rk_vec(d, ptrs, 5, out_aux, aux_dtype, ld_aux)) {
+    const rk_grid g = rk_plan(batch, d, 4, 8);
     B2_LAUNCH(gdcn_fwd_kernel<4>, g.grid, g.threads, 0, (cudaStream_t) stream, P, b, x0, xi, batch, d, g.tx_n,
               out, out_aux, aux_dtype, ld_aux);
   } else {
-    const gd_grid g = gd_plan(batch, d, 1, 8);
+    const rk_grid g = rk_plan(batch, d, 1, 8);
     B2_LAUNCH(gdcn_fwd_kernel<1>, g.grid, g.threads, 0, (cudaStream_t) stream, P, b, x0, xi, batch, d, g.tx_n,
               out, out_aux, aux_dtype, ld_aux);
   }
@@ -238,15 +154,15 @@ extern "C" B2_API int b2_gdcn_bwd(const float* P, const float* b, const float* x
                                   void* stream) {
   B2_REQUIRE(P && b && x0 && g && dP && gx0 && db, "NULL pointer");
   if (int rc = gd_check(batch, d)) return rc;
-  if (int rc = gd_check_aux(dp_aux, aux_dtype, ld_aux, 2 * d)) return rc;
+  if (int rc = rk_check_aux(dp_aux, aux_dtype, ld_aux, 2 * d)) return rc;
   if (batch == 0) return B2_OK;
   const void* ptrs[] = {P, b, x0, g, dP, gx0, db};
-  if (gd_vec(d, ptrs, 7, dp_aux, aux_dtype, ld_aux)) {
-    const gd_grid p = gd_plan(batch, d, 4, 4);
+  if (rk_vec(d, ptrs, 7, dp_aux, aux_dtype, ld_aux)) {
+    const rk_grid p = rk_plan(batch, d, 4, 4);
     B2_LAUNCH(gdcn_bwd_kernel<4>, p.grid, p.threads, 0, (cudaStream_t) stream, P, b, x0, g, batch, d, p.tx_n, dP,
               dp_aux, aux_dtype, ld_aux, gx0, db);
   } else {
-    const gd_grid p = gd_plan(batch, d, 1, 4);
+    const rk_grid p = rk_plan(batch, d, 1, 4);
     B2_LAUNCH(gdcn_bwd_kernel<1>, p.grid, p.threads, 0, (cudaStream_t) stream, P, b, x0, g, batch, d, p.tx_n, dP,
               dp_aux, aux_dtype, ld_aux, gx0, db);
   }

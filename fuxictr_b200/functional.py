@@ -1191,6 +1191,146 @@ def gated_cross_layer(x0, xi, w, wg, b):
     return _GatedCrossLayer.apply(x0, xi, w, wg, b)
 
 
+class _FsGate(torch.autograd.Function):
+    """FinalMLP's gating products f_s = e * (2 g_s), s = 1, 2 (FinalMLP.py, FeatureSelection.forward) in one launch
+    (include/fuxictr_b200.h "FinalMLP"), which also writes f1's and f2's auxiliary operands for the towers' first
+    GEMMs.  A gate of one row (1, d) is broadcast over the batch; its gradient is the column sum over the batch, so
+    the gate MLP behind it runs its forward and backward on that one row.  Backward: one launch for de, dg1, dg2."""
+
+    @staticmethod
+    def forward(ctx, e, g1, g2):
+        e, g1, g2 = _f32c(e), _f32c(g1), _f32c(g2)
+        B, d = e.shape
+        f1, f2 = torch.empty_like(e), torch.empty_like(e)
+        a1, a2 = empty_aux(B, d, e.device), empty_aux(B, d, e.device)
+        rows = (int(g1.shape[0] != 1), int(g2.shape[0] != 1))
+        if B:                   # an empty batch has no rows to gate (and NULL data pointers)
+            _lib.call("b2_fs_gate_fwd", _ptr(e), _ptr(g1), _ptr(g2), *rows, B, d, _ptr(f1), _ptr(f2), _ptr(a1),
+                      _ptr(a2), *_aux_args(a1)[1:], _stream())
+        for f, a in ((f1, a1), (f2, a2)):
+            if a is not None:           # the tower's first layer (make_aux) finds it
+                f._b2_aux = (_MATMUL["mode"], a, f._version)
+        ctx.save_for_backward(e, g1, g2)
+        ctx.rows = rows
+        return f1, f2
+
+    @staticmethod
+    def backward(ctx, df1, df2):
+        e, g1, g2 = ctx.saved_tensors
+        df1, df2 = _f32c(df1), _f32c(df2)
+        B, d = e.shape
+        de = torch.empty_like(e)
+        dg1 = torch.empty_like(g1) if ctx.rows[0] else torch.zeros_like(g1)
+        dg2 = torch.empty_like(g2) if ctx.rows[1] else torch.zeros_like(g2)
+        if B:
+            _lib.call("b2_fs_gate_bwd", _ptr(e), _ptr(g1), _ptr(g2), *ctx.rows, _ptr(df1), _ptr(df2), B, d, _ptr(de),
+                      _ptr(dg1), _ptr(dg2), _stream())
+        return de, dg1, dg2
+
+
+def fs_gate(flat_emb, g1, g2):
+    """(flat_emb * (2 g1), flat_emb * (2 g2)): flat_emb (B, d); each gate (B, d), or (1, d) for every row."""
+    _require_cuda(flat_emb, g1, g2)
+    if flat_emb.dim() != 2:
+        raise ValueError("fs_gate: flat_emb%s must be (B, d)" % (tuple(flat_emb.shape),))
+    B, d = flat_emb.shape
+    for g in (g1, g2):
+        if g.dim() != 2 or g.shape[1] != d or g.shape[0] not in (1, B):
+            raise ValueError("fs_gate: a gate%s must be (1, %d) or (%d, %d)" % (tuple(g.shape), d, B, d))
+    return _FsGate.apply(flat_emb, g1, g2)
+
+
+class _InteractionAggregation(torch.autograd.Function):
+    """FinalMLP's InteractionAggregation at output_dim 1 (FinalMLP.py), out = w_x(x) + w_y(y) + sum_h x_h^T W_h y_h,
+    as one GEMM between two row kernels (include/fuxictr_b200.h "FinalMLP"): W_aug = [block diagonal of the W_h^T;
+    w_x; 0] and bias_aug = [w_y, 0] (b2_agg_pack), Q = x W_aug^T + bias_aug, out = y.Q[:, :dy] + Q[:, dy] + b_x + b_y
+    (b2_agg_fwd).  Backward: dy, ys = [g y | g | 0] and the w_y, b_x, b_y gradients (b2_agg_bwd), dx = ys W_aug
+    (one dgrad, which includes g w_x), dW_aug = ys^T x (one wgrad) and one b2_agg_unpack into the w_xy, w_x
+    gradients.  W_aug changes every step, so its auxiliary operand is made here by make_aux and handed to gemm_ex as
+    it is (None where the precision has none), never looked up in weight_aux's per-weight cache."""
+
+    @staticmethod
+    def forward(ctx, x, y, wx, bx, wy, by, wxy, heads):
+        ctx.params = (wx, bx, wy, by, wxy)         # their gradients may live in an arena
+        x, y = _f32c(x), _f32c(y)
+        wx, bx, wy, by, wxy = _f32c(wx), _f32c(bx), _f32c(wy), _f32c(by), _f32c(wxy)
+        B, dx = x.shape
+        dy = y.shape[1]
+        n = (dy + 4) // 4 * 4                      # B2_AGG_COLS
+        dev = x.device
+        W = torch.empty((n, dx), dtype=torch.float32, device=dev)
+        bias = torch.empty((n,), dtype=torch.float32, device=dev)
+        _lib.call("b2_agg_pack", _ptr(wxy), _ptr(wx), _ptr(wy), dx, dy, heads, _ptr(W), _ptr(bias), _stream())
+        tc = _tc_layer_ok(W) and x.data_ptr() % 16 == 0 and B > 0
+        x_aux = make_aux(x) if tc else None
+        w_aux = make_aux(W) if tc else None
+        Q = torch.empty((B, n), dtype=torch.float32, device=dev)
+        out = torch.empty((B, 1), dtype=torch.float32, device=dev)
+        if B:                   # an empty batch: nothing to multiply (and NULL data pointers)
+            if tc:
+                gemm_ex(x, W, Q, a_small=x_aux, b_small=w_aux, bias=bias)
+            else:
+                gemm_f32(x, W, Q, b_t=True, bias=bias)
+            _lib.call("b2_agg_fwd", _ptr(Q), _ptr(y), _ptr(bx), _ptr(by), B, dy, _ptr(out), _stream())
+        ctx.save_for_backward(x, y, Q, W)
+        ctx.tc, ctx.aux, ctx.heads = tc, (x_aux, w_aux), heads
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, y, Q, W = ctx.saved_tensors
+        g = _f32c(g)
+        x_aux, w_aux = ctx.aux
+        tc = ctx.tc
+        B, dx = x.shape
+        dy = y.shape[1]
+        dev = x.device
+        wx, bx, wy, by, wxy = ctx.params
+        need = ctx.needs_input_grad
+        gy = torch.empty_like(y)
+        ys = torch.empty((B, W.shape[0]), dtype=torch.float32, device=dev)
+        ys_aux = empty_aux(B, W.shape[0], dev) if tc else None
+        gwy = _grad_buffer(wy, zero=True) if need[4] else torch.zeros_like(wy)
+        gbx = _grad_buffer(bx, zero=True) if need[3] else torch.zeros_like(bx)
+        gby = _grad_buffer(by, zero=True) if need[5] else torch.zeros_like(by)
+        gx = torch.empty_like(x)
+        if B:
+            _lib.call("b2_agg_bwd", _ptr(Q), _ptr(y), _ptr(g), B, dy, _ptr(gy), _ptr(ys), *_aux_args(ys_aux),
+                      _ptr(gwy), _ptr(gbx), _ptr(gby), _stream())
+            if tc:                                                                       # dx = ys W_aug
+                gemm_ex(ys, W, gx, b_mn=True, a_small=ys_aux, b_small=w_aux)
+            else:
+                gemm_f32(ys, W, gx)
+        gwx = gwxy = None
+        if need[2] or need[6]:
+            dW = torch.empty_like(W) if B else torch.zeros_like(W)
+            if B:
+                _linear_wgrad(tc, ys, ys_aux, x, x_aux, dW)                              # dW_aug = ys^T x
+            gwx = _grad_buffer(wx, zero=False) if need[2] else torch.empty_like(wx)
+            gwxy = _grad_buffer(wxy, zero=False) if need[6] else torch.empty_like(wxy)
+            _lib.call("b2_agg_unpack", _ptr(dW), dx, dy, ctx.heads, _ptr(gwxy), _ptr(gwx), _stream())
+        return (gx, gy, gwx if need[2] else None, gbx if need[3] else None, gwy if need[4] else None,
+                gby if need[5] else None, gwxy if need[6] else None, None)
+
+
+def interaction_aggregation(x, y, w_x, b_x, w_y, b_y, w_xy, num_heads):
+    """InteractionAggregation.forward at output_dim 1, (B, 1): x (B, dx), y (B, dy); w_x (1, dx), b_x (1,), w_y (1, dy),
+    b_y (1,) the w_x / w_y Linears' parameters; w_xy (num_heads * (dx / num_heads) * (dy / num_heads), 1)."""
+    _require_cuda(x, y, w_x, b_x, w_y, b_y, w_xy)
+    if x.dim() != 2 or y.dim() != 2 or x.shape[0] != y.shape[0]:
+        raise ValueError("interaction_aggregation: x%s and y%s must be (B, dx) and (B, dy)"
+                         % (tuple(x.shape), tuple(y.shape)))
+    dx, dy = x.shape[1], y.shape[1]
+    if num_heads < 1 or dx % num_heads or dy % num_heads:
+        raise ValueError("interaction_aggregation: num_heads %d must divide dx %d and dy %d" % (num_heads, dx, dy))
+    if w_x.numel() != dx or w_y.numel() != dy or b_x.numel() != 1 or b_y.numel() != 1 \
+            or w_xy.numel() != dx * dy // num_heads:
+        raise ValueError("interaction_aggregation: shapes w_x%s b_x%s w_y%s b_y%s w_xy%s do not match dx %d, dy %d"
+                         % (tuple(w_x.shape), tuple(b_x.shape), tuple(w_y.shape), tuple(b_y.shape),
+                            tuple(w_xy.shape), dx, dy))
+    return _InteractionAggregation.apply(x, y, w_x, b_x, w_y, b_y, w_xy, num_heads)
+
+
 # --------------------------------------------------------------------------------------
 # MultiHeadTargetAttention
 # --------------------------------------------------------------------------------------

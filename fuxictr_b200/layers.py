@@ -19,6 +19,7 @@ Reference files (relative to the reference root):
   ScaledDotProductAttention                fuxictr/pytorch/layers/attentions/dot_product_attention.py:24-58
   Dice                                     fuxictr/pytorch/layers/activations.py:24-51
   MLP_Block                                fuxictr/pytorch/layers/blocks/mlp_block.py:24-96
+  FeatureSelection / InteractionAggregation model_zoo/FinalMLP/src/FinalMLP.py
 """
 import sys
 from collections import OrderedDict
@@ -545,6 +546,71 @@ class GateCorssLayer(nn.Module):
         for i in range(self.cn_layers):
             x = F2.gated_cross_layer(x0, x, self.w[i].weight, self.wg[i].weight, self.b[i])
         return x
+
+
+class FeatureSelection(nn.Module):
+    """FinalMLP's feature selection (model_zoo/FinalMLP/src/FinalMLP.py, FeatureSelection): per stream s, a gate MLP
+    ending in a sigmoid gives g_s and the stream's input is flat_emb * (2 g_s).  A stream without context features
+    feeds its gate the learned row fs<s>_ctx_bias; the reference repeats that row over the batch, here the gate MLP
+    runs once on the one row and the gating kernel broadcasts it (functional._FsGate).  Children and initial draws in
+    the reference's order."""
+
+    def __init__(self, feature_map, feature_dim, embedding_dim, fs_hidden_units=[], fs1_context=[], fs2_context=[]):
+        super(FeatureSelection, self).__init__()
+        self.fs1_context = fs1_context
+        if len(fs1_context) == 0:
+            self.fs1_ctx_bias = nn.Parameter(torch.zeros(1, embedding_dim))
+        else:
+            self.fs1_ctx_emb = FeatureEmbedding(feature_map, embedding_dim, required_feature_columns=fs1_context)
+        self.fs2_context = fs2_context
+        if len(fs2_context) == 0:
+            self.fs2_ctx_bias = nn.Parameter(torch.zeros(1, embedding_dim))
+        else:
+            self.fs2_ctx_emb = FeatureEmbedding(feature_map, embedding_dim, required_feature_columns=fs2_context)
+        self.fs1_gate = MLP_Block(input_dim=embedding_dim * max(1, len(fs1_context)), output_dim=feature_dim,
+                                  hidden_units=fs_hidden_units, hidden_activations="ReLU", output_activation="Sigmoid",
+                                  batch_norm=False)
+        self.fs2_gate = MLP_Block(input_dim=embedding_dim * max(1, len(fs2_context)), output_dim=feature_dim,
+                                  hidden_units=fs_hidden_units, hidden_activations="ReLU", output_activation="Sigmoid",
+                                  batch_norm=False)
+
+    def forward(self, X, flat_emb):
+        if len(self.fs1_context) == 0:
+            g1 = self.fs1_gate(self.fs1_ctx_bias)
+        else:
+            g1 = self.fs1_gate(self.fs1_ctx_emb(X, flatten_emb=True))
+        if len(self.fs2_context) == 0:
+            g2 = self.fs2_gate(self.fs2_ctx_bias)
+        else:
+            g2 = self.fs2_gate(self.fs2_ctx_emb(X, flatten_emb=True))
+        return F2.fs_gate(flat_emb, g1, g2)
+
+
+class InteractionAggregation(nn.Module):
+    """FinalMLP's fusion of its two towers (model_zoo/FinalMLP/src/FinalMLP.py, InteractionAggregation):
+    w_x(x) + w_y(y) + the multi-head bilinear sum_h x_h^T W_h y_h, one autograd node (functional.
+    _InteractionAggregation).  `w_xy` gets its xavier draw here, as in the reference; a model's reset_parameters
+    re-draws only the two Linears.  FinalMLP builds it with output_dim 1 only, the one width implemented."""
+
+    def __init__(self, x_dim, y_dim, output_dim=1, num_heads=1):
+        super(InteractionAggregation, self).__init__()
+        assert x_dim % num_heads == 0 and y_dim % num_heads == 0, \
+            "Input dim must be divisible by num_heads!"
+        if output_dim != 1:
+            raise NotImplementedError("InteractionAggregation is implemented for output_dim 1 (FinalMLP's), got %r"
+                                      % (output_dim,))
+        self.num_heads = num_heads
+        self.output_dim = output_dim
+        self.head_x_dim = x_dim // num_heads
+        self.head_y_dim = y_dim // num_heads
+        self.w_x = nn.Linear(x_dim, output_dim)
+        self.w_y = nn.Linear(y_dim, output_dim)
+        self.w_xy = nn.Parameter(torch.Tensor(num_heads * self.head_x_dim * self.head_y_dim, output_dim))
+        nn.init.xavier_normal_(self.w_xy)
+
+    def forward(self, x, y):
+        return F2.interaction_aggregation(x, y, self.w_x.weight, self.w_x.bias, self.w_y.weight, self.w_y.bias,
+                                          self.w_xy, self.num_heads)
 
 
 # --------------------------------------------------------------------------------------

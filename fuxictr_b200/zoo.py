@@ -13,6 +13,8 @@ same RNG consumption) and nothing else.
   DIN      model_zoo/DIN/src/DIN.py:50-149
   xDeepFM  model_zoo/xDeepFM/src/xDeepFM.py:41-97
   GDCN, GDCNP  model_zoo/GDCN/src/GDCN.py
+  FinalMLP     model_zoo/FinalMLP/src/FinalMLP.py
+  DualMLP      model_zoo/FinalMLP/src/DualMLP.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -22,8 +24,8 @@ import torch
 from torch import nn
 
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
-                     CrossNetV2, GateCorssLayer, InnerProductInteraction, DIN_Attention, Dice,
-                     CompressedInteractionNet, LogisticRegression, not_in_whitelist)
+                     CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
+                     DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
 
@@ -171,14 +173,15 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP) may be sharded: any other forward would keep reading the
-        1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP) may be sharded: any other forward
+        would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
         from . import sharded as SH
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
-                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN and GDCNP" % type(self).__name__)
+                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP and "
+                                      "DualMLP" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -559,6 +562,91 @@ class GDCNP(RankModel):
 
     def forward(self, inputs):
         return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class FinalMLP(RankModel):
+    """model_zoo/FinalMLP/src/FinalMLP.py, FinalMLP: two MLP towers over the flattened embedding, each fed through its
+    feature-selection gate (use_fs), fused into the logit by the multi-head bilinear InteractionAggregation.  A gate
+    without context features runs its MLP on one row (layers.FeatureSelection).  Unknown keyword arguments are
+    accepted and ignored, as the reference's **kwargs are."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="FinalMLP", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 mlp1_hidden_units=[64, 64, 64], mlp1_hidden_activations="ReLU", mlp1_dropout=0, mlp1_batch_norm=False,
+                 mlp2_hidden_units=[64, 64, 64], mlp2_hidden_activations="ReLU", mlp2_dropout=0, mlp2_batch_norm=False,
+                 use_fs=True, fs_hidden_units=[64], fs1_context=[], fs2_context=[], num_heads=1,
+                 embedding_regularizer=None, net_regularizer=None, **kwargs):
+        if not mlp1_hidden_units or not mlp2_hidden_units:
+            # the reference fails here too (an IndexError on mlp*_hidden_units[-1]): the fusion needs both towers
+            raise ValueError("FinalMLP needs non-empty mlp1_hidden_units and mlp2_hidden_units (the towers the "
+                             "fusion module combines)")
+        super(FinalMLP, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                       embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                       **kwargs)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        feature_dim = embedding_dim * feature_map.num_fields
+        self.mlp1 = MLP_Block(input_dim=feature_dim, output_dim=None, hidden_units=mlp1_hidden_units,
+                              hidden_activations=mlp1_hidden_activations, output_activation=None,
+                              dropout_rates=mlp1_dropout, batch_norm=mlp1_batch_norm)
+        self.mlp2 = MLP_Block(input_dim=feature_dim, output_dim=None, hidden_units=mlp2_hidden_units,
+                              hidden_activations=mlp2_hidden_activations, output_activation=None,
+                              dropout_rates=mlp2_dropout, batch_norm=mlp2_batch_norm)
+        self.use_fs = use_fs
+        if self.use_fs:
+            self.fs_module = FeatureSelection(feature_map, feature_dim, embedding_dim, fs_hidden_units, fs1_context,
+                                              fs2_context)
+        self.fusion_module = InteractionAggregation(mlp1_hidden_units[-1], mlp2_hidden_units[-1], output_dim=1,
+                                                    num_heads=num_heads)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=True):
+        """RankModel.enable_sharding for a FinalMLP whose gates have no context features: context features are
+        looked up in tables of their own, which the row-sharded front does not carry."""
+        if self.use_fs and (self.fs_module.fs1_context or self.fs_module.fs2_context):
+            raise NotImplementedError("FinalMLP with fs1_context / fs2_context cannot be row-sharded: the gates' "
+                                      "context tables are not part of the sharded front")
+        return super(FinalMLP, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype,
+                                                     want_fm=want_fm)
+
+    def forward_logits(self, inputs):
+        flat_emb = self._flat_embedding(inputs)
+        if self.use_fs:
+            feat1, feat2 = self.fs_module(self.get_inputs(inputs), flat_emb)
+        else:
+            feat1, feat2 = flat_emb, flat_emb
+        return (self.fusion_module(self.mlp1(feat1), self.mlp2(feat2)),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class DualMLP(RankModel):
+    """model_zoo/FinalMLP/src/DualMLP.py, DualMLP: two MLP towers over the flattened embedding, each ending in a
+    logit, summed.  Unknown keyword arguments are accepted and ignored, as the reference's **kwargs are."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="DualMLP", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 mlp1_hidden_units=[64, 64, 64], mlp1_hidden_activations="ReLU", mlp1_dropout=0, mlp1_batch_norm=False,
+                 mlp2_hidden_units=[64, 64, 64], mlp2_hidden_activations="ReLU", mlp2_dropout=0, mlp2_batch_norm=False,
+                 embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(DualMLP, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                      embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                      **kwargs)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.mlp1 = MLP_Block(input_dim=embedding_dim * feature_map.num_fields, output_dim=1,
+                              hidden_units=mlp1_hidden_units, hidden_activations=mlp1_hidden_activations,
+                              output_activation=None, dropout_rates=mlp1_dropout, batch_norm=mlp1_batch_norm)
+        self.mlp2 = MLP_Block(input_dim=embedding_dim * feature_map.num_fields, output_dim=1,
+                              hidden_units=mlp2_hidden_units, hidden_activations=mlp2_hidden_activations,
+                              output_activation=None, dropout_rates=mlp2_dropout, batch_norm=mlp2_batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def forward_logits(self, inputs):
+        flat_emb = self._flat_embedding(inputs)
+        return (self.mlp1(flat_emb), self.mlp2(flat_emb))
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(sum(self.forward_logits(inputs)))}
 
 
 class DLRM(RankModel):

@@ -438,6 +438,52 @@ B2_API int b2_gdcn_bwd(const float* P, const float* b, const float* x0, const fl
 B2_API int b2_gdcn_unpack(const float* dWp, int d, float* gW, float* gWg, void* stream);
 
 /*
+ * FinalMLP (model_zoo/FinalMLP/src/FinalMLP.py): FeatureSelection's gating products and InteractionAggregation at
+ * output_dim 1.  All row-major fp32.
+ *
+ * Gate: e (B, d) is the flattened embedding; g1, g2 the two gate MLPs' sigmoid outputs, each one broadcast row (1, d)
+ * (per_row 0: the gate has no context features) or one row per sample (B, d) (per_row 1).
+ * b2_fs_gate_fwd: f1, f2 (B, d) "=" e * (2 g1), e * (2 g2) (2 g first, then the product, as the reference rounds);
+ *   f1_aux, f2_aux (both or neither, row pitch ld_aux) receive their GEMM operand copies for the towers' first
+ *   layers: the bf16 rounding (aux_dtype B2_BF16) or the 3xTF32 small part (B2_F32).
+ * b2_fs_gate_bwd: de (B, d) "=" df1 (2 g1) + df2 (2 g2); dg_s = 2 (df_s e): (B, d) "=" for a per-row gate, or for a
+ *   broadcast gate its column sum (d) "+=" (caller zeroes): a per-CTA sum, then one float atomic per column and CTA.
+ *
+ * Aggregation: x (B, dx), y (B, dy) the towers' outputs, H heads of widths hx = dx / H, hy = dy / H, and
+ *   out_b = w_x.x_b + b_x + w_y.y_b + b_y + sum_h x_{b,h}^T W_h y_{b,h},  W_h[i, j] = w_xy[(h hx + i) hy + j]
+ * with w_x (dx), w_y (dy), b_x, b_y (1) and w_xy (H hx hy) the reference's w_x, w_y and w_xy.  With
+ * n_aug = B2_AGG_COLS(dy), the smallest multiple of 4 above dy:
+ *   W_aug (n_aug, dx) K-major: row h hy + j holds W_h[:, j] in columns h hx .. h hx + hx - 1 and zeros elsewhere,
+ *     row dy is w_x, rows dy + 1 .. are zero; bias_aug (n_aug) = [w_y, 0 ...]
+ *   Q (B, n_aug) = x W_aug^T + bias_aug (the caller's GEMM): Q[:, :dy] = T + w_y with T_b = [x_{b,h}^T W_h]_h,
+ *     Q[:, dy] = x w_x
+ *   ys (B, n_aug) = [g y | g | 0] for the output gradient g (B): dx = ys W_aug, dW_aug = ys^T x (the caller's GEMMs)
+ * Range: dx, dy >= 1, H divides both, batch * n_aug < 2^31; dy % 4 == 0 with 16-byte aligned rows takes a float4
+ * path, anything else a scalar one.  Outside the range, or given a NULL pointer, every entry point returns
+ * B2_E_INVALID.
+ * b2_agg_pack:   W_aug, bias_aug "=" from w_xy, w_x, w_y; one launch.
+ * b2_agg_fwd:    out (B) "=" sum_{j < dy} y_j Q_j + Q_dy + b_x + b_y; one warp per row.
+ * b2_agg_bwd:    gy (B, dy) "=" g Q[:, :dy]; ys "=" (+ ys_aux as the gate's f1_aux, row width n_aug); gw_y (dy) "+="
+ *   the column sums of g y, gb_x and gb_y (1) each "+=" the sum of g (caller zeroes all three).
+ * b2_agg_unpack: gw_xy (H hx hy) "=" the diagonal blocks of dW_aug, gw_x (dx) "=" its row dy.
+ */
+#define B2_AGG_COLS(dy) (((dy) + 4) / 4 * 4)
+B2_API int b2_fs_gate_fwd(const float* e, const float* g1, const float* g2, int per_row1, int per_row2, int64_t batch,
+                          int d, float* f1, float* f2, void* f1_aux, void* f2_aux, int aux_dtype, int64_t ld_aux,
+                          void* stream);
+B2_API int b2_fs_gate_bwd(const float* e, const float* g1, const float* g2, int per_row1, int per_row2,
+                          const float* df1, const float* df2, int64_t batch, int d, float* de, float* dg1, float* dg2,
+                          void* stream);
+B2_API int b2_agg_pack(const float* w_xy, const float* w_x, const float* w_y, int dx, int dy, int heads, float* W_aug,
+                       float* bias_aug, void* stream);
+B2_API int b2_agg_fwd(const float* Q, const float* y, const float* b_x, const float* b_y, int64_t batch, int dy,
+                      float* out, void* stream);
+B2_API int b2_agg_bwd(const float* Q, const float* y, const float* g, int64_t batch, int dy, float* gy, float* ys,
+                      void* ys_aux, int aux_dtype, int64_t ld_aux, float* gw_y, float* gb_x, float* gb_y,
+                      void* stream);
+B2_API int b2_agg_unpack(const float* dW_aug, int dx, int dy, int heads, float* gw_xy, float* gw_x, void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
