@@ -20,6 +20,7 @@ B2_GEMM_C_IS_ZERO, B2_GEMM_COLSUM_IS_ZERO, B2_GEMM_X3_INLINE, B2_GEMM_BACKFILL =
 B2_MAX_FIELDS = 128
 B2_CROSSMIX_MAX_RANK, B2_CROSSMIX_MAX_COLS = 64, 256
 B2_MHTA_MAX_WIDTH, B2_MHTA_MAX_HEADS = 1024, 32
+B2_HEAD_MAX_K = 28672
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
 c_void_p, c_int, c_int32, c_int64, c_float, c_double = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,

@@ -698,7 +698,7 @@ split_tf32_kernel(const float* __restrict__ x, float* __restrict__ small, int64_
 //   out    = v            (R, C)            out_small  = tf32_small(v)
 //   outT   = v^T          (C, R)            outT_small = tf32_small(v^T)
 //   colsum[c] += sum_r v[r, c]              (bias gradient)
-// Any output pointer may be NULL.  32 x 32 tiles through padded shared memory.
+// Any output pointer may be NULL, but outT_small comes with outT.  32 x 32 tiles through padded shared memory.
 // DROP: x is the gradient of a dropout layer's output, y that dropped output: v = act'(y) * keep * scale * x
 // (the mask first; sigmoid's s = y / scale on kept elements).
 // ---------------------------------------------------------------------------------
@@ -1178,6 +1178,7 @@ extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, i
   B2_REQUIRE(R >= 0 && C >= 0, "bad shape");
   B2_REQUIRE((act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID) || act == B2_PREP_MUL, "bad activation code %d", act);
   B2_REQUIRE(drop_rng == nullptr || act != B2_PREP_MUL, "B2_PREP_MUL takes no dropout mask");
+  B2_REQUIRE(outT_small == nullptr || outT != nullptr, "outT_small needs outT");
   const int rc = check_drop(drop_rng, drop_layer, drop_scale);
   if (rc != B2_OK) return rc;
   cudaStream_t st = (cudaStream_t) stream;
@@ -1216,13 +1217,27 @@ extern "C" B2_API int b2_head_bwd(const float* x, const float* w, const float* y
                         stream);
 }
 
+// head_bwd_kernel stages 2 * K floats (the partial sums of gw and gb_prev) in dynamic shared memory.  A launch whose
+// dynamic and static shared memory together pass the default 48 KB per block needs the instantiation's opt-in first.
+template <bool DROP>
+static int head_bwd_smem_optin(size_t dyn) {
+  const void* kern = (const void*) tc::head_bwd_kernel<DROP>;
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaFuncGetAttributes(&fa, kern);
+  if (e == cudaSuccess && fa.sharedSizeBytes + dyn > 48 * 1024)
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) dyn);
+  if (e != cudaSuccess) return b2_fail(B2_E_CUDA, "b2_head_bwd: smem attribute: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
 extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float* y, const float* gy, int64_t M,
                                      int K, int act, float* gx, float* gw, float* gb, int prev_act,
                                      float* gx_small, float* gb_prev, int grads_zeroed, const int64_t* prev_drop_rng,
                                      int64_t prev_drop_layer, uint32_t prev_drop_thresh, float prev_drop_scale,
                                      void* stream) {
   B2_REQUIRE(x && w && gy && gw, "NULL pointer");
-  B2_REQUIRE(K >= 1 && K <= 6144 && act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad K/act");
+  B2_REQUIRE(K >= 1 && K <= B2_HEAD_MAX_K, "K=%d outside [1, B2_HEAD_MAX_K=%d]", K, B2_HEAD_MAX_K);
+  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad activation code %d", act);
   B2_REQUIRE(prev_act >= B2_ACT_NONE && prev_act <= B2_ACT_SIGMOID, "bad prev_act");
   B2_REQUIRE(act == B2_ACT_NONE || y != nullptr, "activation backward needs y");
   B2_REQUIRE(gx != nullptr || (gx_small == nullptr && gb_prev == nullptr && prev_act == B2_ACT_NONE &&
@@ -1244,12 +1259,15 @@ extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float
   const int64_t rows_per_cta = b2_ceil_div(M, ctas);
   ctas = b2_ceil_div(M, rows_per_cta);
   const float* y_arg = (act == B2_ACT_NONE) ? nullptr : y;
+  const size_t smem = 2 * sizeof(float) * (size_t) K;
+  const int smem_rc = prev_drop_rng != nullptr ? head_bwd_smem_optin<true>(smem) : head_bwd_smem_optin<false>(smem);
+  if (smem_rc != B2_OK) return smem_rc;
   if (prev_drop_rng != nullptr)
-    B2_LAUNCH(tc::head_bwd_kernel<true>, (int) ctas, 256, 2 * sizeof(float) * (size_t) K, st,
+    B2_LAUNCH(tc::head_bwd_kernel<true>, (int) ctas, 256, smem, st,
               x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
               prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
   else
-    B2_LAUNCH(tc::head_bwd_kernel<false>, (int) ctas, 256, 2 * sizeof(float) * (size_t) K, st,
+    B2_LAUNCH(tc::head_bwd_kernel<false>, (int) ctas, 256, smem, st,
               x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
               prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
   B2_CUDA_LAUNCH_CHECK("b2_head_bwd");

@@ -383,6 +383,9 @@ def gemm_f32(a, b, out, a_t=False, b_t=False, bias=None, act=B2_ACT_NONE, mul=No
         b_rs, b_cs = b.stride(0), b.stride(1)
     if K != K2 or tuple(out.shape) != (M, N) or out.stride(1) != 1:
         raise ValueError("gemm shape mismatch: a%s b%s out%s" % (tuple(a.shape), tuple(b.shape), tuple(out.shape)))
+    for t in (mul, add):        # the kernel reads them at out's element offsets
+        if t is not None and (tuple(t.shape) != (M, N) or t.stride() != out.stride()):
+            raise ValueError("gemm_f32: mul and add must share out's shape and leading dimension")
     _lib.call("b2_gemm_f32", _ptr(a), a_rs, a_cs, _ptr(b), b_rs, b_cs, _ptr(out), out.stride(0), M, N, K,
               _ptr(bias), act, _ptr(mul), _ptr(add), 1 if accumulate else 0, _stream())
     return out
@@ -678,6 +681,12 @@ def _tc_layer_ok(weight):
             and weight.is_contiguous() and weight.data_ptr() % 16 == 0)
 
 
+def _head_ok(weight):
+    """nn.Linear weight (1, K) that the N = 1 head kernels take: contiguous, K within the backward's
+    shared-memory staging (B2_HEAD_MAX_K).  A wider one runs as a general GEMM."""
+    return weight.shape[0] == 1 and weight.shape[1] <= _lib.B2_HEAD_MAX_K and weight.is_contiguous()
+
+
 def _linear_fwd(tc, a, a_aux, W, out, w_aux=None, **epilogue):
     """out = epi(a W^T), W (N, K) as nn.Linear keeps it: on the tensor cores (a_aux, w_aux: the operands' auxiliary
     ones; w_aux None: weight_aux(W), a parameter's cached one, itself None in a precision that has none) or,
@@ -721,7 +730,7 @@ class _LinearAct(torch.autograd.Function):
         N = weight.shape[0]
         y = torch.empty((M, N), dtype=torch.float32, device=x.device)
         ctx.act, ctx.bias, ctx.has_bias = act, bias, bias is not None
-        if N == 1 and weight.is_contiguous():
+        if _head_ok(weight):
             ctx.kind = "head"
             _lib.call("b2_head_fwd", _ptr(x), _ptr(weight), _ptr(bias), M, K, act, _ptr(y), _stream())
         else:
@@ -846,7 +855,7 @@ class _MLPChain(torch.autograd.Function):
                 dl[i] = (snap, sum(1 for q in drops[:i] if q > 0)) + dropout_consts(p)
         kinds = []
         for W in Ws:
-            if W.shape[0] == 1 and W.is_contiguous():
+            if _head_ok(W):
                 kinds.append("head")
             elif _tc_layer_ok(W):
                 kinds.append("tc")

@@ -690,8 +690,8 @@ B2_API int b2_split_tf32(const float* x, float* small, int64_t n, void* stream);
  *   v = act'(y) * x when y != NULL (y = activation OUTPUT; fuses the activation backward);
  *   act == B2_PREP_MUL: v = x * y
  *   out (R,C) = v, out_small = 3xTF32 small part, outT (C,R) = v^T, outT_small, colsum[c] = sum_r v[r,c]
- * Every output may be NULL.  One pass where an activation backward, a transpose, a 3xTF32 split and a
- * column sum would each read x again.
+ * Every output may be NULL, but outT_small needs outT.  One pass where an activation backward, a transpose,
+ * a 3xTF32 split and a column sum would each read x again.
  * drop_rng != NULL: x is the gradient of a dropout layer's output and y (if any) that DROPPED output:
  *   v = act'(y) * keep * drop_scale * x  with the mask of (R, C) at counter offset snapshot offset + drop_layer
  *   (not with B2_PREP_MUL).  drop_rng == NULL: no mask, the other drop arguments are ignored.
@@ -704,7 +704,11 @@ B2_API int b2_prep_operand(const float* x, const float* y, int act, int64_t R, i
  * The N = 1 output head of MLP_Block (Linear(K, 1), mlp_block.py:82): warp-per-row GEMV forward,
  * y[m] = act(<x[m,:], w> + b); and one fused backward: gz = act'(y)*gy, gx[m,:] = gz[m]*w (gx may
  * be NULL), gw (K) = sum_m gz[m]*x[m,:], gb (1) = sum_m gz[m]  ("=" semantics).
+ * The backward takes K <= B2_HEAD_MAX_K: it stages 2 * K floats of partial sums in shared memory, and
+ * 2 * 28672 * 4 B = 224 KB, with the kernel's static part, stays within the 227 KB per block of sm_90.
+ * A wider Linear(K, 1) runs as a general GEMM.
  */
+#define B2_HEAD_MAX_K 28672
 B2_API int b2_head_fwd(const float* x, const float* w, const float* b, int64_t M, int K, int act, float* y,
                        void* stream);
 B2_API int b2_head_bwd(const float* x, const float* w, const float* y, const float* gy, int64_t M, int K,
