@@ -323,6 +323,10 @@ int check_front(const b2_field* emb, const b2_field* lr, int nfields, bool bwd) 
                (f.table == nullptr || ((uintptr_t) f.table % 16) == 0), "field %d: rows must be 16-byte aligned", i);
     if (lr != nullptr) {
       B2_REQUIRE(lr[i].idx == f.idx && lr[i].idx_stride == f.idx_stride, "field %d: LR and embedding must share indices", i);
+      // the kernels bound an LR row by the embedding's vocab and skip the embedding's padding row in both packs
+      B2_REQUIRE(lr[i].vocab == f.vocab && lr[i].padding_idx == f.padding_idx,
+                 "field %d: LR and embedding must share vocab and padding_idx (%lld/%d vs %lld/%d)", i,
+                 (long long) lr[i].vocab, lr[i].padding_idx, (long long) f.vocab, f.padding_idx);
       B2_REQUIRE(bwd || lr[i].table != nullptr, "field %d: NULL LR table", i);
     }
   }

@@ -252,13 +252,14 @@ class ShardedFront(object):
         g = group
         # ids_all[p] = batch matrix of rank p: every rank BROADCASTS its ids into slot `rank` of all
         # peers (one launch of P2P stores), so the push kernel walks local memory only.
-        # the slots hold int32 row numbers: the exchange narrows the collator's float64 on the fly
-        self.ids_all, self._ids_all_ptrs, self._ids_peer = g.alloc("ids_all", (g.world, batch_local, matrix_width),
-                                                                   torch.int32)
+        # the slots hold int32 row numbers: the exchange narrows the collator's float64 on the fly.  The exchange
+        # stores 16-byte vectors, so each slot starts 16-byte aligned: its pitch is rounded up to 4 ids.
+        slot_ids = -(-batch_local * matrix_width // 4) * 4
+        self.ids_all, self._ids_all_ptrs, self._ids_peer = g.alloc("ids_all", (g.world, slot_ids), torch.int32)
         esz = self.ids_all.element_size()
         self.src_code = self.idx_code          # dtype of the batch matrix handed to phase_ids
         self.idx_code = F2._IDX_CODE[torch.int32]
-        self._slot_bytes = batch_local * matrix_width * esz
+        self._slot_bytes = slot_ids * esz
         self.ids_ptrs = [self.ids_all.data_ptr() + p * self._slot_bytes for p in range(g.world)]
         self._ids_src = torch.empty((batch_local, matrix_width), dtype=idx_dtype, device="cuda")
         # rows this rank served in the forward (filled by the push, walked by the pull): int32[4] entries

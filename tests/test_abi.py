@@ -67,6 +67,39 @@ def test_entry_points_reject_bad_arguments_without_a_gpu(lib):
         lib.call("b2_split_tf32", null, null, 8, null)
 
 
+def test_front_rejects_lr_fields_that_disagree_with_the_embedding(lib):
+    """The front kernels bound an LR row by the embedding field's vocab and skip the embedding's padding row in both
+    tables, so b2_front_fwd / b2_front_bwd refuse LR fields whose vocab or padding_idx differ.  batch = 0, and the
+    pointers are aligned stand-ins that are never dereferenced: nothing reaches a device."""
+    L = lib.load()
+    null = ctypes.c_void_p(0)
+    p = ctypes.c_void_p(1 << 20)
+
+    def packs(lr_vocab, lr_pad):
+        emb, lr = (lib.b2_field * 2)(), (lib.b2_field * 2)()
+        for i in range(2):
+            emb[i].table, emb[i].idx, emb[i].out = p.value, p.value + 64 * i, p.value + 4096 + 64 * i
+            emb[i].vocab, emb[i].idx_stride, emb[i].out_stride = 50, 2, 32
+            emb[i].dim, emb[i].seq_len, emb[i].pool, emb[i].padding_idx = 16, 1, 0, 0
+            lr[i].table, lr[i].idx, lr[i].idx_stride = p.value + 8192, emb[i].idx, 2
+            lr[i].vocab, lr[i].dim, lr[i].seq_len, lr[i].padding_idx = 50, 1, 1, 0
+        lr[1].vocab, lr[1].padding_idx = lr_vocab, lr_pad
+        return emb, lr
+
+    def fwd(emb, lr):
+        return L.b2_front_fwd(emb, lr, 2, 0, lib.B2_I64, 1, null, p, p, null, None, null, null)
+
+    def bwd(emb, lr):
+        return L.b2_front_bwd(emb, lr, 2, 0, lib.B2_I64, 1, p, p, p, p, null, None, None, null)
+
+    assert fwd(*packs(50, 0)) == 0 and bwd(*packs(50, 0)) == 0          # agreeing packs pass the checks
+    for lr_vocab, lr_pad in ((49, 0), (51, 0), (50, -1), (50, 7)):
+        for call in (fwd, bwd):
+            assert call(*packs(lr_vocab, lr_pad)) == -1, (call.__name__, lr_vocab, lr_pad)
+            msg = L.b2_last_error()
+            assert b"field 1" in msg and b"vocab and padding_idx" in msg, msg
+
+
 def test_missing_library_is_a_hard_error(lib, monkeypatch):
     monkeypatch.setattr(lib, "_lib", None)
     monkeypatch.setattr(lib, "LIB_PATH", "/nonexistent/libfuxictr_b200.so")

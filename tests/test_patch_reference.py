@@ -35,11 +35,19 @@ def build_ref_deepfm(ref, g):
     return fm, model
 
 
+def calls_since(patch, before):
+    """The kernel-path calls of each patched forward since the snapshot `before` (patch.call_counts()): the counters
+    are process-wide, and GPU tests in the same process run the patched forwards on CUDA."""
+    now = patch.call_counts()
+    return {k: n - before.get(k, 0) for k, n in now.items() if n != before.get(k, 0)}
+
+
 def test_enable_keeps_identity_and_cpu_results(ref):
     from fuxictr_b200 import patch
     g = Golden("model_DeepFM")
     cls_before = ref.L.FeatureEmbeddingDict
     patch.enable()
+    before = patch.call_counts()
     try:
         assert ref.L.FeatureEmbeddingDict is cls_before                       # same class object
         fm, model = build_ref_deepfm(ref, g)
@@ -50,7 +58,7 @@ def test_enable_keeps_identity_and_cpu_results(ref):
         batch = {c: mat[:, fm.get_column_index(c)] for c in list(fm.features.keys()) + fm.labels}
         y = model.forward(batch)["y_pred"]                                    # CPU tensors -> original forwards
         assert rel_err(y, g["out"]["y_pred"]) <= 1e-6
-        assert patch.call_counts() == {}
+        assert calls_since(patch, before) == {}
     finally:
         patch.disable()
 
@@ -61,6 +69,7 @@ def test_cuda_tensors_are_routed_to_the_kernels(ref, monkeypatch):
     from fuxictr_b200 import patch
     g = Golden("model_DeepFM")
     patch.enable()
+    before = patch.call_counts()
     try:
         fm, model = build_ref_deepfm(ref, g)
         B = g.meta["batch"]
@@ -69,7 +78,7 @@ def test_cuda_tensors_are_routed_to_the_kernels(ref, monkeypatch):
         monkeypatch.setattr(patch, "_on_cuda", lambda a, k: True)
         with pytest.raises(RuntimeError, match="CUDA"):
             model.forward(batch)
-        assert patch.call_counts().get("FeatureEmbedding", 0) >= 1
+        assert calls_since(patch, before).get("FeatureEmbedding", 0) >= 1
     finally:
         patch.disable()
 
@@ -84,6 +93,7 @@ def test_evaluate_is_patched_but_cpu_models_use_the_reference_path(ref, monkeypa
     from oracle import fuxictr_oracle as O
     g = Golden("model_DeepFM")
     patch.enable()
+    before = patch.call_counts()
     try:
         fm, model = build_ref_deepfm(ref, g)
         model._verbose = 0
@@ -93,18 +103,19 @@ def test_evaluate_is_patched_but_cpu_models_use_the_reference_path(ref, monkeypa
         gen = [{c: m[:, fm.get_column_index(c)] for c in cols} for m in mats]
         logs = model.evaluate(gen, metrics=["logloss", "AUC"])
         preds = model.predict(gen)
-        assert patch.call_counts().get("evaluate", 0) == 0 and patch.call_counts().get("predict", 0) == 0
+        calls = calls_since(patch, before)
+        assert calls.get("evaluate", 0) == 0 and calls.get("predict", 0) == 0
         y = np.concatenate([m[:, -1].numpy() for m in mats])
         want = O.evaluate_metrics(y, preds, ["logloss", "AUC"])
         assert abs(logs["logloss"] - want["logloss"]) <= 1e-12 and abs(logs["AUC"] - want["AUC"]) <= 1e-12
         monkeypatch.setattr(model, "device", torch.device("cuda:0"))
         with pytest.raises((RuntimeError, AssertionError)):
             model.evaluate(gen, metrics=["logloss", "AUC"])
-        assert patch.call_counts().get("evaluate", 0) == 1
+        assert calls_since(patch, before).get("evaluate", 0) == 1
         # group metrics stay on the reference path even for a CUDA model
         fm.group_id = "C0"
         with pytest.raises(Exception):
             model.evaluate(gen, metrics=["gAUC"])
-        assert patch.call_counts().get("evaluate", 0) == 1
+        assert calls_since(patch, before).get("evaluate", 0) == 1
     finally:
         patch.disable()
