@@ -1200,6 +1200,370 @@ def gated_cross_layer(x0, xi, w, wg, b):
     return _GatedCrossLayer.apply(x0, xi, w, wg, b)
 
 
+# --------------------------------------------------------------------------------------
+# MaskNet (include/fuxictr_b200.h "MaskNet")
+# --------------------------------------------------------------------------------------
+def masknet_width_bound(n, what="width"):
+    """None when the MaskNet row kernels cover a row of n values, else the bound it breaks."""
+    if not 1 <= n <= _lib.B2_MASKNET_MAX_WIDTH:
+        return "%s must lie in [1, %d], got %d" % (what, _lib.B2_MASKNET_MAX_WIDTH, n)
+    return None
+
+
+class EmbeddingGrad(object):
+    """The gradient of MaskNet's flattened embedding V_emb, ONE buffer: every mask block's first mask Linear adds its
+    dgrad into it (GEMM accumulate), and so do the embedding LayerNorm's backward and, when V_hidden is V_emb itself,
+    the blocks' v_in gradients.  shared_grad() hands it to autograd once all of them have run.  It also keeps V_emb's
+    GEMM operand copy, made once per forward for all blocks."""
+
+    def __init__(self):
+        self.buf = None
+        self._aux = None
+
+    def target(self, like):
+        """(buffer, accumulate): the first writer of a backward gets an uninitialised buffer to overwrite."""
+        if self.buf is None:
+            self.buf = torch.empty_like(like)
+            return self.buf, False
+        return self.buf, True
+
+    def emb_aux(self, v_emb):
+        key = (_MATMUL["mode"], _MATMUL["x3_inline"], v_emb.data_ptr(), v_emb._version, tuple(v_emb.shape))
+        if self._aux is None or self._aux[0] != key:
+            self._aux = (key, make_aux(v_emb))
+        return self._aux[1]
+
+
+class _SharedGrad(torch.autograd.Function):
+    """x -> x (a view), whose backward returns the EmbeddingGrad buffer the consumers of the view added into (they
+    return no gradient for it themselves).  Autograd runs this backward after every consumer's."""
+
+    @staticmethod
+    def forward(ctx, x, sink):
+        ctx.set_materialize_grads(False)
+        ctx.sink = sink
+        sink.buf = None
+        return x.view_as(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        if g is not None:
+            raise RuntimeError("shared_grad: the view's consumers must add into the EmbeddingGrad buffer")
+        buf, ctx.sink.buf = ctx.sink.buf, None
+        return buf, None
+
+
+def shared_grad(v_emb):
+    """(V_emb view, EmbeddingGrad) for field_layernorm and mask_blocks, which add V_emb's gradient into one buffer."""
+    _require_cuda(v_emb)
+    sink = EmbeddingGrad()
+    return _SharedGrad.apply(_f32c(v_emb), sink), sink
+
+
+def field_param_layout(weights, biases):
+    """(gamma_0, beta_0, pstride) when the F LayerNorms' weights and biases lie at one stride (weight f at
+    &weight_0 + f pstride, bias f at &bias_0 + f pstride, as pack_field_params and the fused optimizer's arena place
+    them), else None."""
+    F = len(weights)
+    w0, b0 = weights[0], biases[0]
+    if any(not t.is_contiguous() or t.dtype != torch.float32 for t in list(weights) + list(biases)):
+        return None
+    if F == 1:
+        return w0, b0, 0
+    step = weights[1].data_ptr() - w0.data_ptr()
+    if step <= 0 or step % 4:
+        return None
+    for f in range(F):
+        if weights[f].data_ptr() != w0.data_ptr() + f * step or biases[f].data_ptr() != b0.data_ptr() + f * step:
+            return None
+    if step // 4 < w0.numel():
+        return None
+    return w0, b0, step // 4
+
+
+def pack_field_params(norms):
+    """Re-home the weights and biases of the LayerNorms `norms` (one per field) into one buffer,
+    [weight_0 | bias_0 | weight_1 | ...] with every slice 16-byte aligned, the layout the fused optimizer's arena gives
+    them: the embedding LayerNorm then reads all F of them at one stride.  The Parameter objects stay (only their .data
+    moves), so optimizers and state_dict keys are unchanged."""
+    params = [p for m in norms for p in (m.weight, m.bias)]
+    D = params[0].numel()
+    pitch = (D + 3) // 4 * 4
+    buf = torch.zeros(len(params) * pitch, dtype=torch.float32, device=params[0].device)
+    with torch.no_grad():
+        for i, p in enumerate(params):
+            dst = buf[i * pitch:i * pitch + D].view(p.shape)
+            dst.copy_(p.data)
+            p.data = dst
+
+
+def _strided_grads(params, pstride):
+    """Zeroed gradient buffers of params (the weights then the biases of F LayerNorms at one stride) that lie at
+    that same stride: the fused optimizer's arena views when they do, else views of one fresh buffer."""
+    F = len(params) // 2
+    grads = [_grad_buffer(p, zero=True) for p in params]
+    layout = field_param_layout(grads[:F], grads[F:])
+    if layout is not None and layout[2] == pstride and \
+            grads[F].data_ptr() - grads[0].data_ptr() == params[F].data_ptr() - params[0].data_ptr():
+        return grads
+    base = min(p.data_ptr() for p in params)
+    span = (max(p.data_ptr() for p in params) - base) // 4 + params[0].numel()
+    buf = torch.zeros(span, dtype=torch.float32, device=params[0].device)
+    out = []
+    for p in params:
+        o = (p.data_ptr() - base) // 4
+        out.append(buf[o:o + p.numel()].view(p.shape))
+    return out
+
+
+class _FieldLayerNorm(torch.autograd.Function):
+    """MaskNet's embedding LayerNorm, V_hidden = cat_f LayerNorm_f(V_emb[:, f]) (MaskNet.py, MaskNet.forward), one
+    launch each way for all F fields (b2_field_ln_fwd / _bwd).  The backward adds the input gradient into the
+    EmbeddingGrad buffer and the weight and bias gradients into buffers at the parameters' stride."""
+
+    @staticmethod
+    def forward(ctx, x, sink, F, D, eps, *params):
+        gamma, beta, pstride = field_param_layout(params[:F], params[F:])
+        B = x.shape[0]
+        out = torch.empty_like(x)
+        ctx.sink, ctx.F, ctx.D, ctx.pstride, ctx.params = sink, F, D, pstride, params
+        if B == 0:          # nothing to normalise: no launch (an empty tensor has no device address)
+            ctx.save_for_backward(x, None, None)
+            return out
+        mean = torch.empty((B, F), dtype=torch.float32, device=x.device)
+        rstd = torch.empty_like(mean)
+        _lib.call("b2_field_ln_fwd", _ptr(x), B, F, D, _ptr(gamma), _ptr(beta), pstride, eps, _ptr(out), _ptr(mean),
+                  _ptr(rstd), _stream())
+        ctx.save_for_backward(x, mean, rstd)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, mean, rstd = ctx.saved_tensors
+        F, D, params = ctx.F, ctx.D, ctx.params
+        grads = _strided_grads(params, ctx.pstride)
+        dx, acc = ctx.sink.target(x)
+        if x.shape[0] == 0:
+            return (None, None, None, None, None) + tuple(grads)
+        _lib.call("b2_field_ln_bwd", _ptr(x), _ptr(mean), _ptr(rstd), _ptr(_f32c(g)), x.shape[0], F, D,
+                  _ptr(params[0]), ctx.pstride, _ptr(dx), 1 if acc else 0, _ptr(grads[0]), _ptr(grads[F]), _stream())
+        return (None, None, None, None, None) + tuple(grads)
+
+
+def field_layernorm(x, sink, weights, biases, eps=1e-5):
+    """cat_f LayerNorm_f(x[:, f D:(f + 1) D]) of a shared_grad view x (B, F D): the F LayerNorms' weights and biases
+    (D) must lie at one stride (field_param_layout; pack_field_params places them so)."""
+    F = len(weights)
+    _require_cuda(x, *weights)
+    if F < 1 or len(biases) != F:
+        raise ValueError("field_layernorm: one weight and one bias per field")
+    D = weights[0].numel()
+    bound = masknet_width_bound(D, "embedding_dim")
+    if bound:
+        raise ValueError("field_layernorm: " + bound)
+    if x.dim() != 2 or x.shape[1] != F * D:
+        raise ValueError("field_layernorm: x%s is not (B, %d * %d)" % (tuple(x.shape), F, D))
+    if field_param_layout(weights, biases) is None:
+        raise ValueError("field_layernorm: the LayerNorms' weights and biases do not lie at one stride; "
+                         "re-home them with pack_field_params")
+    return _FieldLayerNorm.apply(x, sink, F, D, float(eps), *weights, *biases)
+
+
+_MASK_PARAMS = 7        # per block: W1, b1, W2, b2, W3, gamma, beta (gamma, beta None without LayerNorm)
+
+
+class _MaskBlocks(torch.autograd.Function):
+    """nb MaskBlocks on one (V_emb, v_in) (MaskNet.py, MaskBlock.forward), their outputs side by side in one
+    (B, nb n) tensor: ParallelMaskNet's concatenation without a copy (nb = 1: one block of SerialMaskNet).  Block k:
+      h = ReLU(V_emb W1^T + b1)                    GEMM, bias + ReLU epilogue
+      u = V_mask * v_in,  V_mask = h W2^T + b2     GEMM, bias + mul epilogue keeping V_mask (out_pre)
+      z = u W3^T                                   GEMM
+      out[:, k n:(k + 1) n] = drop(act(LN(z)))     b2_mask_row_fwd (+ the operand copy a GEMM consumer wants)
+    Backward of block k: dz (b2_mask_row_bwd, with the LayerNorm weight and bias gradients), dV_mask = v_in * (dz W3)
+    with du = dz W3 kept (one dgrad, mul epilogue, out_pre, colsum = the b2 gradient), dW3, dv_in += du * V_mask
+    (b2_mask_mul), dh = ReLU'(h) * (dV_mask W2) (one dgrad, colsum = the b1 gradient), dW2, and V_emb's gradient added
+    into the EmbeddingGrad buffer (dgrad, accumulate), dW1.  v_in None: v_in is V_emb, its gradient goes to the
+    buffer too.  Where the tensor cores cannot take a Linear it runs on the SIMT GEMM, and the product the mul
+    epilogue would form takes one b2_mask_mul (its sum one b2_prep_operand)."""
+
+    @staticmethod
+    def forward(ctx, v_emb, v_in, sink, cfg, *params):
+        act, eps, drops, want_aux = cfg
+        nb = len(params) // _MASK_PARAMS
+        x = v_in if v_in is not None else v_emb
+        B = v_emb.shape[0]
+        dev = v_emb.device
+        n = params[4].shape[0]
+        out = torch.empty((B, nb * n), dtype=torch.float32, device=dev)
+        ctx.sink, ctx.cfg, ctx.params, ctx.nb = sink, cfg, params, nb
+        if B == 0:          # no rows: no launch (an empty tensor has no device address)
+            ctx.save_for_backward(v_emb, v_in)
+            return out
+        out_aux = empty_aux(B, nb * n, dev) if want_aux else None
+        emb_aligned = v_emb.data_ptr() % 16 == 0 and x.data_ptr() % 16 == 0
+        saved, meta = [], []
+        for k in range(nb):
+            W1, b1, W2, b2, W3, gamma, beta = params[k * _MASK_PARAMS:(k + 1) * _MASK_PARAMS]
+            r, hd = W1.shape[0], W2.shape[0]
+            tc = [_tc_layer_ok(W) and emb_aligned for W in (W1, W2, W3)]
+            emb_aux = sink.emb_aux(v_emb) if tc[0] else None
+            h = torch.empty((B, r), dtype=torch.float32, device=dev)
+            h_aux = empty_aux(B, r, dev) if (tc[1] and tc[0]) else None
+            _linear_fwd(tc[0], v_emb, emb_aux, W1, h, bias=b1, act=B2_ACT_RELU,
+                        **({"out_small": h_aux} if tc[0] else {}))
+            if tc[1] and h_aux is None:
+                h_aux = make_aux(h)
+            vmask = torch.empty((B, hd), dtype=torch.float32, device=dev)
+            u = torch.empty_like(vmask)
+            u_aux = empty_aux(B, hd, dev) if (tc[2] and tc[1]) else None
+            if tc[1]:
+                _linear_fwd(True, h, h_aux, W2, u, bias=b2, mul=x, out_pre=vmask, out_small=u_aux)
+            else:
+                _linear_fwd(False, h, None, W2, vmask, bias=b2)
+                _lib.call("b2_mask_mul", _ptr(vmask), _ptr(x), B * hd, _ptr(u), 0, _stream())
+            if tc[2] and u_aux is None:
+                u_aux = make_aux(u)
+            z = torch.empty((B, n), dtype=torch.float32, device=dev)
+            _linear_fwd(tc[2], u, u_aux, W3, z)
+            ln = gamma is not None
+            mean = torch.empty(B, dtype=torch.float32, device=dev) if ln else None
+            rstd = torch.empty(B, dtype=torch.float32, device=dev) if ln else None
+            dl = drops[k] if drops is not None else None
+            seg_aux = out_aux[:, k * n:] if out_aux is not None else None
+            _lib.call("b2_mask_row_fwd", _ptr(z), B, n, _ptr(gamma), _ptr(beta), eps, act,
+                      *_drop_args(dl), ctypes.c_void_p(out.data_ptr() + 4 * k * n), nb * n,
+                      *_aux_args(seg_aux), _ptr(mean), _ptr(rstd), _stream())
+            saved += [h, vmask, u, z, mean, rstd]
+            meta.append((tc, emb_aux, h_aux, u_aux, dl))
+        if out_aux is not None:
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        ctx.save_for_backward(v_emb, v_in, *saved)
+        ctx.meta = meta
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        v_emb, v_in = ctx.saved_tensors[:2]
+        saved = ctx.saved_tensors[2:]
+        act = ctx.cfg[0]
+        nb, params, sink = ctx.nb, ctx.params, ctx.sink
+        x = v_in if v_in is not None else v_emb
+        g = _f32c(g)
+        B = v_emb.shape[0]
+        dev = v_emb.device
+        grads = [None] * len(params)
+        gx = None
+        if B == 0:          # every gradient is zero; V_emb's buffer is left to the other writers
+            grads = [_grad_buffer(p, zero=True) if p is not None else None for p in params]
+            return (None, torch.zeros_like(v_in) if v_in is not None else None, None, None) + tuple(grads)
+        for k in range(nb):
+            W1, b1, W2, b2, W3, gamma, beta = params[k * _MASK_PARAMS:(k + 1) * _MASK_PARAMS]
+            h, vmask, u, z, mean, rstd = saved[6 * k:6 * k + 6]
+            tc, emb_aux, h_aux, u_aux, dl = ctx.meta[k]
+            r, hd, n = W1.shape[0], W2.shape[0], W3.shape[0]
+            base = k * _MASK_PARAMS
+            # the block's tail: dz (+ its operand copy for W3's dgrad and wgrad) and the LayerNorm's gradients
+            dz = torch.empty((B, n), dtype=torch.float32, device=dev)
+            dz_aux = empty_aux(B, n, dev) if tc[2] else None
+            dgamma = dbeta = None
+            if gamma is not None:
+                dgamma, dbeta = _grad_buffer(gamma, zero=True), _grad_buffer(beta, zero=True)
+                grads[base + 5], grads[base + 6] = dgamma, dbeta
+            _lib.call("b2_mask_row_bwd", _ptr(z), _ptr(mean), _ptr(rstd), _ptr(gamma), _ptr(beta), act,
+                      *_drop_args(dl), ctypes.c_void_p(g.data_ptr() + 4 * k * n), g.stride(0), B, n, _ptr(dz),
+                      *_aux_args(dz_aux), _ptr(dgamma), _ptr(dbeta), _stream())
+            if tc[2] and dz_aux is None:
+                dz_aux = make_aux(dz)
+            # hidden Linear: du = dz W3, dV_mask = v_in * du (+ b2's gradient), dW3
+            gb2 = _grad_buffer(b2, zero=False)
+            du = torch.empty((B, hd), dtype=torch.float32, device=dev)
+            dvm = torch.empty_like(du)
+            dvm_aux = empty_aux(B, hd, dev) if (tc[1] and tc[2]) else None
+            if tc[2]:
+                _linear_dgrad(True, dz, dz_aux, W3, dvm, mul=x, out_pre=du, out_small=dvm_aux, colsum=gb2)
+                if tc[1] and dvm_aux is None:
+                    dvm_aux = make_aux(dvm)
+            else:
+                _linear_dgrad(False, dz, None, W3, du)
+                dvm, dvm_aux = _grad_operand(du, x, B2_PREP_MUL, tc[1], colsum=gb2)
+            grads[base + 3] = gb2
+            gw3 = _grad_buffer(W3, zero=False)
+            _linear_wgrad(tc[2], dz, dz_aux, u, u_aux, gw3)
+            grads[base + 4] = gw3
+            # v_in's gradient, du * V_mask: summed over the blocks (V_emb's buffer when v_in is V_emb)
+            if v_in is not None:
+                if gx is None:
+                    gx, acc = torch.empty_like(v_in), False
+                else:
+                    acc = True
+            else:
+                gx, acc = sink.target(v_emb)
+            _lib.call("b2_mask_mul", _ptr(du), _ptr(vmask), B * hd, _ptr(gx), 1 if acc else 0, _stream())
+            # mask MLP: dh = ReLU'(h) * (dV_mask W2) (+ b1's gradient), dW2, V_emb's gradient, dW1
+            gb1 = _grad_buffer(b1, zero=False)
+            dh = torch.empty((B, r), dtype=torch.float32, device=dev)
+            if tc[1]:
+                dh_aux = empty_aux(B, r, dev) if tc[0] else None
+                _linear_dgrad(True, dvm, dvm_aux, W2, dh, ybwd=h, act_bwd=B2_ACT_RELU, out_small=dh_aux, colsum=gb1)
+                if tc[0] and dh_aux is None:
+                    dh_aux = make_aux(dh)
+            else:
+                _linear_dgrad(False, dvm, None, W2, dh)
+                dh, dh_aux = _grad_operand(dh, h, B2_ACT_RELU, tc[0], colsum=gb1)
+            grads[base + 1] = gb1
+            gw2 = _grad_buffer(W2, zero=False)
+            _linear_wgrad(tc[1], dvm, dvm_aux, h, h_aux, gw2)
+            grads[base + 2] = gw2
+            gemb, acc = sink.target(v_emb)
+            _linear_dgrad(tc[0], dh, dh_aux, W1, gemb, accumulate=acc)
+            gw1 = _grad_buffer(W1, zero=False)
+            _linear_wgrad(tc[0], dh, dh_aux, v_emb, emb_aux, gw1)
+            grads[base] = gw1
+        return (None, gx if v_in is not None else None, None, None) + tuple(grads)
+
+
+def _drop_args(dl):
+    """The (drop_rng, drop_layer, drop_thresh, drop_scale) arguments of a (snapshot, layer, thresh, scale) or None."""
+    if dl is None:
+        return _ptr(None), 0, 0, 0.0
+    return _ptr(dl[0]), dl[1], dl[2], dl[3]
+
+
+def mask_blocks(v_emb, sink, v_in, blocks, act, eps=1e-5, dropout=0.0, snapshot=None, first_layer=0, want_aux=False):
+    """The outputs of the MaskBlocks `blocks` on one (V_emb, v_in), side by side in one (B, nb n) tensor.  v_emb and
+    sink come from shared_grad; v_in None: the blocks' input is V_emb itself.  A block is (W1, b1, W2, b2, W3,
+    gamma, beta) (gamma, beta None: no LayerNorm): its mask_layer.0, mask_layer.2 and hidden_layer Linear weights
+    and biases, and its LayerNorm's.  act: B2_ACT_RELU or B2_ACT_SIGMOID.  dropout > 0: block k draws the mask of
+    layer first_layer + k of `snapshot` (dropout_snapshot).  want_aux: also write the output's GEMM operand copy for
+    a GEMM consumer."""
+    _require_cuda(v_emb, v_in)
+    if act not in (B2_ACT_RELU, B2_ACT_SIGMOID, B2_ACT_NONE):
+        raise NotImplementedError("mask_blocks: activation code %r" % (act,))
+    x = v_in if v_in is not None else v_emb
+    B, d = v_emb.shape
+    params = []
+    n = blocks[0][4].shape[0]
+    for blk in blocks:
+        W1, b1, W2, b2, W3, gamma, beta = blk
+        r, hd = W1.shape[0], W2.shape[0]
+        if (tuple(W1.shape) != (r, d) or tuple(b1.shape) != (r,) or tuple(W2.shape) != (hd, r)
+                or tuple(b2.shape) != (hd,) or tuple(W3.shape) != (n, hd) or x.shape != (B, hd)
+                or (gamma is None) != (beta is None)
+                or (gamma is not None and (tuple(gamma.shape) != (n,) or tuple(beta.shape) != (n,)))):
+            raise ValueError("mask_blocks: shapes V_emb%s v_in%s W1%s W2%s W3%s do not match"
+                             % tuple(tuple(t.shape) for t in (v_emb, x, W1, W2, W3)))
+        params += [W1, b1, W2, b2, W3, gamma, beta]
+    bound = masknet_width_bound(n, "output_dim")
+    if bound:
+        raise ValueError("mask_blocks: " + bound)
+    drops = None
+    if dropout > 0:
+        consts = dropout_consts(dropout)
+        drops = [(snapshot, first_layer + k) + consts for k in range(len(blocks))]
+    return _MaskBlocks.apply(v_emb, None if v_in is None else _f32c(v_in), sink, (act, float(eps), drops, want_aux),
+                             *params)
+
+
 class _FsGate(torch.autograd.Function):
     """FinalMLP's gating products f_s = e * (2 g_s), s = 1, 2 (FinalMLP.py, FeatureSelection.forward) in one launch
     (include/fuxictr_b200.h "FinalMLP"), which also writes f1's and f2's auxiliary operands for the towers' first

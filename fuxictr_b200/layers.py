@@ -20,6 +20,7 @@ Reference files (relative to the reference root):
   Dice                                     fuxictr/pytorch/layers/activations.py:24-51
   MLP_Block                                fuxictr/pytorch/layers/blocks/mlp_block.py:24-96
   FeatureSelection / InteractionAggregation model_zoo/FinalMLP/src/FinalMLP.py
+  MaskBlock / SerialMaskNet / ParallelMaskNet model_zoo/MaskNet/src/MaskNet.py
 """
 import sys
 from collections import OrderedDict
@@ -546,6 +547,171 @@ class GateCorssLayer(nn.Module):
         for i in range(self.cn_layers):
             x = F2.gated_cross_layer(x0, x, self.w[i].weight, self.wg[i].weight, self.b[i])
         return x
+
+
+def _mask_act(module):
+    """The B2_ACT_* code of a MaskBlock's hidden activation module; the row kernel implements ReLU and Sigmoid."""
+    if type(module) == nn.ReLU:
+        return B2_ACT_RELU
+    if type(module) == nn.Sigmoid:
+        return B2_ACT_SIGMOID
+    raise NotImplementedError("MaskBlock: hidden activation %s is not implemented on the H100 path (ReLU and "
+                              "Sigmoid are)" % type(module).__name__)
+
+
+class MaskBlock(nn.Module):
+    """MaskNet's mask block (model_zoo/MaskNet/src/MaskNet.py, MaskBlock):
+    out = hidden_layer(mask_layer(V_emb) * V_hidden), mask_layer = Linear -> ReLU -> Linear,
+    hidden_layer = Linear(bias=False) -> [LayerNorm] -> activation -> [Dropout].  Children, registration order and
+    initial draws are the reference's.  The forward runs on the kernels (functional.mask_blocks): three GEMMs and one
+    row kernel for LayerNorm, activation and dropout.  Output widths beyond the row kernel's bound and activations
+    other than ReLU and Sigmoid are refused here, before any CUDA call."""
+
+    def __init__(self, input_dim, hidden_dim, output_dim, hidden_activation="ReLU", reduction_ratio=1,
+                 dropout_rate=0, layer_norm=True):
+        super(MaskBlock, self).__init__()
+        bound = F2.masknet_width_bound(output_dim, "MaskBlock output_dim")
+        if bound:
+            raise ValueError(bound)
+        self.mask_layer = nn.Sequential(nn.Linear(input_dim, int(hidden_dim * reduction_ratio)),
+                                        nn.ReLU(),
+                                        nn.Linear(int(hidden_dim * reduction_ratio), hidden_dim))
+        hidden_layers = [nn.Linear(hidden_dim, output_dim, bias=False)]
+        if layer_norm:
+            hidden_layers.append(nn.LayerNorm(output_dim))
+        hidden_layers.append(get_activation(hidden_activation))
+        if dropout_rate > 0:
+            hidden_layers.append(nn.Dropout(p=dropout_rate))
+        self.hidden_layer = nn.Sequential(*hidden_layers)
+        self._act = _mask_act(hidden_layers[2 if layer_norm else 1])
+        if dropout_rate > 0:
+            F2.dropout_consts(dropout_rate)         # a rate outside (0, 1) is refused here, as nn.Dropout does
+
+    def block_params(self):
+        """(W1, b1, W2, b2, W3, gamma, beta) of functional.mask_blocks."""
+        ln = self.hidden_layer[1] if type(self.hidden_layer[1]) == nn.LayerNorm else None
+        return (self.mask_layer[0].weight, self.mask_layer[0].bias, self.mask_layer[2].weight, self.mask_layer[2].bias,
+                self.hidden_layer[0].weight, ln.weight if ln is not None else None, ln.bias if ln is not None else None)
+
+    def dropout_rate(self):
+        """The block's dropout probability in training mode, 0 in eval mode (nn.Dropout is then the identity)."""
+        last = self.hidden_layer[-1]
+        return last.p if (type(last) == nn.Dropout and last.training) else 0.0
+
+    def forward(self, V_emb, V_hidden):
+        return _run_mask_blocks([self], V_emb, V_hidden)
+
+
+def _masknet_eps(blocks):
+    ln = blocks[0].hidden_layer[1]
+    return ln.eps if type(ln) == nn.LayerNorm else 1e-5
+
+
+def _run_mask_blocks(blocks, V_emb, V_hidden, sink=None, snapshot=None, first_layer=0, want_aux=False):
+    """The outputs of `blocks` (same act, dropout, LayerNorm and output width) on (V_emb, V_hidden), side by side.
+    sink: the EmbeddingGrad of a shared_grad view V_emb; None: a view and buffer of these blocks alone.
+    V_hidden is V_emb: the blocks' input gradient goes to V_emb's buffer too."""
+    same = V_hidden is V_emb
+    if sink is None:
+        V_emb, sink = F2.shared_grad(V_emb)
+    p = blocks[0].dropout_rate()
+    if p > 0 and snapshot is None:
+        snapshot, first_layer = F2.dropout_snapshot(V_emb.device, len(blocks)), 0
+    return F2.mask_blocks(V_emb, sink, None if same else V_hidden, [b.block_params() for b in blocks], blocks[0]._act,
+                          eps=_masknet_eps(blocks), dropout=p, snapshot=snapshot, first_layer=first_layer,
+                          want_aux=want_aux)
+
+
+class SerialMaskNet(nn.Module):
+    """MaskNet.py, SerialMaskNet: MaskBlocks chained over [input_dim] + hidden_units, every block's mask MLP reading
+    V_emb, then fc = Linear(h_last, output_dim) -> output activation.  One dropout snapshot per forward: block i
+    draws the mask of layer i."""
+
+    def __init__(self, input_dim, output_dim=None, output_activation=None, hidden_units=[],
+                 hidden_activations="ReLU", reduction_ratio=1, dropout_rates=0, layer_norm=True):
+        super(SerialMaskNet, self).__init__()
+        if not isinstance(dropout_rates, list):
+            dropout_rates = [dropout_rates] * len(hidden_units)
+        if not isinstance(hidden_activations, list):
+            hidden_activations = [hidden_activations] * len(hidden_units)
+        self.hidden_units = [input_dim] + hidden_units
+        self.mask_blocks = nn.ModuleList()
+        for idx in range(len(self.hidden_units) - 1):
+            self.mask_blocks.append(MaskBlock(input_dim,
+                                              self.hidden_units[idx],
+                                              self.hidden_units[idx + 1],
+                                              hidden_activations[idx],
+                                              reduction_ratio,
+                                              dropout_rates[idx],
+                                              layer_norm))
+        fc_layers = []
+        if output_dim is not None:
+            fc_layers.append(nn.Linear(self.hidden_units[-1], output_dim))
+        if output_activation is not None:
+            fc_layers.append(get_activation(output_activation))
+        self.fc = None
+        if len(fc_layers) > 0:
+            self.fc = nn.Sequential(*fc_layers)
+
+    def blocks_out(self, V_emb, V_hidden, sink=None):
+        """The last block's output (what fc reads)."""
+        same = V_hidden is V_emb
+        if sink is None:
+            V_emb, sink = F2.shared_grad(V_emb)
+        n_drop = sum(1 for b in self.mask_blocks if b.dropout_rate() > 0)
+        snap = F2.dropout_snapshot(V_emb.device, n_drop) if n_drop else None
+        v_out, ordinal = (V_emb if same else V_hidden), 0
+        for blk in self.mask_blocks:
+            v_out = _run_mask_blocks([blk], V_emb, v_out, sink, snap, ordinal)
+            ordinal += 1 if blk.dropout_rate() > 0 else 0
+        return v_out
+
+    def forward(self, V_emb, V_hidden):
+        v_out = self.blocks_out(V_emb, V_hidden)
+        if self.fc is not None:
+            lin = self.fc[0] if type(self.fc[0]) == nn.Linear else None
+            if lin is not None:
+                act = B2_ACT_SIGMOID if (len(self.fc) > 1 and type(self.fc[1]) == nn.Sigmoid) else B2_ACT_NONE
+                v_out = F2.linear_act(v_out, lin.weight, lin.bias, act)
+                rest = list(self.fc)[2 if act != B2_ACT_NONE else 1:]
+            else:
+                rest = list(self.fc)
+            for m in rest:
+                v_out = m(v_out)
+        return v_out
+
+
+class ParallelMaskNet(nn.Module):
+    """MaskNet.py, ParallelMaskNet: num_blocks MaskBlock(input_dim, input_dim, block_dim) on the same (V_emb,
+    V_hidden), concatenated, then MLP_Block to output_dim.  The blocks run as one autograd node that writes each
+    output straight into its column slice of the concatenation, with the MLP's first-GEMM operand copy."""
+
+    def __init__(self, input_dim, output_dim=None, output_activation=None, num_blocks=1, block_dim=64,
+                 hidden_units=[], hidden_activations="ReLU", reduction_ratio=1, dropout_rates=0,
+                 layer_norm=True):
+        super(ParallelMaskNet, self).__init__()
+        self.num_blocks = num_blocks
+        self.mask_blocks = nn.ModuleList([MaskBlock(input_dim,
+                                                    input_dim,
+                                                    block_dim,
+                                                    hidden_activations,
+                                                    reduction_ratio,
+                                                    dropout_rates,
+                                                    layer_norm) for _ in range(num_blocks)])
+
+        self.dnn = MLP_Block(input_dim=block_dim * num_blocks,
+                             output_dim=output_dim,
+                             hidden_units=hidden_units,
+                             hidden_activations=hidden_activations,
+                             output_activation=output_activation,
+                             dropout_rates=dropout_rates)
+
+    def blocks_out(self, V_emb, V_hidden, sink=None):
+        """The concatenated block outputs (what dnn reads)."""
+        return _run_mask_blocks(list(self.mask_blocks), V_emb, V_hidden, sink, want_aux=True)
+
+    def forward(self, V_emb, V_hidden):
+        return self.dnn(self.blocks_out(V_emb, V_hidden))
 
 
 class FeatureSelection(nn.Module):

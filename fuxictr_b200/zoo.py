@@ -15,6 +15,7 @@ same RNG consumption) and nothing else.
   GDCN, GDCNP  model_zoo/GDCN/src/GDCN.py
   FinalMLP     model_zoo/FinalMLP/src/FinalMLP.py
   DualMLP      model_zoo/FinalMLP/src/DualMLP.py
+  MaskNet      model_zoo/MaskNet/src/MaskNet.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -25,6 +26,7 @@ from torch import nn
 
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
+                     SerialMaskNet, ParallelMaskNet,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -173,15 +175,15 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP) may be sharded: any other forward
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet) may be sharded: any other forward
         would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
         from . import sharded as SH
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
-                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP and "
-                                      "DualMLP" % type(self).__name__)
+                                      "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
+                                      "DualMLP and MaskNet" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -647,6 +649,100 @@ class DualMLP(RankModel):
 
     def forward(self, inputs):
         return {"y_pred": self.output_activation(sum(self.forward_logits(inputs)))}
+
+
+class MaskNet(RankModel):
+    """model_zoo/MaskNet/src/MaskNet.py, MaskNet: MaskBlocks over the flattened embedding V_emb and its per-field
+    LayerNorm V_hidden (emb_layernorm), chained (SerialMaskNet, ending in fc) or side by side under an MLP
+    (ParallelMaskNet).  Every block's mask MLP reads V_emb, not V_hidden, as in the reference.  V_emb's gradient is one
+    buffer that every block and the embedding LayerNorm add into (functional.shared_grad).  The F embedding
+    LayerNorms' weights and biases are kept in one buffer at one stride (functional.pack_field_params; the fused
+    optimizer's arena keeps that layout), so their kernel reads them where they live.  Unknown keyword arguments are
+    accepted and ignored, as the reference's **kwargs are."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="MaskNet", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 dnn_hidden_units=[64, 64, 64], dnn_hidden_activations="ReLU", model_type="SerialMaskNet",
+                 parallel_num_blocks=1, parallel_block_dim=64, reduction_ratio=1, embedding_regularizer=None,
+                 net_regularizer=None, net_dropout=0, emb_layernorm=True, net_layernorm=True, **kwargs):
+        if model_type not in ("SerialMaskNet", "ParallelMaskNet"):
+            raise ValueError("MaskNet: model_type must be 'SerialMaskNet' or 'ParallelMaskNet', got %r" % (model_type,))
+        if model_type == "SerialMaskNet" and not dnn_hidden_units:
+            # the reference would build no block and a bare Linear(d, 1): not a MaskNet
+            raise ValueError("SerialMaskNet needs a non-empty dnn_hidden_units (its chain of mask blocks)")
+        if emb_layernorm:
+            bound = F2.masknet_width_bound(embedding_dim, "MaskNet embedding_dim (emb_layernorm)")
+            if bound:
+                raise ValueError(bound)
+        super(MaskNet, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                      embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                      **kwargs)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        if model_type == "SerialMaskNet":
+            self.mask_net = SerialMaskNet(input_dim=feature_map.num_fields * embedding_dim,
+                                          output_dim=1,
+                                          output_activation=self.output_activation,
+                                          hidden_units=dnn_hidden_units,
+                                          hidden_activations=dnn_hidden_activations,
+                                          reduction_ratio=reduction_ratio,
+                                          dropout_rates=net_dropout,
+                                          layer_norm=net_layernorm)
+        else:
+            self.mask_net = ParallelMaskNet(input_dim=feature_map.num_fields * embedding_dim,
+                                            output_dim=1,
+                                            output_activation=self.output_activation,
+                                            num_blocks=parallel_num_blocks,
+                                            block_dim=parallel_block_dim,
+                                            hidden_units=dnn_hidden_units,
+                                            hidden_activations=dnn_hidden_activations,
+                                            reduction_ratio=reduction_ratio,
+                                            dropout_rates=net_dropout,
+                                            layer_norm=net_layernorm)
+        self.num_fields = feature_map.num_fields
+        if emb_layernorm:
+            self.emb_norm = nn.ModuleList(nn.LayerNorm(embedding_dim) for _ in range(self.num_fields))
+        else:
+            self.emb_norm = None
+        self._finish(kwargs, learning_rate)
+
+    def model_to_device(self):
+        super(MaskNet, self).model_to_device()
+        if self.emb_norm is not None:
+            F2.pack_field_params(self.emb_norm)
+
+    def _logit_mlp(self):
+        """ParallelMaskNet's MLP without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_dnn")
+        if ent is None:
+            dnn = self.mask_net.dnn
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(dnn.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_dnn"] = ent
+        return ent
+
+    def forward_logits(self, inputs):
+        return (self.dense_logit(self._flat_embedding(inputs)),)
+
+    def dense_logit(self, flat_emb):
+        """The pre-sigmoid logit from the flattened embedding (B, F D): the embedding LayerNorm, the mask blocks and
+        the head."""
+        emb, sink = F2.shared_grad(flat_emb)
+        v_hidden = emb
+        if self.emb_norm is not None:
+            ws, bs = [m.weight for m in self.emb_norm], [m.bias for m in self.emb_norm]
+            if F2.field_param_layout(ws, bs) is None:       # moved since model_to_device (e.g. by .to())
+                F2.pack_field_params(self.emb_norm)
+            v_hidden = F2.field_layernorm(emb, sink, ws, bs, self.emb_norm[0].eps)
+        net = self.mask_net
+        if isinstance(net, SerialMaskNet):
+            fc = net.fc[0]
+            return F2.linear_act(net.blocks_out(emb, v_hidden, sink), fc.weight, fc.bias)
+        return self._logit_mlp()(net.blocks_out(emb, v_hidden, sink))
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
 
 
 class DLRM(RankModel):

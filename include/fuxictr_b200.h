@@ -484,6 +484,51 @@ B2_API int b2_agg_bwd(const float* Q, const float* y, const float* g, int64_t ba
 B2_API int b2_agg_unpack(const float* dW_aug, int dx, int dy, int heads, float* gw_xy, float* gw_x, void* stream);
 
 /*
+ * MaskNet (model_zoo/MaskNet/src/MaskNet.py).  All row-major fp32.  LayerNorm is nn.LayerNorm's: biased variance
+ * over the row, eps inside the square root, y = (x - mean) rstd gamma + beta; the kernels take the mean first and
+ * then the variance from the centred values.  Widths (dim, n) lie in [1, B2_MASKNET_MAX_WIDTH]; dim % 4 == 0 (n % 4)
+ * with 16-byte aligned rows, parameters and pitches takes a float4 path, anything else a scalar one.  Outside the
+ * range, or given a NULL pointer, every entry point returns B2_E_INVALID.
+ *
+ * Embedding LayerNorm: x (B, F, D) = the embedding, field f normalised by its own nn.LayerNorm(D), whose weight and
+ * bias lie at gamma + f pstride and beta + f pstride (pstride in floats; the fused optimizer's arena interleaves
+ * them as [gamma_0 | beta_0 | gamma_1 | ...], so gamma = &gamma_0, beta = &beta_0 and pstride = 2 round4(D)).  One
+ * launch each way covers all F fields.
+ * b2_field_ln_fwd: out (B, F, D) "="; mean, rstd (B, F) "=" (saved for the backward).
+ * b2_field_ln_bwd: dx (B, F, D) "=" (accumulate 0) or "+=" (accumulate 1) the input gradient for the output
+ *   gradient g (B, F, D); dgamma, dbeta (at the parameters' stride) "+=" (caller zeroes) the sums over the batch:
+ *   a per-CTA sum, then one float atomic per column and CTA.
+ *
+ * MaskBlock, out = dropout(act(LN(z))) with z = (V_mask * v_in) W^T (B, n) the hidden Linear's output (the GEMM
+ * before this kernel).  gamma, beta (n) NULL: the block has no LayerNorm (out = dropout(act(z))).  act: B2_ACT_NONE,
+ * B2_ACT_RELU or B2_ACT_SIGMOID.  drop_rng != NULL: dropout with the mask of "Dropout masks" over the (B, n) block
+ * output at counter offset snapshot offset + drop_layer.
+ * b2_mask_row_fwd: out "=" at row pitch ld_out (a column slice of a wider buffer); out_aux (optional, row pitch ld_aux)
+ *   receives out's GEMM operand copy: its bf16 rounding (aux_dtype B2_BF16) or its 3xTF32 small part (B2_F32);
+ *   mean, rstd (B) "=" with LayerNorm.
+ * b2_mask_row_bwd: dz (B, n) "=" from the output gradient g (row pitch ld_g): the mask regenerated, act' of the LN
+ *   output recomputed from z, mean and rstd (the value the forward had before dropout), the LN backward; dz_aux as
+ *   out_aux; dgamma, dbeta (n) "+=" (caller zeroes) as in b2_field_ln_bwd.
+ * b2_mask_mul: out (n) "=" (accumulate 0) or "+=" (accumulate 1) a * b: the gradient of the block input
+ *   v_in = du * V_mask, du the hidden Linear's input gradient.
+ */
+#define B2_MASKNET_MAX_WIDTH 1024
+B2_API int b2_field_ln_fwd(const float* x, int64_t batch, int fields, int dim, const float* gamma, const float* beta,
+                           int64_t pstride, float eps, float* out, float* mean, float* rstd, void* stream);
+B2_API int b2_field_ln_bwd(const float* x, const float* mean, const float* rstd, const float* g, int64_t batch,
+                           int fields, int dim, const float* gamma, int64_t pstride, float* dx, int accumulate,
+                           float* dgamma, float* dbeta, void* stream);
+B2_API int b2_mask_row_fwd(const float* z, int64_t batch, int n, const float* gamma, const float* beta, float eps,
+                           int act, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                           float drop_scale, float* out, int64_t ld_out, void* out_aux, int aux_dtype,
+                           int64_t ld_aux, float* mean, float* rstd, void* stream);
+B2_API int b2_mask_row_bwd(const float* z, const float* mean, const float* rstd, const float* gamma, const float* beta,
+                           int act, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                           float drop_scale, const float* g, int64_t ld_g, int64_t batch, int n, float* dz,
+                           void* dz_aux, int aux_dtype, int64_t ld_aux, float* dgamma, float* dbeta, void* stream);
+B2_API int b2_mask_mul(const float* a, const float* b, int64_t n, float* out, int accumulate, void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
