@@ -1564,6 +1564,140 @@ def mask_blocks(v_emb, sink, v_in, blocks, act, eps=1e-5, dropout=0.0, snapshot=
                              *params)
 
 
+# --------------------------------------------------------------------------------------
+# AutoInt (include/fuxictr_b200.h "AutoInt")
+# --------------------------------------------------------------------------------------
+def autoint_bound(fields, attention_dim, heads):
+    """None when the AutoInt row kernels cover F fields, attention_dim A and `heads` heads, else the bound it breaks."""
+    if not 1 <= fields <= _lib.B2_AUTOINT_MAX_FIELDS:
+        return "the number of fields must lie in [1, %d], got %d" % (_lib.B2_AUTOINT_MAX_FIELDS, fields)
+    if not 1 <= attention_dim <= _lib.B2_AUTOINT_MAX_DIM:
+        return "attention_dim must lie in [1, %d], got %d" % (_lib.B2_AUTOINT_MAX_DIM, attention_dim)
+    if heads < 1 or attention_dim % heads:
+        return "num_heads=%d does not divide attention_dim=%d" % (heads, attention_dim)
+    return None
+
+
+class _SelfAttentionLayer(torch.autograd.Function):
+    """One AutoInt MultiHeadSelfAttention layer (AutoInt.py, MultiHeadSelfAttention.forward) on X (B, F, d_in) as one
+    GEMM and one row kernel (include/fuxictr_b200.h "AutoInt"): Wp = [W_q; W_k; W_v (; W_res)] (b2_autoint_pack),
+    P = X Wp^T, out = ReLU(LN(attention(P) + residual)) (b2_autoint_fwd, which also writes out's auxiliary operand for
+    the next layer's GEMM when asked).  Backward: dP with the residual's and the LayerNorm's gradients
+    (b2_autoint_bwd), dX = dP Wp (+ dR for an identity residual, as the dgrad's epilogue add), dWp = dP^T X and one
+    b2_autoint_unpack into the gradients of W_q, W_k, W_v (, W_res)."""
+
+    @staticmethod
+    def forward(ctx, x, cfg, wq, wk, wv, wres, gamma, beta):
+        heads, scale, eps, res_mode, drop, want_aux = cfg
+        ctx.params = (wq, wk, wv, wres, gamma, beta)     # their gradients may live in an arena
+        B, F, din = x.shape
+        A = wq.shape[0]
+        dev = x.device
+        x2 = _f32c(x).view(B * F, din)
+        parts = 4 if wres is not None else 3
+        NP = parts * A
+        out = torch.empty((B, F, A), dtype=torch.float32, device=dev)
+        ctx.cfg, ctx.shape = cfg, (B, F, din, A, NP)
+        if B == 0:          # no rows: no launch (an empty tensor has no device address)
+            ctx.tc = False
+            return out
+        Wp = torch.empty((NP, din), dtype=torch.float32, device=dev)
+        _lib.call("b2_autoint_pack", _ptr(_f32c(wq)), _ptr(_f32c(wk)), _ptr(_f32c(wv)),
+                  _ptr(_f32c(wres) if wres is not None else None), din, A, _ptr(Wp), _stream())
+        tc = _tc_layer_ok(Wp) and x2.data_ptr() % 16 == 0
+        x_aux = make_aux(x2) if tc else None
+        wp_aux = make_aux(Wp) if tc else None
+        P = torch.empty((B * F, NP), dtype=torch.float32, device=dev)
+        _linear_fwd(tc, x2, x_aux, Wp, P, wp_aux)
+        out_aux = empty_aux(B * F, A, dev) if want_aux else None
+        smax = torch.empty((B, heads, F), dtype=torch.float32, device=dev)
+        ssum = torch.empty_like(smax)
+        ln = gamma is not None
+        mean = torch.empty(B * F, dtype=torch.float32, device=dev) if ln else None
+        rstd = torch.empty_like(mean) if ln else None
+        _lib.call("b2_autoint_fwd", _ptr(P), _ptr(x2), B, F, din, A, heads, res_mode, scale, _ptr(gamma), _ptr(beta),
+                  eps, *_drop_args(drop), _ptr(out), *_aux_args(out_aux), _ptr(smax), _ptr(ssum), _ptr(mean),
+                  _ptr(rstd), _stream())
+        if out_aux is not None:         # the next layer's make_aux finds it
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        ctx.save_for_backward(x2, P, Wp, out, smax, ssum, mean, rstd)
+        ctx.tc, ctx.aux = tc, (x_aux, wp_aux)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        heads, scale, _, res_mode, drop, _ = ctx.cfg
+        B, F, din, A, NP = ctx.shape
+        wq, wk, wv, wres, gamma, beta = ctx.params
+        need = ctx.needs_input_grad
+        ln = gamma is not None
+        dgamma = _grad_buffer(gamma, zero=True) if ln and need[6] else (torch.zeros_like(gamma) if ln else None)
+        dbeta = _grad_buffer(beta, zero=True) if ln and need[7] else (torch.zeros_like(beta) if ln else None)
+        ws = [w for w in (wq, wk, wv, wres) if w is not None]
+        if B == 0:
+            gws = [_grad_buffer(w, zero=True) for w in ws] + [None] * (4 - len(ws))
+            return (torch.zeros((B, F, din), dtype=torch.float32, device=g.device), None) + tuple(gws) + (dgamma, dbeta)
+        x2, P, Wp, out, smax, ssum, mean, rstd = ctx.saved_tensors
+        x_aux, wp_aux = ctx.aux
+        tc = ctx.tc
+        dev = x2.device
+        g = _f32c(g)
+        dP = torch.empty((B * F, NP), dtype=torch.float32, device=dev)
+        dp_aux = empty_aux(B * F, NP, dev) if tc else None
+        gres = torch.empty((B * F, A), dtype=torch.float32, device=dev) if res_mode == 1 else None
+        _lib.call("b2_autoint_bwd", _ptr(P), _ptr(x2), _ptr(out), _ptr(g), _ptr(smax), _ptr(ssum), _ptr(mean),
+                  _ptr(rstd), B, F, din, A, heads, res_mode, scale, _ptr(gamma), *_drop_args(drop), _ptr(dP),
+                  *_aux_args(dp_aux), _ptr(gres), _ptr(dgamma), _ptr(dbeta), _stream())
+        gx = torch.empty((B * F, din), dtype=torch.float32, device=dev)
+        _linear_dgrad(tc, dP, dp_aux, Wp, gx, wp_aux, **({"add": gres} if gres is not None else {}))   # dX = dP Wp
+        dWp = torch.empty_like(Wp)
+        _linear_wgrad(tc, dP, dp_aux, x2, x_aux, dWp)                                                   # dWp = dP^T X
+        gws = [_grad_buffer(w, zero=False) if need[2 + k] else torch.empty_like(w)
+               for k, w in enumerate((wq, wk, wv, wres)) if w is not None]
+        _lib.call("b2_autoint_unpack", _ptr(dWp), din, A, _ptr(gws[0]), _ptr(gws[1]), _ptr(gws[2]),
+                  _ptr(gws[3] if wres is not None else None), _stream())
+        gws += [None] * (4 - len(gws))
+        gws = [gw if need[2 + k] else None for k, gw in enumerate(gws)]
+        return (gx.view(B, F, din), None) + tuple(gws) + (dgamma if ln and need[6] else None,
+                                                          dbeta if ln and need[7] else None)
+
+
+def self_attention_layer(x, w_q, w_k, w_v, w_res=None, num_heads=1, use_residual=True, use_scale=False, gamma=None,
+                         beta=None, eps=1e-5, dropout=0.0, snapshot=None, layer=0, want_aux=False):
+    """out (B, F, A) of one AutoInt MultiHeadSelfAttention layer on x (B, F, d_in): w_q, w_k, w_v (and w_res, when
+    use_residual and d_in != A) the (A, d_in) weights of W_q, W_k, W_v (and W_res); gamma, beta (A) the LayerNorm's
+    weight and bias (None: no LayerNorm).  dropout > 0: the attention weights take the mask of layer `layer` of
+    `snapshot` (dropout_snapshot; None: a snapshot of its own).  want_aux: also write out's GEMM operand copy for a
+    following layer's projection GEMM."""
+    _require_cuda(x, w_q, w_k, w_v, w_res, gamma, beta)
+    if x.dim() != 3:
+        raise ValueError("self_attention_layer: x%s is not (B, F, d_in)" % (tuple(x.shape),))
+    B, F, din = x.shape
+    A = w_q.shape[0]
+    bound = autoint_bound(F, A, num_heads)
+    if bound is not None:
+        raise NotImplementedError("AutoInt kernels: " + bound)
+    if any(tuple(w.shape) != (A, din) for w in (w_q, w_k, w_v) + ((w_res,) if w_res is not None else ())):
+        raise ValueError("self_attention_layer: x%s and the projection weights %s do not match"
+                         % (tuple(x.shape), [tuple(w.shape) for w in (w_q, w_k, w_v, w_res) if w is not None]))
+    if (gamma is None) != (beta is None) or (gamma is not None and (gamma.numel() != A or beta.numel() != A)):
+        raise ValueError("self_attention_layer: the LayerNorm needs a weight and a bias of %d" % A)
+    if use_residual and w_res is None and din != A:
+        raise ValueError("self_attention_layer: a residual with input_dim %d != attention_dim %d needs w_res"
+                         % (din, A))
+    res_mode = (2 if w_res is not None else 1) if use_residual else 0
+    if not use_residual:
+        w_res = None
+    drop = None
+    if dropout > 0:
+        if snapshot is None:
+            snapshot, layer = dropout_snapshot(x.device, 1), 0
+        drop = (snapshot, layer) + dropout_consts(dropout)
+    scale = float((A // num_heads) ** 0.5) if use_scale else 0.0
+    cfg = (num_heads, scale, float(eps), res_mode, drop, want_aux)
+    return _SelfAttentionLayer.apply(x, cfg, w_q, w_k, w_v, w_res, gamma, beta)
+
+
 class _FsGate(torch.autograd.Function):
     """FinalMLP's gating products f_s = e * (2 g_s), s = 1, 2 (FinalMLP.py, FeatureSelection.forward) in one launch
     (include/fuxictr_b200.h "FinalMLP"), which also writes f1's and f2's auxiliary operands for the towers' first

@@ -21,6 +21,7 @@ Reference files (relative to the reference root):
   MLP_Block                                fuxictr/pytorch/layers/blocks/mlp_block.py:24-96
   FeatureSelection / InteractionAggregation model_zoo/FinalMLP/src/FinalMLP.py
   MaskBlock / SerialMaskNet / ParallelMaskNet model_zoo/MaskNet/src/MaskNet.py
+  MultiHeadSelfAttention                   model_zoo/AutoInt/src/AutoInt.py
 """
 import sys
 from collections import OrderedDict
@@ -966,3 +967,52 @@ class MultiHeadTargetAttention(nn.Module):
         weights = (self.W_q.weight, self.W_k.weight, self.W_v.weight, self.W_o.weight) if self.use_qkvo else ()
         return F2.target_attention(target_item, history_sequence, mask, self.num_heads, self.scale is not None,
                                    *weights)
+
+
+class MultiHeadSelfAttention(nn.Module):
+    """model_zoo/AutoInt/src/AutoInt.py, MultiHeadSelfAttention: field-wise multi-head self-attention with an optional
+    residual (X, or X W_res^T when input_dim != attention_dim), LayerNorm and a final ReLU.  One autograd node per layer
+    (functional._SelfAttentionLayer): one GEMM on the stacked [W_q; W_k; W_v (; W_res)] and one row kernel that never
+    writes the (B, H, F, F) attention weights.  The constructor, its assert, the children (`dot_attention` is the
+    ScaledDotProductAttention mirror and holds the dropout), their registration order and initial draws are the
+    reference's."""
+
+    def __init__(self, input_dim, attention_dim=None, num_heads=1, dropout_rate=0., use_residual=True,
+                 use_scale=False, layer_norm=False):
+        super(MultiHeadSelfAttention, self).__init__()
+        if attention_dim is None:
+            attention_dim = input_dim
+        assert attention_dim % num_heads == 0, \
+            "attention_dim={} is not divisible by num_heads={}".format(attention_dim, num_heads)
+        bound = F2.autoint_bound(1, attention_dim, num_heads)
+        if bound is not None:
+            raise NotImplementedError("MultiHeadSelfAttention kernels: " + bound)
+        self.head_dim = attention_dim // num_heads
+        self.num_heads = num_heads
+        self.use_residual = use_residual
+        self.scale = self.head_dim ** 0.5 if use_scale else None
+        self.W_q = nn.Linear(input_dim, attention_dim, bias=False)
+        self.W_k = nn.Linear(input_dim, attention_dim, bias=False)
+        self.W_v = nn.Linear(input_dim, attention_dim, bias=False)
+        if self.use_residual and input_dim != attention_dim:
+            self.W_res = nn.Linear(input_dim, attention_dim, bias=False)
+        else:
+            self.W_res = None
+        self.dot_attention = ScaledDotProductAttention(dropout_rate)
+        self.layer_norm = nn.LayerNorm(attention_dim) if layer_norm else None
+
+    def forward(self, X, snapshot=None, layer=0, want_aux=False):
+        """X (B, F, input_dim) -> (B, F, attention_dim).  In training mode with dropout the attention weights take the
+        mask of layer `layer` of `snapshot` (functional.dropout_snapshot; None: one of its own).  want_aux: also write
+        the output's GEMM operand copy for a following layer."""
+        drop = self.dot_attention.dropout
+        p = drop.p if (drop is not None and self.training) else 0.0
+        ln = self.layer_norm
+        return F2.self_attention_layer(X, self.W_q.weight, self.W_k.weight, self.W_v.weight,
+                                       self.W_res.weight if self.W_res is not None else None,
+                                       num_heads=self.num_heads, use_residual=self.use_residual,
+                                       use_scale=self.scale is not None,
+                                       gamma=ln.weight if ln is not None else None,
+                                       beta=ln.bias if ln is not None else None,
+                                       eps=ln.eps if ln is not None else 1e-5, dropout=p, snapshot=snapshot,
+                                       layer=layer, want_aux=want_aux)

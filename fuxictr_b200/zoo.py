@@ -16,6 +16,7 @@ same RNG consumption) and nothing else.
   FinalMLP     model_zoo/FinalMLP/src/FinalMLP.py
   DualMLP      model_zoo/FinalMLP/src/DualMLP.py
   MaskNet      model_zoo/MaskNet/src/MaskNet.py
+  AutoInt      model_zoo/AutoInt/src/AutoInt.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -26,7 +27,7 @@ from torch import nn
 
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
-                     SerialMaskNet, ParallelMaskNet,
+                     SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -175,7 +176,7 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet) may be sharded: any other forward
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt) may be sharded: any other forward
         would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
@@ -183,7 +184,7 @@ class RankModel(nn.Module):
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
                                       "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
-                                      "DualMLP and MaskNet" % type(self).__name__)
+                                      "DualMLP, MaskNet and AutoInt" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -743,6 +744,90 @@ class MaskNet(RankModel):
 
     def forward(self, inputs):
         return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class AutoInt(RankModel):
+    """model_zoo/AutoInt/src/AutoInt.py, AutoInt (AutoInt+ with a DNN): a stack of MultiHeadSelfAttention layers over
+    the field embeddings, y = sigmoid(fc(flatten(attention(E))) [+ dnn(flatten(E))] [+ LR(X)]).  Each attention layer
+    is one projection GEMM and one row kernel (layers.MultiHeadSelfAttention); in training mode with net_dropout the
+    layers draw their attention-weight masks from one dropout snapshot.  An empty dnn_hidden_units builds no DNN, as
+    in the reference.  Unknown keyword arguments are accepted and ignored, as the reference's **kwargs are."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="AutoInt", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 dnn_hidden_units=[64, 64, 64], dnn_activations="ReLU", attention_layers=2, num_heads=1,
+                 attention_dim=8, net_dropout=0, batch_norm=False, layer_norm=False, use_scale=False,
+                 use_wide=False, use_residual=True, embedding_regularizer=None, net_regularizer=None, **kwargs):
+        assert attention_dim % num_heads == 0, \
+            "attention_dim={} is not divisible by num_heads={}".format(attention_dim, num_heads)
+        bound = F2.autoint_bound(feature_map.num_fields, attention_dim, num_heads)
+        if bound is not None:
+            raise NotImplementedError("AutoInt kernels: " + bound)
+        super(AutoInt, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                      embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                      **kwargs)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.lr_layer = LogisticRegression(feature_map, use_bias=False) if use_wide else None
+        self.dnn = MLP_Block(input_dim=feature_map.sum_emb_out_dim(), output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=None, dropout_rates=net_dropout,
+                             batch_norm=batch_norm) if dnn_hidden_units else None
+        self.self_attention = nn.Sequential(
+            *[MultiHeadSelfAttention(embedding_dim if i == 0 else attention_dim, attention_dim=attention_dim,
+                                     num_heads=num_heads, dropout_rate=net_dropout, use_residual=use_residual,
+                                     use_scale=use_scale, layer_norm=layer_norm)
+              for i in range(attention_layers)])
+        self.fc = nn.Linear(feature_map.num_fields * attention_dim, 1)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which AutoInt does not have: with use_wide the sharded
+        front's logit is the LR term alone."""
+        if want_fm:
+            raise ValueError("AutoInt has no FM term: enable_sharding(..., want_fm=False)")
+        return super(AutoInt, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype,
+                                                    want_fm=False)
+
+    def _front(self, inputs):
+        """(feature_emb (B, F, D), LR logit or None)."""
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables (and LR), P2P push/pull
+            from .sharded import sharded_front
+            feature_emb, logit = sharded_front(self._sharded_front, self._batch_matrix(inputs))
+            return feature_emb, (logit if self.lr_layer is not None else None)
+        X = self.get_inputs(inputs)
+        if self.lr_layer is None:
+            return self.embedding_layer(X), None
+        fused = fused_front(self.embedding_layer, self.lr_layer, X, want_fm=False)
+        if fused is not None:     # gather + LR in one launch
+            return fused
+        return self.embedding_layer(X), self.lr_layer(X)
+
+    def attention(self, feature_emb):
+        """The self-attention stack on (B, F, D)."""
+        mods = list(self.self_attention)
+        snap = None
+        if mods and self.training and mods[0].dot_attention.dropout is not None:
+            snap = F2.dropout_snapshot(feature_emb.device, len(mods))
+        x = feature_emb
+        for i, m in enumerate(mods):
+            x = m(x, snapshot=snap, layer=i, want_aux=i + 1 < len(mods))
+        return x
+
+    def forward_logits(self, inputs):
+        feature_emb, lr_logit = self._front(inputs)
+        attention_out = self.attention(feature_emb)
+        terms = [F2.linear_act(attention_out.flatten(start_dim=1), self.fc.weight, self.fc.bias)]
+        if self.dnn is not None:
+            terms.append(self.dnn(feature_emb.flatten(start_dim=1)))
+        if lr_logit is not None:
+            terms.append(lr_logit)
+        return tuple(terms)
+
+    def forward(self, inputs):
+        terms = self.forward_logits(inputs)
+        y_pred = terms[0]
+        for t in terms[1:]:
+            y_pred = y_pred + t
+        return {"y_pred": self.output_activation(y_pred)}
 
 
 class DLRM(RankModel):

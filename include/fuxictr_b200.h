@@ -529,6 +529,51 @@ B2_API int b2_mask_row_bwd(const float* z, const float* mean, const float* rstd,
 B2_API int b2_mask_mul(const float* a, const float* b, int64_t n, float* out, int accumulate, void* stream);
 
 /*
+ * AutoInt's multi-head field self-attention (model_zoo/AutoInt/src/AutoInt.py, MultiHeadSelfAttention), one layer on
+ * X (B, F, d_in):
+ *   Z = concat_h dropout(softmax(Q_h K_h^T [/ scale])) V_h + R,   out = ReLU(LN(Z))   (LN optional)
+ * with Q, K, V = X W_q^T, X W_k^T, X W_v^T of width A = attention_dim, H heads of width dh = A / H, scale = sqrt(dh)
+ * or 0 (no scaling), and R = X (res_mode 1, d_in == A), X W_res^T (res_mode 2) or 0 (res_mode 0).  All row-major
+ * fp32; NP = 4A with W_res, 3A without:
+ *   Wp (NP, d_in) K-major: rows 0 .. A-1 W_q, A .. 2A-1 W_k, 2A .. 3A-1 W_v, 3A .. 4A-1 W_res
+ *   P  (B F, NP) = X Wp^T (the caller's GEMM): columns [Q | K | V | X W_res^T] per field row
+ *   dP (B F, NP): [dQ | dK | dV | dR]; dX = dP Wp (+ dR for an identity residual) and dWp = dP^T X (the caller's
+ *     GEMMs)
+ * Saved for the backward: P, X, out, the softmax max and sum per (b, h, i) (stat_max, stat_sum (B, H, F)) and with
+ * LayerNorm its mean and rstd per row (ln_mean, ln_rstd (B F)).  No (B, H, F, F) tensor is stored: the backward
+ * recomputes the probabilities.  Dropout (drop_rng != NULL) drops attention weight (b, h, i, j) with the mask of
+ * "Dropout masks" over the (B H F, F) weights at counter offset snapshot offset + drop_layer.  LayerNorm is
+ * nn.LayerNorm(A)'s (mean first, then the biased variance from the centred values, eps inside the square root).
+ * Range: 1 <= F <= B2_AUTOINT_MAX_FIELDS, 1 <= A <= B2_AUTOINT_MAX_DIM, any H dividing A, d_in >= 1, batch >= 0
+ * (0: no launch) with batch F 4A < 2^31.  A % 4 == 0 with a 16-byte aligned P stages through float4 loads, anything
+ * else through scalar ones.  Outside the range, or given a NULL pointer, every entry point returns B2_E_INVALID.
+ * b2_autoint_pack:   Wp "=" from W_q, W_k, W_v and W_res (NULL: none); one launch.
+ * b2_autoint_fwd:    out (B F, A) "="; out_aux (optional, row pitch ld_aux) receives out's GEMM operand copy for the
+ *   next layer: its bf16 rounding (aux_dtype B2_BF16) or its 3xTF32 small part (B2_F32); the statistics "=".
+ * b2_autoint_bwd:    dP "=" (+ dp_aux as out_aux, row width NP) from the output gradient g (B F, A) and the saved
+ *   tensors; gres (B F, A) "=" dR for an identity residual; dgamma, dbeta (A) "+=" (caller zeroes): a per-CTA sum,
+ *   then one float atomic per column and CTA.
+ * b2_autoint_unpack: gW_q, gW_k, gW_v (, gW_res) (A, d_in) "=" from dWp.
+ */
+#define B2_AUTOINT_MAX_FIELDS 64
+#define B2_AUTOINT_MAX_DIM 64
+B2_API int b2_autoint_pack(const float* Wq, const float* Wk, const float* Wv, const float* Wres, int din, int A,
+                           float* Wp, void* stream);
+B2_API int b2_autoint_fwd(const float* P, const float* X, int64_t batch, int fields, int din, int A, int heads,
+                          int res_mode, float scale, const float* gamma, const float* beta, float eps,
+                          const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale,
+                          float* out, void* out_aux, int aux_dtype, int64_t ld_aux, float* stat_max, float* stat_sum,
+                          float* ln_mean, float* ln_rstd, void* stream);
+B2_API int b2_autoint_bwd(const float* P, const float* X, const float* out, const float* g, const float* stat_max,
+                          const float* stat_sum, const float* ln_mean, const float* ln_rstd, int64_t batch,
+                          int fields, int din, int A, int heads, int res_mode, float scale, const float* gamma,
+                          const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale,
+                          float* dP, void* dp_aux, int aux_dtype, int64_t ld_aux, float* gres, float* dgamma,
+                          float* dbeta, void* stream);
+B2_API int b2_autoint_unpack(const float* dWp, int din, int A, float* gWq, float* gWk, float* gWv, float* gWres,
+                             void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
