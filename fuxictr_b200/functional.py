@@ -1698,6 +1698,237 @@ def self_attention_layer(x, w_q, w_k, w_v, w_res=None, num_heads=1, use_residual
     return _SelfAttentionLayer.apply(x, cfg, w_q, w_k, w_v, w_res, gamma, beta)
 
 
+# --------------------------------------------------------------------------------------
+# WuKong (include/fuxictr_b200.h "WuKong")
+# --------------------------------------------------------------------------------------
+def wukong_bound(fields, out_fields, embedding_dim, rank_k):
+    """None when the WuKong row kernels cover a layer of `fields` input and `out_fields` output fields, embedding_dim
+    D and rank k, else the bound it breaks."""
+    if rank_k is None:
+        return "fmp_rank_k=None (the vanilla FM, F^2 wide) is not implemented; give a rank"
+    for name, v, hi in (("the number of input fields", fields, _lib.B2_WUKONG_MAX_FIELDS),
+                        ("lcb_features + fmb_features", out_fields, _lib.B2_WUKONG_MAX_FIELDS),
+                        ("embedding_dim", embedding_dim, _lib.B2_WUKONG_MAX_DIM),
+                        ("fmp_rank_k", rank_k, _lib.B2_WUKONG_MAX_RANK)):
+        if not 1 <= v <= hi:
+            return "%s must lie in [1, %d], got %d" % (name, hi, v)
+    if fields * rank_k > _lib.B2_WUKONG_MAX_FM_WIDTH:
+        return "input fields * fmp_rank_k must be at most %d, got %d" % (_lib.B2_WUKONG_MAX_FM_WIDTH, fields * rank_k)
+    return None
+
+
+def wukong_pitch(fields):
+    """The field pitch of a WuKong layer's X' (B D, fp): fields rounded up to a multiple of 4."""
+    return (fields + 3) // 4 * 4
+
+
+def _wukong_tc_shape(n, k):
+    """True when a field-axis GEMM with a stacked weight of (n, k) would take the tensor cores (_tc_layer_ok)."""
+    return _MATMUL["mode"] != "fp32" and n >= 16 and k >= 16 and n % 4 == 0 and k % 4 == 0
+
+
+class _WuKongFM(torch.autograd.Function):
+    """The factorization-machine half of a WuKong layer (WuKong.py, FactorizationMachineBlock.optimized_fm and its
+    LayerNorm), one launch each way (b2_wukong_fm_fwd / _bwd): fm = LN(flatten(x (x^T Y))).  Layout 0 reads the
+    embedding (B, F, D) and also returns X'_0 (B D, fp), the layer's field-axis GEMM operand; layout 1 reads X' (a
+    shared_grad view) and adds its gradient into the sink's buffer."""
+
+    @staticmethod
+    def forward(ctx, x, sink, cfg, Y, gamma, beta):
+        layout, F, D, k, eps, fm_aux_on, xp_aux_on = cfg
+        ctx.set_materialize_grads(False)
+        ctx.params, ctx.sink, ctx.cfg = (Y, gamma, beta), sink, cfg
+        B = x.shape[0] if layout == 0 else x.shape[0] // D
+        dev = x.device
+        fp = wukong_pitch(F)
+        fm = torch.empty((B, F * k), dtype=torch.float32, device=dev)
+        xp = torch.empty((B * D, fp), dtype=torch.float32, device=dev) if layout == 0 else None
+        ctx.B = B
+        if B == 0:
+            ctx.save_for_backward(x, None, None)
+            return (fm, xp) if layout == 0 else fm
+        fm_aux = empty_aux(B, F * k, dev) if fm_aux_on else None
+        xp_aux = empty_aux(B * D, fp, dev) if (xp_aux_on and xp is not None) else None
+        mean = torch.empty(B, dtype=torch.float32, device=dev)
+        rstd = torch.empty_like(mean)
+        _lib.call("b2_wukong_fm_fwd", _ptr(x), layout, B, F, D, k, _ptr(_f32c(Y)), _ptr(gamma), _ptr(beta), eps,
+                  _ptr(fm), *_aux_args(fm_aux), _ptr(xp), _ptr(xp_aux), xp_aux.stride(0) if xp_aux is not None else 0,
+                  _ptr(mean), _ptr(rstd), _stream())
+        for t, aux in ((fm, fm_aux), (xp, xp_aux)):
+            if aux is not None:         # the consuming GEMM's make_aux finds it
+                t._b2_aux = (_MATMUL["mode"], aux, t._version)
+        ctx.save_for_backward(x, mean, rstd)
+        return (fm, xp) if layout == 0 else fm
+
+    @staticmethod
+    def backward(ctx, g, gxp=None):
+        layout, F, D, k, _, _, _ = ctx.cfg
+        Y, gamma, beta = ctx.params
+        x, mean, rstd = ctx.saved_tensors
+        gY, dgamma, dbeta = (_grad_buffer(p, zero=True) for p in (Y, gamma, beta))
+        if layout == 0:
+            gx, acc = torch.zeros_like(x) if ctx.B == 0 else torch.empty_like(x), False
+        else:
+            gx, acc = ctx.sink.target(x)
+        if ctx.B > 0:
+            if g is None:
+                g = torch.zeros((ctx.B, F * k), dtype=torch.float32, device=x.device)
+            _lib.call("b2_wukong_fm_bwd", _ptr(x), layout, ctx.B, F, D, k, _ptr(_f32c(Y)), _ptr(gamma), _ptr(mean),
+                      _ptr(rstd), _ptr(_f32c(g)), _ptr(_f32c(gxp) if gxp is not None else None), _ptr(gx),
+                      1 if acc else 0, _ptr(gY), _ptr(dgamma), _ptr(dbeta), _stream())
+        elif layout == 1 and not acc:
+            gx.zero_()
+        return (gx if layout == 0 else None, None, None, gY, dgamma, dbeta)
+
+
+class _WuKongMix(torch.autograd.Function):
+    """The rest of a WuKong layer (WuKong.py, WuKongLayer.forward after the FMB's MLP): one field-axis GEMM
+    C = X' Ws^T + bs on Ws = [W_lcb; W_res] (packed by b2_wukong_pack with a projection residual or an X' pitch wider
+    than F; W_lcb itself otherwise) and one row kernel (b2_wukong_out_fwd) that forms cat(FMB, LCB) + residual and the
+    LayerNorm(D), writing the next layer's X' or, for the last layer, the (B, Fo D) flatten.  Backward: the row kernel
+    (b2_wukong_out_bwd) writes the MLP output's gradient, dC and, for an identity residual, X''s gradient; the dgrad
+    adds dC Ws into it, the wgrad forms dWs = dC^T X' (split by b2_wukong_unpack when packed).  X''s gradient goes into
+    the sink's buffer (a shared_grad view), or is returned (layer 0, whose FM node takes it)."""
+
+    @staticmethod
+    def forward(ctx, xp, sink, mlp_out, cfg, W_lcb, W_res, b_res, gamma, beta):
+        B, F, D, lcb, fmb, eps, last, want_aux = cfg
+        ctx.set_materialize_grads(False)
+        ctx.params, ctx.sink, ctx.cfg = (W_lcb, W_res, b_res, gamma, beta), sink, cfg
+        Fo = lcb + fmb
+        fpi, fpo = wukong_pitch(F), wukong_pitch(Fo)
+        dev = xp.device
+        proj = W_res is not None
+        N = lcb + (Fo if proj else 0)
+        out = torch.empty((B, Fo * D) if last else (B * D, fpo), dtype=torch.float32, device=dev)
+        packed = proj or fpi != F
+        ctx.shape = (N, fpi, packed)
+        if B == 0:
+            ctx.tc = False
+            ctx.save_for_backward(xp, None, None, None, None, None)
+            return out
+        if packed:
+            Ws = torch.empty((N, fpi), dtype=torch.float32, device=dev)
+            bs = torch.empty(N, dtype=torch.float32, device=dev) if proj else None
+            _lib.call("b2_wukong_pack", _ptr(_f32c(W_lcb)), _ptr(_f32c(W_res) if proj else None),
+                      _ptr(_f32c(b_res) if proj else None), F, lcb, Fo, _ptr(Ws), _ptr(bs), _stream())
+        else:
+            Ws, bs = _f32c(W_lcb), None
+        tc = _tc_layer_ok(Ws) and xp.data_ptr() % 16 == 0
+        x_aux = make_aux(xp) if tc else None
+        ws_aux = (make_aux(Ws) if packed else weight_aux(Ws)) if tc else None
+        C = torch.empty((B * D, N), dtype=torch.float32, device=dev)
+        _linear_fwd(tc, xp, x_aux, Ws, C, ws_aux, bias=bs)
+        out_aux = (empty_aux(B, Fo * D, dev) if last else empty_aux(B * D, fpo, dev)) if want_aux else None
+        ln = gamma is not None
+        mean = torch.empty(B * Fo, dtype=torch.float32, device=dev) if ln else None
+        rstd = torch.empty_like(mean) if ln else None
+        _lib.call("b2_wukong_out_fwd", _ptr(mlp_out), _ptr(C), _ptr(xp), B, F, D, lcb, fmb, 2 if proj else 1,
+                  _ptr(gamma), _ptr(beta), eps, 0 if last else 1, _ptr(out), *_aux_args(out_aux), _ptr(mean),
+                  _ptr(rstd), _stream())
+        if out_aux is not None:
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        ctx.save_for_backward(xp, mlp_out, C, Ws, mean, rstd)
+        ctx.tc, ctx.aux = tc, (x_aux, ws_aux)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        B, F, D, lcb, fmb, _, last, _ = ctx.cfg
+        W_lcb, W_res, b_res, gamma, beta = ctx.params
+        xp, mlp_out, C, Ws, mean, rstd = ctx.saved_tensors
+        N, fpi, packed = ctx.shape
+        proj, ln = W_res is not None, gamma is not None
+        sink = ctx.sink
+        dev = xp.device
+        if sink is not None:
+            gx, acc = sink.target(xp)
+        else:
+            gx, acc = torch.empty_like(xp), False
+        dgamma = _grad_buffer(gamma, zero=True) if ln else None
+        dbeta = _grad_buffer(beta, zero=True) if ln else None
+        dbias = _grad_buffer(b_res, zero=True) if proj else None
+        gW_lcb = _grad_buffer(W_lcb, zero=False)
+        gW_res = _grad_buffer(W_res, zero=False) if proj else None
+        g_mlp = torch.zeros((B, fmb * D), dtype=torch.float32, device=dev) if B == 0 else \
+            torch.empty((B, fmb * D), dtype=torch.float32, device=dev)
+        if B == 0 or g is None:
+            if not acc:
+                gx.zero_()
+            g_mlp.zero_()
+            gW_lcb.zero_()
+            if proj:
+                gW_res.zero_()
+            return (gx if sink is None else None, None, g_mlp, None, gW_lcb, gW_res, dbias, dgamma, dbeta)
+        x_aux, ws_aux = ctx.aux
+        tc = ctx.tc
+        dC = torch.empty((B * D, N), dtype=torch.float32, device=dev)
+        dc_aux = empty_aux(B * D, N, dev) if tc else None
+        _lib.call("b2_wukong_out_bwd", _ptr(mlp_out), _ptr(C), _ptr(xp), B, F, D, lcb, fmb, 2 if proj else 1,
+                  _ptr(gamma), _ptr(mean), _ptr(rstd), 0 if last else 1, _ptr(_f32c(g)), _ptr(g_mlp), _ptr(dC),
+                  *_aux_args(dc_aux), _ptr(gx if not proj else None), 1 if acc else 0, _ptr(dbias), _ptr(dgamma),
+                  _ptr(dbeta), _stream())
+        _linear_dgrad(tc, dC, dc_aux, Ws, gx, ws_aux, accumulate=acc or not proj)               # dX' (+)= dC Ws
+        if packed:
+            dWs = torch.empty_like(Ws)
+            _linear_wgrad(tc, dC, dc_aux, xp, x_aux, dWs)                                        # dWs = dC^T X'
+            _lib.call("b2_wukong_unpack", _ptr(dWs), F, lcb, lcb + fmb, _ptr(gW_lcb), _ptr(gW_res), _stream())
+        else:
+            _linear_wgrad(tc, dC, dc_aux, xp, x_aux, gW_lcb)
+        return (gx if sink is None else None, None, g_mlp, None, gW_lcb, gW_res, dbias, dgamma, dbeta)
+
+
+def wukong_layer(x, proj_Y, fm_gamma, fm_beta, mlp, W_lcb, W_res=None, b_res=None, gamma=None, beta=None,
+                 fm_eps=1e-5, eps=1e-5, embedding_dim=None, sink=None, last=True, fm_aux=False, want_aux=False):
+    """One WuKong layer.  x: the embedding (B, F, D), or X' (B D, fp) as a shared_grad view with its sink and
+    embedding_dim given (the previous layer's output with last=False).  proj_Y (F, k), fm_gamma, fm_beta (F k): the
+    FMB's projection and LayerNorm; mlp: the FMB's MLP, a callable (B, F k) -> (B, fmb D); W_lcb (lcb, F): the LCB's
+    weight; W_res (Fo, F), b_res (Fo): the residual projection (None: the identity, F == Fo); gamma, beta (D): the
+    output LayerNorm (None: none).  Returns the (B, Fo D) flatten [b, f, d] when last, else X' (B D, fpo) for the
+    next layer.  fm_aux: write the MLP input's GEMM operand copy; want_aux: the output's, for the GEMM that reads it."""
+    _require_cuda(x, proj_Y, fm_gamma, fm_beta, W_lcb, W_res, b_res, gamma, beta)
+    F, k = proj_Y.shape
+    lcb = W_lcb.shape[0]
+    if sink is None:
+        if x.dim() != 3 or x.shape[1] != F:
+            raise ValueError("wukong_layer: x%s is not (B, %d, D)" % (tuple(x.shape), F))
+        B, _, D = x.shape
+        layout = 0
+    else:
+        D = embedding_dim
+        if D is None or x.dim() != 2 or x.shape[1] != wukong_pitch(F) or x.shape[0] % D:
+            raise ValueError("wukong_layer: X'%s is not (B * %s, %d)" % (tuple(x.shape), D, wukong_pitch(F)))
+        B = x.shape[0] // D
+        layout = 1
+    if W_res is not None:
+        Fo = W_res.shape[0]
+    else:
+        Fo = F
+    fmb = Fo - lcb
+    bound = wukong_bound(F, Fo, D, k)
+    if bound is not None:
+        raise NotImplementedError("WuKong kernels: " + bound)
+    if fmb < 1 or tuple(W_lcb.shape) != (lcb, F) or fm_gamma.numel() != F * k or fm_beta.numel() != F * k \
+            or (W_res is not None and (tuple(W_res.shape) != (Fo, F) or b_res is None or b_res.numel() != Fo)):
+        raise ValueError("wukong_layer: shapes x%s proj_Y%s W_lcb%s W_res%s do not match"
+                         % (tuple(x.shape), tuple(proj_Y.shape), tuple(W_lcb.shape),
+                            tuple(W_res.shape) if W_res is not None else None))
+    if (gamma is None) != (beta is None) or (gamma is not None and (gamma.numel() != D or beta.numel() != D)):
+        raise ValueError("wukong_layer: the output LayerNorm needs a weight and a bias of %d" % D)
+    N = lcb + (Fo if W_res is not None else 0)
+    x = _f32c(x)
+    cfg = (layout, F, D, k, float(fm_eps), fm_aux, layout == 0 and _wukong_tc_shape(N, wukong_pitch(F)))
+    if layout == 0:
+        fm, xp = _WuKongFM.apply(x, None, cfg, proj_Y, fm_gamma, fm_beta)
+    else:
+        fm, xp = _WuKongFM.apply(x, sink, cfg, proj_Y, fm_gamma, fm_beta), x
+    mlp_out = _f32c(mlp(fm)) if B > 0 else fm.new_zeros((0, fmb * D))     # an empty batch: nothing to multiply
+    if tuple(mlp_out.shape) != (B, fmb * D):
+        raise ValueError("wukong_layer: the FMB's MLP returned %s, not (%d, %d)" % (tuple(mlp_out.shape), B, fmb * D))
+    cfg = (B, F, D, lcb, fmb, float(eps), bool(last), want_aux)
+    return _WuKongMix.apply(xp, sink, mlp_out, cfg, W_lcb, W_res, b_res, gamma, beta)
+
+
 class _FsGate(torch.autograd.Function):
     """FinalMLP's gating products f_s = e * (2 g_s), s = 1, 2 (FinalMLP.py, FeatureSelection.forward) in one launch
     (include/fuxictr_b200.h "FinalMLP"), which also writes f1's and f2's auxiliary operands for the towers' first

@@ -22,6 +22,7 @@ Reference files (relative to the reference root):
   FeatureSelection / InteractionAggregation model_zoo/FinalMLP/src/FinalMLP.py
   MaskBlock / SerialMaskNet / ParallelMaskNet model_zoo/MaskNet/src/MaskNet.py
   MultiHeadSelfAttention                   model_zoo/AutoInt/src/AutoInt.py
+  FactorizationMachineBlock / LinearCompressionBlock / WuKongLayer model_zoo/WuKong/src/WuKong.py
 """
 import sys
 from collections import OrderedDict
@@ -1016,3 +1017,94 @@ class MultiHeadSelfAttention(nn.Module):
                                        beta=ln.bias if ln is not None else None,
                                        eps=ln.eps if ln is not None else 1e-5, dropout=p, snapshot=snapshot,
                                        layer=layer, want_aux=want_aux)
+
+
+class FactorizationMachineBlock(nn.Module):
+    """model_zoo/WuKong/src/WuKong.py, FactorizationMachineBlock: the rank-k FM x (x^T proj_Y), its LayerNorm over
+    F k and an MLP to fmb D with a ReLU output.  The constructor, its draws (proj_Y = randn(F, k), then the MLP's
+    Linears), the children and their registration order are the reference's; the forward runs inside
+    WuKongLayer.forward (functional.wukong_layer).  rank_k=None (the vanilla FM, F^2 wide) is refused."""
+
+    def __init__(self, input_features=16, output_features=16, embedding_dim=16, rank_k=8, mlp_hidden_units=[16, 16],
+                 mlp_hidden_activations="relu", mlp_dropout=0):
+        super(FactorizationMachineBlock, self).__init__()
+        if rank_k is None:
+            raise NotImplementedError("FactorizationMachineBlock kernels: " + F2.wukong_bound(input_features,
+                                                                                              output_features, 1, None))
+        self.embedding_dim = embedding_dim
+        self.output_features = output_features
+        self.rank_k = rank_k
+        self.input_features = input_features
+        self.proj_Y = nn.Parameter(torch.randn(self.input_features, self.rank_k))
+        fm_out_dim = input_features * rank_k
+        self.layer_norm = nn.LayerNorm(fm_out_dim)
+        self.mlp = MLP_Block(input_dim=fm_out_dim, output_dim=output_features * embedding_dim,
+                             hidden_units=mlp_hidden_units, hidden_activations=mlp_hidden_activations,
+                             output_activation="relu", dropout_rates=mlp_dropout)
+
+    def first_linear(self):
+        return next(m for m in self.mlp.mlp if type(m) == nn.Linear)
+
+
+class LinearCompressionBlock(nn.Module):
+    """model_zoo/WuKong/src/WuKong.py, LinearCompressionBlock: Linear(F -> lcb, bias=False) over the field axis; it
+    runs as the LCB columns of WuKongLayer's field-axis GEMM."""
+
+    def __init__(self, input_features=16, output_features=8):
+        super(LinearCompressionBlock, self).__init__()
+        self.linear = nn.Linear(input_features, output_features, bias=False)
+
+
+class WuKongLayer(nn.Module):
+    """model_zoo/WuKong/src/WuKong.py, WuKongLayer: out = [LayerNorm(D)](cat(FMB(x), LCB(x)) + residual), the residual
+    x itself or, when input_features != lcb + fmb, residual_proj over the field axis.  Constructor, children, their
+    registration order and draws are the reference's.  One layer is the FM row kernel, the FMB's MLP, one field-axis
+    GEMM and the combine row kernel (functional.wukong_layer); between layers of a stack the activations stay in the
+    (B D, fp) layout (forward_stack)."""
+
+    def __init__(self, input_features=16, lcb_features=8, fmb_features=8, embedding_dim=16, fmp_rank_k=4,
+                 fmb_mlp_units=[16, 16], fmb_mlp_activations="relu", fmb_dropout=0.1, layer_norm=True):
+        super(WuKongLayer, self).__init__()
+        bound = F2.wukong_bound(input_features, lcb_features + fmb_features, embedding_dim, fmp_rank_k)
+        if bound is None and (lcb_features < 1 or fmb_features < 1):
+            bound = "lcb_features and fmb_features must be at least 1, got %d and %d" % (lcb_features, fmb_features)
+        if bound is not None:
+            raise NotImplementedError("WuKongLayer kernels: " + bound)
+        self.fmb = FactorizationMachineBlock(input_features, fmb_features, embedding_dim, fmp_rank_k, fmb_mlp_units,
+                                             fmb_mlp_activations, fmb_dropout)
+        self.lcb = LinearCompressionBlock(input_features, lcb_features)
+        self.layer_norm = nn.LayerNorm(embedding_dim) if layer_norm else None
+        if input_features != lcb_features + fmb_features:
+            self.residual_proj = nn.Linear(input_features, lcb_features + fmb_features)
+
+    def run(self, x, sink=None, last=True, want_aux=False):
+        """functional.wukong_layer on x (the embedding (B, F, D), or X' with its shared_grad sink)."""
+        fmb, ln = self.fmb, self.layer_norm
+        res = getattr(self, "residual_proj", None)
+        return F2.wukong_layer(x, fmb.proj_Y, fmb.layer_norm.weight, fmb.layer_norm.bias, fmb.mlp,
+                               self.lcb.linear.weight, res.weight if res is not None else None,
+                               res.bias if res is not None else None, ln.weight if ln is not None else None,
+                               ln.bias if ln is not None else None, fm_eps=fmb.layer_norm.eps,
+                               eps=ln.eps if ln is not None else 1e-5, embedding_dim=fmb.embedding_dim, sink=sink,
+                               last=last, fm_aux=F2._tc_layer_ok(fmb.first_linear().weight), want_aux=want_aux)
+
+    def forward(self, x):
+        """x (B, F, D) -> (B, lcb + fmb, D)."""
+        out = self.run(x)
+        return out.view(x.shape[0], -1, self.fmb.embedding_dim)
+
+
+def wukong_stack(layers, feature_emb, want_aux=False):
+    """The WuKong layers `layers` on feature_emb (B, F, D) -> the last layer's (B, Fo D) flatten [b, f, d].  Between
+    layers the activations stay as X' (B D, fp), whose gradient is one buffer (functional.shared_grad) that the
+    combine backward, the dgrad and the FM backward all add into.  want_aux: the flatten's GEMM operand copy."""
+    x, sink = feature_emb, None
+    for i, layer in enumerate(layers):
+        last = i + 1 == len(layers)
+        if last:
+            return layer.run(x, sink, last=True, want_aux=want_aux)
+        nxt = layers[i + 1]
+        res = getattr(nxt, "residual_proj", None)
+        n = nxt.lcb.linear.weight.shape[0] + (res.weight.shape[0] if res is not None else 0)
+        x = layer.run(x, sink, last=False, want_aux=F2._wukong_tc_shape(n, F2.wukong_pitch(nxt.fmb.input_features)))
+        x, sink = F2.shared_grad(x)

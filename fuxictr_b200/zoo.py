@@ -17,6 +17,7 @@ same RNG consumption) and nothing else.
   DualMLP      model_zoo/FinalMLP/src/DualMLP.py
   MaskNet      model_zoo/MaskNet/src/MaskNet.py
   AutoInt      model_zoo/AutoInt/src/AutoInt.py
+  WuKong       model_zoo/WuKong/src/WuKong.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -27,7 +28,7 @@ from torch import nn
 
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
-                     SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention,
+                     SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -176,15 +177,15 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt) may be sharded: any other forward
-        would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong) may be sharded: any
+        other forward would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
         from . import sharded as SH
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
                                       "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
-                                      "DualMLP, MaskNet and AutoInt" % type(self).__name__)
+                                      "DualMLP, MaskNet, AutoInt and WuKong" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -828,6 +829,81 @@ class AutoInt(RankModel):
         for t in terms[1:]:
             y_pred = y_pred + t
         return {"y_pred": self.output_activation(y_pred)}
+
+
+class WuKong(RankModel):
+    """model_zoo/WuKong/src/WuKong.py, WuKong: num_wukong_layers WuKongLayers over the field embeddings, then
+    y = sigmoid(fc(flatten(stack(E)))).  Each layer is the FM row kernel, the FMB's MLP, one field-axis GEMM and the
+    combine row kernel (layers.WuKongLayer); the last layer writes the flatten fc reads.  fc is the reference's
+    MLP_Block (with mlp_batch_norm, torch's BatchNorm1d between our Linears, as every batch_norm MLP runs).  Unknown
+    keyword arguments are accepted and ignored, as the reference's **kwargs are.  Refused: fmp_rank_k=None (the
+    vanilla FM), num_wukong_layers < 1 and shapes outside functional.wukong_bound."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="WuKong", gpu=-1, learning_rate=1e-3, embedding_dim=64,
+                 num_wukong_layers=3, lcb_features=40, fmb_features=40, fmb_mlp_units=[32, 32],
+                 fmb_mlp_activations="relu", fmp_rank_k=8, mlp_hidden_units=[32, 32], mlp_hidden_activations="relu",
+                 mlp_batch_norm=True, layer_norm=True, net_dropout=0, embedding_regularizer=None, net_regularizer=None,
+                 **kwargs):
+        if num_wukong_layers < 1:
+            raise NotImplementedError("WuKong needs num_wukong_layers >= 1, got %d (the reference then builds an fc "
+                                      "for lcb + fmb fields over the embedding's fields)" % num_wukong_layers)
+        output_features = lcb_features + fmb_features
+        for fields in ((feature_map.num_fields, output_features) if num_wukong_layers > 1 or
+                       feature_map.num_fields == output_features else (feature_map.num_fields,)):
+            bound = F2.wukong_bound(fields, output_features, embedding_dim, fmp_rank_k)
+            if bound is not None:
+                raise NotImplementedError("WuKong kernels: " + bound)
+        super(WuKong, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                     embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                     **kwargs)
+        self.embedding_dim = embedding_dim
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.wukong_stack = nn.Sequential(*[
+            WuKongLayer(input_features=feature_map.num_fields if i == 0 else output_features,
+                        lcb_features=lcb_features, fmb_features=fmb_features, embedding_dim=embedding_dim,
+                        fmp_rank_k=fmp_rank_k, fmb_mlp_units=fmb_mlp_units, fmb_mlp_activations=fmb_mlp_activations,
+                        fmb_dropout=net_dropout, layer_norm=layer_norm)
+            for i in range(num_wukong_layers)])
+        self.fc = MLP_Block(input_dim=output_features * embedding_dim, output_dim=1, hidden_units=mlp_hidden_units,
+                            hidden_activations=mlp_hidden_activations, output_activation=self.output_activation,
+                            batch_norm=mlp_batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which WuKong does not have."""
+        if want_fm:
+            raise ValueError("WuKong has no FM term: enable_sharding(..., want_fm=False)")
+        return super(WuKong, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype,
+                                                   want_fm=False)
+
+    def _logit_mlp(self):
+        """fc without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_fc")
+        if ent is None:
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(self.fc.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_fc"] = ent
+        return ent
+
+    def _feature_emb(self, inputs):
+        """The field embeddings (B, F, D), from the row-sharded front after enable_sharding()."""
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull
+            from .sharded import sharded_front
+            return sharded_front(self._sharded_front, self._batch_matrix(inputs))[0]
+        return self.embedding_layer(self.get_inputs(inputs))
+
+    def forward_logits(self, inputs):
+        fc = self._logit_mlp()
+        first = next(m for m in fc.mlp if type(m) == nn.Linear)
+        flat = wukong_stack(list(self.wukong_stack), self._feature_emb(inputs),
+                            want_aux=F2._tc_layer_ok(first.weight) and fc.chain_layers() is not None)
+        return (fc(flat),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
 
 
 class DLRM(RankModel):

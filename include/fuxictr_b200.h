@@ -574,6 +574,64 @@ B2_API int b2_autoint_unpack(const float* dWp, int din, int A, float* gWq, float
                              void* stream);
 
 /*
+ * WuKong's layer (model_zoo/WuKong/src/WuKong.py, WuKongLayer) on x (B, F, D) with rank k, lcb + fmb = Fo output
+ * fields:
+ *   fm   = LN_fk(flatten(x (x^T Y)))                 Y = proj_Y (F, k); LN over F k, always affine
+ *   z    = cat(FMB_MLP(fm).view(B, fmb, D), x W_lcb^T over the field axis) + R,   R = x (F == Fo) or the projection
+ *          x W_res^T + b_res over the field axis
+ *   out  = LN_D(z) per (b, field) (optional, one LayerNorm(D) for all fields)
+ * Layouts, row-major fp32 (fp = F rounded up to a multiple of 4; pad columns are zero where written "="):
+ *   X    (B, F, D)    [b, f, d]: the embedding (layout 0)
+ *   X'   (B D, fp)    [b, d, f]: a layer's input (layout 1); X'_{i+1} is written at fpo = Fo rounded up to 4
+ *   Ws   (N, fp)      [W_lcb; W_res] zero-padded, N = lcb (+ Fo with a projection); bs (N) = [0; b_res]
+ *   C    (B D, N)     = X' Ws^T + bs (the caller's GEMM): columns [LCB out | projection]
+ *   fm   (B, F k)     the FMB MLP's input; mlp (B, fmb D) its output, [b, j, d]
+ *   flat (B, Fo D)    [b, f, d]: the last layer's output (out_layout 0), what the model's fc reads
+ * Range: 1 <= F, Fo <= B2_WUKONG_MAX_FIELDS, 1 <= D <= B2_WUKONG_MAX_DIM, 1 <= k <= B2_WUKONG_MAX_RANK,
+ * F k <= B2_WUKONG_MAX_FM_WIDTH, lcb, fmb >= 1, batch >= 0 (0: no launch) with every (B, row) tensor below 2^31
+ * elements.  X' and a 16-byte aligned X with D % 4 == 0 stage through float4 loads, anything else through scalar
+ * ones.  Outside the range, or given a NULL pointer, every entry point returns B2_E_INVALID.  An aux pointer (optional,
+ * row pitch ld) receives the GEMM operand copy of the tensor written beside it: its bf16 rounding (aux_dtype B2_BF16)
+ * or its 3xTF32 small part (B2_F32).
+ * b2_wukong_fm_fwd:  fm "=" (+ fm_aux) from X (layout 0) or X' (layout 1); ln_mean, ln_rstd (B) "="; layout 0 may
+ *   also write X'_0 "=" (xp_out, + xp_aux).
+ * b2_wukong_fm_bwd:  from g = d fm, recomputing fm: gx "=" (accumulate 0) or "+=" in the input's layout (layout 0
+ *   adds gxp, the gradient of X'_0, transposed); gY, dgamma, dbeta (F k) "+=" (caller zeroes): a per-CTA sum, then
+ *   one float atomic per element and CTA.
+ * b2_wukong_out_fwd: out "=" as X'_{i+1} (out_layout 1) or flat (out_layout 0) (+ out_aux); res_mode 1 reads the
+ *   residual from X' (xp), 2 from C's projection columns; ln_mean, ln_rstd (B Fo) "=" with LayerNorm (gamma != NULL).
+ * b2_wukong_out_bwd: from g in out's layout (g_layout): g_mlp (B, fmb D) "=", dC (B D, N) "=" (+ dc_aux); res_mode 1:
+ *   gxp (B D, fp) "=" or "+=" (accumulate); res_mode 2: dbias (Fo) "+="; dgamma, dbeta (D) "+=" (caller zeroes).
+ * b2_wukong_pack:    Ws "=" and, with W_res, bs "=".
+ * b2_wukong_unpack:  gW_lcb (lcb, F) and, when gW_res != NULL, gW_res (Fo, F) "=" from dWs (N, fp).
+ */
+#define B2_WUKONG_MAX_FIELDS 128
+#define B2_WUKONG_MAX_DIM 128
+#define B2_WUKONG_MAX_RANK 32
+#define B2_WUKONG_MAX_FM_WIDTH 1024
+B2_API int b2_wukong_fm_fwd(const float* x, int layout, int64_t batch, int fields, int D, int k, const float* Y,
+                            const float* gamma, const float* beta, float eps, float* fm_out, void* fm_aux,
+                            int aux_dtype, int64_t ld_aux, float* xp_out, void* xp_aux, int64_t ld_xp_aux,
+                            float* ln_mean, float* ln_rstd, void* stream);
+B2_API int b2_wukong_fm_bwd(const float* x, int layout, int64_t batch, int fields, int D, int k, const float* Y,
+                            const float* gamma, const float* ln_mean, const float* ln_rstd, const float* g,
+                            const float* gxp, float* gx, int accumulate, float* gY, float* dgamma, float* dbeta,
+                            void* stream);
+B2_API int b2_wukong_out_fwd(const float* mlp_out, const float* C, const float* xp, int64_t batch, int fields, int D,
+                             int lcb, int fmb, int res_mode, const float* gamma, const float* beta, float eps,
+                             int out_layout, float* out, void* out_aux, int aux_dtype, int64_t ld_aux, float* ln_mean,
+                             float* ln_rstd, void* stream);
+B2_API int b2_wukong_out_bwd(const float* mlp_out, const float* C, const float* xp, int64_t batch, int fields, int D,
+                             int lcb, int fmb, int res_mode, const float* gamma, const float* ln_mean,
+                             const float* ln_rstd, int g_layout, const float* g, float* g_mlp, float* dC,
+                             void* dc_aux, int aux_dtype, int64_t ld_aux, float* gxp, int accumulate, float* dbias,
+                             float* dgamma, float* dbeta, void* stream);
+B2_API int b2_wukong_pack(const float* W_lcb, const float* W_res, const float* b_res, int fields, int lcb,
+                          int out_fields, float* Ws, float* bs, void* stream);
+B2_API int b2_wukong_unpack(const float* dWs, int fields, int lcb, int out_fields, float* gW_lcb, float* gW_res,
+                            void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
