@@ -342,7 +342,7 @@ class OracleTrainer(object):
     def train_step(self, batch):
         self.optimizer.zero_grad()
         y_pred, y = self.forward(batch)
-        loss = bce_mean(y_pred, y)
+        loss = bce_mean(y_pred, y.to(y_pred.dtype))      # labels in the state's dtype (float64 runs)
         loss.backward()
         torch.nn.utils.clip_grad_norm_(self.params, self.max_norm)
         self.optimizer.step()
