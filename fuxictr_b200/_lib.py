@@ -24,6 +24,8 @@ B2_HEAD_MAX_K = 28672
 B2_MASKNET_MAX_WIDTH = 1024
 B2_AUTOINT_MAX_FIELDS, B2_AUTOINT_MAX_DIM = 64, 64
 B2_WUKONG_MAX_FIELDS, B2_WUKONG_MAX_DIM, B2_WUKONG_MAX_RANK, B2_WUKONG_MAX_FM_WIDTH = 128, 128, 32, 1024
+B2_FINALNET_CONCAT, B2_FINALNET_SUM = 0, 1
+B2_FINALNET_MAX_WIDTH, B2_FINALNET_MAX_FIELDS, B2_FINALNET_MAX_DIM, B2_FINALNET_MAX_GATE_WIDTH = 1024, 128, 128, 8192
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
 c_void_p, c_int, c_int32, c_int64, c_float, c_double = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,
@@ -183,6 +185,18 @@ SIGNATURES = {
                                   c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_wukong_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_wukong_unpack": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_finalnet_fi_fwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_float, c_float, c_int,
+                                   c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, ctypes.c_uint32,
+                                   c_float, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
+    "b2_finalnet_fi_bwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                   c_void_p, c_int, c_int, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p,
+                                   c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_finalnet_gate_fwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                     c_int64, c_void_p]),
+    "b2_finalnet_gate_bwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                     c_void_p, c_void_p, c_void_p]),
+    "b2_finalnet_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
     "b2_mhta_pack":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                              c_void_p, c_void_p]),
     "b2_mhta_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float,

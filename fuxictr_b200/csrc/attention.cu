@@ -9,7 +9,7 @@
 // HBM-bound elementwise + column/row reductions: no tensor cores.  Train-mode Dice needs batch
 // statistics over all B*L rows: a column-statistics pass (fp64 block partials, one atomic per
 // column per CTA) followed by one elementwise pass; the backward mirrors it.
-#include "b2_common.cuh"
+#include "bn_common.cuh"
 
 namespace {
 // ---- column sums of up to three derived quantities -------------------------------------------------
@@ -63,16 +63,8 @@ __global__ void dice_finalize_kernel(const double* __restrict__ stats, int64_t M
                                      float* __restrict__ running_mean, float* __restrict__ running_var) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const double mu = stats[c] / (double) M;
-  double var = stats[C + c] / (double) M - mu * mu;
-  if (var < 0.0) var = 0.0;
-  mean[c] = (float) mu;
-  rstd[c] = (float) (1.0 / sqrt(var + (double) eps));
-  if (running_mean != nullptr) {
-    const double unbiased = (M > 1) ? var * (double) M / (double) (M - 1) : var;
-    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float) mu;
-    running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float) unbiased;
-  }
+  b2_bn_finalize(stats[c], stats[C + c], M, eps, momentum, mean + c, rstd + c,
+                 running_mean != nullptr ? running_mean + c : nullptr, running_mean != nullptr ? running_var + c : nullptr);
 }
 
 // eval mode: normalise with the running statistics

@@ -1699,6 +1699,243 @@ def self_attention_layer(x, w_q, w_k, w_v, w_res=None, num_heads=1, use_residual
 
 
 # --------------------------------------------------------------------------------------
+# FinalNet (include/fuxictr_b200.h "FinalNet")
+# --------------------------------------------------------------------------------------
+FINALNET_RESIDUAL = {"concat": _lib.B2_FINALNET_CONCAT, "sum": _lib.B2_FINALNET_SUM}
+
+
+def finalnet_bound(widths=(), fields=None, embedding_dim=None):
+    """None when the FinalNet kernels cover FinalBlock layers of output widths `widths` and, with `fields`, a
+    FeatureGating over (fields, embedding_dim); else the bound it breaks."""
+    for n in widths:
+        if not 1 <= n <= _lib.B2_FINALNET_MAX_WIDTH:
+            return "FinalBlock hidden units must lie in [1, %d], got %d" % (_lib.B2_FINALNET_MAX_WIDTH, n)
+    if fields is not None:
+        if not 1 <= fields <= _lib.B2_FINALNET_MAX_FIELDS:
+            return "feature gating needs 1 to %d fields, got %d" % (_lib.B2_FINALNET_MAX_FIELDS, fields)
+        if not 1 <= embedding_dim <= _lib.B2_FINALNET_MAX_DIM:
+            return "feature gating needs embedding_dim in [1, %d], got %d" % (_lib.B2_FINALNET_MAX_DIM, embedding_dim)
+        if fields * embedding_dim > _lib.B2_FINALNET_MAX_GATE_WIDTH:
+            return "feature gating needs fields * embedding_dim <= %d, got %d" % (_lib.B2_FINALNET_MAX_GATE_WIDTH,
+                                                                                  fields * embedding_dim)
+    return None
+
+
+class _FactorizedInteraction(torch.autograd.Function):
+    """One FinalBlock layer (FinalNet.py, FinalBlock.forward with FactorizedInteraction) as one GEMM and the row
+    kernels of include/fuxictr_b200.h "FinalNet": h = x W^T + b (bias in the epilogue), out = dropout(act(BN(z))) with
+    z the product form of h (b2_finalnet_fi_fwd, which also writes out's operand copy for the next layer's GEMM when
+    asked).  Backward: dh, the bias and the BatchNorm gradients (b2_finalnet_fi_bwd), dx = dh W (added into the
+    EmbeddingGrad buffer when x is a shared_grad view), dW = dh^T x.  bn: None, or (training, eps, momentum,
+    running_mean, running_var, num_batches_tracked) of the layer's nn.BatchNorm1d, whose buffers the kernels update."""
+
+    @staticmethod
+    def forward(ctx, x, sink, cfg, W, b, gamma, beta):
+        residual, act, bn, drop, want_aux = cfg
+        ctx.params, ctx.cfg, ctx.sink = (W, b, gamma, beta), cfg, sink
+        B = x.shape[0]
+        H = W.shape[0]
+        half = H // 2
+        n = 2 * half if residual == _lib.B2_FINALNET_CONCAT else half
+        dev = x.device
+        out = torch.empty((B, n), dtype=torch.float32, device=dev)
+        if B == 0:          # no rows: no launch (an empty tensor has no device address)
+            ctx.tc, ctx.x_aux, ctx.ws = False, None, None
+            ctx.save_for_backward(x, None, None, None)
+            return out
+        tc = _tc_layer_ok(W) and x.data_ptr() % 16 == 0
+        x_aux = (sink.emb_aux(x) if sink is not None else make_aux(x)) if tc else None
+        h = torch.empty((B, H), dtype=torch.float32, device=dev)
+        _linear_fwd(tc, x, x_aux, W, h, bias=b)
+        out_aux = empty_aux(B, n, dev) if want_aux else None
+        mean = rstd = ws = None
+        training, eps, momentum, rm, rv, nbt = bn if bn is not None else (0, 0.0, 0.0, None, None, None)
+        if bn is not None:
+            mean = torch.empty(n, dtype=torch.float32, device=dev)
+            rstd = torch.empty_like(mean)
+            ws = torch.empty(4 * n, dtype=torch.float64, device=dev)
+        _lib.call("b2_finalnet_fi_fwd", _ptr(h), B, half, residual, _ptr(gamma), _ptr(beta), eps, momentum,
+                  int(training), _ptr(rm), _ptr(rv), _ptr(nbt), _ptr(ws), act, *_drop_args(drop), _ptr(out),
+                  *_aux_args(out_aux), _ptr(mean), _ptr(rstd), _stream())
+        if out_aux is not None:         # the next layer's make_aux finds it
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        ctx.save_for_backward(x, h, mean, rstd)
+        ctx.tc, ctx.x_aux, ctx.ws = tc, x_aux, ws
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, h, mean, rstd = ctx.saved_tensors
+        W, b, gamma, beta = ctx.params
+        residual, act, bn, drop, _ = ctx.cfg
+        sink, tc = ctx.sink, ctx.tc
+        B = x.shape[0]
+        H = W.shape[0]
+        half = H // 2
+        n = 2 * half if residual == _lib.B2_FINALNET_CONCAT else half
+        gW = _grad_buffer(W, zero=False)
+        gb = _grad_buffer(b, zero=True) if b is not None else None
+        gg = _grad_buffer(gamma, zero=False) if gamma is not None else None
+        gbe = _grad_buffer(beta, zero=False) if beta is not None else None
+        if B == 0:          # every gradient is zero; a shared buffer is left to its other writers
+            for t in (gW, gg, gbe):
+                if t is not None:
+                    t.zero_()
+            gx = torch.zeros_like(x) if sink is None and ctx.needs_input_grad[0] else None
+            return gx, None, None, gW, gb, gg, gbe
+        g = _f32c(g)
+        dh = torch.empty((B, H), dtype=torch.float32, device=x.device)
+        dh_aux = empty_aux(B, H, x.device) if tc else None
+        training = bool(bn[0]) if bn is not None else False
+        ws = ctx.ws[2 * n:] if bn is not None else None
+        _lib.call("b2_finalnet_fi_bwd", _ptr(h), B, half, residual, _ptr(gamma), _ptr(beta), _ptr(mean), _ptr(rstd),
+                  int(training), _ptr(ws), 0 if training else 1, act, *_drop_args(drop), _ptr(g), _ptr(dh),
+                  *_aux_args(dh_aux), _ptr(gb), _ptr(gg), _ptr(gbe), _stream())
+        if tc and dh_aux is None:
+            dh_aux = make_aux(dh)
+        gx = None
+        if sink is not None:
+            target, acc = sink.target(x)
+            _linear_dgrad(tc, dh, dh_aux, W, target, accumulate=acc)
+        elif ctx.needs_input_grad[0]:
+            gx = torch.empty_like(x)
+            _linear_dgrad(tc, dh, dh_aux, W, gx)
+        _linear_wgrad(tc, dh, dh_aux, x, ctx.x_aux, gW)
+        return gx, None, None, gW, gb, gg, gbe
+
+
+def factorized_interaction(x, weight, bias=None, residual_type="sum", sink=None, batch_norm=None, act=B2_ACT_NONE,
+                           dropout=None, want_aux=False):
+    """One FinalBlock layer on x (B, K): FactorizedInteraction(x) with weight (2m, K) and bias (2m,), then the optional
+    BatchNorm1d, activation and dropout.  batch_norm: (nn.BatchNorm1d, training) or None; act: B2_ACT_NONE,
+    B2_ACT_RELU or B2_ACT_SIGMOID; dropout: (snapshot, layer, p) (dropout_snapshot) or None.  sink: x is a shared_grad
+    view whose gradient is added into that EmbeddingGrad.  want_aux: also write the output's GEMM operand copy."""
+    _require_cuda(x, weight)
+    if residual_type not in FINALNET_RESIDUAL:
+        raise ValueError("residual_type must be 'concat' or 'sum', got %r" % (residual_type,))
+    if act not in (B2_ACT_NONE, B2_ACT_RELU, B2_ACT_SIGMOID):
+        raise NotImplementedError("factorized_interaction: activation code %r" % (act,))
+    H, K = weight.shape
+    residual = FINALNET_RESIDUAL[residual_type]
+    if x.dim() != 2 or x.shape[1] != K or H % 2 or (bias is not None and tuple(bias.shape) != (H,)):
+        raise ValueError("factorized_interaction: shapes x%s weight%s do not match" % (tuple(x.shape),
+                                                                                      tuple(weight.shape)))
+    n = H if residual == _lib.B2_FINALNET_CONCAT else H // 2
+    bound = finalnet_bound([n])
+    if bound:
+        raise NotImplementedError("FinalNet kernels: " + bound)
+    bn = gamma = beta = None
+    if batch_norm is not None:
+        norm, training = batch_norm
+        if norm.num_features != n or not norm.affine or not norm.track_running_stats or norm.momentum is None:
+            raise NotImplementedError("FinalNet kernels: BatchNorm1d(%d) with affine, running statistics and a "
+                                      "momentum, got %r" % (n, norm))
+        if training and x.shape[0] == 1:
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % ((1, n),))
+        bn = (int(bool(training)), float(norm.eps), float(norm.momentum), norm.running_mean, norm.running_var,
+              norm.num_batches_tracked)
+        gamma, beta = norm.weight, norm.bias
+    drop = None
+    if dropout is not None:
+        snap, layer, p = dropout
+        drop = (snap, layer) + dropout_consts(p)
+    return _FactorizedInteraction.apply(_f32c(x), sink, (residual, act, bn, drop, want_aux), weight, bias, gamma, beta)
+
+
+class _FeatureGating(torch.autograd.Function):
+    """FinalNet's FeatureGating with gate_residual "concat" (FinalNet.py, FeatureGating.forward) on e (B, F D), one
+    row kernel each way: out = [e, e * (W e + b)] over the field axis, flattened (b2_finalnet_gate_fwd, with the
+    operand copy block 1's first GEMM reads).  Backward: e's gradient added into the EmbeddingGrad buffer (or a fresh
+    one without a sink), dW and db (b2_finalnet_gate_bwd)."""
+
+    @staticmethod
+    def forward(ctx, e, sink, want_aux, W, b):
+        ctx.params, ctx.sink = (W, b), sink
+        B, FD = e.shape
+        F = W.shape[0]
+        out = torch.empty((B, 2 * FD), dtype=torch.float32, device=e.device)
+        ctx.save_for_backward(e)
+        if B == 0:
+            return out
+        out_aux = empty_aux(B, 2 * FD, e.device) if want_aux else None
+        _lib.call("b2_finalnet_gate_fwd", _ptr(e), B, F, FD // F, _ptr(_f32c(W)), _ptr(_f32c(b)), _ptr(out),
+                  *_aux_args(out_aux), _stream())
+        if out_aux is not None:
+            out._b2_aux = (_MATMUL["mode"], out_aux, out._version)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (e,) = ctx.saved_tensors
+        W, b = ctx.params
+        sink = ctx.sink
+        B, FD = e.shape
+        F = W.shape[0]
+        gW, gb = _grad_buffer(W, zero=True), _grad_buffer(b, zero=True)
+        if sink is not None:
+            de, acc = sink.target(e) if B > 0 else (None, False)
+        else:
+            de, acc = torch.empty_like(e), False
+        if B > 0:
+            _lib.call("b2_finalnet_gate_bwd", _ptr(e), B, F, FD // F, _ptr(_f32c(W)), _ptr(_f32c(b)), _ptr(_f32c(g)),
+                      _ptr(de), 1 if acc else 0, _ptr(gW), _ptr(gb), _stream())
+        return (de if sink is None else None), None, None, gW, gb
+
+
+def feature_gating(feature_emb, weight, bias, sink=None, want_aux=False):
+    """[e, e * gates] flattened to (B, 2 F D), gates = Linear(F, F) over the field axis of feature_emb (B, F, D) or
+    its flatten (B, F D) (a shared_grad view with its `sink`).  want_aux: also write the operand copy of the output."""
+    _require_cuda(feature_emb, weight, bias)
+    F = weight.shape[0]
+    B = feature_emb.shape[0]
+    e = feature_emb.reshape(B, -1) if feature_emb.dim() == 3 else feature_emb
+    if tuple(weight.shape) != (F, F) or tuple(bias.shape) != (F,) or e.dim() != 2 or e.shape[1] % F:
+        raise ValueError("feature_gating: shapes feature_emb%s weight%s bias%s do not match"
+                         % (tuple(feature_emb.shape), tuple(weight.shape), tuple(bias.shape)))
+    bound = finalnet_bound(fields=F, embedding_dim=e.shape[1] // F)
+    if bound:
+        raise NotImplementedError("FinalNet kernels: " + bound)
+    return _FeatureGating.apply(e if sink is not None else _f32c(e), sink, want_aux, weight, bias)
+
+
+class _FinalNetLoss(torch.autograd.Function):
+    """FinalNet's two-block loss (FinalNet.py, add_loss with block_type "2B") from the logits y1, y2 in one launch
+    (b2_finalnet_loss); also returns y_pred = sigmoid((y1 + y2) / 2) (not differentiable)."""
+
+    @staticmethod
+    def forward(ctx, label, y1, y2):
+        ctx.shapes = (y1.shape, y2.shape)
+        y1, y2 = _f32c(y1).view(-1), _f32c(y2).view(-1)
+        B = y1.numel()
+        dev = y1.device
+        label = _f32c(label).view(-1)
+        y_pred = torch.empty((B, 1), dtype=torch.float32, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        g1 = torch.empty((B,), dtype=torch.float32, device=dev)
+        g2 = torch.empty_like(g1)
+        _lib.call("b2_finalnet_loss", _ptr(y1), _ptr(y2), _ptr(label), B, _ptr(loss), _ptr(y_pred), _ptr(g1),
+                  _ptr(g2), _stream())
+        ctx.save_for_backward(g1, g2)
+        ctx.mark_non_differentiable(y_pred)
+        return loss, y_pred
+
+    @staticmethod
+    def backward(ctx, gloss, _gy):
+        g1, g2 = ctx.saved_tensors
+        return None, (g1 * gloss).view(ctx.shapes[0]), (g2 * gloss).view(ctx.shapes[1])
+
+
+def finalnet_loss(label, y1, y2):
+    """(loss, y_pred) of FinalNet's 2B loss, BCE(y_pred, y) + BCE(sigmoid(y1), p) + BCE(sigmoid(y2), p) with
+    y_pred = p = sigmoid((y1 + y2) / 2) held constant in the last two terms; y1, y2 (B, 1) or (B,) logits."""
+    _require_cuda(label, y1, y2)
+    if y1.numel() != y2.numel() or y1.numel() != label.numel() or y1.numel() < 1:
+        raise ValueError("finalnet_loss: y1, y2 and label must hold the same number (>= 1) of values")
+    return _FinalNetLoss.apply(label, y1, y2)
+
+
+# --------------------------------------------------------------------------------------
 # WuKong (include/fuxictr_b200.h "WuKong")
 # --------------------------------------------------------------------------------------
 def wukong_bound(fields, out_fields, embedding_dim, rank_k):

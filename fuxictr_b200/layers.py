@@ -23,6 +23,7 @@ Reference files (relative to the reference root):
   MaskBlock / SerialMaskNet / ParallelMaskNet model_zoo/MaskNet/src/MaskNet.py
   MultiHeadSelfAttention                   model_zoo/AutoInt/src/AutoInt.py
   FactorizationMachineBlock / LinearCompressionBlock / WuKongLayer model_zoo/WuKong/src/WuKong.py
+  FeatureGating / FactorizedInteraction / FinalBlock model_zoo/FinalNet/src/FinalNet.py
 """
 import sys
 from collections import OrderedDict
@@ -1108,3 +1109,115 @@ def wukong_stack(layers, feature_emb, want_aux=False):
         n = nxt.lcb.linear.weight.shape[0] + (res.weight.shape[0] if res is not None else 0)
         x = layer.run(x, sink, last=False, want_aux=F2._wukong_tc_shape(n, F2.wukong_pitch(nxt.fmb.input_features)))
         x, sink = F2.shared_grad(x)
+
+
+# --------------------------------------------------------------------------------------
+# FinalNet (model_zoo/FinalNet/src/FinalNet.py)
+# --------------------------------------------------------------------------------------
+def _finalnet_act(module):
+    """The B2_ACT_* code of a FinalBlock activation module (get_activation's result), refusing what the kernels lack."""
+    if module is None:
+        return B2_ACT_NONE
+    if type(module) == nn.ReLU:
+        return B2_ACT_RELU
+    if type(module) == nn.Sigmoid:
+        return B2_ACT_SIGMOID
+    raise NotImplementedError("FinalBlock kernels: activation %s is not supported (None, ReLU and Sigmoid are)"
+                              % type(module).__name__)
+
+
+class FeatureGating(nn.Module):
+    """model_zoo/FinalNet/src/FinalNet.py, FeatureGating: gates = Linear(F, F) over the field axis, out =
+    cat([e, e * gates], dim=1) (gate_residual "concat"; "sum" is refused).  init_weights sets the gate's weight to 0
+    and its bias to 1, as the reference's.  One row kernel each way (functional.feature_gating)."""
+
+    def __init__(self, num_fields, gate_residual="concat"):
+        super(FeatureGating, self).__init__()
+        self.linear = nn.Linear(num_fields, num_fields)
+        assert gate_residual in ["concat", "sum"]
+        if gate_residual != "concat":
+            raise NotImplementedError("FeatureGating kernels: gate_residual='sum' is not supported ('concat' is)")
+        self.gate_residual = gate_residual
+
+    def init_weights(self):
+        nn.init.zeros_(self.linear.weight)
+        nn.init.ones_(self.linear.bias)
+
+    def run(self, feature_emb, sink=None, want_aux=False):
+        """(B, 2 F D): the flattened output block 1 reads; feature_emb (B, F, D), or its (B, F D) shared_grad view."""
+        return F2.feature_gating(feature_emb, self.linear.weight, self.linear.bias, sink=sink, want_aux=want_aux)
+
+    def forward(self, feature_emb):
+        """(B, F, D) -> (B, 2 F, D)."""
+        return self.run(feature_emb).view(feature_emb.shape[0], -1, feature_emb.shape[2])
+
+
+class FactorizedInteraction(nn.Module):
+    """model_zoo/FinalNet/src/FinalNet.py, FactorizedInteraction: h = Linear(x), h2, h1 = chunk(h, 2),
+    cat([h2, h1 * h2]) (concat, which asserts an even output_dim) or h2 + h1 * h2 (sum, whose Linear is 2 output_dim
+    wide).  One GEMM and one row kernel (functional.factorized_interaction)."""
+
+    def __init__(self, input_dim, output_dim, bias=True, residual_type="sum"):
+        super(FactorizedInteraction, self).__init__()
+        self.residual_type = residual_type
+        if residual_type == "sum":
+            output_dim = output_dim * 2
+        else:
+            assert output_dim % 2 == 0, "output_dim should be divisible by 2."
+        self.linear = nn.Linear(input_dim, output_dim, bias=bias)
+
+    def forward(self, x):
+        return F2.factorized_interaction(x, self.linear.weight, self.linear.bias, self.residual_type)
+
+
+class FinalBlock(nn.Module):
+    """model_zoo/FinalNet/src/FinalNet.py, FinalBlock: per layer FactorizedInteraction, then BatchNorm1d (the real
+    nn.BatchNorm1d children, whose running statistics the kernels update in place), the activation and dropout.  As in
+    the reference, layer i applies self.dropout[i] whenever there is one, and self.dropout only holds the rates > 0: per
+    layer rates [0, 0.5] put the 0.5 after layer 0.  Activations: None, ReLU, Sigmoid; others are refused here."""
+
+    def __init__(self, input_dim, hidden_units=[], hidden_activations=None, dropout_rates=[], batch_norm=True,
+                 residual_type="sum"):
+        super(FinalBlock, self).__init__()
+        if type(dropout_rates) != list:
+            dropout_rates = [dropout_rates] * len(hidden_units)
+        if type(hidden_activations) != list:
+            hidden_activations = [hidden_activations] * len(hidden_units)
+        bound = F2.finalnet_bound(hidden_units)
+        if bound is not None:
+            raise NotImplementedError("FinalBlock kernels: " + bound)
+        self.layer = nn.ModuleList()
+        self.norm = nn.ModuleList()
+        self.dropout = nn.ModuleList()
+        self.activation = nn.ModuleList()
+        hidden_units = [input_dim] + hidden_units
+        for idx in range(len(hidden_units) - 1):
+            self.layer.append(FactorizedInteraction(hidden_units[idx], hidden_units[idx + 1],
+                                                    residual_type=residual_type))
+            if batch_norm:
+                self.norm.append(nn.BatchNorm1d(hidden_units[idx + 1]))
+            if dropout_rates[idx] > 0:
+                self.dropout.append(nn.Dropout(dropout_rates[idx]))
+            self.activation.append(get_activation(hidden_activations[idx]))
+        self._acts = [_finalnet_act(a) for a in self.activation]
+
+    def run(self, X, sink=None, want_aux=False):
+        """The block on X (B, input_dim); sink: X is a shared_grad view.  want_aux: the output's operand copy."""
+        L = len(self.layer)
+        rates = [self.dropout[i].p if len(self.dropout) > i else 0.0 for i in range(L)]
+        snap = None
+        if self.training and any(p > 0 for p in rates):
+            snap = F2.dropout_snapshot(X.device, L)
+        x = X
+        for i in range(L):
+            lin = self.layer[i].linear
+            norm = (self.norm[i], self.norm[i].training) if len(self.norm) > i else None
+            drop = (snap, i, rates[i]) if snap is not None and rates[i] > 0 else None
+            aux = F2._tc_layer_ok(self.layer[i + 1].linear.weight) if i + 1 < L else want_aux
+            x = F2.factorized_interaction(x, lin.weight, lin.bias, self.layer[i].residual_type,
+                                          sink=sink if i == 0 else None, batch_norm=norm, act=self._acts[i],
+                                          dropout=drop, want_aux=aux)
+        return x
+
+    def forward(self, X):
+        return self.run(X)

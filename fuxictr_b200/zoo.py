@@ -18,6 +18,7 @@ same RNG consumption) and nothing else.
   MaskNet      model_zoo/MaskNet/src/MaskNet.py
   AutoInt      model_zoo/AutoInt/src/AutoInt.py
   WuKong       model_zoo/WuKong/src/WuKong.py
+  FinalNet     model_zoo/FinalNet/src/FinalNet.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -29,6 +30,7 @@ from torch import nn
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
+                     FeatureGating, FinalBlock,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -177,7 +179,8 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong) may be sharded: any
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong, FinalNet) may be
+        sharded: any
         other forward would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
         categorical features only.  Anything else is refused before a table is touched."""
@@ -185,7 +188,7 @@ class RankModel(nn.Module):
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
                                       "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
-                                      "DualMLP, MaskNet, AutoInt and WuKong" % type(self).__name__)
+                                      "DualMLP, MaskNet, AutoInt, WuKong and FinalNet" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -355,7 +358,7 @@ class RankModel(nn.Module):
         y_true = self.get_labels(batch_data)
         fused_logit = hasattr(self, "forward_logits") and not regularised
         if fused_logit:
-            loss, _ = F2.logit_bce(y_true, *self.forward_logits(batch_data))
+            loss = self.fused_loss(batch_data, y_true)
         else:
             loss = self.compute_loss(self.forward(batch_data), y_true)
         seed = getattr(self, "_loss_grad", None)      # 1/world for row-sharded runs (see enable_sharding)
@@ -373,6 +376,11 @@ class RankModel(nn.Module):
             opt.arena.defer_join = False
         opt.step()
         return loss
+
+    def fused_loss(self, batch_data, y_true):
+        """The loss of fused_train_step's fused path: the fused logit + BCE kernel over the sum of the model's
+        pre-sigmoid logit terms (`forward_logits`).  A model whose loss is not a BCE of such a sum overrides this."""
+        return F2.logit_bce(y_true, *self.forward_logits(batch_data))[0]
 
 
 def _parse_regularizer(reg):
@@ -1081,3 +1089,100 @@ class xDeepFM(RankModel):
         if len(terms) > 2:
             y_pred = y_pred + terms[2]
         return {"y_pred": self.output_activation(y_pred)}
+
+
+class FinalNet(RankModel):
+    """model_zoo/FinalNet/src/FinalNet.py, FinalNet: block 1 (a FinalBlock over the flattened embedding, or over the
+    feature gating's [e, e * gates] with use_feature_gating) and fc1; with block_type "2B" also block 2 over the plain
+    flattened embedding and fc2, y_pred = sigmoid((y1 + y2) / 2) and the self-distillation loss of add_loss, which the
+    fused step takes in one launch (functional.finalnet_loss).  The embedding's gradient is one shared_grad buffer that
+    the gating's backward and the blocks' first dgrads add into.  Unknown keyword arguments are accepted and ignored,
+    as the reference's **kwargs are.  Refused: activations other than None, ReLU and Sigmoid, shapes outside
+    functional.finalnet_bound, lazy tables and enable_sharding(want_fm=True)."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="FinalNet", gpu=-1, learning_rate=1e-3, embedding_dim=10,
+                 block_type="2B", batch_norm=True, use_feature_gating=False, block1_hidden_units=[64, 64, 64],
+                 block1_hidden_activations=None, block1_dropout=0, block2_hidden_units=[64, 64, 64],
+                 block2_hidden_activations=None, block2_dropout=0, residual_type="concat", embedding_regularizer=None,
+                 net_regularizer=None, **kwargs):
+        super(FinalNet, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                       embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                       **kwargs)
+        assert block_type in ["1B", "2B"], "block_type={} not supported.".format(block_type)
+        num_fields = feature_map.num_fields
+        bound = F2.finalnet_bound(fields=num_fields, embedding_dim=embedding_dim) if use_feature_gating else None
+        if bound is not None:
+            raise NotImplementedError("FinalNet kernels: " + bound)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.use_feature_gating = use_feature_gating
+        if use_feature_gating:
+            self.feature_gating = FeatureGating(num_fields, gate_residual="concat")
+            gate_out_dim = embedding_dim * num_fields * 2
+        self.block_type = block_type
+        self.block1 = FinalBlock(input_dim=gate_out_dim if use_feature_gating else embedding_dim * num_fields,
+                                 hidden_units=block1_hidden_units, hidden_activations=block1_hidden_activations,
+                                 dropout_rates=block1_dropout, batch_norm=batch_norm, residual_type=residual_type)
+        self.fc1 = nn.Linear(block1_hidden_units[-1], 1)
+        if block_type == "2B":
+            self.block2 = FinalBlock(input_dim=embedding_dim * num_fields, hidden_units=block2_hidden_units,
+                                     hidden_activations=block2_hidden_activations, dropout_rates=block2_dropout,
+                                     batch_norm=batch_norm, residual_type=residual_type)
+            self.fc2 = nn.Linear(block2_hidden_units[-1], 1)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which FinalNet does not have."""
+        if want_fm:
+            raise ValueError("FinalNet has no FM term: enable_sharding(..., want_fm=False)")
+        return super(FinalNet, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype,
+                                                     want_fm=False)
+
+    def _feature_emb(self, inputs):
+        """The field embeddings (B, F, D), from the row-sharded front after enable_sharding()."""
+        if getattr(self, "_sharded_front", None) is not None:   # row-sharded tables, P2P push/pull
+            from .sharded import sharded_front
+            return sharded_front(self._sharded_front, self._batch_matrix(inputs))[0]
+        return self.embedding_layer(self.get_inputs(inputs))
+
+    def forward_logits(self, inputs):
+        """(y1,) or, with 2B, (y1, y2): the blocks' pre-sigmoid logits (B, 1)."""
+        feature_emb = self._feature_emb(inputs)
+        flat, sink = F2.shared_grad(feature_emb.flatten(start_dim=1))
+        first = F2._tc_layer_ok(self.block1.layer[0].linear.weight) if len(self.block1.layer) else False
+        if self.use_feature_gating:
+            x1 = self.feature_gating.run(flat, sink=sink, want_aux=first)
+            out1 = self.block1.run(x1)
+        else:
+            out1 = self.block1.run(flat, sink=sink)
+        y1 = F2.linear_act(out1, self.fc1.weight, self.fc1.bias)
+        if self.block_type == "1B":
+            return (y1,)
+        out2 = self.block2.run(flat, sink=sink)
+        return (y1, F2.linear_act(out2, self.fc2.weight, self.fc2.bias))
+
+    def forward(self, inputs):
+        logits = self.forward_logits(inputs)
+        if self.block_type == "1B":
+            return {"y_pred": self.output_activation(logits[0]), "y1": None, "y2": None}
+        y1, y2 = logits
+        return {"y_pred": self.output_activation(0.5 * (y1 + y2)), "y1": y1, "y2": y2}
+
+    def add_loss(self, return_dict, y_true):
+        """FinalNet.add_loss: BCE of y_pred, plus with 2B the two self-distillation terms against y_pred detached."""
+        loss = self.loss_fn(return_dict["y_pred"], y_true, reduction="mean")
+        if self.block_type == "2B":
+            y1 = self.output_activation(return_dict["y1"])
+            y2 = self.output_activation(return_dict["y2"])
+            loss1 = self.loss_fn(y1, return_dict["y_pred"].detach(), reduction="mean")
+            loss2 = self.loss_fn(y2, return_dict["y_pred"].detach(), reduction="mean")
+            loss = loss + loss1 + loss2
+        return loss
+
+    def compute_loss(self, return_dict, y_true):
+        return self.add_loss(return_dict, y_true) + self.regularization_loss()
+
+    def fused_loss(self, batch_data, y_true):
+        if self.block_type == "1B":
+            return super(FinalNet, self).fused_loss(batch_data, y_true)
+        return F2.finalnet_loss(y_true, *self.forward_logits(batch_data))[0]

@@ -632,6 +632,59 @@ B2_API int b2_wukong_unpack(const float* dWs, int fields, int lcb, int out_field
                             void* stream);
 
 /*
+ * FinalNet (model_zoo/FinalNet/src/FinalNet.py).  One FactorizedInteraction layer of a FinalBlock on the caller's
+ * GEMM output h = x W^T + b (B, 2 half), row-major fp32:
+ *   h2 = h[:, :half], h1 = h[:, half:]
+ *   z   = [h2, h1 h2] (residual B2_FINALNET_CONCAT, n = 2 half)  |  h2 + h1 h2 (B2_FINALNET_SUM, n = half)
+ *   out = dropout(act(BatchNorm1d(z))) (B, n), each stage optional: gamma == NULL is no batch norm, act a B2_ACT_*
+ *         code, drop_rng == NULL no dropout (the Philox mask of element (b, c) of out, as the MLP chain's).
+ * Batch norm: eps, momentum as nn.BatchNorm1d; training normalises with the batch's biased variance, updates
+ *   running_mean / running_var (unbiased variance) and num_batches (int64) in place, and refuses batch 1; eval
+ *   normalises with the running statistics.  mean, rstd (n) "=" are what the backward reads.  stats_ws (fp64): 4 n
+ *   doubles, the forward's column sums and, at stats_ws + 2 n, the backward's; a training forward clears all 4 n.
+ * Range: 1 <= n <= B2_FINALNET_MAX_WIDTH, batch >= 0 (0: no launch), batch * 2 half < 2^31.  half % 4 == 0 with
+ *   16-byte aligned rows runs the float4 path, anything else the scalar one.  Outside the range, or given a NULL
+ *   pointer, every entry point returns B2_E_INVALID.  An aux pointer (optional, row pitch ld_aux) receives the GEMM
+ *   operand copy of the tensor written beside it: its bf16 rounding (aux_dtype B2_BF16) or 3xTF32 small part (B2_F32).
+ * b2_finalnet_fi_fwd: out "=" (+ out_aux); with batch norm in training a zero fill, a statistics pass and the apply
+ *   pass, else the apply pass alone.
+ * b2_finalnet_fi_bwd: from g = d out (B, n): dh (B, 2 half) "=" (+ dh_aux); dbias (2 half) "+=" (caller zeroes);
+ *   with batch norm dgamma, dbeta (n) "=", from the sums at stats_ws (2 n doubles; zero_ws clears them first, which
+ *   a training forward has already done).  training selects the batch-statistics backward.
+ * FeatureGating (gate_residual "concat") of e (B, F, D) with W (F, F), bias (F):
+ *   g = W e + bias over the field axis, out (B, 2 F D) = [e, e * g] flattened.
+ *   Range: 1 <= F <= B2_FINALNET_MAX_FIELDS, 1 <= D <= B2_FINALNET_MAX_DIM, F D <= B2_FINALNET_MAX_GATE_WIDTH.
+ * b2_finalnet_gate_fwd: out "=" (+ out_aux).
+ * b2_finalnet_gate_bwd: from g = d out: de (B, F, D) "=" (accumulate 0) or "+="; dW, db "+=" (caller zeroes).
+ * b2_finalnet_loss: the two-block loss of logits y1, y2 (B) and labels (B), batch >= 1, in one launch:
+ *   y_pred = sigmoid((y1 + y2) / 2), loss "=" mean_b [BCE(y_pred, y) + BCE(sigmoid(y1), p) + BCE(sigmoid(y2), p)]
+ *   with p = y_pred held constant; g1, g2 "=" d loss / d y1, y2.  Log terms clamped at -100 (b2_logit_bce_fwd).
+ */
+#define B2_FINALNET_CONCAT 0
+#define B2_FINALNET_SUM 1
+#define B2_FINALNET_MAX_WIDTH 1024
+#define B2_FINALNET_MAX_FIELDS 128
+#define B2_FINALNET_MAX_DIM 128
+#define B2_FINALNET_MAX_GATE_WIDTH 8192
+B2_API int b2_finalnet_fi_fwd(const float* h, int64_t batch, int half, int residual, const float* gamma,
+                              const float* beta, float eps, float momentum, int training, float* running_mean,
+                              float* running_var, int64_t* num_batches, double* stats_ws, int act,
+                              const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh, float drop_scale,
+                              float* out, void* out_aux, int aux_dtype, int64_t ld_aux, float* mean, float* rstd,
+                              void* stream);
+B2_API int b2_finalnet_fi_bwd(const float* h, int64_t batch, int half, int residual, const float* gamma,
+                              const float* beta, const float* mean, const float* rstd, int training, double* stats_ws,
+                              int zero_ws, int act, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                              float drop_scale, const float* g, float* dh, void* dh_aux, int aux_dtype, int64_t ld_aux,
+                              float* dbias, float* dgamma, float* dbeta, void* stream);
+B2_API int b2_finalnet_gate_fwd(const float* e, int64_t batch, int fields, int dim, const float* W, const float* bias,
+                                float* out, void* out_aux, int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_finalnet_gate_bwd(const float* e, int64_t batch, int fields, int dim, const float* W, const float* bias,
+                                const float* g, float* de, int accumulate, float* dW, float* db, void* stream);
+B2_API int b2_finalnet_loss(const float* y1, const float* y2, const float* label, int64_t batch, float* loss,
+                            float* y_pred, float* g1, float* g2, void* stream);
+
+/*
  * MultiHeadTargetAttention (layers/attentions/target_attention.py:95-172 with ScaledDotProductAttention,
  * dot_product_attention.py:32-58): one query, the target t (B, d), per sample over its history x (B, L, d).
  * With use_qkvo, W_q, W_k, W_v (A, d) and W_o (d, A), A = H*hd; W_?,h is head h's hd rows of W_q, W_k, W_v,
