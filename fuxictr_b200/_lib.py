@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(HERE, "libfuxictr_b200.so")
 B2_F32, B2_BF16, B2_F64, B2_I64, B2_I32 = 0, 1, 2, 3, 4
 B2_POOL_NONE, B2_POOL_SUM, B2_POOL_MEAN = 0, 1, 2
 B2_ACT_NONE, B2_ACT_RELU, B2_ACT_SIGMOID = 0, 1, 2
+B2_ACT_LEAKY_RELU = 4
 B2_PREP_MUL = 3
 B2_GEMM_C_IS_ZERO, B2_GEMM_COLSUM_IS_ZERO, B2_GEMM_X3_INLINE, B2_GEMM_BACKFILL = 1, 2, 4, 8
 B2_MAX_FIELDS = 128
@@ -26,6 +27,8 @@ B2_AUTOINT_MAX_FIELDS, B2_AUTOINT_MAX_DIM = 64, 64
 B2_WUKONG_MAX_FIELDS, B2_WUKONG_MAX_DIM, B2_WUKONG_MAX_RANK, B2_WUKONG_MAX_FM_WIDTH = 128, 128, 32, 1024
 B2_FINALNET_CONCAT, B2_FINALNET_SUM = 0, 1
 B2_FINALNET_MAX_WIDTH, B2_FINALNET_MAX_FIELDS, B2_FINALNET_MAX_DIM, B2_FINALNET_MAX_GATE_WIDTH = 1024, 128, 128, 8192
+B2_BST_MAX_LEN, B2_BST_MAX_DIM, B2_BST_MAX_HEAD_DIM, B2_BST_MAX_HEADS, B2_BST_MAX_PARTS = 256, 512, 64, 16, 8
+B2_BST_POOL_MEAN, B2_BST_POOL_SUM, B2_BST_POOL_TARGET = 0, 1, 2
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
 c_void_p, c_int, c_int32, c_int64, c_float, c_double = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int32,
@@ -197,6 +200,24 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p]),
     "b2_finalnet_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
+    "b2_bst_tokens_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int, c_int,
+                                  c_void_p, c_void_p, c_int, c_int64, c_void_p]),
+    "b2_bst_tokens_bwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                  c_void_p, c_void_p]),
+    "b2_bst_attn_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int64,
+                                ctypes.c_uint32, c_float, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p,
+                                c_void_p]),
+    "b2_bst_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int,
+                                c_int, c_int, c_float, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p, c_void_p,
+                                c_int, c_int64, c_void_p]),
+    "b2_bst_addnorm_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int64,
+                                   ctypes.c_uint32, c_float, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p,
+                                   c_void_p]),
+    "b2_bst_addnorm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p, c_void_p, c_int,
+                                   c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_bst_pool_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "b2_bst_pool_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b2_mhta_pack":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                              c_void_p, c_void_p]),
     "b2_mhta_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float,

@@ -28,6 +28,11 @@ int b2_fail(int code, const char* fmt, ...);
 
 static inline int64_t b2_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// A B2_ACT_* code that the GEMM epilogues, the head kernels and b2_prep_operand take.
+static inline bool b2_act_ok(int act) {
+  return (act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID) || act == B2_ACT_LEAKY_RELU;
+}
+
 // ---- programmatic dependent launch (on by default; B2_PDL=0 launches plainly) --------------------
 // The step is a chain of ~45 short kernels; with PDL a kernel's CTAs are scheduled while its predecessor
 // drains and sit at griddepcontrol.wait (which returns only when the predecessor has COMPLETED and its

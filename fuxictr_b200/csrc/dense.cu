@@ -148,6 +148,7 @@ sgemm_kernel(const GemmArgs g, bool a_vec, bool b_vec) {
       if (g.add != nullptr) v += __ldg(g.add + m * g.ldc + n);
       if (g.act == B2_ACT_RELU) v = fmaxf(v, 0.f);
       else if (g.act == B2_ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
+      else if (g.act == B2_ACT_LEAKY_RELU) v = v > 0.f ? v : __fmul_rn(v, B2_LEAKY_SLOPE);
       if (g.beta) v += *cp;
       *cp = v;
     }
@@ -171,7 +172,7 @@ extern "C" B2_API int b2_gemm_f32(const float* a, int64_t a_rs, int64_t a_cs, co
              (long long) M, (long long) N, (long long) K, (long long) ldc);
   B2_REQUIRE(a_rs == 1 || a_cs == 1, "A must have a unit stride");
   B2_REQUIRE(b_rs == 1 || b_cs == 1, "B must have a unit stride");
-  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad activation code %d", act);
+  B2_REQUIRE(b2_act_ok(act), "bad activation code %d", act);
   if (M == 0 || N == 0) return B2_OK;
   cudaStream_t st = (cudaStream_t) stream;
   GemmArgs g;

@@ -360,19 +360,28 @@ __device__ __forceinline__ void seg_store_bf16(__nv_bfloat16* p, const float4& v
 // DROP: keep is the element's dropout mask bit.  The mask multiplies after the activation (forward: y = act(z) *
 // keep * scale) and before the activation backward (dgrad: dZ = act'(.) * keep * scale * dH), where ybwd holds the
 // dropped output: ReLU's act' is ybwd > 0 as before; sigmoid's s is recovered as ybwd / scale on kept elements.
-template <bool DROP>
+// LEAKY: the instantiation that also knows B2_ACT_LEAKY_RELU (forward and act_bwd; its act' is ybwd > 0 ? 1 : slope,
+// which a dropped element's zero gradient leaves zero).  Every other launch runs the LEAKY = false code, which is the
+// epilogue without it.
+template <bool DROP, bool LEAKY>
 __device__ __forceinline__ float epilogue_elem(const Params& p, float t, float mv, float av, float yv, float cv,
                                               bool keep) {
   if (p.mul != nullptr) t = __fmul_rn(t, mv);
   if (p.add != nullptr) t = __fadd_rn(t, av);
   if (p.act == B2_ACT_RELU) t = fmaxf(t, 0.f);
   else if (p.act == B2_ACT_SIGMOID) t = 1.f / (1.f + expf(-t));
+  if constexpr (LEAKY) {
+    if (p.act == B2_ACT_LEAKY_RELU) t = t > 0.f ? t : __fmul_rn(t, B2_LEAKY_SLOPE);
+  }
   if constexpr (DROP) t = keep ? __fmul_rn(t, p.drop_scale) : 0.f;
   if (p.ybwd != nullptr) {     // activation backward of the PRODUCER of this gradient, fused
     if (p.act_bwd == B2_ACT_RELU) t = (yv > 0.f) ? t : 0.f;
     else if (p.act_bwd == B2_ACT_SIGMOID) {
       const float s = DROP ? __fdiv_rn(yv, p.drop_scale) : yv;
       t = __fmul_rn(t, __fmul_rn(__fsub_rn(1.f, s), s));
+    }
+    if constexpr (LEAKY) {
+      if (p.act_bwd == B2_ACT_LEAKY_RELU) t = (yv > 0.f) ? t : __fmul_rn(t, B2_LEAKY_SLOPE);
     }
   }
   if (p.beta) t = __fadd_rn(t, cv);
@@ -382,7 +391,7 @@ __device__ __forceinline__ float epilogue_elem(const Params& p, float t, float m
 // The two consumer warpgroups (threads 128-383) meet; barrier 0 is __syncthreads.
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-template <int BN, int MODE, bool DROP>
+template <int BN, int MODE, bool DROP, bool LEAKY>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
   constexpr int NR = BN / 2;                            // accumulators per thread: 64 x BN per warpgroup
@@ -649,10 +658,10 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
         if constexpr (DROP) {
           if (k > 0) kb = b2_drop_keep4(dseed, doff, (uint64_t) m * (uint64_t) p.N + (uint64_t) n, k, p.drop_thresh);
         }
-        t.x = epilogue_elem<DROP>(p, t.x, mv[i].x, av[i].x, yv[i].x, cv[i].x, kb & 1u);
-        t.y = epilogue_elem<DROP>(p, t.y, mv[i].y, av[i].y, yv[i].y, cv[i].y, kb & 2u);
-        t.z = epilogue_elem<DROP>(p, t.z, mv[i].z, av[i].z, yv[i].z, cv[i].z, kb & 4u);
-        t.w = epilogue_elem<DROP>(p, t.w, mv[i].w, av[i].w, yv[i].w, cv[i].w, kb & 8u);
+        t.x = epilogue_elem<DROP, LEAKY>(p, t.x, mv[i].x, av[i].x, yv[i].x, cv[i].x, kb & 1u);
+        t.y = epilogue_elem<DROP, LEAKY>(p, t.y, mv[i].y, av[i].y, yv[i].y, cv[i].y, kb & 2u);
+        t.z = epilogue_elem<DROP, LEAKY>(p, t.z, mv[i].z, av[i].z, yv[i].z, cv[i].z, kb & 4u);
+        t.w = epilogue_elem<DROP, LEAKY>(p, t.w, mv[i].w, av[i].w, yv[i].w, cv[i].w, kb & 8u);
         seg_store(p.c + o, t, v, k);
         if (p.c_small != nullptr) {
           const int64_t oa = (int64_t) m * p.ld_aux + n;
@@ -702,7 +711,7 @@ split_tf32_kernel(const float* __restrict__ x, float* __restrict__ small, int64_
 // DROP: x is the gradient of a dropout layer's output, y that dropped output: v = act'(y) * keep * scale * x
 // (the mask first; sigmoid's s = y / scale on kept elements).
 // ---------------------------------------------------------------------------------
-template <bool DROP>
+template <bool DROP, bool LEAKY>      // LEAKY: the twin that also knows B2_ACT_LEAKY_RELU (as the GEMM's)
 __global__ void __launch_bounds__(256)
 prep_operand_kernel(const float* __restrict__ x, const float* __restrict__ y, int act, int64_t R,
                     int64_t C, int64_t ld_in, float* __restrict__ out, float* __restrict__ out_small,
@@ -734,6 +743,9 @@ prep_operand_kernel(const float* __restrict__ x, const float* __restrict__ y, in
           v = v * ((1.f - s) * s);
         }
         else if (act == B2_PREP_MUL) v = v * yv;
+        if constexpr (LEAKY) {
+          if (act == B2_ACT_LEAKY_RELU) v = (yv > 0.f) ? v : __fmul_rn(v, B2_LEAKY_SLOPE);
+        }
       }
       if (out != nullptr) out[r * C + c] = v;
       if (out_small != nullptr) out_small[r * C + c] = tf32_small(v);
@@ -773,6 +785,7 @@ prep_operand_kernel(const float* __restrict__ x, const float* __restrict__ y, in
 //   together with its 3xTF32 small part (gx_small) and its bias gradient gb_prev[k] = sum_m gx[m,k].
 //   DROP: the previous layer ends on dropout, x is its dropped output: its mask multiplies gx before prev_act'.
 // ---------------------------------------------------------------------------------
+template <bool LEAKY>
 __global__ void __launch_bounds__(256)
 head_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
                 int64_t M, int K, int act, float* __restrict__ y) {
@@ -790,13 +803,16 @@ head_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
       float v = acc + bv;
       if (act == B2_ACT_RELU) v = fmaxf(v, 0.f);
       else if (act == B2_ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
+      if constexpr (LEAKY) {
+        if (act == B2_ACT_LEAKY_RELU) v = v > 0.f ? v : __fmul_rn(v, B2_LEAKY_SLOPE);
+      }
       y[m] = v;
     }
   }
 }
 
 // CTA = 256 threads = 8 warps; each CTA owns a contiguous block of rows; lane k-strided columns.
-template <bool DROP>
+template <bool DROP, bool LEAKY>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ y,
                 const float* __restrict__ gy, int64_t M, int K, int act, int64_t rows_per_cta,
@@ -830,6 +846,9 @@ head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
         const float yv = __ldg(y + m);
         if (act == B2_ACT_RELU) gz = (yv > 0.f) ? gz : 0.f;
         else if (act == B2_ACT_SIGMOID) gz = gz * ((1.f - yv) * yv);
+        if constexpr (LEAKY) {
+          if (act == B2_ACT_LEAKY_RELU) gz = (yv > 0.f) ? gz : __fmul_rn(gz, B2_LEAKY_SLOPE);
+        }
       }
       if (kb == 0 && lane == 0) gb_acc += gz;
 #pragma unroll
@@ -846,6 +865,9 @@ head_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
             else if (prev_act == B2_ACT_SIGMOID) {
               const float s = DROP ? __fdiv_rn(xv, drop_scale) : xv;
               val = val * ((1.f - s) * s);
+            }
+            if constexpr (LEAKY) {
+              if (prev_act == B2_ACT_LEAKY_RELU) val = (xv > 0.f) ? val : __fmul_rn(val, B2_LEAKY_SLOPE);
             }
             gx[m * K + k] = val;
             if (gx_small != nullptr) gx_small[m * K + k] = tf32_small(val);
@@ -962,9 +984,9 @@ static bool tma_ok(const float* p, int64_t ld) { return tma_ok_e(p, ld, 4); }
 
 // plan != NULL: fill in the launch plan (tile shape, ring depths, shared memory) and return without
 // touching the device — pure host arithmetic, so the CPU test-suite can sweep it (tests/test_abi.py).
-template <int BN, int MODE, bool DROP>
+template <int BN, int MODE, bool DROP, bool LEAKY>
 static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
-  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE, DROP>;
+  void (*kern)(tc::Params) = tc::gemm_tc_kernel<BN, MODE, DROP, LEAKY>;
   // opt-in to > 48 KB of dynamic shared memory, for the largest ring this instantiation launches with: an
   // idempotent per-process property (C++11 guarantees the initialiser runs once, thread-safely)
   static const cudaError_t attr_rc =
@@ -977,24 +999,26 @@ static int gemm_launch(const tc::Params& p, int grid, cudaStream_t st) {
 }
 
 // One kernel instantiation per tile width and arithmetic mode (tf32 and bf16 single pass, 3xTF32 up to bn = 64),
-// and per dropout: a launch with a dropout mask in its epilogue runs the DROP twin of its instantiation.
+// per dropout (a launch with a dropout mask in its epilogue runs the DROP twin of its instantiation) and per
+// LeakyReLU (a launch with B2_ACT_LEAKY_RELU as act or act_bwd runs the LEAKY twin, so no other launch pays for it).
 typedef int (*GemmLaunch)(const tc::Params&, int, cudaStream_t);
-template <bool DROP>
+template <bool DROP, bool LEAKY>
 static GemmLaunch gemm_inst_t(int bn, int mode) {
   switch (bn * 4 + mode) {
-    case 32 * 4 + tc::TF32: return gemm_launch<32, tc::TF32, DROP>;
-    case 64 * 4 + tc::TF32: return gemm_launch<64, tc::TF32, DROP>;
-    case 128 * 4 + tc::TF32: return gemm_launch<128, tc::TF32, DROP>;
-    case 32 * 4 + tc::BF16: return gemm_launch<32, tc::BF16, DROP>;
-    case 64 * 4 + tc::BF16: return gemm_launch<64, tc::BF16, DROP>;
-    case 128 * 4 + tc::BF16: return gemm_launch<128, tc::BF16, DROP>;
-    case 32 * 4 + tc::X3: return gemm_launch<32, tc::X3, DROP>;
-    case 64 * 4 + tc::X3: return gemm_launch<64, tc::X3, DROP>;
+    case 32 * 4 + tc::TF32: return gemm_launch<32, tc::TF32, DROP, LEAKY>;
+    case 64 * 4 + tc::TF32: return gemm_launch<64, tc::TF32, DROP, LEAKY>;
+    case 128 * 4 + tc::TF32: return gemm_launch<128, tc::TF32, DROP, LEAKY>;
+    case 32 * 4 + tc::BF16: return gemm_launch<32, tc::BF16, DROP, LEAKY>;
+    case 64 * 4 + tc::BF16: return gemm_launch<64, tc::BF16, DROP, LEAKY>;
+    case 128 * 4 + tc::BF16: return gemm_launch<128, tc::BF16, DROP, LEAKY>;
+    case 32 * 4 + tc::X3: return gemm_launch<32, tc::X3, DROP, LEAKY>;
+    case 64 * 4 + tc::X3: return gemm_launch<64, tc::X3, DROP, LEAKY>;
     default: return nullptr;
   }
 }
-static GemmLaunch gemm_inst(int bn, int mode, bool drop) {
-  return drop ? gemm_inst_t<true>(bn, mode) : gemm_inst_t<false>(bn, mode);
+static GemmLaunch gemm_inst(int bn, int mode, bool drop, bool leaky) {
+  if (leaky) return drop ? gemm_inst_t<true, true>(bn, mode) : gemm_inst_t<false, true>(bn, mode);
+  return drop ? gemm_inst_t<true, false>(bn, mode) : gemm_inst_t<false, false>(bn, mode);
 }
 
 static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan) {
@@ -1007,8 +1031,8 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   B2_REQUIRE(M >= 1 && N >= 1 && K >= 1 && ldc >= N, "bad shape");
   B2_REQUIRE(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "shape exceeds 31 bits");
   B2_REQUIRE(lda >= (d->a_mn_major ? M : K) && ldb >= (d->b_mn_major ? N : K), "leading dimension too small");
-  B2_REQUIRE(d->act >= B2_ACT_NONE && d->act <= B2_ACT_SIGMOID, "bad activation code %d", d->act);
-  B2_REQUIRE(d->act_bwd >= B2_ACT_NONE && d->act_bwd <= B2_ACT_SIGMOID, "bad act_bwd code %d", d->act_bwd);
+  B2_REQUIRE(b2_act_ok(d->act), "bad activation code %d", d->act);
+  B2_REQUIRE(b2_act_ok(d->act_bwd), "bad act_bwd code %d", d->act_bwd);
   B2_REQUIRE(d->act_bwd == B2_ACT_NONE || d->ybwd != nullptr, "act_bwd needs ybwd");
   B2_REQUIRE((d->a_small == nullptr) == (d->b_small == nullptr), "3xTF32 needs both small operands");
   B2_REQUIRE(esz == 4 || d->a_small == nullptr, "bf16 operands are single-pass (no small parts)");
@@ -1099,7 +1123,8 @@ static int gemm_tc_impl(const b2_gemm_desc* d, void* stream, b2_gemm_plan* plan)
   B2_REQUIRE(total_tiles < (1ll << 31), "too many tiles");
   p.tiles_m = (int) tiles_m; p.tiles_n = (int) tiles_n; p.splits = splits;
   const int mode = three_pass ? tc::X3 : (esz == 2 ? tc::BF16 : tc::TF32);
-  const GemmLaunch launch = gemm_inst(best_bn, mode, drop);
+  const GemmLaunch launch = gemm_inst(best_bn, mode, drop,
+                                       d->act == B2_ACT_LEAKY_RELU || d->act_bwd == B2_ACT_LEAKY_RELU);
   B2_REQUIRE(launch != nullptr, "no GEMM instantiation for bn %d", best_bn);
   p.ring = tc::ring_layout(best_bn, mode, p.a_mn != 0, p.b_mn != 0);
   B2_REQUIRE(p.ring.stages >= 2 && p.ring.smem <= tc::SMEM_MAX, "tile does not fit shared memory");
@@ -1176,7 +1201,7 @@ extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, i
                                       uint32_t drop_thresh, float drop_scale, void* stream) {
   B2_REQUIRE(x != nullptr, "NULL input");
   B2_REQUIRE(R >= 0 && C >= 0, "bad shape");
-  B2_REQUIRE((act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID) || act == B2_PREP_MUL, "bad activation code %d", act);
+  B2_REQUIRE(b2_act_ok(act) || act == B2_PREP_MUL, "bad activation code %d", act);
   B2_REQUIRE(drop_rng == nullptr || act != B2_PREP_MUL, "B2_PREP_MUL takes no dropout mask");
   B2_REQUIRE(outT_small == nullptr || outT != nullptr, "outT_small needs outT");
   const int rc = check_drop(drop_rng, drop_layer, drop_scale);
@@ -1189,12 +1214,17 @@ extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, i
   if (R == 0 || C == 0) return B2_OK;
   dim3 grid((unsigned) b2_ceil_div(C, 32), (unsigned) b2_ceil_div(R, 32));
   B2_REQUIRE(grid.y <= 65535, "too many rows for this launch geometry");
-  if (drop_rng != nullptr)
-    B2_LAUNCH(tc::prep_operand_kernel<true>, grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT, outT_small,
-              colsum, drop_rng, drop_layer, drop_thresh, drop_scale);
-  else
-    B2_LAUNCH(tc::prep_operand_kernel<false>, grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT, outT_small,
-              colsum, drop_rng, drop_layer, drop_thresh, drop_scale);
+#define PREP_LAUNCH(DROP, LEAKY)                                                                                 \
+  B2_LAUNCH((tc::prep_operand_kernel<DROP, LEAKY>), grid, 256, 0, st, x, y, act, R, C, C, out, out_small, outT,      \
+            outT_small, colsum, drop_rng, drop_layer, drop_thresh, drop_scale)
+  if (act == B2_ACT_LEAKY_RELU) {
+    if (drop_rng != nullptr) PREP_LAUNCH(true, true);
+    else PREP_LAUNCH(false, true);
+  } else {
+    if (drop_rng != nullptr) PREP_LAUNCH(true, false);
+    else PREP_LAUNCH(false, false);
+  }
+#undef PREP_LAUNCH
   B2_CUDA_LAUNCH_CHECK("b2_prep_operand");
   return B2_OK;
 }
@@ -1202,11 +1232,14 @@ extern "C" B2_API int b2_prep_operand(const float* x, const float* y, int act, i
 extern "C" B2_API int b2_head_fwd(const float* x, const float* w, const float* b, int64_t M, int K, int act,
                                   float* y, void* stream) {
   B2_REQUIRE(x && w && y, "NULL pointer");
-  B2_REQUIRE(K >= 1 && act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad K/act");
+  B2_REQUIRE(K >= 1 && b2_act_ok(act), "bad K/act");
   if (M <= 0) return B2_OK;
   int64_t blocks = b2_ceil_div(M * 32, 256);
   if (blocks > (int64_t) B2_NUM_SMS * 8) blocks = (int64_t) B2_NUM_SMS * 8;
-  B2_LAUNCH(tc::head_fwd_kernel, (int) blocks, 256, 0, (cudaStream_t) stream, x, w, b, M, K, act, y);
+  if (act == B2_ACT_LEAKY_RELU)
+    B2_LAUNCH(tc::head_fwd_kernel<true>, (int) blocks, 256, 0, (cudaStream_t) stream, x, w, b, M, K, act, y);
+  else
+    B2_LAUNCH(tc::head_fwd_kernel<false>, (int) blocks, 256, 0, (cudaStream_t) stream, x, w, b, M, K, act, y);
   B2_CUDA_LAUNCH_CHECK("b2_head_fwd");
   return B2_OK;
 }
@@ -1219,9 +1252,9 @@ extern "C" B2_API int b2_head_bwd(const float* x, const float* w, const float* y
 
 // head_bwd_kernel stages 2 * K floats (the partial sums of gw and gb_prev) in dynamic shared memory.  A launch whose
 // dynamic and static shared memory together pass the default 48 KB per block needs the instantiation's opt-in first.
-template <bool DROP>
+template <bool DROP, bool LEAKY>
 static int head_bwd_smem_optin(size_t dyn) {
-  const void* kern = (const void*) tc::head_bwd_kernel<DROP>;
+  const void* kern = (const void*) tc::head_bwd_kernel<DROP, LEAKY>;
   cudaFuncAttributes fa;
   cudaError_t e = cudaFuncGetAttributes(&fa, kern);
   if (e == cudaSuccess && fa.sharedSizeBytes + dyn > 48 * 1024)
@@ -1237,8 +1270,8 @@ extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float
                                      void* stream) {
   B2_REQUIRE(x && w && gy && gw, "NULL pointer");
   B2_REQUIRE(K >= 1 && K <= B2_HEAD_MAX_K, "K=%d outside [1, B2_HEAD_MAX_K=%d]", K, B2_HEAD_MAX_K);
-  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_SIGMOID, "bad activation code %d", act);
-  B2_REQUIRE(prev_act >= B2_ACT_NONE && prev_act <= B2_ACT_SIGMOID, "bad prev_act");
+  B2_REQUIRE(b2_act_ok(act), "bad activation code %d", act);
+  B2_REQUIRE(b2_act_ok(prev_act), "bad prev_act");
   B2_REQUIRE(act == B2_ACT_NONE || y != nullptr, "activation backward needs y");
   B2_REQUIRE(gx != nullptr || (gx_small == nullptr && gb_prev == nullptr && prev_act == B2_ACT_NONE &&
                                prev_drop_rng == nullptr),
@@ -1260,16 +1293,23 @@ extern "C" B2_API int b2_head_bwd_ex(const float* x, const float* w, const float
   ctas = b2_ceil_div(M, rows_per_cta);
   const float* y_arg = (act == B2_ACT_NONE) ? nullptr : y;
   const size_t smem = 2 * sizeof(float) * (size_t) K;
-  const int smem_rc = prev_drop_rng != nullptr ? head_bwd_smem_optin<true>(smem) : head_bwd_smem_optin<false>(smem);
-  if (smem_rc != B2_OK) return smem_rc;
-  if (prev_drop_rng != nullptr)
-    B2_LAUNCH(tc::head_bwd_kernel<true>, (int) ctas, 256, smem, st,
-              x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
-              prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
-  else
-    B2_LAUNCH(tc::head_bwd_kernel<false>, (int) ctas, 256, smem, st,
-              x, w, y_arg, gy, M, K, act, rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev,
-              prev_drop_rng, prev_drop_layer, prev_drop_thresh, prev_drop_scale);
+  const bool leaky = act == B2_ACT_LEAKY_RELU || prev_act == B2_ACT_LEAKY_RELU;
+#define HEAD_BWD(DROP, LEAKY)                                                                                      \
+  do {                                                                                                             \
+    const int smem_rc = head_bwd_smem_optin<DROP, LEAKY>(smem);                                                    \
+    if (smem_rc != B2_OK) return smem_rc;                                                                          \
+    B2_LAUNCH((tc::head_bwd_kernel<DROP, LEAKY>), (int) ctas, 256, smem, st, x, w, y_arg, gy, M, K, act,           \
+              rows_per_cta, gx, gw, gb, prev_act, gx_small, gb_prev, prev_drop_rng, prev_drop_layer,               \
+              prev_drop_thresh, prev_drop_scale);                                                                  \
+  } while (0)
+  if (leaky) {
+    if (prev_drop_rng != nullptr) HEAD_BWD(true, true);
+    else HEAD_BWD(false, true);
+  } else {
+    if (prev_drop_rng != nullptr) HEAD_BWD(true, false);
+    else HEAD_BWD(false, false);
+  }
+#undef HEAD_BWD
   B2_CUDA_LAUNCH_CHECK("b2_head_bwd");
   return B2_OK;
 }

@@ -5,6 +5,7 @@ tape; all arithmetic happens in libfuxictr_b200.so.  Every function requires CUD
 tensors and raises otherwise — there is no eager/CPU fallback on this path.
 """
 import ctypes
+import math
 import os
 import weakref
 
@@ -1696,6 +1697,286 @@ def self_attention_layer(x, w_q, w_k, w_v, w_res=None, num_heads=1, use_residual
     scale = float((A // num_heads) ** 0.5) if use_scale else 0.0
     cfg = (num_heads, scale, float(eps), res_mode, drop, want_aux)
     return _SelfAttentionLayer.apply(x, cfg, w_q, w_k, w_v, w_res, gamma, beta)
+
+
+# --------------------------------------------------------------------------------------
+# BST (include/fuxictr_b200.h "BST")
+# --------------------------------------------------------------------------------------
+BST_POOL = {"mean": _lib.B2_BST_POOL_MEAN, "sum": _lib.B2_BST_POOL_SUM, "target": _lib.B2_BST_POOL_TARGET}
+
+
+def bst_bound(seq_len, model_dim, num_heads, parts=1, heads_apply=True):
+    """None when the BST kernels cover L = seq_len tokens of width model_dim in num_heads heads, built from `parts`
+    fields per token; else the bound it breaks.  heads_apply=False: the kernels that see no heads (tokens, pooling)."""
+    if not 2 <= seq_len <= _lib.B2_BST_MAX_LEN:
+        return "max_len + 1 must lie in [2, %d], got %d" % (_lib.B2_BST_MAX_LEN, seq_len)
+    if not 1 <= model_dim <= _lib.B2_BST_MAX_DIM:
+        return "model_dim must lie in [1, %d], got %d" % (_lib.B2_BST_MAX_DIM, model_dim)
+    if not 1 <= parts <= _lib.B2_BST_MAX_PARTS:
+        return "a token takes 1 to %d fields, got %d" % (_lib.B2_BST_MAX_PARTS, parts)
+    if not heads_apply:
+        return None
+    if not 1 <= num_heads <= _lib.B2_BST_MAX_HEADS:
+        return "num_heads must lie in [1, %d], got %d" % (_lib.B2_BST_MAX_HEADS, num_heads)
+    if model_dim % num_heads:
+        return "num_heads=%d does not divide model_dim=%d" % (num_heads, model_dim)
+    if model_dim // num_heads > _lib.B2_BST_MAX_HEAD_DIM:
+        return "the head width model_dim / num_heads must be at most %d, got %d" % (_lib.B2_BST_MAX_HEAD_DIM,
+                                                                                 model_dim // num_heads)
+    return None
+
+
+def _set_aux_hint(out, aux):
+    """The next GEMM's make_aux(out) finds the operand copy its producer wrote."""
+    if aux is not None:
+        out._b2_aux = (_MATMUL["mode"], aux, out._version)
+
+
+def _arr(ctype, values):
+    return (ctype * len(values))(*values)
+
+
+class _BstTokens(torch.autograd.Function):
+    """X (B L, md): per sample the L - 1 history tokens [seq_0[b, t] .. | pos[t]] and the target token
+    [tgt_0[b] .. | pos[L - 1]] (b2_bst_tokens_fwd).  Backward: each view's gradient and the position table's batch sum
+    in one launch (b2_bst_tokens_bwd)."""
+
+    @staticmethod
+    def forward(ctx, cfg, pos, *views):
+        want_aux, = cfg
+        nf = len(views) // 2
+        # a view's samples may lie at any pitch (an arena slice, a sharded front's landed rows); within a sample
+        # the tokens must be contiguous
+        seqs = [v if (v.dtype == torch.float32 and v.stride(2) == 1 and v.stride(1) == v.shape[2]) else
+                v.float().contiguous() for v in views[:nf]]
+        tgts = [v if (v.dtype == torch.float32 and v.stride(1) == 1) else v.float().contiguous() for v in views[nf:]]
+        B, Lm1, D = seqs[0].shape
+        L = Lm1 + 1
+        md = D * (nf + (pos is not None))
+        dev = seqs[0].device
+        out = torch.empty((B * L, md), dtype=torch.float32, device=dev)
+        ctx.shape = (B, L, D, nf, pos is not None)
+        ctx.pos = pos
+        if B == 0:
+            return out
+        aux = empty_aux(B * L, md, dev) if want_aux else None
+        _lib.call("b2_bst_tokens_fwd", _arr(ctypes.c_void_p, [v.data_ptr() for v in seqs]),
+                  _arr(ctypes.c_int64, [v.stride(0) for v in seqs]), _arr(ctypes.c_void_p, [v.data_ptr() for v in tgts]),
+                  _arr(ctypes.c_int64, [v.stride(0) for v in tgts]), nf, _ptr(_f32c(pos) if pos is not None else None),
+                  B, L, D, _ptr(out), *_aux_args(aux), _stream())
+        _set_aux_hint(out, aux)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        B, L, D, nf, use_pos = ctx.shape
+        dev = g.device
+        dseq = [torch.empty((B, L - 1, D), dtype=torch.float32, device=dev) for _ in range(nf)]
+        dtgt = [torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(nf)]
+        dpos = None
+        if use_pos:
+            dpos = _grad_buffer(ctx.pos, zero=True) if ctx.needs_input_grad[1] else torch.zeros_like(ctx.pos)
+        if B > 0:
+            _lib.call("b2_bst_tokens_bwd", _ptr(_f32c(g)), None, B, L, D, nf, int(use_pos),
+                      _arr(ctypes.c_void_p, [t.data_ptr() for t in dseq]), _arr(ctypes.c_void_p, [t.data_ptr() for t in dtgt]),
+                      _ptr(dpos), _stream())
+        return (None, dpos if use_pos and ctx.needs_input_grad[1] else None) + tuple(dseq) + tuple(dtgt)
+
+
+def bst_tokens(sequence_embs, target_embs, position_emb=None, want_aux=False):
+    """The (B L, model_dim) token matrix of one (target, sequence) pair: sequence_embs nf views (B, L - 1, D),
+    target_embs nf views (B, D) (a tuple of fields: their embeddings side by side), position_emb (L, D) or None.
+    want_aux: also write the matrix's GEMM operand copy for the in-projection."""
+    seqs, tgts = list(sequence_embs), list(target_embs)
+    _require_cuda(*(seqs + tgts + [position_emb]))
+    if len(seqs) != len(tgts) or not seqs:
+        raise ValueError("bst_tokens: %d sequence fields and %d target fields" % (len(seqs), len(tgts)))
+    B, Lm1, D = seqs[0].shape
+    for v in seqs:
+        if v.dim() != 3 or tuple(v.shape) != (B, Lm1, D):
+            raise ValueError("bst_tokens: sequence embeddings %s differ" % [tuple(t.shape) for t in seqs])
+    for v in tgts:
+        if tuple(v.shape) != (B, D):
+            raise ValueError("bst_tokens: target embeddings %s are not (%d, %d)" % ([tuple(t.shape) for t in tgts], B, D))
+    if position_emb is not None and tuple(position_emb.shape) != (Lm1 + 1, D):
+        raise ValueError("bst_tokens: position_emb%s is not (%d, %d)" % (tuple(position_emb.shape), Lm1 + 1, D))
+    md = D * (len(seqs) + (position_emb is not None))
+    bound = bst_bound(Lm1 + 1, md, 1, len(seqs), heads_apply=False)
+    if bound is not None:
+        raise NotImplementedError("BST kernels: " + bound)
+    return _BstTokens.apply((want_aux,), position_emb, *(seqs + tgts))
+
+
+class _BstAttention(torch.autograd.Function):
+    """ctx (B L, md) of the masked multi-head self-attention on QKV (B L, 3 md) (b2_bst_attn_fwd), the probabilities
+    never stored; backward: dQKV in one launch (b2_bst_attn_bwd), which feeds the in-projection's dgrad and wgrad."""
+
+    @staticmethod
+    def forward(ctx, qkv, valid, cfg):
+        B, L, md, heads, causal, scale, drop, want_aux = cfg
+        dev = qkv.device
+        out = torch.empty((B * L, md), dtype=torch.float32, device=dev)
+        ctx.cfg = cfg
+        if B == 0:
+            return out
+        qkv = _f32c(qkv)
+        aux = empty_aux(B * L, md, dev) if want_aux else None
+        smax = torch.empty((B, heads, L), dtype=torch.float32, device=dev)
+        ssum = torch.empty_like(smax)
+        _lib.call("b2_bst_attn_fwd", _ptr(qkv), _ptr(valid), B, L, md, heads, int(causal), scale, *_drop_args(drop),
+                  _ptr(out), *_aux_args(aux), _ptr(smax), _ptr(ssum), _stream())
+        _set_aux_hint(out, aux)
+        ctx.save_for_backward(qkv, valid, out, smax, ssum)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        B, L, md, heads, causal, scale, drop, _ = ctx.cfg
+        if B == 0:
+            return torch.zeros((0, 3 * md), dtype=torch.float32, device=g.device), None, None
+        qkv, valid, out, smax, ssum = ctx.saved_tensors
+        dqkv = torch.empty_like(qkv)
+        _lib.call("b2_bst_attn_bwd", _ptr(qkv), _ptr(valid), _ptr(out), _ptr(_f32c(g)), _ptr(smax), _ptr(ssum), B, L,
+                  md, heads, int(causal), scale, *_drop_args(drop), _ptr(dqkv), *_aux_args(None), _stream())
+        return dqkv, None, None
+
+
+def bst_attention(qkv, valid, batch, seq_len, num_heads, causal=False, dropout=0.0, snapshot=None, layer=0,
+                  want_aux=False):
+    """torch's nn.MultiheadAttention core on the in-projection's output qkv (B L, 3 md) = [Q | K | V]: per head
+    softmax((q sqrt(1 / dh)) k^T + mask) v with BST's mask: key j hidden from query i != j when j is a padded history
+    slot (valid (B, L - 1) uint8, 0 = padding) or, causal, j > i.  dropout > 0: the weights take the mask of layer
+    `layer` of `snapshot` (dropout_snapshot; None: one of its own).  Returns (B L, md), before out_proj."""
+    _require_cuda(qkv, valid)
+    B, L = batch, seq_len
+    md = qkv.shape[1] // 3 if qkv.dim() == 2 else 0
+    if qkv.dim() != 2 or qkv.shape[0] != B * L or qkv.shape[1] != 3 * md:
+        raise ValueError("bst_attention: qkv%s is not (%d, 3 model_dim)" % (tuple(qkv.shape), B * L))
+    if valid.dtype != torch.uint8 or tuple(valid.shape) != (B, L - 1) or not valid.is_contiguous():
+        raise ValueError("bst_attention: valid must be a contiguous (%d, %d) uint8 mask" % (B, L - 1))
+    bound = bst_bound(L, md, num_heads)
+    if bound is not None:
+        raise NotImplementedError("BST kernels: " + bound)
+    drop = None
+    if dropout > 0:
+        if snapshot is None:
+            snapshot, layer = dropout_snapshot(qkv.device, 1), 0
+        drop = (snapshot, layer) + dropout_consts(dropout)
+    scale = float(ctypes.c_float(math.sqrt(1.0 / (md // num_heads))).value)
+    return _BstAttention.apply(qkv, valid, (B, L, md, num_heads, bool(causal), scale, drop, want_aux))
+
+
+class _BstAddNorm(torch.autograd.Function):
+    """out = LN(res + dropout(a)) (b2_bst_addnorm_fwd), each stage optional; backward in one launch
+    (b2_bst_addnorm_bwd): d(res) is dz itself, da the masked dz."""
+
+    @staticmethod
+    def forward(ctx, a, res, cfg, gamma, beta):
+        eps, drop, want_aux = cfg
+        a = _f32c(a)
+        res = _f32c(res) if res is not None else None
+        R, n = a.shape
+        dev = a.device
+        out = torch.empty((R, n), dtype=torch.float32, device=dev)
+        ln = gamma is not None
+        mean = torch.empty(R, dtype=torch.float32, device=dev) if ln else None
+        rstd = torch.empty_like(mean) if ln else None
+        ctx.cfg, ctx.ln_params = cfg, (gamma, beta)
+        ctx.has_res = res is not None
+        if R > 0:
+            aux = empty_aux(R, n, dev) if want_aux else None
+            _lib.call("b2_bst_addnorm_fwd", _ptr(a), _ptr(res), R, n, _ptr(gamma), _ptr(beta), eps, *_drop_args(drop),
+                      _ptr(out), *_aux_args(aux), _ptr(mean), _ptr(rstd), _stream())
+            _set_aux_hint(out, aux)
+        ctx.save_for_backward(a if ln else None, res if ln else None, mean, rstd)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        eps, drop, _ = ctx.cfg
+        gamma, beta = ctx.ln_params
+        a, res, mean, rstd = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        ln = gamma is not None
+        R, n = g.shape
+        dev = g.device
+        dgamma = (_grad_buffer(gamma, zero=True) if need[3] else torch.zeros_like(gamma)) if ln else None
+        dbeta = (_grad_buffer(beta, zero=True) if need[4] else torch.zeros_like(beta)) if ln else None
+        da = torch.empty((R, n), dtype=torch.float32, device=dev)
+        dres = torch.empty_like(da) if (ctx.has_res and drop is not None) else None
+        if R > 0:
+            _lib.call("b2_bst_addnorm_bwd", _ptr(a), _ptr(res), _ptr(_f32c(g)), None, R, n, _ptr(gamma), _ptr(mean),
+                      _ptr(rstd), *_drop_args(drop), _ptr(da), *_aux_args(None), _ptr(dres), _ptr(dgamma),
+                      _ptr(dbeta), _stream())
+        if ctx.has_res and dres is None:
+            dres = da                   # no dropout: the residual's gradient is the same dz
+        return (da, dres if ctx.has_res else None, None, dgamma if ln and need[3] else None,
+                dbeta if ln and need[4] else None)
+
+
+def bst_add_norm(a, res=None, gamma=None, beta=None, eps=1e-5, dropout=0.0, snapshot=None, layer=0, want_aux=False):
+    """LN(res + dropout(a)) on (rows, n): TransformerBlock's `s = LN1(x + dropout1(attn))` and
+    `LN2(s + dropout2(ffn))`; res None: no residual; gamma, beta None: no LayerNorm.  dropout > 0: the mask of layer
+    `layer` of `snapshot`.  want_aux: also write the output's GEMM operand copy."""
+    _require_cuda(a, res, gamma, beta)
+    if a.dim() != 2 or (res is not None and res.shape != a.shape):
+        raise ValueError("bst_add_norm: a%s and res%s" % (tuple(a.shape), None if res is None else tuple(res.shape)))
+    n = a.shape[1]
+    if not 1 <= n <= _lib.B2_BST_MAX_DIM:
+        raise NotImplementedError("BST kernels: model_dim must lie in [1, %d], got %d" % (_lib.B2_BST_MAX_DIM, n))
+    if (gamma is None) != (beta is None) or (gamma is not None and (gamma.numel() != n or beta.numel() != n)):
+        raise ValueError("bst_add_norm: the LayerNorm needs a weight and a bias of %d" % n)
+    drop = None
+    if dropout > 0:
+        if snapshot is None:
+            snapshot, layer = dropout_snapshot(a.device, 1), 0
+        drop = (snapshot, layer) + dropout_consts(dropout)
+    return _BstAddNorm.apply(a, res, (float(eps), drop, want_aux), gamma, beta)
+
+
+class _BstPool(torch.autograd.Function):
+    """(B, md) pooling of the L tokens of x (B L, md) (b2_bst_pool_fwd / _bwd)."""
+
+    @staticmethod
+    def forward(ctx, x, valid, cfg):
+        B, L, mode = cfg
+        md = x.shape[1]
+        out = torch.empty((B, md), dtype=torch.float32, device=x.device)
+        ctx.cfg = cfg
+        ctx.save_for_backward(valid)
+        if B > 0:
+            _lib.call("b2_bst_pool_fwd", _ptr(_f32c(x)), _ptr(valid), B, L, md, mode, _ptr(out), md, _stream())
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        B, L, mode = ctx.cfg
+        valid, = ctx.saved_tensors
+        md = g.shape[1]
+        dx = torch.empty((B * L, md), dtype=torch.float32, device=g.device)
+        if B > 0:
+            g = _f32c(g)
+            _lib.call("b2_bst_pool_bwd", _ptr(g), g.stride(0), _ptr(valid), B, L, md, mode, _ptr(dx), _stream())
+        return dx, None, None
+
+
+def bst_pooling(x, valid, batch, seq_len, pooling="mean"):
+    """BST.sequence_pooling of the transformer output x (B L, md): "mean" / "sum" over the real history slots and the
+    target (mean divides by their count + 1e-12), "target" the last token, "concat" all L tokens flattened (a view)."""
+    _require_cuda(x, valid)
+    B, L = batch, seq_len
+    if x.dim() != 2 or x.shape[0] != B * L:
+        raise ValueError("bst_pooling: x%s is not (%d, model_dim)" % (tuple(x.shape), B * L))
+    if pooling == "concat":
+        return x.reshape(B, L * x.shape[1])
+    if pooling not in BST_POOL:
+        raise ValueError("seq_pooling_type={} not supported.".format(pooling))
+    if valid.dtype != torch.uint8 or tuple(valid.shape) != (B, L - 1) or not valid.is_contiguous():
+        raise ValueError("bst_pooling: valid must be a contiguous (%d, %d) uint8 mask" % (B, L - 1))
+    bound = bst_bound(L, x.shape[1], 1, heads_apply=False)
+    if bound is not None:
+        raise NotImplementedError("BST kernels: " + bound)
+    return _BstPool.apply(x, valid, (B, L, BST_POOL[pooling]))
 
 
 # --------------------------------------------------------------------------------------

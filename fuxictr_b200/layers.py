@@ -24,6 +24,7 @@ Reference files (relative to the reference root):
   MultiHeadSelfAttention                   model_zoo/AutoInt/src/AutoInt.py
   FactorizationMachineBlock / LinearCompressionBlock / WuKongLayer model_zoo/WuKong/src/WuKong.py
   FeatureGating / FactorizedInteraction / FinalBlock model_zoo/FinalNet/src/FinalNet.py
+  TransformerBlock / BehaviorTransformer   model_zoo/BST/src/BST.py
 """
 import sys
 from collections import OrderedDict
@@ -36,7 +37,7 @@ from torch import nn
 from . import _lib
 from . import functional as F2
 from ._lib import (B2_POOL_NONE, B2_POOL_SUM, B2_POOL_MEAN, B2_ACT_NONE, B2_ACT_RELU,
-                   B2_ACT_SIGMOID, FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT)
+                   B2_ACT_SIGMOID, B2_ACT_LEAKY_RELU, FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT)
 
 layers = sys.modules[__name__]  # so feature_encoder strings like "layers.MaskedSumPooling()" resolve
 
@@ -1221,3 +1222,112 @@ class FinalBlock(nn.Module):
 
     def forward(self, X):
         return self.run(X)
+
+
+class TransformerBlock(nn.Module):
+    """model_zoo/BST/src/BST.py, TransformerBlock: s = LN1(x [+ dropout1(MHA(x))]), out = LN2(s [+ dropout2(FFN(s))]) with
+    FFN = Linear -> LeakyReLU -> Linear.  `attention` is a real nn.MultiheadAttention and holds the projections
+    (in_proj_weight = [W_q; W_k; W_v], in_proj_bias, out_proj) and the attention dropout; the kernels read it, its
+    forward is never called.  On the kernels (run): the in-projection GEMM, the masked attention row kernel, the
+    out-projection GEMM, the residual + dropout + LayerNorm row kernel, the FFN as one MLP chain with LeakyReLU
+    (B2_ACT_LEAKY_RELU) in its first epilogue and dropout2 in its second, and the residual + LayerNorm row kernel.
+    Constructor, children, registration order and initial draws are the reference's."""
+
+    def __init__(self, model_dim=64, ffn_dim=64, num_heads=8, attn_dropout=0.0, net_dropout=0.0, layer_norm=True,
+                 use_residual=True):
+        super(TransformerBlock, self).__init__()
+        self.attention = nn.MultiheadAttention(model_dim, num_heads=num_heads, dropout=attn_dropout, batch_first=True)
+        self.ffn = nn.Sequential(nn.Linear(model_dim, ffn_dim), nn.LeakyReLU(), nn.Linear(ffn_dim, model_dim))
+        self.use_residual = use_residual
+        self.dropout1 = nn.Dropout(net_dropout)
+        self.dropout2 = nn.Dropout(net_dropout)
+        self.layer_norm1 = nn.LayerNorm(model_dim) if layer_norm else None
+        self.layer_norm2 = nn.LayerNorm(model_dim) if layer_norm else None
+
+    def _p(self, drop):
+        return drop.p if (drop.training and drop.p > 0) else 0.0
+
+    def run(self, x, valid, batch, seq_len, causal=False, snapshot=None, layer=0, want_aux=False):
+        """x (B L, model_dim) -> (B L, model_dim).  valid (B, L - 1) uint8: 1 for a real history slot.  In training
+        mode with dropout the attention weights take the mask of layer `layer` of `snapshot` and dropout1 that of
+        layer + 1 (functional.dropout_snapshot; None: their own); dropout2 is the MLP chain's, drawn from the chain's
+        own snapshot (its layer 0).  want_aux: also
+        write the output's GEMM operand copy for a following block.  An empty batch makes no launch."""
+        att = self.attention
+        if not isinstance(self.ffn[1], nn.LeakyReLU) or self.ffn[1].negative_slope != 0.01:
+            raise NotImplementedError("TransformerBlock kernels: the FFN activation must be nn.LeakyReLU(0.01)")
+        if batch == 0:
+            return x.view_as(x)
+        ln1, ln2 = self.layer_norm1, self.layer_norm2
+        W1, W2 = self.ffn[0], self.ffn[2]
+        qkv = F2.linear_act(x, att.in_proj_weight, att.in_proj_bias)
+        ctx = F2.bst_attention(qkv, valid, batch, seq_len, att.num_heads, causal=causal,
+                               dropout=att.dropout if self.training else 0.0, snapshot=snapshot, layer=layer,
+                               want_aux=F2._tc_layer_ok(att.out_proj.weight))
+        attn = F2.linear_act(ctx, att.out_proj.weight, att.out_proj.bias)
+        s = F2.bst_add_norm(attn, x if self.use_residual else None, ln1.weight if ln1 is not None else None,
+                            ln1.bias if ln1 is not None else None, ln1.eps if ln1 is not None else 1e-5,
+                            dropout=self._p(self.dropout1), snapshot=snapshot, layer=layer + 1,
+                            want_aux=F2._tc_layer_ok(W1.weight))
+        p2 = self._p(self.dropout2)
+        f = F2.mlp_chain(s, [(W1.weight, W1.bias, B2_ACT_LEAKY_RELU), (W2.weight, W2.bias, B2_ACT_NONE, p2)])
+        return F2.bst_add_norm(f, s if self.use_residual else None, ln2.weight if ln2 is not None else None,
+                               ln2.bias if ln2 is not None else None, ln2.eps if ln2 is not None else 1e-5,
+                               want_aux=want_aux)
+
+    def forward(self, x, attn_mask=None):
+        raise NotImplementedError("TransformerBlock runs on the kernels through run(x, valid, ...), which takes the "
+                                  "key-padding mask as a (B, L - 1) byte mask instead of a (B H, L, L) attn_mask")
+
+
+class BehaviorTransformer(nn.Module):
+    """model_zoo/BST/src/BST.py, BehaviorTransformer: [tokens | position_emb] through stacked TransformerBlocks.
+    position_emb (seq_len, position_dim) is a trained parameter initialised sinusoidally by its own reset_parameters
+    (RankModel.reset_parameters does not touch it).  In training mode with dropout the blocks draw their attention and
+    dropout1 masks from one dropout snapshot, two layers per block (each FFN chain takes a snapshot of its own)."""
+
+    def __init__(self, seq_len=1, model_dim=64, num_heads=8, stacked_transformer_layers=1, attn_dropout=0.0,
+                 net_dropout=0.0, use_position_emb=True, position_dim=4, layer_norm=True, use_residual=True):
+        super(BehaviorTransformer, self).__init__()
+        self.position_dim = position_dim
+        self.use_position_emb = use_position_emb
+        self.transformer_blocks = nn.ModuleList(TransformerBlock(model_dim=model_dim, ffn_dim=model_dim,
+                                                                 num_heads=num_heads, attn_dropout=attn_dropout,
+                                                                 net_dropout=net_dropout, layer_norm=layer_norm,
+                                                                 use_residual=use_residual)
+                                                for _ in range(stacked_transformer_layers))
+        if self.use_position_emb:
+            self.position_emb = nn.Parameter(torch.Tensor(seq_len, position_dim))
+            self.reset_parameters()
+
+    def reset_parameters(self):
+        """The sinusoidal table: pe[t, 2k] = sin(t w_k), pe[t, 2k + 1] = cos(t w_k), w_k = 10000^(-2k / dim)."""
+        seq_len = self.position_emb.size(0)
+        pe = torch.zeros(seq_len, self.position_dim)
+        position = torch.arange(0, seq_len).float().unsqueeze(1)
+        freq = torch.exp(torch.arange(0, self.position_dim, 2).float() * (-np.log(10000.0) / self.position_dim))
+        pe[:, 0::2] = torch.sin(position * freq)
+        pe[:, 1::2] = torch.cos(position * freq)
+        self.position_emb.data = pe
+
+    def run(self, sequence_embs, target_embs, valid, causal=False, want_aux=False):
+        """The (B L, model_dim) output of the stack on one (target, sequence) pair: sequence_embs the nf (B, L - 1, D)
+        embeddings of the sequence fields, target_embs the nf (B, D) ones of the target fields, valid (B, L - 1)
+        uint8.  want_aux: also write the output's GEMM operand copy."""
+        blocks = list(self.transformer_blocks)
+        B, Lm1 = valid.shape
+        L = Lm1 + 1
+        x = F2.bst_tokens(sequence_embs, target_embs, self.position_emb if self.use_position_emb else None,
+                          want_aux=bool(blocks) and F2._tc_layer_ok(blocks[0].attention.in_proj_weight))
+        snap = None
+        if self.training and blocks and (blocks[0].attention.dropout > 0 or blocks[0]._p(blocks[0].dropout1) > 0):
+            snap = F2.dropout_snapshot(x.device, 2 * len(blocks))
+        for k, blk in enumerate(blocks):
+            last = k + 1 == len(blocks)
+            x = blk.run(x, valid, B, L, causal=causal, snapshot=snap, layer=2 * k,
+                        want_aux=want_aux if last else F2._tc_layer_ok(blocks[k + 1].attention.in_proj_weight))
+        return x
+
+    def forward(self, x, attn_mask=None):
+        raise NotImplementedError("BehaviorTransformer runs on the kernels through run(sequence_embs, target_embs, "
+                                  "valid)")

@@ -19,6 +19,7 @@ same RNG consumption) and nothing else.
   AutoInt      model_zoo/AutoInt/src/AutoInt.py
   WuKong       model_zoo/WuKong/src/WuKong.py
   FinalNet     model_zoo/FinalNet/src/FinalNet.py
+  BST          model_zoo/BST/src/BST.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -30,7 +31,7 @@ from torch import nn
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
-                     FeatureGating, FinalBlock,
+                     FeatureGating, FinalBlock, BehaviorTransformer,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -179,7 +180,7 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong, FinalNet) may be
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong, FinalNet, BST) may be
         sharded: any
         other forward would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
@@ -188,7 +189,7 @@ class RankModel(nn.Module):
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
                                       "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
-                                      "DualMLP, MaskNet, AutoInt, WuKong and FinalNet" % type(self).__name__)
+                                      "DualMLP, MaskNet, AutoInt, WuKong, FinalNet and BST" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -1186,3 +1187,111 @@ class FinalNet(RankModel):
         if self.block_type == "1B":
             return super(FinalNet, self).fused_loss(batch_data, y_true)
         return F2.finalnet_loss(y_true, *self.forward_logits(batch_data))[0]
+
+
+class BST(RankModel):
+    """model_zoo/BST/src/BST.py, BST: per (target, sequence) field pair a BehaviorTransformer over the L = max_len + 1
+    tokens [history | target] (a tuple of fields: their embeddings side by side, then the position embedding), pooled
+    ("mean", "sum", "target" or "concat") into a vector that replaces the sequence fields; the DNN reads the remaining
+    embeddings in FeatureMap order, then the pooled vectors in pair order.  The target fields' embeddings stay in the
+    DNN input too.  Each block runs on the kernels (layers.TransformerBlock); the key-padding mask comes from the
+    first sequence field's ids (0 = padding).  Unknown keyword arguments are accepted and ignored, as the reference's
+    **kwargs are.  Refused: model_dim % num_heads != 0 (the reference's assert), shapes outside functional.bst_bound,
+    lazy tables and enable_sharding(want_fm=True)."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="BST", gpu=-1, dnn_hidden_units=[256, 128, 64], dnn_activations="ReLU",
+                 num_heads=2, stacked_transformer_layers=1, attention_dropout=0, learning_rate=1e-3, embedding_dim=10,
+                 net_dropout=0, batch_norm=False, layer_norm=True, use_residual=True,
+                 bst_target_field=[("item_id", "cate_id")], bst_sequence_field=[("click_history", "cate_history")],
+                 seq_pooling_type="mean", use_position_emb=True, use_causal_mask=False, embedding_regularizer=None,
+                 net_regularizer=None, **kwargs):
+        as_list = lambda v: v if type(v) == list else [v]                       # noqa: E731
+        targets, sequences = as_list(bst_target_field), as_list(bst_sequence_field)
+        assert len(targets) == len(sequences), "len(self.bst_target_field) != len(self.bst_sequence_field)"
+        if seq_pooling_type not in ("mean", "sum", "target", "concat"):
+            raise ValueError("seq_pooling_type={} not supported.".format(seq_pooling_type))
+        dims = []
+        for target, sequence in zip(targets, sequences):
+            names = list(_flatten([sequence]))
+            if len(list(_flatten([target]))) != len(names):
+                raise ValueError("BST: target %r and sequence %r have different numbers of fields" % (target, sequence))
+            model_dim = embedding_dim * (int(use_position_emb) + len(names))
+            seq_len = feature_map.features[names[0]]["max_len"] + 1
+            assert model_dim % num_heads == 0, "embed_dim must be divisible by num_heads"
+            bound = F2.bst_bound(seq_len, model_dim, num_heads, len(names))
+            if bound is not None:
+                raise NotImplementedError("BST kernels: " + bound)
+            dims.append((model_dim, seq_len, len(names)))
+        super(BST, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                  embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                  **kwargs)
+        self.bst_target_field, self.bst_sequence_field = targets, sequences
+        self.use_causal_mask = use_causal_mask
+        self.seq_pooling_type = seq_pooling_type
+        self.embedding_dim = embedding_dim
+        self.num_heads = num_heads
+        self.embedding_layer = FeatureEmbeddingDict(feature_map, embedding_dim)
+        self.transformer_encoders = nn.ModuleList()
+        seq_out_dim = 0
+        for model_dim, seq_len, parts in dims:
+            width = seq_len * model_dim if seq_pooling_type == "concat" else model_dim
+            seq_out_dim += width - parts * embedding_dim
+            self.transformer_encoders.append(
+                BehaviorTransformer(seq_len=seq_len, model_dim=model_dim, num_heads=num_heads,
+                                    stacked_transformer_layers=stacked_transformer_layers,
+                                    attn_dropout=attention_dropout, net_dropout=net_dropout,
+                                    position_dim=embedding_dim, use_position_emb=use_position_emb,
+                                    layer_norm=layer_norm, use_residual=use_residual))
+        self.dnn = MLP_Block(input_dim=feature_map.sum_emb_out_dim() + seq_out_dim, output_dim=1,
+                             hidden_units=dnn_hidden_units, hidden_activations=dnn_activations,
+                             output_activation=self.output_activation, dropout_rates=net_dropout,
+                             batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which BST does not have."""
+        if want_fm:
+            raise ValueError("BST has no FM term: enable_sharding(..., want_fm=False)")
+        return super(BST, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype, want_fm=False)
+
+    def _logit_mlp(self):
+        """dnn without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_dnn")
+        if ent is None:
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(self.dnn.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_dnn"] = ent
+        return ent
+
+    def dnn_input(self, inputs):
+        """The DNN's input (B, width): the embeddings left after the sequence fields are dropped, in FeatureMap order,
+        then each pair's pooled transformer output."""
+        X = self.get_inputs(inputs)
+        front = getattr(self, "_sharded_front", None)
+        if front is not None:       # row-sharded tables: (B, D) / (B, L, D) views of the landed rows
+            from .sharded import sharded_front
+            landed, _ = sharded_front(front, self._batch_matrix(inputs))
+            views = front.field_views(landed)
+            emb = OrderedDict((name, views[name]) for name in self.feature_map.features.keys() if name in views)
+        else:
+            emb = self.embedding_layer(X)
+        pooled = []
+        for enc, target, sequence in zip(self.transformer_encoders, self.bst_target_field, self.bst_sequence_field):
+            tnames, snames = list(_flatten([target])), list(_flatten([sequence]))
+            valid = torch.ne(X[snames[0]], 0).to(torch.uint8)
+            B, L = valid.shape[0], valid.shape[1] + 1
+            out = enc.run([emb[n] for n in snames], [emb[n] for n in tnames], valid, causal=self.use_causal_mask)
+            pooled.append(F2.bst_pooling(out, valid, B, L, self.seq_pooling_type))
+        for sequence in self.bst_sequence_field:
+            for name in _flatten([sequence]):
+                emb.pop(name, None)
+        return torch.cat(list(emb.values()) + pooled, dim=-1)
+
+    def forward_logits(self, inputs):
+        return (self._logit_mlp()(self.dnn_input(inputs)),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}

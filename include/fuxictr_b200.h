@@ -56,6 +56,8 @@ extern "C" {
 #define B2_ACT_NONE 0
 #define B2_ACT_RELU 1
 #define B2_ACT_SIGMOID 2
+#define B2_ACT_LEAKY_RELU 4 /* nn.LeakyReLU(): y = z > 0 ? z : z * B2_LEAKY_SLOPE; its backward reads y (y > 0 iff z > 0) */
+#define B2_LEAKY_SLOPE 0.01f
 #define B2_PREP_MUL 3 /* b2_prep_operand only: v = x * y (plain elementwise product, CrossNetV2 backward) */
 
 #define B2_MAX_FIELDS 128
@@ -572,6 +574,79 @@ B2_API int b2_autoint_bwd(const float* P, const float* X, const float* out, cons
                           float* dbeta, void* stream);
 B2_API int b2_autoint_unpack(const float* dWp, int din, int A, float* gWq, float* gWk, float* gWv, float* gWres,
                              void* stream);
+
+/*
+ * BST, the Behavior Sequence Transformer (model_zoo/BST/src/BST.py): TransformerBlocks over the L = max_len + 1 tokens
+ * of a (target, sequence) pair, model_dim md = D (nf + use_pos) for nf fields per token of width D.  All row-major
+ * fp32.  Token b L + t of X (B L, md) is [seq_0[b, t] .. seq_{nf-1}[b, t] | pos[t]] for t < L - 1 and
+ * [tgt_0[b] .. tgt_{nf-1}[b] | pos[L - 1]] for t = L - 1.  valid (B, L - 1) bytes: 1 for a real history slot,
+ * 0 for padding (sequence id 0).  A block on X, with the caller's GEMMs (bias in their epilogues):
+ *   QKV = X W_in^T + b_in (B L, 3 md)            columns [Q | K | V], head h the columns h dh .. h dh + dh - 1
+ *   ctx = b2_bst_attn_fwd(QKV)                   per head: dropout(softmax((q scale) k^T + mask)) v, scale =
+ *                                                sqrt(1 / dh) as the caller rounds it; key j masked for query i iff
+ *                                                j != i and (j is padding, or causal and j > i)
+ *   s   = b2_bst_addnorm_fwd(ctx W_o^T + b_o, X)  LN1(X + dropout1(.))
+ *   out = b2_bst_addnorm_fwd(FFN(s), s)           LN2(s + FFN(s)), FFN = dropout2(W2 LeakyReLU(W1 s + b1) + b2) as a
+ *                                                two-layer MLP chain (B2_ACT_LEAKY_RELU in the first epilogue)
+ * Saved for the backward: QKV, ctx and the softmax max and sum per (b, h, i) (stat_max, stat_sum (B, H, L)); no
+ * (B H, L, L) tensor is stored.  Attention dropout drops weight (b, h, i, j) with the mask of "Dropout masks" over the
+ * (B H L, L) weights, the add-norm's dropout element (r, c) of its (rows, n) input a; each at counter offset
+ * snapshot offset + drop_layer.  LayerNorm is nn.LayerNorm's (mean first, then the biased variance from the centred
+ * values, eps inside the square root).  Every output with an aux argument (row pitch ld_aux) also receives its GEMM
+ * operand copy: bf16 rounding (aux_dtype B2_BF16) or 3xTF32 small part (B2_F32).
+ * Range: 2 <= L <= B2_BST_MAX_LEN, 1 <= md <= B2_BST_MAX_DIM, 1 <= heads <= B2_BST_MAX_HEADS dividing md with
+ * dh = md / heads <= B2_BST_MAX_HEAD_DIM, 1 <= nf <= B2_BST_MAX_PARTS, batch >= 0 (0: no launch) with batch L < 2^31.
+ * The attention kernels stage 2 L (dh + 1) floats per (sample, head) in shared memory.  Outside the range, or given a
+ * NULL pointer, every entry point returns B2_E_INVALID.
+ * b2_bst_tokens_fwd:  X "=" from nf sequence views seq[f] (B, L - 1, D; sample b at seq[f] + b seq_ld[f], its tokens
+ *   contiguous), nf target views tgt[f] (B, D; row pitch tgt_ld[f]) and the position table pos (L, D; NULL: none).
+ *   seq, seq_ld, tgt, tgt_ld are host arrays of nf entries.
+ * b2_bst_tokens_bwd:  from G = g (+ g2, NULL: none) (B L, md): dseq[f] (B, L - 1, D) and dtgt[f] (B, D) "=" (host
+ *   arrays of device pointers, contiguous), dpos (L, D) "+=" the batch sum of G's position columns (use_pos).
+ * b2_bst_attn_fwd:    ctx (B L, md) and the statistics "=".
+ * b2_bst_attn_bwd:    dQKV (B L, 3 md) "=" [dQ | dK | dV] from dctx and the saved tensors.
+ * b2_bst_addnorm_fwd: out (rows, n) "=" LN(res + dropout(a)); res NULL: no residual; gamma, beta NULL: no LayerNorm
+ *   (then ln_mean, ln_rstd are not written).
+ * b2_bst_addnorm_bwd: from G = g (+ g2): dres "=" dz (NULL: not written), da "=" keep scale dz, with
+ *   dz = LN'(G); dgamma, dbeta (n) "+=" (caller zeroes): a per-CTA sum, then one float atomic per column and CTA.
+ * b2_bst_pool_fwd:    out[b, :] (row pitch ld_out) "=" the pooling of sample b's L tokens of x (B L, md):
+ *   B2_BST_POOL_SUM sum of the real slots and the target, B2_BST_POOL_MEAN that sum / (count + 1e-12),
+ *   B2_BST_POOL_TARGET the last token.  (concat pooling is X's flat view and needs no kernel.)
+ * b2_bst_pool_bwd:    dx (B L, md) "=" from g (row pitch ld_g).
+ */
+#define B2_BST_MAX_LEN 256
+#define B2_BST_MAX_DIM 512
+#define B2_BST_MAX_HEAD_DIM 64
+#define B2_BST_MAX_HEADS 16
+#define B2_BST_MAX_PARTS 8
+#define B2_BST_POOL_MEAN 0
+#define B2_BST_POOL_SUM 1
+#define B2_BST_POOL_TARGET 2
+B2_API int b2_bst_tokens_fwd(const float* const* seq, const int64_t* seq_ld, const float* const* tgt,
+                             const int64_t* tgt_ld, int nf, const float* pos, int64_t batch, int L, int D, float* tok,
+                             void* tok_aux, int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_bst_tokens_bwd(const float* g, const float* g2, int64_t batch, int L, int D, int nf, int use_pos,
+                             float* const* dseq, float* const* dtgt, float* dpos, void* stream);
+B2_API int b2_bst_attn_fwd(const float* qkv, const uint8_t* valid, int64_t batch, int L, int md, int heads, int causal,
+                           float scale, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                           float drop_scale, float* ctx, void* ctx_aux, int aux_dtype, int64_t ld_aux, float* stat_max,
+                           float* stat_sum, void* stream);
+B2_API int b2_bst_attn_bwd(const float* qkv, const uint8_t* valid, const float* ctx, const float* dctx,
+                           const float* stat_max, const float* stat_sum, int64_t batch, int L, int md, int heads,
+                           int causal, float scale, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                           float drop_scale, float* dqkv, void* dqkv_aux, int aux_dtype, int64_t ld_aux, void* stream);
+B2_API int b2_bst_addnorm_fwd(const float* a, const float* res, int64_t rows, int n, const float* gamma,
+                              const float* beta, float eps, const int64_t* drop_rng, int64_t drop_layer,
+                              uint32_t drop_thresh, float drop_scale, float* out, void* out_aux, int aux_dtype,
+                              int64_t ld_aux, float* ln_mean, float* ln_rstd, void* stream);
+B2_API int b2_bst_addnorm_bwd(const float* a, const float* res, const float* g, const float* g2, int64_t rows, int n,
+                              const float* gamma, const float* ln_mean, const float* ln_rstd, const int64_t* drop_rng,
+                              int64_t drop_layer, uint32_t drop_thresh, float drop_scale, float* da, void* da_aux,
+                              int aux_dtype, int64_t ld_aux, float* dres, float* dgamma, float* dbeta, void* stream);
+B2_API int b2_bst_pool_fwd(const float* x, const uint8_t* valid, int64_t batch, int L, int md, int mode, float* out,
+                           int64_t ld_out, void* stream);
+B2_API int b2_bst_pool_bwd(const float* g, int64_t ld_g, const uint8_t* valid, int64_t batch, int L, int md, int mode,
+                           float* dx, void* stream);
 
 /*
  * WuKong's layer (model_zoo/WuKong/src/WuKong.py, WuKongLayer) on x (B, F, D) with rank k, lcb + fmb = Fo output
