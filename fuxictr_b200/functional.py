@@ -1980,6 +1980,241 @@ def bst_pooling(x, valid, batch, seq_len, pooling="mean"):
 
 
 # --------------------------------------------------------------------------------------
+# DIEN (include/fuxictr_b200.h "DIEN")
+# --------------------------------------------------------------------------------------
+DIEN_CELL = {"GRU": _lib.B2_DIEN_GRU, "AUGRU": _lib.B2_DIEN_AUGRU, "AGRU": _lib.B2_DIEN_AGRU}
+
+
+def dien_bound(model_dim, seq_len):
+    """None when the DIEN kernels cover a GRU of width model_dim over seq_len positions, else the bound it breaks."""
+    if not 1 <= model_dim <= _lib.B2_DIEN_MAX_DIM:
+        return "the GRU width model_dim must lie in [1, %d], got %d" % (_lib.B2_DIEN_MAX_DIM, model_dim)
+    if not 1 <= seq_len <= _lib.B2_DIEN_MAX_LEN:
+        return "the sequence's max_len must lie in [1, %d], got %d" % (_lib.B2_DIEN_MAX_LEN, seq_len)
+    return None
+
+
+def _dien_seq(x):
+    """x (B, L, H) as the kernels read it: fp32, each sample's tokens contiguous, samples at any pitch."""
+    if x.dtype == torch.float32 and x.stride(2) == 1 and x.stride(1) == x.shape[2] and x.stride(0) >= x.shape[1] * x.shape[2]:
+        return x
+    return x.float().contiguous()
+
+
+def _param_grad(param, need):
+    return _grad_buffer(param, zero=True) if need else torch.zeros_like(param)
+
+
+class _GruSequence(torch.autograd.Function):
+    """(h_seq (B, L, H), h_last (B, H)) of one GRU over the sequence (b2_gru_fwd); backward: the reverse-time
+    recurrence in one launch (b2_gru_bwd).  With a sink, x's gradient goes into the sink's buffer (x is a shared_grad
+    view) and none is returned."""
+
+    @staticmethod
+    def forward(ctx, x, mask, att, cfg, W_ih, b_ih, W_hh, b_hh):
+        cell, sink = cfg
+        ctx.set_materialize_grads(False)
+        x = _dien_seq(x)
+        B, L, H = x.shape
+        dev = x.device
+        a = _f32c(att) if att is not None else None
+        h_seq = torch.empty((B, L, H), dtype=torch.float32, device=dev)
+        h_last = torch.empty((B, H), dtype=torch.float32, device=dev)
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_gru_fwd", _ptr(x), x.stride(0), _ptr(mask), _ptr(W_ih), _ptr(b_ih), _ptr(W_hh), _ptr(b_hh),
+                      _ptr(a), cell, B, L, H, _ptr(h_seq), _ptr(h_last), _stream())
+        ctx.cfg = cfg
+        ctx.params = (W_ih, b_ih, W_hh, b_hh)
+        ctx.save_for_backward(x, mask, a, h_seq)
+        return h_seq, h_last
+
+    @staticmethod
+    def backward(ctx, dh_seq, dh_last):
+        cell, sink = ctx.cfg
+        x, mask, a, h_seq = ctx.saved_tensors
+        W_ih, b_ih, W_hh, b_hh = ctx.params
+        need = ctx.needs_input_grad
+        B, L, H = x.shape
+        if sink is not None:
+            dx, acc = sink.target(h_seq)
+        else:
+            dx, acc = torch.empty((B, L, H), dtype=torch.float32, device=x.device), False
+        da = torch.empty((B, L), dtype=torch.float32, device=x.device) if a is not None else None
+        gW_ih, gb_ih, gW_hh, gb_hh = (_param_grad(p, need[4 + i]) for i, p in enumerate(ctx.params))
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_gru_bwd", _ptr(x), x.stride(0), _ptr(mask), _ptr(W_ih), _ptr(b_ih), _ptr(W_hh), _ptr(b_hh),
+                      _ptr(a), cell, B, L, H, _ptr(h_seq), _ptr(_f32c(dh_seq) if dh_seq is not None else None),
+                      _ptr(_f32c(dh_last) if dh_last is not None else None), _ptr(dx), int(acc), _ptr(da), _ptr(gW_ih),
+                      _ptr(gb_ih), _ptr(gW_hh), _ptr(gb_hh), _stream())
+        grads = tuple(g if need[4 + i] else None for i, g in enumerate((gW_ih, gb_ih, gW_hh, gb_hh)))
+        return (dx if sink is None else None, None, da if a is not None and need[2] else None, None) + grads
+
+
+def _dien_mask(mask, B, L):
+    if mask.dtype != torch.uint8 or tuple(mask.shape) != (B, L) or not mask.is_contiguous():
+        raise ValueError("DIEN: the mask must be a contiguous (%d, %d) uint8 tensor" % (B, L))
+    return mask
+
+
+def gru_sequence(x, mask, W_ih, b_ih, W_hh, b_hh, cell="GRU", att=None, sink=None):
+    """One GRU over x (B, L, H) from h = 0: (h_seq (B, L, H), h_last (B, H)).  mask (B, L) uint8: a sample's length is
+    its number of non-zero bytes (pad_mask.sum(1)), the recurrence runs over positions [0, len) and h_seq is zero from
+    len on; h_last is the state after step len - 1, zero for an empty history (pack_padded_sequence, nn.GRU,
+    pad_packed_sequence and DIEN.get_unmasked_tensor).  cell: "GRU" (nn.GRU's gates r, z, n), "AUGRU" or "AGRU"
+    (DIEN's AUGRUCell / AGRUCell, chunks u, r, n of x2h / h2h, with the attention att (B, L)).  sink: x is a
+    shared_grad view whose gradient this adds into the sink's buffer."""
+    _require_cuda(x, mask, W_ih, b_ih, W_hh, b_hh, att)
+    if cell not in DIEN_CELL:
+        raise ValueError("gru_sequence: cell must be one of %s, got %r" % (sorted(DIEN_CELL), cell))
+    if x.dim() != 3:
+        raise ValueError("gru_sequence: x%s is not (B, L, H)" % (tuple(x.shape),))
+    B, L, H = x.shape
+    bound = dien_bound(H, L)
+    if bound is not None:
+        raise NotImplementedError("DIEN kernels: " + bound)
+    _dien_mask(mask, B, L)
+    if tuple(W_ih.shape) != (3 * H, H) or tuple(W_hh.shape) != (3 * H, H) or b_ih.numel() != 3 * H \
+            or b_hh.numel() != 3 * H:
+        raise ValueError("gru_sequence: the weights must be (3H, H) and the biases (3H,) for H = %d" % H)
+    if (cell == "GRU") != (att is None) or (att is not None and tuple(att.shape) != (B, L)):
+        raise ValueError("gru_sequence: AUGRU and AGRU take an attention (%d, %d), GRU none" % (B, L))
+    return _GruSequence.apply(x, mask, att, (DIEN_CELL[cell], sink), W_ih, b_ih, W_hh, b_hh)
+
+
+class _DienScores(torch.autograd.Function):
+    """s (B, L) = <h_t, W t> mask (bilinear) or <h_t, t> mask (dot) (b2_dien_scores_fwd); backward: dh added into the
+    sink's buffer (or returned), dt, and dW = dq^T t on the SIMT GEMM."""
+
+    @staticmethod
+    def forward(ctx, h, target, mask, sink, W):
+        B, L, H = h.shape
+        dev = h.device
+        t = target if (target.dtype == torch.float32 and target.stride(1) == 1) else target.float().contiguous()
+        q = torch.empty((B, H), dtype=torch.float32, device=dev)
+        s = torch.empty((B, L), dtype=torch.float32, device=dev)
+        Wc = _f32c(W) if W is not None else None
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_dien_scores_fwd", _ptr(h), _ptr(t), t.stride(0), _ptr(Wc), _ptr(mask), B, L, H, _ptr(q), _ptr(s),
+                      _stream())
+        ctx.sink, ctx.W = sink, W
+        ctx.save_for_backward(h, t, mask, q)
+        return s
+
+    @staticmethod
+    def backward(ctx, ds):
+        h, t, mask, q = ctx.saved_tensors
+        sink, W = ctx.sink, ctx.W
+        B, L, H = h.shape
+        if sink is not None:
+            dh, acc = sink.target(h)
+        else:
+            dh, acc = torch.empty_like(h), False
+        dq = torch.empty((B, H), dtype=torch.float32, device=h.device)
+        dt = torch.empty((B, H), dtype=torch.float32, device=h.device)
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_dien_scores_bwd", _ptr(h), _ptr(t), t.stride(0), _ptr(W), _ptr(mask), _ptr(q), _ptr(_f32c(ds)),
+                      B, L, H, _ptr(dh), int(acc), _ptr(dq), _ptr(dt), _stream())
+        gW = None
+        if W is not None and ctx.needs_input_grad[4]:
+            gW = _grad_buffer(W, zero=False)
+            if B > 0:
+                gemm_f32(dq, t, gW, a_t=True)
+            else:
+                gW.zero_()
+        return (dh if sink is None else None), dt, None, None, gW
+
+
+def dien_scores(interest, target, mask, W_kernel=None, sink=None):
+    """AttentionLayer's bilinear (W_kernel (H, H)) or dot (W_kernel None) scores on the interests (B, L, H) against
+    the target (B, H), times mask (B, L) uint8: (B, L).  sink: interest is a shared_grad view."""
+    _require_cuda(interest, target, mask, W_kernel)
+    if interest.dim() != 3:
+        raise ValueError("dien_scores: interest%s is not (B, L, H)" % (tuple(interest.shape),))
+    B, L, H = interest.shape
+    bound = dien_bound(H, L)
+    if bound is not None:
+        raise NotImplementedError("DIEN kernels: " + bound)
+    _dien_mask(mask, B, L)
+    if tuple(target.shape) != (B, H) or (W_kernel is not None and tuple(W_kernel.shape) != (H, H)):
+        raise ValueError("dien_scores: target%s or W_kernel does not match H = %d" % (tuple(target.shape), H))
+    return _DienScores.apply(_f32c(interest), target, mask, sink, W_kernel)
+
+
+def dien_softmax(scores, mask):
+    """softmax_L(s mask - 1e9 (1 - mask)), AttentionLayer's use_attention_softmax (b2_din_softmax_fwd / _bwd)."""
+    return _DinSoftmax.apply(scores, mask)
+
+
+class _DienDinInput(torch.autograd.Function):
+    """[t, h, t - h, t h] ((B L), 4H) of din_attention (b2_din_input_fwd); backward adds dh into the sink's buffer."""
+
+    @staticmethod
+    def forward(ctx, target, hist, sink):
+        target = _f32c(target)
+        B, L, d = hist.shape
+        out = torch.empty((B * L, 4 * d), dtype=torch.float32, device=hist.device)
+        _lib.call("b2_din_input_fwd", _ptr(target), _ptr(hist), B, L, d, _ptr(out), _stream())
+        ctx.sink = sink
+        ctx.save_for_backward(target, hist)
+        return out
+
+    @staticmethod
+    def backward(ctx, gin):
+        target, hist = ctx.saved_tensors
+        B, L, d = hist.shape
+        gt = torch.empty_like(target)
+        gh, acc = ctx.sink.target(hist)
+        _lib.call("b2_din_input_bwd", _ptr(target), _ptr(hist), _ptr(_f32c(gin)), B, L, d, _ptr(gt), _ptr(gh),
+                  int(acc), _stream())
+        return gt, None, None
+
+
+def dien_din_input(target, interest, sink):
+    """din_attention's MLP input from the target (B, H) and the interests (B, L, H), a shared_grad view with its sink."""
+    _require_cuda(target, interest)
+    return _DienDinInput.apply(target, _f32c(interest), sink)
+
+
+class _DienSumPool(torch.autograd.Function):
+    """[sum_t x_t | t * sum_t x_t] (B, 2H) of DIEN's enable_sum_pooling (b2_dien_sum_pool_fwd / _bwd)."""
+
+    @staticmethod
+    def forward(ctx, x, target):
+        x = x.float().contiguous()
+        t = target if (target.dtype == torch.float32 and target.stride(1) == 1) else target.float().contiguous()
+        B, L, H = x.shape
+        out = torch.empty((B, 2 * H), dtype=torch.float32, device=x.device)
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_dien_sum_pool_fwd", _ptr(x), _ptr(t), t.stride(0), B, L, H, _ptr(out), 2 * H, _stream())
+        ctx.save_for_backward(x, t)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, t = ctx.saved_tensors
+        B, L, H = x.shape
+        g = _f32c(g)
+        dx = torch.empty_like(x)
+        dt = torch.empty((B, H), dtype=torch.float32, device=x.device)
+        if B > 0:       # an empty batch makes no launch
+            _lib.call("b2_dien_sum_pool_bwd", _ptr(x), _ptr(t), t.stride(0), _ptr(g), g.stride(0), B, L, H, _ptr(dx),
+                      _ptr(dt), 0, _stream())
+        return dx, dt
+
+
+def dien_sum_pool(sequence_emb, target):
+    """(B, 2H): MaskedSumPooling of the zero-padded sequence (B, L, H) and its product with the target (B, H)."""
+    _require_cuda(sequence_emb, target)
+    B, L, H = sequence_emb.shape
+    bound = dien_bound(H, L)
+    if bound is not None:
+        raise NotImplementedError("DIEN kernels: " + bound)
+    if tuple(target.shape) != (B, H):
+        raise ValueError("dien_sum_pool: target%s is not (%d, %d)" % (tuple(target.shape), B, H))
+    return _DienSumPool.apply(sequence_emb, target)
+
+
+# --------------------------------------------------------------------------------------
 # FinalNet (include/fuxictr_b200.h "FinalNet")
 # --------------------------------------------------------------------------------------
 FINALNET_RESIDUAL = {"concat": _lib.B2_FINALNET_CONCAT, "sum": _lib.B2_FINALNET_SUM}

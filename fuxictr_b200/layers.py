@@ -1331,3 +1331,92 @@ class BehaviorTransformer(nn.Module):
     def forward(self, x, attn_mask=None):
         raise NotImplementedError("BehaviorTransformer runs on the kernels through run(sequence_embs, target_embs, "
                                   "valid)")
+
+
+class AGRUCell(nn.Module):
+    """model_zoo/DIEN/src/DIEN.py, AGRUCell: h' = h + a (n - h), r = s(i_r + h_r), n = tanh(i_n + r h_n), with the
+    chunks u, r, n of x2h(x) and h2h(h) (u unused).  The kernels read x2h and h2h (functional.gru_sequence)."""
+
+    def __init__(self, input_size, hidden_size, bias=True):
+        super(AGRUCell, self).__init__()
+        self.x2h = nn.Linear(input_size, 3 * hidden_size, bias=bias)
+        self.h2h = nn.Linear(hidden_size, 3 * hidden_size, bias=bias)
+
+    def forward(self, x, hx, attn):
+        raise NotImplementedError("AGRUCell runs over whole sequences on the kernels (DynamicGRU.run)")
+
+
+class AUGRUCell(AGRUCell):
+    """model_zoo/DIEN/src/DIEN.py, AUGRUCell: h' = h + a s(i_u + h_u) (n - h), r and n as AGRUCell's."""
+
+    def forward(self, x, hx, attn):
+        raise NotImplementedError("AUGRUCell runs over whole sequences on the kernels (DynamicGRU.run)")
+
+
+class DynamicGRU(nn.Module):
+    """model_zoo/DIEN/src/DIEN.py, DynamicGRU with an AUGRU or AGRU cell: the recurrence over each sample's first len
+    positions from h = 0, one kernel launch each way (functional.gru_sequence) instead of a Python loop over time."""
+
+    def __init__(self, input_size, hidden_size, bias=True, gru_type="AUGRU"):
+        super(DynamicGRU, self).__init__()
+        self.hidden_size = hidden_size
+        self.gru_type = gru_type
+        if gru_type == "AUGRU":
+            self.gru_cell = AUGRUCell(input_size, hidden_size, bias=bias)
+        elif gru_type == "AGRU":
+            self.gru_cell = AGRUCell(input_size, hidden_size, bias=bias)
+
+    def run(self, x, mask, attn, sink=None):
+        """h_last (B, H) of the cell over x (B, L, H) with the attention attn (B, L); mask (B, L) uint8 gives the
+        lengths.  sink: x is a shared_grad view (functional.gru_sequence)."""
+        cell = self.gru_cell
+        if cell.x2h.bias is None or cell.h2h.bias is None:
+            raise NotImplementedError("DynamicGRU kernels: the cell's Linears need their biases (bias=True)")
+        return F2.gru_sequence(x, mask, cell.x2h.weight, cell.x2h.bias, cell.h2h.weight, cell.h2h.bias,
+                               cell=self.gru_type, att=attn, sink=sink)[1]
+
+    def forward(self, packed_seq_emb, attn_score=None, h=None):
+        raise NotImplementedError("DynamicGRU runs on the kernels through run(x, mask, attn), which takes padded "
+                                  "sequences and a mask instead of PackedSequences")
+
+
+class AttentionLayer(nn.Module):
+    """model_zoo/DIEN/src/DIEN.py, AttentionLayer: the scores of the interests against the target, times the mask,
+    optionally softmaxed.  bilinear_attention <h_t, W_kernel t> and dot_attention <h_t, t> are one kernel each way
+    (functional.dien_scores); din_attention is the DIN input kernel, attn_mlp (an MLP_Block) and the masked softmax.
+    A Dice attn_mlp is refused: the reference takes its batch statistics over the rows of non-empty histories only."""
+
+    def __init__(self, model_dim, attention_type="bilinear_attention", attention_hidden_units=[80, 40],
+                 attention_activation="Dice", use_attention_softmax=True, attention_dropout=0.0):
+        super(AttentionLayer, self).__init__()
+        assert attention_type in ["bilinear_attention", "dot_attention", "din_attention"], \
+            "attention_type={} is not supported.".format(attention_type)
+        self.attention_type = attention_type
+        self.use_attention_softmax = use_attention_softmax
+        if attention_type == "bilinear_attention":
+            self.W_kernel = nn.Parameter(torch.eye(model_dim))
+        elif attention_type == "din_attention":
+            self.attn_mlp = MLP_Block(input_dim=model_dim * 4, output_dim=1, hidden_units=attention_hidden_units,
+                                      hidden_activations=attention_activation, output_activation=None,
+                                      dropout_rates=attention_dropout, batch_norm=False)
+
+    def run(self, interest, target, mask, sink=None):
+        """(B, L) scores of interest (B, L, H) (a shared_grad view with its sink, or None) against target (B, H);
+        mask (B, L) uint8."""
+        if self.attention_type == "din_attention":
+            if any(type(m) == Dice for m in self.attn_mlp.modules()):
+                raise NotImplementedError("DIEN din_attention: Dice in attn_mlp is not supported (the reference takes "
+                                          "Dice's batch statistics over the rows of non-empty histories only)")
+            if sink is None:
+                raise ValueError("AttentionLayer din_attention: pass the interests' shared_grad sink")
+            B, L = mask.shape
+            w = self.attn_mlp(F2.dien_din_input(target, interest, sink)).view(B, L)
+            if not self.use_attention_softmax:
+                return w * mask
+        else:
+            w = F2.dien_scores(interest, target, mask,
+                               self.W_kernel if self.attention_type == "bilinear_attention" else None, sink=sink)
+        return F2.dien_softmax(w, mask) if self.use_attention_softmax else w
+
+    def forward(self, sequence_emb, target_emb, mask=None):
+        raise NotImplementedError("AttentionLayer runs on the kernels through run(interest, target, mask)")

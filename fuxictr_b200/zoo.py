@@ -20,6 +20,7 @@ same RNG consumption) and nothing else.
   WuKong       model_zoo/WuKong/src/WuKong.py
   FinalNet     model_zoo/FinalNet/src/FinalNet.py
   BST          model_zoo/BST/src/BST.py
+  DIEN         model_zoo/DIEN/src/DIEN.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -31,7 +32,7 @@ from torch import nn
 from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbeddingDict, MLP_Block, FactorizationMachine,
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
-                     FeatureGating, FinalBlock, BehaviorTransformer,
+                     FeatureGating, FinalBlock, BehaviorTransformer, DynamicGRU, AttentionLayer, MaskedSumPooling,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
@@ -180,7 +181,8 @@ class RankModel(nn.Module):
         """Row-shard every embedding / LR table over `group` (fuxictr_b200.sharded) and route the
         sparse front through the peer-memory push/pull kernels.  Call after model_to_device() and
         before use_fused_optimizer().  Only models whose forward consumes `self._sharded_front`
-        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong, FinalNet, BST) may be
+        (DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, DualMLP, MaskNet, AutoInt, WuKong, FinalNet, BST, DIEN)
+        may be
         sharded: any
         other forward would keep reading the 1/world row shards with global ids.  Features: categorical, and unpooled sequences (DIN's histories;
         a table shared by several fields is sharded once), one common embedding dim; an LR term needs
@@ -189,7 +191,7 @@ class RankModel(nn.Module):
         if not getattr(type(self), "_routes_sharded_front", False):
             raise NotImplementedError("%s does not route its lookups through the sharded front; row-sharding "
                                       "is implemented for DeepFM, DLRM, DCNv2, xDeepFM, DIN, GDCN, GDCNP, FinalMLP, "
-                                      "DualMLP, MaskNet, AutoInt, WuKong, FinalNet and BST" % type(self).__name__)
+                                      "DualMLP, MaskNet, AutoInt, WuKong, FinalNet, BST and DIEN" % type(self).__name__)
         fed = self.embedding_layer
         if not isinstance(fed, FeatureEmbeddingDict):       # FeatureEmbedding wraps it; DIN holds it directly
             fed = fed.embedding_layer
@@ -1289,6 +1291,162 @@ class BST(RankModel):
             for name in _flatten([sequence]):
                 emb.pop(name, None)
         return torch.cat(list(emb.values()) + pooled, dim=-1)
+
+    def forward_logits(self, inputs):
+        return (self._logit_mlp()(self.dnn_input(inputs)),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class DIEN(RankModel):
+    """model_zoo/DIEN/src/DIEN.py, DIEN: per (target, sequence) field pair (a tuple of fields: their embeddings side by
+    side) an interest extractor GRU over the history, then the interest-evolution GRU: an AUGRU or AGRU (DynamicGRU)
+    driven by AttentionLayer's scores against the target, or an nn.GRU.  Its last state, then (enable_sum_pooling) the
+    sequence's sum pooling and its product with the target, join the remaining 2-D embeddings in FeatureMap order
+    (the neg-sequence fields left out) as the DNN's input.  A sample's length is the number of non-zero ids of its
+    pair's first sequence field, and the attention mask is id > 0 position by position, as in the reference; an empty
+    history gives a zero state.  The lengths are formed on the device: no row compaction, no host sync, so the step can
+    be captured in a CUDA graph.  The extractor and a gru_type="GRU" evolution keep real nn.GRU children, which hold
+    the weights; their forward is never called.  Unknown keyword arguments are accepted and ignored.
+    Refused: gru_type="AIGRU" and aux_loss_alpha > 0 (both fail in the reference), a DNN input whose width the
+    reference's formula gets wrong, din_attention with Dice, shapes outside functional.dien_bound, lazy tables and
+    enable_sharding(want_fm=True)."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="DIEN", gpu=-1, dnn_hidden_units=[200, 80], dnn_activations="ReLU",
+                 learning_rate=1e-3, embedding_dim=16, net_dropout=0, batch_norm=True,
+                 dien_target_field=[("item_id", "cate_id")], dien_sequence_field=[("click_history", "cate_history")],
+                 dien_neg_seq_field=[("neg_click_history", "neg_cate_history")], gru_type="AUGRU",
+                 enable_sum_pooling=False, attention_dropout=0, attention_type="bilinear_attention",
+                 attention_hidden_units=[80, 40], attention_activation="Dice", use_attention_softmax=True,
+                 aux_hidden_units=[100, 50], aux_activation="ReLU", aux_loss_alpha=0, embedding_regularizer=None,
+                 net_regularizer=None, **kwargs):
+        # a tuple of fields may arrive as a list (a JSON or YAML config)
+        as_list = lambda v: [tuple(f) if isinstance(f, list) else f for f in (v if isinstance(v, list) else [v])]  # noqa
+        targets, sequences, negs = as_list(dien_target_field), as_list(dien_sequence_field), as_list(dien_neg_seq_field)
+        assert len(targets) == len(sequences), "dien_sequence_field or dien_target_field not supported."
+        if gru_type == "AIGRU":
+            raise NotImplementedError("DIEN gru_type='AIGRU' is not supported: the reference fails in "
+                                      "interest_emb * attn_scores, a (B, L, H) x (B, L) broadcast")
+        if gru_type not in ("GRU", "AGRU", "AUGRU"):
+            raise ValueError("DIEN gru_type={} is not supported.".format(gru_type))
+        if aux_loss_alpha > 0:
+            raise NotImplementedError("DIEN aux_loss_alpha > 0 is not supported: the reference fails in add_loss, "
+                                      "where loss += alpha * aux_loss adds an (N,) vector in place into a 0-d tensor")
+        if gru_type != "GRU" and attention_type == "din_attention" and \
+                any(str(a).lower() == "dice" for a in as_list(attention_activation)):
+            raise NotImplementedError("DIEN din_attention with Dice is not supported: the reference takes Dice's "
+                                      "batch statistics over the rows of non-empty histories only")
+        specs = feature_map.features
+        dims = []
+        for target, sequence in zip(targets, sequences):
+            names = list(_flatten([sequence]))
+            model_dim = embedding_dim * len(list(_flatten([target])))
+            bound = F2.dien_bound(model_dim, int(specs[names[0]]["max_len"]))
+            if bound is not None:
+                raise NotImplementedError("DIEN kernels: " + bound)
+            dims.append(model_dim)
+        neg_names = list(_flatten(negs))
+        ref_width = 2 * sum(dims) + feature_map.sum_emb_out_dim() - embedding_dim * len(neg_names)
+        if not enable_sum_pooling:
+            ref_width -= embedding_dim * len(list(_flatten(targets))) * 2
+        dflt = feature_map.default_emb_dim
+        width = sum(dims) * (3 if enable_sum_pooling else 1) + sum(
+            spec.get("emb_output_dim", spec.get("embedding_dim", dflt)) for name, spec in specs.items()
+            if spec["type"] not in ("sequence", "meta") or (spec["type"] == "sequence" and spec.get("feature_encoder")))
+        if width != ref_width:
+            raise NotImplementedError("DIEN: the reference sizes the DNN input as %d but feeds it %d values (neg-sequence "
+                                      "fields not in the feature map, or sequence fields outside the pairs)"
+                                      % (ref_width, width))
+        super(DIEN, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                   embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                   **kwargs)
+        self.dien_target_field, self.dien_sequence_field = targets, sequences
+        self.aux_loss_alpha = aux_loss_alpha
+        self.dien_neg_seq_field = negs
+        self.embedding_dim = embedding_dim
+        self.embedding_layer = FeatureEmbeddingDict(feature_map, embedding_dim)
+        self.sum_pooling = MaskedSumPooling()
+        self.gru_type = gru_type
+        self.extraction_modules = nn.ModuleList()
+        self.evolving_modules = nn.ModuleList()
+        self.attention_modules = nn.ModuleList()
+        for model_dim in dims:
+            self.extraction_modules.append(nn.GRU(input_size=model_dim, hidden_size=model_dim, batch_first=True))
+            if gru_type in ("AGRU", "AUGRU"):
+                self.evolving_modules.append(DynamicGRU(model_dim, model_dim, gru_type=gru_type))
+            else:
+                self.evolving_modules.append(nn.GRU(input_size=model_dim, hidden_size=model_dim, batch_first=True))
+            if gru_type in ("AGRU", "AUGRU"):
+                self.attention_modules.append(
+                    AttentionLayer(model_dim, attention_type=attention_type,
+                                   attention_hidden_units=attention_hidden_units,
+                                   attention_activation=attention_activation,
+                                   use_attention_softmax=use_attention_softmax, attention_dropout=attention_dropout))
+        self.enable_sum_pooling = enable_sum_pooling
+        self.dnn = MLP_Block(input_dim=width, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which DIEN does not have."""
+        if want_fm:
+            raise ValueError("DIEN has no FM term: enable_sharding(..., want_fm=False)")
+        return super(DIEN, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype, want_fm=False)
+
+    def _logit_mlp(self):
+        """dnn without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_dnn")
+        if ent is None:
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(self.dnn.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_dnn"] = ent
+        return ent
+
+    @staticmethod
+    def get_embedding(field, emb):
+        """A tuple of fields means their embeddings side by side (DIEN.get_embedding)."""
+        parts = [emb[name] for name in (field if type(field) == tuple else (field,))]
+        return parts[0] if len(parts) == 1 else torch.cat(parts, dim=-1)
+
+    def interest(self, k, sequence_emb, target_emb, mask):
+        """h_out (B, H) of pair k: the extractor GRU, the attention and the evolution GRU.  The interests' gradient is
+        one buffer that the attention and the evolution GRU add into (functional.shared_grad)."""
+        ext, evo = self.extraction_modules[k], self.evolving_modules[k]
+        h_seq, _ = F2.gru_sequence(sequence_emb, mask, ext.weight_ih_l0, ext.bias_ih_l0, ext.weight_hh_l0,
+                                   ext.bias_hh_l0)
+        interest, sink = F2.shared_grad(h_seq)
+        if self.gru_type == "GRU":
+            return F2.gru_sequence(interest, mask, evo.weight_ih_l0, evo.bias_ih_l0, evo.weight_hh_l0,
+                                   evo.bias_hh_l0, sink=sink)[1]
+        scores = self.attention_modules[k].run(interest, target_emb, mask, sink=sink)
+        return evo.run(interest, mask, scores, sink=sink)
+
+    def dnn_input(self, inputs):
+        X = self.get_inputs(inputs)
+        front = getattr(self, "_sharded_front", None)
+        if front is not None:       # row-sharded tables: (B, D) / (B, L, D) views of the landed rows
+            from .sharded import sharded_front
+            landed, _ = sharded_front(front, self._batch_matrix(inputs))
+            views = front.field_views(landed)
+            emb = OrderedDict((name, views[name]) for name in self.feature_map.features.keys() if name in views)
+        else:
+            emb = self.embedding_layer(X)
+        parts = []
+        for k, (target, sequence) in enumerate(zip(self.dien_target_field, self.dien_sequence_field)):
+            target_emb = self.get_embedding(target, emb)
+            sequence_emb = self.get_embedding(sequence, emb)
+            mask = torch.ne(X[list(_flatten([sequence]))[0]], 0).to(torch.uint8)
+            parts.append(self.interest(k, sequence_emb, target_emb, mask))
+            if self.enable_sum_pooling:
+                parts.append(F2.dien_sum_pool(sequence_emb, target_emb))
+        negs = set(_flatten(self.dien_neg_seq_field))
+        parts += [e for name, e in emb.items() if e.dim() == 2 and name not in negs]
+        return torch.cat(parts, dim=-1)
 
     def forward_logits(self, inputs):
         return (self._logit_mlp()(self.dnn_input(inputs)),)

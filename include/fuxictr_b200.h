@@ -649,6 +649,60 @@ B2_API int b2_bst_pool_bwd(const float* g, int64_t ld_g, const uint8_t* valid, i
                            float* dx, void* stream);
 
 /*
+ * DIEN, the Deep Interest Evolution Network (model_zoo/DIEN/src/DIEN.py): the interest extractor (nn.GRU), the
+ * attention between the interests and the target, and the interest-evolution GRU (AUGRU, AGRU or nn.GRU) over a
+ * behaviour sequence.  All row-major fp32.
+ * A GRU over x (B, L, H) (sample b at x + b ld_x, its L tokens contiguous) with W_ih, W_hh (3H, H), b_ih, b_hh (3H):
+ *   gi = W_ih x_t + b_ih, gh = W_hh h + b_hh, chunks c0, c1, c2 of H each; one update h' = h + g (n - h) with
+ *   B2_DIEN_GRU   (nn.GRU, chunks r, z, n):     r = s(gi0 + gh0), z = s(gi1 + gh1), n = tanh(gi2 + r gh2), g = 1 - z
+ *   B2_DIEN_AUGRU (AUGRUCell, chunks u, r, n): u = s(gi0 + gh0), r = s(gi1 + gh1), n = tanh(gi2 + r gh2), g = a_t u
+ *   B2_DIEN_AGRU  (AGRUCell, chunks u, r, n):  r = s(gi1 + gh1), n = tanh(gi2 + r gh2), g = a_t (chunk u unused)
+ * with s the logistic sigmoid and a (B, L) the attention (NULL for B2_DIEN_GRU).  Sample b's length len_b is the number
+ * of non-zero bytes of its row of mask (B, L) (pad_mask.sum(1), the first sequence field's id > 0); the recurrence runs
+ * over positions [0, len_b) from h = 0, wherever the zeros are (as pack_padded_sequence does).
+ * b2_gru_fwd: h_seq (B, L, H) "=": the state after step t for t < len_b, 0 from len_b on (pad_packed_sequence's
+ *   padding); h_last (B, H) "=" (NULL: not written): the state after step len_b - 1, 0 for an empty history.
+ * b2_gru_bwd: the reverse-time recurrence from the saved h_seq, recomputing the gates from h_{t-1} and x_t.
+ *   dh_seq (B, L, H) (NULL: none) and dh_last (B, H) (NULL: none) are the gradients of the forward's outputs.
+ *   dx (B, L, H) "=" (accumulate 0: zero from len_b on) or "+=" (accumulate 1); da (B, L) "=" (zero from len_b on;
+ *   NULL for B2_DIEN_GRU); dW_ih, dW_hh (3H, H), db_ih, db_hh (3H) "+=" (caller zeroes): a per-CTA sum in shared
+ *   memory, then one float atomic per element and CTA.
+ * Both keep W_ih and W_hh in shared memory and give each sample a group of G threads, G the power of two >= H: thread j
+ *   of the group owns hidden unit j.  No (B L, 3H) gate tensor is formed.
+ * b2_dien_scores_fwd: the bilinear (W (H, H)) or dot (W NULL) attention of AttentionLayer: q_b = W t_b (t_b for dot),
+ *   q (B, H) "=", s (B, L) "=" <h_seq[b, t], q_b> mask[b, t].  t (B, H) at row pitch ld_t.
+ * b2_dien_scores_bwd: from ds (B, L): dh_seq[b, t] "+=" (accumulate 1) or "=" (0) ds mask q_b; dq (B, H) "=" the sum
+ *   over t of ds mask h_seq[b, t]; dt (B, H) "=" W^T dq (dq for dot).  dW = dq^T t is the caller's GEMM.
+ * b2_dien_sum_pool_fwd: out[b] (row pitch ld_out) "=" [sum_t x[b, t] | t_b * sum_t x[b, t]] (2H), DIEN's sum pooling of
+ *   the zero-padded sequence and its product with the target (enable_sum_pooling).
+ * b2_dien_sum_pool_bwd: from g (B, 2H) at row pitch ld_g: dx[b, t] "+=" (accumulate 1) or "=" (0) g1 + t_b g2 for every
+ *   t; dt (B, H) "+=" (accumulate 1) or "=" (0) sum_t x[b, t] g2.
+ * Range: 1 <= H <= B2_DIEN_MAX_DIM, 1 <= L <= B2_DIEN_MAX_LEN, batch >= 0 (0: no launch), batch L < 2^31.  Outside the
+ * range, or given a NULL pointer, every entry point returns B2_E_INVALID.
+ */
+#define B2_DIEN_MAX_DIM 64
+#define B2_DIEN_MAX_LEN 1024
+#define B2_DIEN_GRU 0
+#define B2_DIEN_AUGRU 1
+#define B2_DIEN_AGRU 2
+B2_API int b2_gru_fwd(const float* x, int64_t ld_x, const uint8_t* mask, const float* W_ih, const float* b_ih,
+                      const float* W_hh, const float* b_hh, const float* att, int cell, int64_t batch, int L, int H,
+                      float* h_seq, float* h_last, void* stream);
+B2_API int b2_gru_bwd(const float* x, int64_t ld_x, const uint8_t* mask, const float* W_ih, const float* b_ih,
+                      const float* W_hh, const float* b_hh, const float* att, int cell, int64_t batch, int L, int H,
+                      const float* h_seq, const float* dh_seq, const float* dh_last, float* dx, int accumulate,
+                      float* da, float* dW_ih, float* db_ih, float* dW_hh, float* db_hh, void* stream);
+B2_API int b2_dien_scores_fwd(const float* h_seq, const float* t, int64_t ld_t, const float* W, const uint8_t* mask,
+                              int64_t batch, int L, int H, float* q, float* s, void* stream);
+B2_API int b2_dien_scores_bwd(const float* h_seq, const float* t, int64_t ld_t, const float* W, const uint8_t* mask,
+                              const float* q, const float* ds, int64_t batch, int L, int H, float* dh_seq,
+                              int accumulate, float* dq, float* dt, void* stream);
+B2_API int b2_dien_sum_pool_fwd(const float* x, const float* t, int64_t ld_t, int64_t batch, int L, int H, float* out,
+                                int64_t ld_out, void* stream);
+B2_API int b2_dien_sum_pool_bwd(const float* x, const float* t, int64_t ld_t, const float* g, int64_t ld_g,
+                                int64_t batch, int L, int H, float* dx, float* dt, int accumulate, void* stream);
+
+/*
  * WuKong's layer (model_zoo/WuKong/src/WuKong.py, WuKongLayer) on x (B, F, D) with rank k, lcb + fmb = Fo output
  * fields:
  *   fm   = LN_fk(flatten(x (x^T Y)))                 Y = proj_Y (F, k); LN over F k, always affine
