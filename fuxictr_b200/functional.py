@@ -2943,6 +2943,214 @@ def target_attention(target_item, history_sequence, mask=None, num_heads=1, use_
     return _TargetAttention.apply(target_item, history_sequence, mask_u8, num_heads, scale, *weights)
 
 
+# --------------------------------------------------------------------------------------
+# LongCTR interest blocks: ETA's SimHash top-k retrieval and SDIM's hash-collision pooling
+# --------------------------------------------------------------------------------------
+def _lsh_common_bound(batch, d, L):
+    if not 1 <= d <= _lib.B2_LSH_MAX_DIM:
+        return "the item width d (item_info_dim) must lie in [1, %d], got %d" % (_lib.B2_LSH_MAX_DIM, d)
+    if not 1 <= L <= _lib.B2_LSH_MAX_LEN:
+        return "the history length L must lie in [1, %d], got %d" % (_lib.B2_LSH_MAX_LEN, L)
+    if batch * (L + 1) >= 2 ** 31:
+        return "batch (L + 1) must stay below 2^31, got %d" % (batch * (L + 1))
+    return None
+
+
+def eta_bound(d, L, topk, hash_bits, batch=1):
+    """None when the ETA kernels cover item width d, history length L, topk and hash_bits, else the bound it breaks."""
+    msg = _lsh_common_bound(batch, d, L)
+    if msg is not None:
+        return msg
+    if not 1 <= hash_bits <= _lib.B2_ETA_MAX_BITS:
+        return "hash_bits must lie in [1, %d], got %d" % (_lib.B2_ETA_MAX_BITS, hash_bits)
+    if not 1 <= topk <= _lib.B2_LSH_MAX_TOPK:
+        return "topk must lie in [1, %d], got %d" % (_lib.B2_LSH_MAX_TOPK, topk)
+    k = min(topk, L)
+    if 4 * d * hash_bits + 4 * k + 4 * hash_bits + L + 16 > _lib.B2_LSH_MAX_SMEM:
+        return "d hash_bits = %d needs more shared memory than a CTA has" % (d * hash_bits)
+    return None
+
+
+def sdim_bound(d, L, num_hashes, hash_bits, batch=1):
+    """None when the SDIM kernels cover item width d, history length L, num_hashes and hash_bits, else the bound it
+    breaks.  hash_bits stops at 24: above it the reference's float bucket code . powers_of_two is no longer exact, so
+    its collisions cannot be reproduced."""
+    msg = _lsh_common_bound(batch, d, L)
+    if msg is not None:
+        return msg
+    if not 1 <= hash_bits <= _lib.B2_SDIM_MAX_BITS:
+        return "hash_bits must lie in [1, %d] (a wider float bucket code is not exact), got %d" \
+            % (_lib.B2_SDIM_MAX_BITS, hash_bits)
+    if not 1 <= num_hashes <= _lib.B2_SDIM_MAX_HASHES:
+        return "num_hashes must lie in [1, %d], got %d" % (_lib.B2_SDIM_MAX_HASHES, num_hashes)
+    pool = 4 * d * num_hashes * hash_bits + 4 * (256 // d) * num_hashes * d + 4 * num_hashes + 4 * L
+    if pool > _lib.B2_LSH_MAX_SMEM or 4 * num_hashes * d + 4 * L > _lib.B2_LSH_MAX_SMEM:
+        return "d num_hashes hash_bits = %d needs more shared memory than a CTA has" % (d * num_hashes * hash_bits)
+    return None
+
+
+class _SavedCtx(object):
+    """Stands in for an autograd ctx, so that an interest block's node can run _TargetAttention's forward and
+    backward inside its own."""
+
+    def save_for_backward(self, *tensors):
+        self.saved_tensors = tensors
+
+
+def _mhta_fwd(t, x, mask_u8, heads, scale, weights):
+    ctx = _SavedCtx()
+    out = _TargetAttention.forward(ctx, t, x, mask_u8, heads, scale, *(weights or (None,) * 4))
+    return out, ctx
+
+
+def _mhta_bwd(ctx, g):
+    """(dt, dx, (dW_q, dW_k, dW_v, dW_o) or ())."""
+    grads = _TargetAttention.backward(ctx, g)
+    return grads[0], grads[1], tuple(w for w in grads[5:] if w is not None)
+
+
+def _mhta_scale(weights, d, heads, use_scale):
+    A = weights[0].shape[0] if weights else d
+    return 1.0 / (A // heads) ** 0.5 if use_scale else 1.0
+
+
+def _short_window(x, mask_u8, S):
+    """The reference's item_feat_emb[:, -short_seq_len:-1] and mask[:, -short_seq_len:-1] with S = short_seq_len - 1:
+    the embeddings of positions [L - S, L) and the mask of positions [L - S - 1, L - 1), one apart as in the reference."""
+    L = mask_u8.shape[1]
+    return x[:, L - S:L], mask_u8[:, L - S - 1:L - 1].contiguous()
+
+
+class _EtaInterest(torch.autograd.Function):
+    """ETA.forward's interest block (ETA.py:150-165) over item_feat_emb x (B, L + 1, d) as one node: the short target
+    attention over the window, SimHash retrieval of the k = min(topk, L) nearest history rows (b2_eta_retrieve_fwd),
+    the long target attention over them.  Returns (target, short interest, long interest), each (B, d).  The backward
+    runs both attentions' backwards and one assembly launch (b2_eta_assemble_bwd) that writes dx once."""
+
+    @staticmethod
+    def forward(ctx, x, mask_u8, R, r_stride, S, k, heads, use_scale, *weights):
+        x = _f32c(x)
+        B, L1, d = x.shape
+        L = L1 - 1
+        ws, wl = weights[:4], weights[4:]
+        target = x[:, L].contiguous()
+        hs, ms = _short_window(x, mask_u8, S)
+        short, sctx = _mhta_fwd(target, hs, ms, heads, _mhta_scale(ws, d, heads, use_scale), ws)
+        bits = R.shape[-1]
+        topk_emb = torch.empty((B, k, d), dtype=torch.float32, device=x.device)
+        topk_mask = torch.empty((B, k), dtype=torch.uint8, device=x.device)
+        pos = torch.empty((B, k), dtype=torch.int32, device=x.device)
+        _lib.call("b2_eta_retrieve_fwd", _ptr(x), _ptr(mask_u8), _ptr(R), r_stride, B, L, d, bits, k, _ptr(topk_emb),
+                  _ptr(topk_mask), _ptr(pos), _stream())
+        long, lctx = _mhta_fwd(target, topk_emb, topk_mask, heads, _mhta_scale(wl, d, heads, use_scale), wl)
+        ctx.parts = (sctx, lctx, S, k, pos, L)
+        ctx.mark_non_differentiable(pos)
+        return target, short, long, pos
+
+    @staticmethod
+    def backward(ctx, g_target, g_short, g_long, _):
+        sctx, lctx, S, k, pos, L = ctx.parts
+        dt_s, dx_s, dws = _mhta_bwd(sctx, _f32c(g_short))
+        dt_l, dx_l, dwl = _mhta_bwd(lctx, _f32c(g_long))
+        B, d = dt_s.shape
+        g_target = _f32c(g_target)
+        dx = torch.empty((B, L + 1, d), dtype=torch.float32, device=dt_s.device)
+        _lib.call("b2_eta_assemble_bwd", _ptr(g_target), _ptr(dt_s), _ptr(dt_l), _ptr(dx_s), S, _ptr(dx_l),
+                  _ptr(pos), B, L, d, k, _ptr(dx), _stream())
+        return (dx, None, None, None, None, None, None, None) + dws + dwl
+
+
+class _SdimInterest(torch.autograd.Function):
+    """SDIM.forward's interest block (SDIM.py:155-167) over item_feat_emb x (B, L + 1, d) as one node: the short target
+    attention over the window and the hash-collision pooling of the history (b2_sdim_pool_fwd).  Returns (target,
+    short interest, long interest), each (B, d).  The backward runs the attention's backward and one assembly launch
+    (b2_sdim_assemble_bwd) that writes dx once."""
+
+    @staticmethod
+    def forward(ctx, x, mask_u8, R, r_stride, S, l2_norm, heads, use_scale, *weights):
+        x = _f32c(x)
+        B, L1, d = x.shape
+        L = L1 - 1
+        target = x[:, L].contiguous()
+        hs, ms = _short_window(x, mask_u8, S)
+        short, sctx = _mhta_fwd(target, hs, ms, heads, _mhta_scale(weights, d, heads, use_scale), weights)
+        nh, bits = R.shape[-2], R.shape[-1]
+        long = torch.empty((B, d), dtype=torch.float32, device=x.device)
+        sums = torch.empty((B, nh, d), dtype=torch.float32, device=x.device)
+        collide = torch.empty((B, L), dtype=torch.int32, device=x.device)
+        _lib.call("b2_sdim_pool_fwd", _ptr(x), _ptr(mask_u8), _ptr(R), r_stride, B, L, d, nh, bits, int(l2_norm),
+                  _ptr(long), _ptr(sums), _ptr(collide), _stream())
+        ctx.parts = (sctx, S, l2_norm, sums, collide, L)
+        return target, short, long
+
+    @staticmethod
+    def backward(ctx, g_target, g_short, g_long):
+        sctx, S, l2_norm, sums, collide, L = ctx.parts
+        dt_s, dx_s, dws = _mhta_bwd(sctx, _f32c(g_short))
+        B, d = dt_s.shape
+        # both held until the launch: a temporary freed inside the argument list would hand its block to the next one
+        g_target, g_long = _f32c(g_target), _f32c(g_long)
+        zero = torch.zeros((B, d), dtype=torch.float32, device=dt_s.device)
+        dx = torch.empty((B, L + 1, d), dtype=torch.float32, device=dt_s.device)
+        _lib.call("b2_sdim_assemble_bwd", _ptr(g_target), _ptr(dt_s), _ptr(zero), _ptr(dx_s), S, _ptr(g_long),
+                  _ptr(sums), _ptr(collide), B, L, d, sums.shape[1], int(l2_norm), _ptr(dx), _stream())
+        return (dx, None, None, None, None, None, None, None) + dws
+
+
+def _lsh_inputs(name, item_emb, mask, R, hash_dims, short_seq_len):
+    _require_cuda(item_emb, mask, R)
+    if item_emb.dim() != 3 or mask.dim() != 2 or mask.shape[0] != item_emb.shape[0] \
+            or item_emb.shape[1] != mask.shape[1] + 1:
+        raise ValueError("%s: item_feat_emb%s must be (B, L + 1, d) and mask%s (B, L)"
+                         % (name, tuple(item_emb.shape), tuple(mask.shape)))
+    B, L1, d = item_emb.shape
+    L = L1 - 1
+    if L == 0:
+        raise ValueError("%s: the batch has an empty history axis (L = 0)" % name)
+    if R.dim() != 2 + hash_dims or R.shape[0] not in (1, B) or R.shape[1] != d:
+        raise ValueError("%s: rotations%s must be (1 or B, d, ...) with d = %d" % (name, tuple(R.shape), d))
+    if short_seq_len < 2:
+        raise ValueError("%s: short_seq_len must be at least 2 (the window [-short_seq_len:-1] would be empty), got %d"
+                         % (name, short_seq_len))
+    if L < short_seq_len:
+        raise ValueError("%s: the history length L = %d is below short_seq_len = %d, where the reference's "
+                         "[-short_seq_len:-1] windows of the embeddings and of the mask differ in length"
+                         % (name, L, short_seq_len))
+    mask_u8 = torch.ne(mask, 0).view(torch.uint8)
+    R = _f32c(R)
+    r_stride = 0 if R.shape[0] == 1 else R[0].numel()
+    return mask_u8, R, r_stride, B, L, d
+
+
+def eta_interest(item_emb, mask, rotations, short_seq_len, topk, num_heads, use_scale, short_weights, long_weights):
+    """ETA's interest block: item_emb (B, L + 1, d) (the last position the target), mask (B, L) (non-zero = valid),
+    rotations (1 or B, d, hash_bits), short_weights and long_weights the (W_q, W_k, W_v, W_o) of the two attentions.
+    Returns (target, short interest, long interest, positions): three (B, d) and the chosen history positions (B, k)
+    int32, k = min(topk, L), sorted by (Hamming distance, position).  Ties at equal distance go to the lower position."""
+    mask_u8, R, r_stride, B, L, d = _lsh_inputs("ETA", item_emb, mask, rotations, 1, short_seq_len)
+    bound = eta_bound(d, L, topk, R.shape[-1], B)
+    if bound is not None:
+        raise NotImplementedError("ETA kernels: " + bound)
+    for w in tuple(short_weights) + tuple(long_weights):
+        _require_cuda(w)
+    return _EtaInterest.apply(item_emb, mask_u8, R, r_stride, short_seq_len - 1, min(topk, L), num_heads, use_scale,
+                              *short_weights, *long_weights)
+
+
+def sdim_interest(item_emb, mask, rotations, short_seq_len, l2_norm, num_heads, use_scale, short_weights):
+    """SDIM's interest block: item_emb (B, L + 1, d) (the last position the target), mask (B, L) (non-zero = valid),
+    rotations (1 or B, d, num_hashes, hash_bits), short_weights (W_q, W_k, W_v, W_o) of the short attention or () for
+    use_qkvo=False.  Returns (target, short interest, long interest), each (B, d)."""
+    mask_u8, R, r_stride, B, L, d = _lsh_inputs("SDIM", item_emb, mask, rotations, 2, short_seq_len)
+    bound = sdim_bound(d, L, R.shape[-2], R.shape[-1], B)
+    if bound is not None:
+        raise NotImplementedError("SDIM kernels: " + bound)
+    for w in short_weights:
+        _require_cuda(w)
+    return _SdimInterest.apply(item_emb, mask_u8, R, r_stride, short_seq_len - 1, bool(l2_norm), num_heads, use_scale,
+                               *short_weights)
+
+
 def mlp_chain_supported():
     return _MATMUL["mode"] != "fp32"
 

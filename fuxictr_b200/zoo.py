@@ -21,6 +21,7 @@ same RNG consumption) and nothing else.
   FinalNet     model_zoo/FinalNet/src/FinalNet.py
   BST          model_zoo/BST/src/BST.py
   DIEN         model_zoo/DIEN/src/DIEN.py
+  ETA, SDIM    model_zoo/LongCTR/ETA/ETA.py, model_zoo/LongCTR/SDIM/SDIM.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -33,7 +34,8 @@ from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbedding
                      CrossNetV2, GateCorssLayer, FeatureSelection, InteractionAggregation, InnerProductInteraction,
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
                      FeatureGating, FinalBlock, BehaviorTransformer, DynamicGRU, AttentionLayer, MaskedSumPooling,
-                     DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, not_in_whitelist)
+                     DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, MultiHeadTargetAttention,
+                     not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
 
@@ -1453,3 +1455,199 @@ class DIEN(RankModel):
 
     def forward(self, inputs):
         return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class _LongCTRModel(RankModel):
+    """What ETA and SDIM share: the LongCTR input triple (batch_dict, item_dict, mask) of the reference's
+    LongCTRDataLoader, the item embeddings `embedding_layer(item_dict, flatten_emb=True)` viewed as (B, L + 1, d) with
+    the target last, and a DNN over [batch embeddings, target, interests].  d = item_info_dim is the sum of the
+    embedding dims of the features with source "item".  Refused: attention_dropout > 0 (the target-attention kernels
+    have none), short_seq_len < 2, accumulation_steps != 1, a batch with L = 0 or L < short_seq_len (the reference's
+    embedding and mask windows then differ in length), a DNN input whose width is not the reference's
+    sum_emb_out_dim() + 2 item_info_dim, lazy tables and enable_sharding()."""
+
+    def _longctr_init(self, feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps):
+        if attention_dropout:
+            raise NotImplementedError("%s: attention_dropout > 0 is not supported: the target-attention kernels have "
+                                      "no dropout" % type(self).__name__)
+        if short_seq_len < 2:
+            raise ValueError("%s: short_seq_len must be at least 2 (the window [-short_seq_len:-1] would be empty), "
+                             "got %d" % (type(self).__name__, short_seq_len))
+        if accumulation_steps != 1:
+            raise NotImplementedError("%s: accumulation_steps != 1 is not supported: every step updates the weights"
+                                      % type(self).__name__)
+        self.feature_map = feature_map
+        self.embedding_dim = embedding_dim
+        self.short_seq_len = short_seq_len
+        self.accumulation_steps = accumulation_steps
+        self.item_info_dim = 0
+        for feat, spec in feature_map.features.items():
+            if spec.get("source") == "item":
+                self.item_info_dim += spec.get("embedding_dim", embedding_dim)
+
+    def get_inputs(self, inputs, feature_source=None):
+        """(X_dict, item_dict, mask) on the model's device (ETA.py / SDIM.py get_inputs)."""
+        batch_dict, item_dict, mask = inputs
+        X_dict = dict()
+        for feature, value in batch_dict.items():
+            if feature in self.feature_map.labels:
+                continue
+            feature_spec = self.feature_map.features[feature]
+            if feature_spec["type"] == "meta":
+                continue
+            if feature_source and not_in_whitelist(feature_spec["source"], feature_source):
+                continue
+            X_dict[feature] = value.to(self.device)
+        for item, value in item_dict.items():
+            item_dict[item] = value.to(self.device)
+        return X_dict, item_dict, mask.to(self.device)
+
+    def get_labels(self, inputs):
+        y = inputs[0][self.feature_map.labels[0]].to(self.device)
+        return y.float().view(-1, 1)
+
+    def get_group_id(self, inputs):
+        return inputs[0][self.feature_map.group_id]
+
+    def _logit_mlp(self):
+        """dnn without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_dnn")
+        if ent is None:
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(self.dnn.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_dnn"] = ent
+        return ent
+
+    def _item_inputs(self, inputs):
+        """(batch embeddings or None, item_feat_emb (B, L + 1, d), mask (B, L)); checks the DNN width."""
+        batch_dict, item_dict, mask = self.get_inputs(inputs)
+        emb_out = self.embedding_layer(batch_dict, flatten_emb=True) if batch_dict else None
+        if mask.dim() != 2 or mask.shape[1] == 0:
+            raise ValueError("%s: mask%s must be (B, L) with L >= 1" % (type(self).__name__, tuple(mask.shape)))
+        B, L = mask.shape
+        item_feat_emb = self.embedding_layer(item_dict, flatten_emb=True)
+        if item_feat_emb.shape[-1] != self.item_info_dim or item_feat_emb.numel() != B * (L + 1) * self.item_info_dim:
+            raise ValueError("%s: item_dict gives %s embeddings, expected B (L + 1) = %d rows of item_info_dim = %d"
+                             % (type(self).__name__, tuple(item_feat_emb.shape), B * (L + 1), self.item_info_dim))
+        width = (0 if emb_out is None else emb_out.shape[-1]) + 3 * self.item_info_dim
+        ref_width = self.feature_map.sum_emb_out_dim() + 2 * self.item_info_dim
+        if width != ref_width:
+            raise NotImplementedError("%s: the reference sizes the DNN input as sum_emb_out_dim() + 2 item_info_dim = "
+                                      "%d but this batch gives it %d values (item features in batch_dict, or a "
+                                      "feature in neither dict)" % (type(self).__name__, ref_width, width))
+        return emb_out, item_feat_emb.view(B, L + 1, self.item_info_dim), mask
+
+    def forward_logits(self, inputs):
+        return (self._logit_mlp()(self.dnn_input(inputs)),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class ETA(_LongCTRModel):
+    """model_zoo/LongCTR/ETA/ETA.py, ETA: a short target attention over the last short_seq_len - 1 history items, and
+    a long one over the topk history items nearest the target in SimHash Hamming distance; the DNN reads [batch
+    embeddings, target, short, long].  The interest block is one autograd node on the kernels (functional.eta_interest);
+    ties at equal distance go to the lower history position.  reuse_hash=False draws (B, d, hash_bits) rotations with
+    torch.randn on the device every forward, as the reference does.  The frozen random_rotations stay outside the
+    optimizer.  Unknown keyword arguments are accepted and ignored.  Refusals: see _LongCTRModel, and shapes outside
+    functional.eta_bound."""
+
+    def __init__(self, feature_map, model_id="ETA", gpu=-1, dnn_hidden_units=[512, 128, 64], dnn_activations="ReLU",
+                 attention_dim=64, num_heads=1, use_scale=True, attention_dropout=0, reuse_hash=True, hash_bits=32,
+                 topk=50, learning_rate=1e-3, embedding_dim=10, net_dropout=0, batch_norm=False, short_seq_len=50,
+                 accumulation_steps=1, embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(ETA, self).__init__(feature_map, model_id=model_id, gpu=gpu, embedding_regularizer=embedding_regularizer,
+                                  net_regularizer=net_regularizer, **kwargs)
+        self._longctr_init(feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps)
+        bound = F2.eta_bound(self.item_info_dim, 1, topk, hash_bits)
+        if bound is not None:
+            raise NotImplementedError("ETA kernels: " + bound)
+        self.reuse_hash = reuse_hash
+        self.hash_bits = hash_bits
+        self.topk = topk
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.short_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                        attention_dropout, use_scale)
+        self.random_rotations = nn.Parameter(torch.randn(1, self.item_info_dim, self.hash_bits), requires_grad=False)
+        self.long_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                       attention_dropout, use_scale)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim * 2
+        self.dnn = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def interest(self, item_feat_emb, mask):
+        """(target, short, long, positions) of functional.eta_interest."""
+        if self.reuse_hash:
+            rotations = self.random_rotations
+        else:
+            rotations = torch.randn(item_feat_emb.size(0), self.item_info_dim, self.hash_bits,
+                                    device=item_feat_emb.device)
+        sa, la = self.short_attention, self.long_attention
+        return F2.eta_interest(item_feat_emb, mask, rotations, self.short_seq_len, self.topk, sa.num_heads,
+                               sa.scale is not None, (sa.W_q.weight, sa.W_k.weight, sa.W_v.weight, sa.W_o.weight),
+                               (la.W_q.weight, la.W_k.weight, la.W_v.weight, la.W_o.weight))
+
+    def dnn_input(self, inputs):
+        emb_out, item_feat_emb, mask = self._item_inputs(inputs)
+        target, short, long, _ = self.interest(item_feat_emb, mask)
+        return torch.cat(([emb_out] if emb_out is not None else []) + [target, short, long], dim=-1)
+
+
+class SDIM(_LongCTRModel):
+    """model_zoo/LongCTR/SDIM/SDIM.py, SDIM: a short target attention over the last short_seq_len - 1 history items, and
+    the long interest as the mean over num_hashes SimHash hashes of the sum of the history items whose bucket matches
+    the target's (each sum L2-normalised with l2_norm); the DNN reads [batch embeddings, target, long, short].  The
+    interest block is one autograd node on the kernels (functional.sdim_interest), with no torch.nonzero, so the step
+    never waits for the host.  reuse_hash=False draws (B, d, num_hashes, hash_bits) rotations with torch.randn on the
+    device every forward.  The frozen powers_of_two and random_rotations stay outside the optimizer.  Unknown keyword
+    arguments are accepted and ignored.  Refusals: see _LongCTRModel, and shapes outside functional.sdim_bound
+    (hash_bits > 24 among them)."""
+
+    def __init__(self, feature_map, model_id="SDIM", gpu=-1, dnn_hidden_units=[512, 128, 64], dnn_activations="ReLU",
+                 attention_dim=64, use_qkvo=True, num_heads=1, use_scale=True, attention_dropout=0, reuse_hash=True,
+                 num_hashes=1, hash_bits=4, learning_rate=1e-3, embedding_dim=10, net_dropout=0, batch_norm=False,
+                 l2_norm=False, short_seq_len=50, accumulation_steps=1, embedding_regularizer=None,
+                 net_regularizer=None, **kwargs):
+        super(SDIM, self).__init__(feature_map, model_id=model_id, gpu=gpu, embedding_regularizer=embedding_regularizer,
+                                   net_regularizer=net_regularizer, **kwargs)
+        self._longctr_init(feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps)
+        bound = F2.sdim_bound(self.item_info_dim, 1, num_hashes, hash_bits)
+        if bound is not None:
+            raise NotImplementedError("SDIM kernels: " + bound)
+        self.reuse_hash = reuse_hash
+        self.num_hashes = num_hashes
+        self.hash_bits = hash_bits
+        self.l2_norm = l2_norm
+        self.powers_of_two = nn.Parameter(torch.tensor([2.0 ** i for i in range(hash_bits)]), requires_grad=False)
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.short_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                        attention_dropout, use_scale, use_qkvo)
+        self.random_rotations = nn.Parameter(torch.randn(1, self.item_info_dim, self.num_hashes, self.hash_bits),
+                                             requires_grad=False)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim * 2
+        self.dnn = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def interest(self, item_feat_emb, mask):
+        """(target, short, long) of functional.sdim_interest."""
+        if self.reuse_hash:
+            rotations = self.random_rotations
+        else:
+            rotations = torch.randn(item_feat_emb.size(0), self.item_info_dim, self.num_hashes, self.hash_bits,
+                                    device=item_feat_emb.device)
+        sa = self.short_attention
+        weights = (sa.W_q.weight, sa.W_k.weight, sa.W_v.weight, sa.W_o.weight) if sa.use_qkvo else ()
+        return F2.sdim_interest(item_feat_emb, mask, rotations, self.short_seq_len, self.l2_norm, sa.num_heads,
+                                sa.scale is not None, weights)
+
+    def dnn_input(self, inputs):
+        emb_out, item_feat_emb, mask = self._item_inputs(inputs)
+        target, short, long = self.interest(item_feat_emb, mask)
+        return torch.cat(([emb_out] if emb_out is not None else []) + [target, long, short], dim=-1)

@@ -703,6 +703,50 @@ B2_API int b2_dien_sum_pool_bwd(const float* x, const float* t, int64_t ld_t, co
                                 int64_t batch, int L, int H, float* dx, float* dt, int accumulate, void* stream);
 
 /*
+ * LSH over a long behaviour sequence: ETA's SimHash top-k retrieval (model_zoo/LongCTR/ETA/ETA.py) and SDIM's
+ * hash-collision pooling (model_zoo/LongCTR/SDIM/SDIM.py).  x is item_feat_emb (B, L + 1, d) row-major fp32: positions
+ * [0, L) the history, position L the target; mask (B, L) bytes, non-zero = valid.  Sample b's rotations start at
+ * R + b r_stride (r_stride 0: one shared set).  SimHash bit j of a row v is v . R[:, j] > 0 (bit 0 at exactly 0), the
+ * projection in fp32 FMA over ascending columns.
+ * b2_eta_retrieve_fwd: R (d, bits).  dist_l = popc(code_l ^ code_target), 1 + bits where mask is 0.  Writes the k
+ *   smallest, sorted by (distance, position): ties go to the lower position.  topk_emb (B, k, d), topk_mask (B, k)
+ *   bytes (mask != 0 at the chosen position) and topk_pos (B, k) int32, all "=".
+ * b2_sdim_pool_fwd: R (d, num_hashes, bits).  Bucket h of a row is its bits-bit code under R[:, h, :]; position l
+ *   collides in hash h when its bucket equals the target's and mask[l] != 0.  sums (B, num_hashes, d) "=" the sum of the
+ *   colliding rows per hash (zero when none), collide (B, L) "=" one bit per hash, out (B, d) "=" the mean over hashes
+ *   of sums, each first divided by max(|sum|, 1e-12) when l2norm (F.normalize).
+ * b2_eta_assemble_bwd / b2_sdim_assemble_bwd: dx (B, L + 1, d) "=", every row written once.  Row L = dt0 + dt1 + dt2
+ *   (each (B, d)).  Rows [L - S, L) add dshort (B, S, d).  ETA adds dlong (B, k, d) at the positions topk_pos.  SDIM
+ *   adds, for each hash h position l collides in, (dlong / num_hashes) times the Jacobian of F.normalize at sums[b, h]
+ *   when l2norm (1 / max(|s|, 1e-12) below the clamp), dlong (B, d) / num_hashes without.
+ * Range: 1 <= d <= B2_LSH_MAX_DIM, 1 <= L <= B2_LSH_MAX_LEN, batch (L + 1) < 2^31, batch >= 0 (0: no launch);
+ * ETA 1 <= bits <= B2_ETA_MAX_BITS and 1 <= k <= min(L, B2_LSH_MAX_TOPK); SDIM 1 <= bits <= B2_SDIM_MAX_BITS (a wider
+ * bucket is no longer exact as the reference's float code . powers_of_two), 1 <= num_hashes <= B2_SDIM_MAX_HASHES,
+ * 1 <= S <= L, and the shared memory a CTA needs within B2_LSH_MAX_SMEM bytes: ETA 4 d bits + 4 k + 4 bits + L + 16,
+ * SDIM 4 d num_hashes bits + 4 (256 / d) num_hashes d + 4 num_hashes + 4 L.  Outside the range, or given a NULL
+ * pointer, every entry point returns B2_E_INVALID.
+ */
+#define B2_LSH_MAX_DIM 256
+#define B2_LSH_MAX_LEN 4096
+#define B2_LSH_MAX_TOPK 256
+#define B2_LSH_MAX_SMEM (227 * 1024 - 1024)
+#define B2_ETA_MAX_BITS 64
+#define B2_SDIM_MAX_BITS 24
+#define B2_SDIM_MAX_HASHES 32
+B2_API int b2_eta_retrieve_fwd(const float* x, const uint8_t* mask, const float* R, int64_t r_stride, int64_t batch,
+                               int L, int d, int bits, int k, float* topk_emb, uint8_t* topk_mask, int32_t* topk_pos,
+                               void* stream);
+B2_API int b2_sdim_pool_fwd(const float* x, const uint8_t* mask, const float* R, int64_t r_stride, int64_t batch,
+                            int L, int d, int num_hashes, int bits, int l2norm, float* out, float* sums,
+                            uint32_t* collide, void* stream);
+B2_API int b2_eta_assemble_bwd(const float* dt0, const float* dt1, const float* dt2, const float* dshort, int S,
+                               const float* dlong, const int32_t* topk_pos, int64_t batch, int L, int d, int k,
+                               float* dx, void* stream);
+B2_API int b2_sdim_assemble_bwd(const float* dt0, const float* dt1, const float* dt2, const float* dshort, int S,
+                                const float* dlong, const float* sums, const uint32_t* collide, int64_t batch, int L,
+                                int d, int num_hashes, int l2norm, float* dx, void* stream);
+
+/*
  * WuKong's layer (model_zoo/WuKong/src/WuKong.py, WuKongLayer) on x (B, F, D) with rank k, lcb + fmb = Fo output
  * fields:
  *   fm   = LN_fk(flatten(x (x^T Y)))                 Y = proj_Y (F, k); LN over F k, always affine
