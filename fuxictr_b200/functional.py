@@ -3098,7 +3098,18 @@ class _SdimInterest(torch.autograd.Function):
 
 
 def _lsh_inputs(name, item_emb, mask, R, hash_dims, short_seq_len):
-    _require_cuda(item_emb, mask, R)
+    _require_cuda(R)
+    mask_u8, B, L, d = _longctr_inputs(name, item_emb, mask, short_seq_len)
+    if R.dim() != 2 + hash_dims or R.shape[0] not in (1, B) or R.shape[1] != d:
+        raise ValueError("%s: rotations%s must be (1 or B, d, ...) with d = %d" % (name, tuple(R.shape), d))
+    R = _f32c(R)
+    r_stride = 0 if R.shape[0] == 1 else R[0].numel()
+    return mask_u8, R, r_stride, B, L, d
+
+
+def _longctr_inputs(name, item_emb, mask, short_seq_len):
+    """(mask bytes, B, L, d) of a LongCTR interest block's item_feat_emb (B, L + 1, d) and mask (B, L)."""
+    _require_cuda(item_emb, mask)
     if item_emb.dim() != 3 or mask.dim() != 2 or mask.shape[0] != item_emb.shape[0] \
             or item_emb.shape[1] != mask.shape[1] + 1:
         raise ValueError("%s: item_feat_emb%s must be (B, L + 1, d) and mask%s (B, L)"
@@ -3107,8 +3118,6 @@ def _lsh_inputs(name, item_emb, mask, R, hash_dims, short_seq_len):
     L = L1 - 1
     if L == 0:
         raise ValueError("%s: the batch has an empty history axis (L = 0)" % name)
-    if R.dim() != 2 + hash_dims or R.shape[0] not in (1, B) or R.shape[1] != d:
-        raise ValueError("%s: rotations%s must be (1 or B, d, ...) with d = %d" % (name, tuple(R.shape), d))
     if short_seq_len < 2:
         raise ValueError("%s: short_seq_len must be at least 2 (the window [-short_seq_len:-1] would be empty), got %d"
                          % (name, short_seq_len))
@@ -3116,10 +3125,7 @@ def _lsh_inputs(name, item_emb, mask, R, hash_dims, short_seq_len):
         raise ValueError("%s: the history length L = %d is below short_seq_len = %d, where the reference's "
                          "[-short_seq_len:-1] windows of the embeddings and of the mask differ in length"
                          % (name, L, short_seq_len))
-    mask_u8 = torch.ne(mask, 0).view(torch.uint8)
-    R = _f32c(R)
-    r_stride = 0 if R.shape[0] == 1 else R[0].numel()
-    return mask_u8, R, r_stride, B, L, d
+    return torch.ne(mask, 0).view(torch.uint8), B, L, d
 
 
 def eta_interest(item_emb, mask, rotations, short_seq_len, topk, num_heads, use_scale, short_weights, long_weights):
@@ -3149,6 +3155,219 @@ def sdim_interest(item_emb, mask, rotations, short_seq_len, l2_norm, num_heads, 
         _require_cuda(w)
     return _SdimInterest.apply(item_emb, mask_u8, R, r_stride, short_seq_len - 1, bool(l2_norm), num_heads, use_scale,
                                *short_weights)
+
+
+# --------------------------------------------------------------------------------------
+# LongCTR interest blocks: SIM's soft-search retrieval and TWIN's top-k attention
+# --------------------------------------------------------------------------------------
+def _topk_common_bound(batch, d, L, topk):
+    if not 1 <= d <= _lib.B2_TOPK_MAX_DIM:
+        return "the item width d (item_info_dim) must lie in [1, %d], got %d" % (_lib.B2_TOPK_MAX_DIM, d)
+    if not 1 <= L <= _lib.B2_TOPK_MAX_LEN:
+        return "the history length L must lie in [1, %d], got %d" % (_lib.B2_TOPK_MAX_LEN, L)
+    if not 1 <= topk <= _lib.B2_TOPK_MAX_K:
+        return "topk must lie in [1, %d], got %d" % (_lib.B2_TOPK_MAX_K, topk)
+    if batch * (L + 1) >= 2 ** 31:
+        return "batch (L + 1) must stay below 2^31, got %d" % (batch * (L + 1))
+    return None
+
+
+def _heads_bound(d, num_heads):
+    if not 1 <= num_heads <= _lib.B2_MHTA_MAX_HEADS or num_heads * d > _lib.B2_MHTA_MAX_WIDTH:
+        return "num_heads must lie in [1, %d] with num_heads d <= %d, got num_heads %d, d %d" \
+            % (_lib.B2_MHTA_MAX_HEADS, _lib.B2_MHTA_MAX_WIDTH, num_heads, d)
+    return None
+
+
+def _part_bytes(d):
+    return 4 * (256 // d) * d
+
+
+def sim_bound(d, L, topk, num_heads, batch=1):
+    """None when the SIM kernels cover item width d, history length L, topk and num_heads, else the bound it breaks."""
+    msg = _topk_common_bound(batch, d, L, topk) or _heads_bound(d, num_heads)
+    if msg is not None:
+        return msg
+    k = min(topk, L)
+    if 8 * L + 4 * d + _part_bytes(d) + 4 * k > _lib.B2_TOPK_MAX_SMEM:
+        return "L = %d needs more shared memory than a CTA has" % L
+    return None
+
+
+def twin_bound(d, L, topk, num_heads, batch=1):
+    """None when the TWIN kernels cover item width d, history length L, topk and num_heads, else the bound it breaks."""
+    msg = _topk_common_bound(batch, d, L, topk) or _heads_bound(d, num_heads)
+    if msg is not None:
+        return msg
+    k, H = min(topk, L), num_heads
+    fwd = 4 * L + 4 * d + 8 * k + _part_bytes(d)
+    bwd = 4 * ((H * L + 1) // 2) + 12 * H * d + 12 * H * k + 4 * H
+    if max(fwd, bwd) > _lib.B2_TOPK_MAX_SMEM:
+        return "num_heads L = %d needs more shared memory than a CTA has" % (H * L)
+    return None
+
+
+class _SimInterest(torch.autograd.Function):
+    """SIM.forward's interest block (SIM.py:128-153) over item_feat_emb x (B, L + 1, d) as one node: the short target
+    attention over the window; the soft-search GSU, u = W_b^T W_a t on two fp32 GEMMs, then the scores
+    qk_l = (u . x_l) mask_l, pooled = sum_l qk_l x_l and the k = min(topk, L) best rows (b2_sim_retrieve_fwd); the long
+    target attention over them.  Returns (target, short, long, pooled, positions).  The backward runs both attentions'
+    backwards, the GSU's (b2_sim_gsu_bwd, then the fp32 GEMMs back to dW_a, dW_b and dt) and one assembly launch
+    (b2_sim_assemble_bwd) that writes dx once."""
+
+    @staticmethod
+    def forward(ctx, x, mask_u8, S, k, heads, use_scale, Wa, Wb, *weights):
+        x = _f32c(x)
+        B, L1, d = x.shape
+        L, dev = L1 - 1, x.device
+        ws, wl = weights[:4], weights[4:]
+        target = x[:, L].contiguous()
+        hs, ms = _short_window(x, mask_u8, S)
+        short, sctx = _mhta_fwd(target, hs, ms, heads, _mhta_scale(ws, d, heads, use_scale), ws)
+        # the scores decide the selection, so they are fp32 in every matmul mode
+        Wa, Wb = _f32c(Wa), _f32c(Wb)
+        a = gemm_f32(target, Wa, torch.empty((B, Wa.shape[0]), dtype=torch.float32, device=dev), b_t=True)
+        u = gemm_f32(a, Wb, torch.empty((B, d), dtype=torch.float32, device=dev))
+        qk = torch.empty((B, L), dtype=torch.float32, device=dev)
+        pooled = torch.empty((B, d), dtype=torch.float32, device=dev)
+        topk_emb = torch.empty((B, k, d), dtype=torch.float32, device=dev)
+        topk_mask = torch.empty((B, k), dtype=torch.uint8, device=dev)
+        pos = torch.empty((B, k), dtype=torch.int32, device=dev)
+        _lib.call("b2_sim_retrieve_fwd", _ptr(x), _ptr(mask_u8), _ptr(u), B, L, d, k, _ptr(qk), _ptr(pooled),
+                  _ptr(topk_emb), _ptr(topk_mask), _ptr(pos), _stream())
+        long, lctx = _mhta_fwd(target, topk_emb, topk_mask, heads, _mhta_scale(wl, d, heads, use_scale), wl)
+        ctx.parts = (sctx, lctx, S, k, L, x, mask_u8, target, a, u, qk, pos, Wa, Wb)
+        ctx.mark_non_differentiable(pos)
+        return target, short, long, pooled, pos
+
+    @staticmethod
+    def backward(ctx, g_target, g_short, g_long, g_pooled, _):
+        sctx, lctx, S, k, L, x, mask_u8, target, a, u, qk, pos, Wa, Wb = ctx.parts
+        dt_s, dx_s, dws = _mhta_bwd(sctx, _f32c(g_short))
+        dt_l, dx_l, dwl = _mhta_bwd(lctx, _f32c(g_long))
+        B, d = dt_s.shape
+        dev = x.device
+        g_target, g_pooled = _f32c(g_target), _f32c(g_pooled)
+        dqk = torch.empty((B, L), dtype=torch.float32, device=dev)
+        du = torch.empty((B, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_sim_gsu_bwd", _ptr(x), _ptr(mask_u8), _ptr(g_pooled), B, L, d, _ptr(dqk), _ptr(du), _stream())
+        da = gemm_f32(du, Wb, torch.empty_like(a), b_t=True)                   # da = du W_b^T
+        dWb = gemm_f32(a, du, torch.empty_like(Wb), a_t=True)                  # dW_b = a^T du
+        dt_g = gemm_f32(da, Wa, torch.empty_like(target))                      # dt = da W_a
+        dWa = gemm_f32(da, target, torch.empty_like(Wa), a_t=True)             # dW_a = da^T t
+        dx = torch.empty((B, L + 1, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_sim_assemble_bwd", _ptr(g_target), _ptr(dt_s), _ptr(dt_l), _ptr(dt_g), _ptr(dx_s), S,
+                  _ptr(dx_l), _ptr(pos), _ptr(qk), _ptr(dqk), _ptr(u), _ptr(g_pooled), B, L, d, k, _ptr(dx),
+                  _stream())
+        return (dx, None, None, None, None, None, dWa, dWb) + dws + dwl
+
+
+class _TwinInterest(torch.autograd.Function):
+    """TWIN.forward's interest block (TWIN.py:125-141 with MultiHeadTopKAttention, TWIN.py:243-293) over item_feat_emb
+    x (B, L + 1, d) as one node: the short target attention over the window, then the top-k attention over the whole
+    history.  W_q, W_h, W_v, W_o fold as MultiHeadTargetAttention's do (b2_mhta_pack, scale 1 / sqrt(head_dim)), so
+    the history is never projected: q' = t W_M^T (fp32 in every matmul mode: the scores decide the selection), the row
+    kernel's per-head selection, softmax and pooled p (b2_twin_topk_fwd), out = p W_N^T (the matmul mode's GEMM).
+    Returns (target, short, long, positions (B, heads, k)).  The backward's row kernel (b2_twin_topk_bwd) writes dq'
+    and all of dx, the target row's dq' W_M included."""
+
+    @staticmethod
+    def forward(ctx, x, mask_u8, S, k, heads, use_scale, *weights):
+        x = _f32c(x)
+        B, L1, d = x.shape
+        L, H, dev = L1 - 1, heads, x.device
+        ws = weights[:4]
+        Wq, Wh, Wv, Wo = (_f32c(w) for w in weights[4:])
+        target = x[:, L].contiguous()
+        hs, ms = _short_window(x, mask_u8, S)
+        short, sctx = _mhta_fwd(target, hs, ms, heads, _mhta_scale(ws, d, heads, use_scale), ws)
+        hd = Wq.shape[0] // H
+        scale = 1.0 / hd ** 0.5
+        WM = torch.empty((H * d, d), dtype=torch.float32, device=dev)
+        WN = torch.empty((d, H * d), dtype=torch.float32, device=dev)
+        _lib.call("b2_mhta_pack", _ptr(Wq), _ptr(Wh), _ptr(Wv), _ptr(Wo), d, H, hd, scale, _ptr(WM), _ptr(WN),
+                  _stream())
+        q = gemm_f32(target, WM, torch.empty((B, H * d), dtype=torch.float32, device=dev), b_t=True)
+        p = torch.empty((B, H * d), dtype=torch.float32, device=dev)
+        stats = torch.empty((B, H, 2), dtype=torch.float32, device=dev)
+        pos = torch.empty((B, H, k), dtype=torch.int32, device=dev)
+        _lib.call("b2_twin_topk_fwd", _ptr(q), _ptr(x), _ptr(mask_u8), B, L, d, H, k, _ptr(p), _ptr(stats), _ptr(pos),
+                  _stream())
+        tc = _tc_layer_ok(WN)
+        p_aux, wn_aux = (make_aux(p), make_aux(WN)) if tc else (None, None)
+        long = _linear_fwd(tc, p, p_aux, WN, torch.empty((B, d), dtype=torch.float32, device=dev), wn_aux)
+        ctx.parts = (sctx, S, k, H, hd, scale, x, mask_u8, target, q, p, stats, pos, WM, WN, tc, p_aux, wn_aux,
+                     (Wq, Wh, Wv, Wo))
+        ctx.mark_non_differentiable(pos)
+        return target, short, long, pos
+
+    @staticmethod
+    def backward(ctx, g_target, g_short, g_long, _):
+        (sctx, S, k, H, hd, scale, x, mask_u8, target, q, p, stats, pos, WM, WN, tc, p_aux, wn_aux,
+         (Wq, Wh, Wv, Wo)) = ctx.parts
+        dt_s, dx_s, dws = _mhta_bwd(sctx, _f32c(g_short))
+        B, L1, d = x.shape
+        dev = x.device
+        g, g_target = _f32c(g_long), _f32c(g_target)
+        g_aux = make_aux(g) if tc else None
+        dp = torch.empty((B, H * d), dtype=torch.float32, device=dev)
+        dWN = torch.empty((d, H * d), dtype=torch.float32, device=dev)
+        _linear_dgrad(tc, g, g_aux, WN, dp, wn_aux)                           # dp = g W_N
+        _linear_wgrad(tc, g, g_aux, p, p_aux, dWN)                           # dW_N = g^T p
+        dq = torch.empty((B, H * d), dtype=torch.float32, device=dev)
+        dx = torch.empty_like(x)
+        _lib.call("b2_twin_topk_bwd", _ptr(q), _ptr(x), _ptr(mask_u8), _ptr(p), _ptr(stats), _ptr(pos), _ptr(dp),
+                  _ptr(WM), _ptr(g_target), _ptr(dt_s), _ptr(dx_s), S, B, L1 - 1, d, H, k, _ptr(dq), _ptr(dx),
+                  _stream())
+        dWM = gemm_f32(dq, target, torch.empty_like(WM), a_t=True)             # dW_M = dq'^T t
+        gWq, gWh, gWv, gWo = (torch.empty_like(w) for w in (Wq, Wh, Wv, Wo))
+        _lib.call("b2_mhta_unpack", _ptr(Wq), _ptr(Wh), _ptr(Wv), _ptr(Wo), _ptr(dWM), _ptr(dWN), d, H, hd, scale,
+                  _ptr(gWq), _ptr(gWh), _ptr(gWv), _ptr(gWo), _stream())
+        return (dx, None, None, None, None, None) + dws + (gWq, gWh, gWv, gWo)
+
+
+def _topk_weights(name, weights, d, heads):
+    for w in weights:
+        _require_cuda(w)
+    A = weights[0].shape[0]
+    if A % heads or any(tuple(w.shape) != (A, d) for w in weights[:-1]) or tuple(weights[-1].shape) != (d, A):
+        raise ValueError("%s: attention_dim %d, num_heads %d and the weights do not match" % (name, A, heads))
+
+
+def sim_interest(item_emb, mask, short_seq_len, topk, num_heads, W_a, W_b, short_weights, long_weights):
+    """SIM's interest block: item_emb (B, L + 1, d) (the last position the target), mask (B, L) (non-zero = valid),
+    W_a, W_b (A, d) the GSU's Linears, short_weights and long_weights the (W_q, W_k, W_v, W_o) of the two attentions
+    (use_scale on, as SIM builds them).  Returns (target, short interest, long interest, pooled, positions): four
+    (B, d) and the chosen history positions (B, k) int32, k = min(topk, L), sorted by (score desc, position asc).
+    Masked positions score 0, as in the reference; ties go to the lower position, and -0.0 ties with +0.0."""
+    mask_u8, B, L, d = _longctr_inputs("SIM", item_emb, mask, short_seq_len)
+    bound = sim_bound(d, L, topk, num_heads, B)
+    if bound is not None:
+        raise NotImplementedError("SIM kernels: " + bound)
+    _topk_weights("SIM", tuple(short_weights), d, num_heads)
+    _topk_weights("SIM", tuple(long_weights), d, num_heads)
+    _require_cuda(W_a, W_b)
+    if W_a.dim() != 2 or tuple(W_b.shape) != tuple(W_a.shape) or W_a.shape[1] != d:
+        raise ValueError("SIM: W_a%s and W_b%s must both be (attention_dim, d = %d)"
+                         % (tuple(W_a.shape), tuple(W_b.shape), d))
+    return _SimInterest.apply(item_emb, mask_u8, short_seq_len - 1, min(topk, L), num_heads, True, W_a, W_b,
+                              *short_weights, *long_weights)
+
+
+def twin_interest(item_emb, mask, short_seq_len, topk, num_heads, short_weights, topk_weights):
+    """TWIN's interest block: item_emb (B, L + 1, d) (the last position the target), mask (B, L) (non-zero = valid),
+    short_weights the (W_q, W_k, W_v, W_o) of the short attention, topk_weights the (W_q, W_h, W_v, W_o) of
+    MultiHeadTopKAttention.  Returns (target, short interest, long interest, positions): three (B, d) and the chosen
+    history positions (B, num_heads, k) int32, k = min(topk, L), per head sorted by (score desc, position asc).  A
+    masked score is exactly -1e9, so masked rows tie and go to the lower positions."""
+    mask_u8, B, L, d = _longctr_inputs("TWIN", item_emb, mask, short_seq_len)
+    bound = twin_bound(d, L, topk, num_heads, B)
+    if bound is not None:
+        raise NotImplementedError("TWIN kernels: " + bound)
+    _topk_weights("TWIN", tuple(short_weights), d, num_heads)
+    _topk_weights("TWIN", tuple(topk_weights), d, num_heads)
+    return _TwinInterest.apply(item_emb, mask_u8, short_seq_len - 1, min(topk, L), num_heads, True, *short_weights,
+                               *topk_weights)
 
 
 def mlp_chain_supported():

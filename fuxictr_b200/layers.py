@@ -972,6 +972,43 @@ class MultiHeadTargetAttention(nn.Module):
                                    *weights)
 
 
+class MultiHeadTopKAttention(nn.Module):
+    """model_zoo/LongCTR/TWIN/TWIN.py, MultiHeadTopKAttention: per head, the target scores the whole history, the top k
+    scores are kept and softmaxed, and their values are pooled.  The constructor, its assert, the children W_q, W_h,
+    W_v, W_o (registration order, state_dict keys, initial draws) and `dropout` are the reference's.  It runs inside
+    TWIN's interest block, one autograd node on the kernels (functional.twin_interest); Kc > 0 (cross features, which
+    the reference can only broadcast at L = 1) and attention dropout have no kernel and raise."""
+
+    def __init__(self, input_dim=64, Kc=0, embedding_dim=16, attention_dim=64, topk=50, num_heads=1, dropout_rate=0):
+        super(MultiHeadTopKAttention, self).__init__()
+        assert attention_dim % num_heads == 0, \
+            "attention_dim={} is not divisible by num_heads={}".format(attention_dim, num_heads)
+        if Kc > 0:
+            raise NotImplementedError("MultiHeadTopKAttention kernels: Kc_cross_features > 0 is not supported: the "
+                                      "reference's cross_feat_seq.view(B, Kc, -1) * W_c broadcasts only at L = 1")
+        if dropout_rate:
+            raise NotImplementedError("MultiHeadTopKAttention kernels: attention dropout has no kernel")
+        self.num_heads = num_heads
+        self.topk = topk
+        self.head_dim = attention_dim // num_heads
+        self.scale = self.head_dim ** 0.5
+        self.Kc = Kc
+        self.Kc_dim = 0
+        self.Kh_dim = input_dim
+        self.W_q = nn.Linear(input_dim, attention_dim, bias=False)
+        self.W_h = nn.Linear(input_dim, attention_dim, bias=False)
+        self.W_v = nn.Linear(input_dim, attention_dim, bias=False)
+        self.W_o = nn.Linear(attention_dim, input_dim, bias=False)
+        self.dropout = None
+
+    def weights(self):
+        return self.W_q.weight, self.W_h.weight, self.W_v.weight, self.W_o.weight
+
+    def forward(self, target_item, item_sequence, mask=None):
+        raise NotImplementedError("MultiHeadTopKAttention runs inside TWIN's interest block: call "
+                                  "functional.twin_interest on item_feat_emb (B, L + 1, d) with the target last")
+
+
 class MultiHeadSelfAttention(nn.Module):
     """model_zoo/AutoInt/src/AutoInt.py, MultiHeadSelfAttention: field-wise multi-head self-attention with an optional
     residual (X, or X W_res^T when input_dim != attention_dim), LayerNorm and a final ReLU.  One autograd node per layer

@@ -22,6 +22,7 @@ same RNG consumption) and nothing else.
   BST          model_zoo/BST/src/BST.py
   DIEN         model_zoo/DIEN/src/DIEN.py
   ETA, SDIM    model_zoo/LongCTR/ETA/ETA.py, model_zoo/LongCTR/SDIM/SDIM.py
+  SIM, TWIN    model_zoo/LongCTR/SIM/SIM.py, model_zoo/LongCTR/TWIN/TWIN.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
 """
@@ -35,7 +36,7 @@ from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbedding
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
                      FeatureGating, FinalBlock, BehaviorTransformer, DynamicGRU, AttentionLayer, MaskedSumPooling,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, MultiHeadTargetAttention,
-                     not_in_whitelist)
+                     MultiHeadTopKAttention, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
 
@@ -1509,15 +1510,15 @@ class _LongCTRModel(RankModel):
     def get_group_id(self, inputs):
         return inputs[0][self.feature_map.group_id]
 
-    def _logit_mlp(self):
-        """dnn without its output Sigmoid (the same modules, not registered a second time)."""
-        ent = self.__dict__.get("_logit_dnn")
+    def _logit_mlp(self, name="dnn"):
+        """The MLP_Block `name` without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_" + name)
         if ent is None:
             ent = MLP_Block.__new__(MLP_Block)
             nn.Module.__init__(ent)
-            mods = list(self.dnn.mlp)
+            mods = list(getattr(self, name).mlp)
             ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
-            self.__dict__["_logit_dnn"] = ent
+            self.__dict__["_logit_" + name] = ent
         return ent
 
     def _item_inputs(self, inputs):
@@ -1651,3 +1652,134 @@ class SDIM(_LongCTRModel):
         emb_out, item_feat_emb, mask = self._item_inputs(inputs)
         target, short, long = self.interest(item_feat_emb, mask)
         return torch.cat(([emb_out] if emb_out is not None else []) + [target, long, short], dim=-1)
+
+
+def _mhta_weights(att):
+    return att.W_q.weight, att.W_k.weight, att.W_v.weight, att.W_o.weight
+
+
+def _check_heads(name, attention_dim, num_heads):
+    if num_heads < 1 or attention_dim % num_heads:
+        raise ValueError("%s: attention_dim=%d is not divisible by num_heads=%d" % (name, attention_dim, num_heads))
+
+
+class SIM(_LongCTRModel):
+    """model_zoo/LongCTR/SIM/SIM.py, SIM: a short target attention over the last short_seq_len - 1 history items; a
+    soft-search GSU that scores every history row as qk_l = (W_a t) . (W_b x_l) mask_l, pools the history with those
+    scores into an auxiliary DNN over [batch embeddings, target, pooled], and keeps the topk best rows for a long target
+    attention; the main DNN reads [batch embeddings, target, short, long].  forward returns {"y_pred", "y_aux"} and the
+    loss is alpha BCE(y_aux) + beta BCE(y_pred).  The interest block is one autograd node on the kernels
+    (functional.sim_interest).  Masked positions score 0, as in the reference, so they outrank negatively scored valid
+    rows; ties go to the lower history position.  Unknown keyword arguments are accepted and ignored.  Refusals:
+    gsu_type != "soft" (the reference asserts), attention_dim not divisible by num_heads, see _LongCTRModel, and shapes
+    outside functional.sim_bound."""
+
+    def __init__(self, feature_map, model_id="SIM", gpu=-1, dnn_hidden_units=[512, 128, 64], dnn_activations="ReLU",
+                 attention_dropout=0, attention_dim=64, num_heads=1, gsu_type="soft", short_seq_len=50, topk=50,
+                 alpha=1, beta=1, learning_rate=1e-3, embedding_dim=10, net_dropout=0, batch_norm=False,
+                 accumulation_steps=1, embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(SIM, self).__init__(feature_map, model_id=model_id, gpu=gpu, embedding_regularizer=embedding_regularizer,
+                                  net_regularizer=net_regularizer, **kwargs)
+        if gsu_type != "soft":
+            raise NotImplementedError("SIM: gsu_type=%r is not supported: only the soft search exists (the reference "
+                                      "asserts gsu_type == 'soft')" % (gsu_type,))
+        self._longctr_init(feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps)
+        _check_heads("SIM", attention_dim, num_heads)
+        bound = F2.sim_bound(self.item_info_dim, 1, topk, num_heads)
+        if bound is not None:
+            raise NotImplementedError("SIM kernels: " + bound)
+        self.topk = topk
+        self.alpha = alpha
+        self.beta = beta
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.W_a = nn.Linear(self.item_info_dim, attention_dim, bias=False)
+        self.W_b = nn.Linear(self.item_info_dim, attention_dim, bias=False)
+        self.short_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                        attention_dropout)
+        self.long_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                       attention_dropout)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim
+        self.dnn_aux = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                                 hidden_activations=dnn_activations, output_activation=self.output_activation,
+                                 dropout_rates=net_dropout, batch_norm=batch_norm)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim * 2
+        self.dnn = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def interest(self, item_feat_emb, mask):
+        """(target, short, long, pooled, positions) of functional.sim_interest."""
+        return F2.sim_interest(item_feat_emb, mask, self.short_seq_len, self.topk, self.short_attention.num_heads,
+                               self.W_a.weight, self.W_b.weight, _mhta_weights(self.short_attention),
+                               _mhta_weights(self.long_attention))
+
+    def _logits(self, inputs):
+        """(main logit, auxiliary logit), each (B, 1) before the output Sigmoid."""
+        emb_out, item_feat_emb, mask = self._item_inputs(inputs)
+        target, short, long, pooled, _ = self.interest(item_feat_emb, mask)
+        emb = [emb_out] if emb_out is not None else []
+        y = self._logit_mlp()(torch.cat(emb + [target, short, long], dim=-1))
+        y_aux = self._logit_mlp("dnn_aux")(torch.cat(emb + [target, pooled], dim=-1))
+        return y, y_aux
+
+    def forward_logits(self, inputs):
+        return (self._logits(inputs)[0],)
+
+    def forward(self, inputs):
+        y, y_aux = self._logits(inputs)
+        return {"y_pred": self.output_activation(y), "y_aux": self.output_activation(y_aux)}
+
+    def compute_loss(self, return_dict, y_true):
+        loss_gsu = self.loss_fn(return_dict["y_aux"], y_true, reduction="mean")
+        loss_esu = self.loss_fn(return_dict["y_pred"], y_true, reduction="mean")
+        return self.alpha * loss_gsu + self.beta * loss_esu + self.regularization_loss()
+
+    def fused_loss(self, batch_data, y_true):
+        y, y_aux = self._logits(batch_data)
+        return self.alpha * F2.logit_bce(y_true, y_aux)[0] + self.beta * F2.logit_bce(y_true, y)[0]
+
+
+class TWIN(_LongCTRModel):
+    """model_zoo/LongCTR/TWIN/TWIN.py, TWIN: a short target attention over the last short_seq_len - 1 history items,
+    and MultiHeadTopKAttention over the whole history: per head the topk best scores, softmaxed over those k; the DNN
+    reads [batch embeddings, target, short, long].  The interest block is one autograd node on the kernels
+    (functional.twin_interest); ties go to the lower history position.  Unknown keyword arguments are accepted and
+    ignored.  Refusals: Kc_cross_features > 0 (the reference can only broadcast its cross features at L = 1),
+    attention_dim not divisible by num_heads, see _LongCTRModel, and shapes outside functional.twin_bound."""
+
+    def __init__(self, feature_map, model_id="TWIN", gpu=-1, dnn_hidden_units=[512, 128, 64], dnn_activations="ReLU",
+                 attention_dropout=0, attention_dim=64, num_heads=1, short_seq_len=50, topk=50, Kc_cross_features=0,
+                 learning_rate=1e-3, embedding_dim=10, net_dropout=0, batch_norm=False, accumulation_steps=1,
+                 embedding_regularizer=None, net_regularizer=None, **kwargs):
+        super(TWIN, self).__init__(feature_map, model_id=model_id, gpu=gpu, embedding_regularizer=embedding_regularizer,
+                                   net_regularizer=net_regularizer, **kwargs)
+        if Kc_cross_features > 0:
+            raise NotImplementedError("TWIN: Kc_cross_features > 0 is not supported: the reference's "
+                                      "cross_feat_seq.view(B, Kc, -1) * W_c broadcasts only at L = 1")
+        self._longctr_init(feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps)
+        _check_heads("TWIN", attention_dim, num_heads)
+        bound = F2.twin_bound(self.item_info_dim, 1, topk, num_heads)
+        if bound is not None:
+            raise NotImplementedError("TWIN kernels: " + bound)
+        self.topk = topk
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.short_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                        attention_dropout)
+        self.long_attention = MultiHeadTopKAttention(self.item_info_dim, Kc_cross_features, embedding_dim,
+                                                     attention_dim, topk, num_heads, attention_dropout)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim * 2
+        self.dnn = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def interest(self, item_feat_emb, mask):
+        """(target, short, long, positions) of functional.twin_interest."""
+        return F2.twin_interest(item_feat_emb, mask, self.short_seq_len, self.topk, self.short_attention.num_heads,
+                                _mhta_weights(self.short_attention), self.long_attention.weights())
+
+    def dnn_input(self, inputs):
+        emb_out, item_feat_emb, mask = self._item_inputs(inputs)
+        target, short, long, _ = self.interest(item_feat_emb, mask)
+        return torch.cat(([emb_out] if emb_out is not None else []) + [target, short, long], dim=-1)

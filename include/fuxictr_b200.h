@@ -747,6 +747,54 @@ B2_API int b2_sdim_assemble_bwd(const float* dt0, const float* dt1, const float*
                                 int d, int num_hashes, int l2norm, float* dx, void* stream);
 
 /*
+ * SIM / TWIN: learned-score top-k retrieval over a long behaviour sequence, SIM's soft-search GSU
+ * (model_zoo/LongCTR/SIM/SIM.py) and TWIN's MultiHeadTopKAttention (model_zoo/LongCTR/TWIN/TWIN.py).  x is
+ * item_feat_emb (B, L + 1, d) row-major fp32: positions [0, L) the history, position L the target; mask (B, L) bytes,
+ * non-zero = valid.  Scores are fp32 FMA dot products over ascending columns.  The selection keeps the k largest
+ * scores, sorted by (score desc, position asc): ties go to the lower position, and -0.0 ties with +0.0.
+ * b2_sim_retrieve_fwd: u (B, d) = W_b^T W_a t.  qk (B, L) "=" (u . x_l) mask_l (masked positions score 0),
+ *   pooled (B, d) "=" sum_l qk_l x_l, and the k best: topk_emb (B, k, d), topk_mask (B, k) bytes (mask != 0 at the
+ *   chosen position) and topk_pos (B, k) int32.
+ * b2_sim_gsu_bwd: dqk (B, L) "=" (dpooled . x_l) mask_l, du (B, d) "=" sum_l dqk_l x_l.
+ * b2_sim_assemble_bwd: dx (B, L + 1, d) "=", every row written once.  Row L = dt0 + dt1 + dt2 + dt3 (each (B, d)).
+ *   Rows [0, L): dshort (B, S, d) on rows [L - S, L), dlong (B, k, d) at the positions topk_pos, and
+ *   qk_l dpooled + dqk_l u.
+ * b2_twin_topk_fwd: q (B, heads d) = t W_M^T of b2_mhta_pack (the 1 / sqrt(head_dim) scale folded in).
+ *   score_hl = q_h . x_l, exactly -1e9 where masked; per head the k best, a softmax over them, p (B, heads d) "="
+ *   sum_s a_hs x_{pos_hs}, stats (B, heads, 2) "=" {the largest chosen score, sum of exp(score - it)} and
+ *   topk_pos (B, heads, k) "=" the chosen positions.  All chosen masked: the weights are uniform over the k.
+ * b2_twin_topk_bwd: from dp (B, heads d) and the forward's q, p, stats and topk_pos: dq (B, heads d) "=" and
+ *   dx (B, L + 1, d) "=", every row written once.  ds_hs = a_hs (dp_h . x_l - dp_h . p_h) (0 where masked),
+ *   dq_h = sum_s ds_hs x_l, dx_l = sum over the heads that chose l of (a_hs dp_h + ds_hs q_h), plus dshort on rows
+ *   [L - S, L); row L = dt0 + dt1 + dq W_M (W_M (heads d, d) the forward's packed weight).
+ * Range: 1 <= d <= B2_TOPK_MAX_DIM, 1 <= L <= B2_TOPK_MAX_LEN, 1 <= k <= min(L, B2_TOPK_MAX_K), batch (L + 1) < 2^31,
+ * batch >= 0 (0: no launch), 1 <= S <= L; TWIN 1 <= heads <= B2_MHTA_MAX_HEADS with heads d <= B2_MHTA_MAX_WIDTH; the
+ * dynamic shared memory a CTA needs within B2_TOPK_MAX_SMEM bytes (G = 256 / d column groups): SIM forward
+ * 8 L + 4 d + 4 G d + 4 k, SIM backward 4 L + 4 d + 4 G d, TWIN forward 4 L + 4 d + 8 k + 4 G d, TWIN backward
+ * 4 ceil(heads L / 2) + 12 heads d + 12 heads k + 4 heads.  Outside the range, or given a NULL pointer, every entry
+ * point returns B2_E_INVALID.
+ */
+#define B2_TOPK_MAX_DIM 256
+#define B2_TOPK_MAX_LEN 4096
+#define B2_TOPK_MAX_K 256
+#define B2_TOPK_MAX_SMEM (220 * 1024)
+B2_API int b2_sim_retrieve_fwd(const float* x, const uint8_t* mask, const float* u, int64_t batch, int L, int d,
+                               int k, float* qk, float* pooled, float* topk_emb, uint8_t* topk_mask,
+                               int32_t* topk_pos, void* stream);
+B2_API int b2_sim_gsu_bwd(const float* x, const uint8_t* mask, const float* dpooled, int64_t batch, int L, int d,
+                          float* dqk, float* du, void* stream);
+B2_API int b2_sim_assemble_bwd(const float* dt0, const float* dt1, const float* dt2, const float* dt3,
+                               const float* dshort, int S, const float* dlong, const int32_t* topk_pos,
+                               const float* qk, const float* dqk, const float* u, const float* dpooled, int64_t batch,
+                               int L, int d, int k, float* dx, void* stream);
+B2_API int b2_twin_topk_fwd(const float* q, const float* x, const uint8_t* mask, int64_t batch, int L, int d,
+                            int heads, int k, float* p, float* stats, int32_t* topk_pos, void* stream);
+B2_API int b2_twin_topk_bwd(const float* q, const float* x, const uint8_t* mask, const float* p, const float* stats,
+                            const int32_t* topk_pos, const float* dp, const float* WM, const float* dt0,
+                            const float* dt1, const float* dshort, int S, int64_t batch, int L, int d, int heads,
+                            int k, float* dq, float* dx, void* stream);
+
+/*
  * WuKong's layer (model_zoo/WuKong/src/WuKong.py, WuKongLayer) on x (B, F, D) with rank k, lcb + fmb = Fo output
  * fields:
  *   fm   = LN_fk(flatten(x (x^T Y)))                 Y = proj_Y (F, k); LN over F k, always affine
