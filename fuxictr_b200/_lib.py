@@ -29,6 +29,8 @@ B2_FINALNET_CONCAT, B2_FINALNET_SUM = 0, 1
 B2_FINALNET_MAX_WIDTH, B2_FINALNET_MAX_FIELDS, B2_FINALNET_MAX_DIM, B2_FINALNET_MAX_GATE_WIDTH = 1024, 128, 128, 8192
 B2_BST_MAX_LEN, B2_BST_MAX_DIM, B2_BST_MAX_HEAD_DIM, B2_BST_MAX_HEADS, B2_BST_MAX_PARTS = 256, 512, 64, 16, 8
 B2_BST_POOL_MEAN, B2_BST_POOL_SUM, B2_BST_POOL_TARGET = 0, 1, 2
+(B2_TRANSACT_MAX_LEN, B2_TRANSACT_MAX_DIM, B2_TRANSACT_MAX_HEAD_DIM, B2_TRANSACT_MAX_HEADS,
+ B2_TRANSACT_MAX_PARTS) = 256, 512, 256, 16, 8
 B2_DIEN_MAX_DIM, B2_DIEN_MAX_LEN = 64, 1024
 B2_DIEN_GRU, B2_DIEN_AUGRU, B2_DIEN_AGRU = 0, 1, 2
 B2_LSH_MAX_DIM, B2_LSH_MAX_LEN, B2_LSH_MAX_TOPK, B2_LSH_MAX_SMEM = 256, 4096, 256, 227 * 1024 - 1024
@@ -223,6 +225,19 @@ SIGNATURES = {
                                    c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_bst_pool_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "b2_bst_pool_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b2_transact_tokens_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64,
+                                       c_int64, c_int, c_int, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p]),
+    "b2_transact_tokens_bwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_transact_attn_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_float, c_void_p, c_int64,
+                                     ctypes.c_uint32, c_float, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p,
+                                     c_void_p]),
+    "b2_transact_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int,
+                                     c_int, c_float, c_void_p, c_int64, ctypes.c_uint32, c_float, c_void_p, c_void_p,
+                                     c_void_p, c_int, c_int64, c_void_p]),
+    "b2_transact_out_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_int, c_int64, c_void_p]),
+    "b2_transact_out_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p,
+                                    c_void_p]),
     "b2_gru_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                            c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_gru_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

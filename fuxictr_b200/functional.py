@@ -1980,6 +1980,221 @@ def bst_pooling(x, valid, batch, seq_len, pooling="mean"):
 
 
 # --------------------------------------------------------------------------------------
+# TransAct (include/fuxictr_b200.h "TransAct")
+# --------------------------------------------------------------------------------------
+_IDS_DTYPE = {torch.float64: _lib.B2_F64, torch.int64: _lib.B2_I64, torch.int32: _lib.B2_I32,
+              torch.float32: _lib.B2_F32}
+
+
+def transact_bound(seq_len, model_dim, num_heads, parts=2, heads_apply=True):
+    """None when the TransAct kernels cover L = seq_len tokens of width model_dim in num_heads heads, built from
+    `parts` fields per token (sequence and target fields together); else the bound it breaks.  heads_apply=False: the
+    kernels that see no heads (tokens, output)."""
+    if not 1 <= seq_len <= _lib.B2_TRANSACT_MAX_LEN:
+        return "max_len must lie in [1, %d], got %d" % (_lib.B2_TRANSACT_MAX_LEN, seq_len)
+    if not 1 <= model_dim <= _lib.B2_TRANSACT_MAX_DIM:
+        return "model_dim must lie in [1, %d], got %d" % (_lib.B2_TRANSACT_MAX_DIM, model_dim)
+    if not 2 <= parts <= _lib.B2_TRANSACT_MAX_PARTS:
+        return "a token takes 2 to %d fields, got %d" % (_lib.B2_TRANSACT_MAX_PARTS, parts)
+    if not heads_apply:
+        return None
+    if not 1 <= num_heads <= _lib.B2_TRANSACT_MAX_HEADS:
+        return "num_heads must lie in [1, %d], got %d" % (_lib.B2_TRANSACT_MAX_HEADS, num_heads)
+    if model_dim % num_heads:
+        return "num_heads=%d does not divide model_dim=%d" % (num_heads, model_dim)
+    if model_dim // num_heads > _lib.B2_TRANSACT_MAX_HEAD_DIM:
+        return "the head width model_dim / num_heads must be at most %d, got %d" % (_lib.B2_TRANSACT_MAX_HEAD_DIM,
+                                                                                 model_dim // num_heads)
+    return None
+
+
+class _TransActTokens(torch.autograd.Function):
+    """(X (B L, md), valid (B, L) uint8): token t of sample b is [seq_0[b, t] .. | tgt_0[b] ..], valid is ids != 0 with
+    an empty history's last slot set (b2_transact_tokens_fwd, one launch).  Backward: the sequence views' gradients and
+    the targets' sums over t in one launch (b2_transact_tokens_bwd)."""
+
+    @staticmethod
+    def forward(ctx, cfg, ids, *views):
+        ns, want_aux = cfg
+        seqs = [v if (v.dtype == torch.float32 and v.stride(2) == 1 and v.stride(1) == v.shape[2]) else
+                v.float().contiguous() for v in views[:ns]]
+        tgts = [v if (v.dtype == torch.float32 and v.stride(1) == 1) else v.float().contiguous() for v in views[ns:]]
+        nt = len(tgts)
+        B, L, D = seqs[0].shape
+        md = D * (ns + nt)
+        dev = seqs[0].device
+        out = torch.empty((B * L, md), dtype=torch.float32, device=dev)
+        valid = torch.empty((B, L), dtype=torch.uint8, device=dev)
+        ctx.shape = (B, L, D, ns, nt)
+        ctx.mark_non_differentiable(valid)
+        if B == 0:
+            return out, valid
+        if ids.dtype not in _IDS_DTYPE:
+            ids = ids.long()
+        if ids.stride(1) != 1:
+            ids = ids.contiguous()
+        aux = empty_aux(B * L, md, dev) if want_aux else None
+        _lib.call("b2_transact_tokens_fwd", _arr(ctypes.c_void_p, [v.data_ptr() for v in seqs]),
+                  _arr(ctypes.c_int64, [v.stride(0) for v in seqs]), ns,
+                  _arr(ctypes.c_void_p, [v.data_ptr() for v in tgts]), _arr(ctypes.c_int64, [v.stride(0) for v in tgts]),
+                  nt, _ptr(ids), _IDS_DTYPE[ids.dtype], ids.stride(0), B, L, D, _ptr(out), *_aux_args(aux),
+                  _ptr(valid), _stream())
+        _set_aux_hint(out, aux)
+        return out, valid
+
+    @staticmethod
+    def backward(ctx, g, _gvalid):
+        B, L, D, ns, nt = ctx.shape
+        dev = g.device
+        dseq = [torch.empty((B, L, D), dtype=torch.float32, device=dev) for _ in range(ns)]
+        dtgt = [torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(nt)]
+        if B > 0:
+            _lib.call("b2_transact_tokens_bwd", _ptr(_f32c(g)), B, L, D, ns, nt,
+                      _arr(ctypes.c_void_p, [t.data_ptr() for t in dseq]),
+                      _arr(ctypes.c_void_p, [t.data_ptr() for t in dtgt]), _stream())
+        return (None, None) + tuple(dseq) + tuple(dtgt)
+
+
+def transact_tokens(sequence_embs, target_embs, ids, want_aux=False):
+    """TransAct's early-fusion tokens of one (target, sequence) pair and its key-padding mask: sequence_embs ns views
+    (B, L, D), target_embs nt views (B, D) (a tuple of fields: their embeddings side by side), ids (B, L) the first
+    sequence field's ids.  Returns (X (B L, D (ns + nt)), valid (B, L) uint8): valid is ids != 0, with the last slot of
+    an all-padding sample set (TransActTransformer.adjust_mask).  want_aux: also write X's GEMM operand copy."""
+    seqs, tgts = list(sequence_embs), list(target_embs)
+    _require_cuda(*(seqs + tgts + [ids]))
+    if not seqs or not tgts:
+        raise ValueError("transact_tokens: %d sequence fields and %d target fields" % (len(seqs), len(tgts)))
+    B, L, D = seqs[0].shape
+    for v in seqs:
+        if v.dim() != 3 or tuple(v.shape) != (B, L, D):
+            raise ValueError("transact_tokens: sequence embeddings %s differ" % [tuple(t.shape) for t in seqs])
+    for v in tgts:
+        if tuple(v.shape) != (B, D):
+            raise ValueError("transact_tokens: target embeddings %s are not (%d, %d)"
+                             % ([tuple(t.shape) for t in tgts], B, D))
+    if tuple(ids.shape) != (B, L):
+        raise ValueError("transact_tokens: ids%s are not (%d, %d)" % (tuple(ids.shape), B, L))
+    bound = transact_bound(L, D * (len(seqs) + len(tgts)), 1, len(seqs) + len(tgts), heads_apply=False)
+    if bound is not None:
+        raise NotImplementedError("TransAct kernels: " + bound)
+    return _TransActTokens.apply((len(seqs), want_aux), ids, *(seqs + tgts))
+
+
+class _TransActAttention(torch.autograd.Function):
+    """ctx (B L, md) of the key-tiled masked self-attention on QKV (B L, 3 md) (b2_transact_attn_fwd), the
+    probabilities never stored; backward: dQKV in two deterministic launches (b2_transact_attn_bwd)."""
+
+    @staticmethod
+    def forward(ctx, qkv, valid, cfg):
+        B, L, md, heads, scale, drop, want_aux = cfg
+        dev = qkv.device
+        out = torch.empty((B * L, md), dtype=torch.float32, device=dev)
+        ctx.cfg = cfg
+        if B == 0:
+            return out
+        qkv = _f32c(qkv)
+        aux = empty_aux(B * L, md, dev) if want_aux else None
+        smax = torch.empty((B, heads, L), dtype=torch.float32, device=dev)
+        ssum = torch.empty_like(smax)
+        _lib.call("b2_transact_attn_fwd", _ptr(qkv), _ptr(valid), B, L, md, heads, scale, *_drop_args(drop),
+                  _ptr(out), *_aux_args(aux), _ptr(smax), _ptr(ssum), _stream())
+        _set_aux_hint(out, aux)
+        ctx.save_for_backward(qkv, valid, out, smax, ssum)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        B, L, md, heads, scale, drop, _ = ctx.cfg
+        if B == 0:
+            return torch.zeros((0, 3 * md), dtype=torch.float32, device=g.device), None, None
+        qkv, valid, out, smax, ssum = ctx.saved_tensors
+        dqkv = torch.empty_like(qkv)
+        delta = torch.empty_like(smax)
+        _lib.call("b2_transact_attn_bwd", _ptr(qkv), _ptr(valid), _ptr(out), _ptr(_f32c(g)), _ptr(smax), _ptr(ssum),
+                  B, L, md, heads, scale, *_drop_args(drop), _ptr(delta), _ptr(dqkv), *_aux_args(None), _stream())
+        return dqkv, None, None
+
+
+def transact_attention(qkv, valid, batch, seq_len, num_heads, dropout=0.0, snapshot=None, layer=0, want_aux=False):
+    """nn.MultiheadAttention's core with a key-padding mask on the in-projection's output qkv (B L, 3 md) =
+    [Q | K | V]: per head softmax((q sqrt(1 / dh)) k^T + mask) v, key j hidden iff valid[b, j] == 0 (valid (B, L)
+    uint8, never all 0 in a row).  Rows of padded queries come out 0.  dropout > 0: the weights take the mask of layer
+    `layer` of `snapshot` (dropout_snapshot; None: one of its own).  Returns (B L, md), before out_proj."""
+    _require_cuda(qkv, valid)
+    B, L = batch, seq_len
+    md = qkv.shape[1] // 3 if qkv.dim() == 2 else 0
+    if qkv.dim() != 2 or qkv.shape[0] != B * L or qkv.shape[1] != 3 * md:
+        raise ValueError("transact_attention: qkv%s is not (%d, 3 model_dim)" % (tuple(qkv.shape), B * L))
+    if valid.dtype != torch.uint8 or tuple(valid.shape) != (B, L) or not valid.is_contiguous():
+        raise ValueError("transact_attention: valid must be a contiguous (%d, %d) uint8 mask" % (B, L))
+    bound = transact_bound(L, md, num_heads)
+    if bound is not None:
+        raise NotImplementedError("TransAct kernels: " + bound)
+    drop = None
+    if dropout > 0:
+        if snapshot is None:
+            snapshot, layer = dropout_snapshot(qkv.device, 1), 0
+        drop = (snapshot, layer) + dropout_consts(dropout)
+    scale = float(ctypes.c_float(math.sqrt(1.0 / (md // num_heads))).value)
+    return _TransActAttention.apply(qkv, valid, (B, L, md, num_heads, scale, drop, want_aux))
+
+
+class _TransActOut(torch.autograd.Function):
+    """The last k slots of y (B L, md), zeroed where padded, flattened to (B, k md), and (max_pool) the max over L with
+    padded slots at -1e9, its winning slot per column saved (b2_transact_out_fwd); backward: dy "=" in one launch
+    (b2_transact_out_bwd)."""
+
+    @staticmethod
+    def forward(ctx, y, valid, cfg):
+        B, L, k, pool, want_aux = cfg
+        md = y.shape[1]
+        dev = y.device
+        last = torch.empty((B, k * md), dtype=torch.float32, device=dev)
+        maxv = torch.empty((B, md), dtype=torch.float32, device=dev) if pool else None
+        arg = torch.empty((B, md), dtype=torch.int32, device=dev) if pool else None
+        ctx.cfg = cfg
+        ctx.save_for_backward(valid, arg)
+        if B > 0:
+            aux = empty_aux(B, md, dev) if (pool and want_aux) else None
+            _lib.call("b2_transact_out_fwd", _ptr(_f32c(y)), _ptr(valid), B, L, md, k, _ptr(last), _ptr(maxv),
+                      _ptr(arg), *_aux_args(aux), _stream())
+            if aux is not None:
+                _set_aux_hint(maxv, aux)
+        return (last, maxv) if pool else last
+
+    @staticmethod
+    def backward(ctx, glast, gmax=None):
+        B, L, k, pool, _ = ctx.cfg
+        valid, arg = ctx.saved_tensors
+        md = glast.shape[1] // k
+        dy = torch.empty((B * L, md), dtype=torch.float32, device=glast.device)
+        if B > 0:
+            if pool and gmax is None:
+                gmax = torch.zeros((B, md), dtype=torch.float32, device=glast.device)
+            _lib.call("b2_transact_out_bwd", _ptr(_f32c(glast)), _ptr(_f32c(gmax) if pool else None),
+                      _ptr(arg), _ptr(valid), B, L, md, k, _ptr(dy), _stream())
+        return dy, None, None
+
+
+def transact_output(y, valid, batch, seq_len, first_k_cols=1, max_pool=True, want_aux=False):
+    """TransActTransformer's head on the encoder output y (B L, md): (last, maxv) with last (B, k md) the last k slots,
+    zeroed where padded, and maxv (B, md) the max over L with padded slots at -1e9 (ties: the first slot), or last
+    alone when not max_pool.  want_aux: also write maxv's GEMM operand copy for out_linear."""
+    _require_cuda(y, valid)
+    B, L = batch, seq_len
+    if y.dim() != 2 or y.shape[0] != B * L:
+        raise ValueError("transact_output: y%s is not (%d, model_dim)" % (tuple(y.shape), B * L))
+    if valid.dtype != torch.uint8 or tuple(valid.shape) != (B, L) or not valid.is_contiguous():
+        raise ValueError("transact_output: valid must be a contiguous (%d, %d) uint8 mask" % (B, L))
+    if not 1 <= first_k_cols <= L:
+        raise ValueError("transact_output: first_k_cols=%d outside [1, %d]" % (first_k_cols, L))
+    bound = transact_bound(L, y.shape[1], 1, heads_apply=False)
+    if bound is not None:
+        raise NotImplementedError("TransAct kernels: " + bound)
+    return _TransActOut.apply(y, valid, (B, L, int(first_k_cols), bool(max_pool), want_aux))
+
+
+# --------------------------------------------------------------------------------------
 # DIEN (include/fuxictr_b200.h "DIEN")
 # --------------------------------------------------------------------------------------
 DIEN_CELL = {"GRU": _lib.B2_DIEN_GRU, "AUGRU": _lib.B2_DIEN_AUGRU, "AGRU": _lib.B2_DIEN_AGRU}

@@ -1370,6 +1370,86 @@ class BehaviorTransformer(nn.Module):
                                   "valid)")
 
 
+class TransActTransformer(nn.Module):
+    """model_zoo/TransAct/src/TransAct.py, TransActTransformer: the early-fusion tokens [sequence | target] of the L
+    slots through a post-norm nn.TransformerEncoder with a key-padding mask (an empty history keeps its last slot),
+    the output zeroed at padded slots, then [last first_k_cols slots | out_linear(max over L)].
+    `transformer_encoder` is a real nn.TransformerEncoder and holds the parameters (its layers start as copies of one
+    layer, as in the reference); its forward is never called.  On the kernels (run), each layer is the in-projection
+    GEMM, the key-tiled attention (functional.transact_attention), out_proj, the residual + dropout1 + norm1 row
+    kernel, the FFN as one MLP chain (ReLU and the inner dropout in its first epilogue, dropout2 in its second) and the
+    residual + norm2 row kernel.  Refused: use_time_window_mask=True (the reference's forward never passes
+    time_interval_seq, so it cannot train)."""
+
+    def __init__(self, transformer_in_dim, dim_feedforward=64, num_heads=1, dropout=0, transformer_layers=1,
+                 use_time_window_mask=False, time_window_ms=86400000, first_k_cols=1, concat_max_pool=True):
+        super(TransActTransformer, self).__init__()
+        if use_time_window_mask:
+            raise NotImplementedError("TransAct use_time_window_mask=True is not supported: the reference's forward "
+                                      "never passes time_interval_seq, so its mask compares None with an int")
+        self.use_time_window_mask = use_time_window_mask
+        self.time_window_ms = time_window_ms
+        self.concat_max_pool = concat_max_pool
+        self.first_k_cols = first_k_cols
+        encoder_layer = nn.TransformerEncoderLayer(d_model=transformer_in_dim, nhead=num_heads,
+                                                   dim_feedforward=dim_feedforward, dropout=dropout, batch_first=True)
+        self.transformer_encoder = nn.TransformerEncoder(encoder_layer, num_layers=transformer_layers)
+        if self.concat_max_pool:
+            self.out_linear = nn.Linear(transformer_in_dim, transformer_in_dim)
+
+    @staticmethod
+    def _p(drop):
+        return drop.p if (drop.training and drop.p > 0) else 0.0
+
+    def run_layers(self, x, valid, batch, seq_len, want_aux=False):
+        """The encoder stack on the tokens x (B L, md) with the adjusted mask valid (B, L) uint8.  Rows of padded slots
+        come out finite but not the reference's: the model zeroes them.  In training mode with dropout, layer k's
+        attention weights take the mask of snapshot layer 2 k and its dropout1 that of 2 k + 1; the FFN chains draw
+        their own."""
+        lyrs = list(self.transformer_encoder.layers)
+        if batch == 0 or not lyrs:
+            return x
+        snap = None
+        if self.training and (lyrs[0].self_attn.dropout > 0 or self._p(lyrs[0].dropout1) > 0):
+            snap = F2.dropout_snapshot(x.device, 2 * len(lyrs))
+        for k, lyr in enumerate(lyrs):
+            if lyr.norm_first or lyr.activation_relu_or_gelu != 1:
+                raise NotImplementedError("TransActTransformer kernels: post-norm layers with ReLU only")
+            att = lyr.self_attn
+            last = k + 1 == len(lyrs)
+            qkv = F2.linear_act(x, att.in_proj_weight, att.in_proj_bias)
+            ctx = F2.transact_attention(qkv, valid, batch, seq_len, att.num_heads,
+                                        dropout=att.dropout if self.training else 0.0, snapshot=snap, layer=2 * k,
+                                        want_aux=F2._tc_layer_ok(att.out_proj.weight))
+            a = F2.linear_act(ctx, att.out_proj.weight, att.out_proj.bias)
+            s = F2.bst_add_norm(a, x, lyr.norm1.weight, lyr.norm1.bias, lyr.norm1.eps, dropout=self._p(lyr.dropout1),
+                                snapshot=snap, layer=2 * k + 1, want_aux=F2._tc_layer_ok(lyr.linear1.weight))
+            p0, p2 = self._p(lyr.dropout), self._p(lyr.dropout2)
+            f = F2.mlp_chain(s, [(lyr.linear1.weight, lyr.linear1.bias, B2_ACT_RELU) + ((p0,) if p0 > 0 else ()),
+                                 (lyr.linear2.weight, lyr.linear2.bias, B2_ACT_NONE) + ((p2,) if p2 > 0 else ())])
+            nxt = want_aux if last else F2._tc_layer_ok(lyrs[k + 1].self_attn.in_proj_weight)
+            x = F2.bst_add_norm(f, s, lyr.norm2.weight, lyr.norm2.bias, lyr.norm2.eps, want_aux=nxt)
+        return x
+
+    def run(self, sequence_embs, target_embs, ids):
+        """The (B, (first_k_cols + concat_max_pool) md) output on one (target, sequence) pair: sequence_embs the ns
+        (B, L, D) embeddings of the sequence fields, target_embs the nt (B, D) ones of the target fields, ids (B, L)
+        the first sequence field's ids (0 = padding)."""
+        lyrs = list(self.transformer_encoder.layers)
+        B, L = ids.shape[0], ids.shape[1]
+        x, valid = F2.transact_tokens(sequence_embs, target_embs, ids,
+                                      want_aux=bool(lyrs) and F2._tc_layer_ok(lyrs[0].self_attn.in_proj_weight))
+        y = self.run_layers(x, valid, B, L)
+        if not self.concat_max_pool:
+            return F2.transact_output(y, valid, B, L, self.first_k_cols, max_pool=False)
+        last, maxv = F2.transact_output(y, valid, B, L, self.first_k_cols, max_pool=True,
+                                        want_aux=F2._tc_layer_ok(self.out_linear.weight))
+        return torch.cat([last, F2.linear_act(maxv, self.out_linear.weight, self.out_linear.bias)], dim=-1)
+
+    def forward(self, target_emb, sequence_emb, time_interval_seq=None, mask=None):
+        raise NotImplementedError("TransActTransformer runs on the kernels through run(sequence_embs, target_embs, ids)")
+
+
 class AGRUCell(nn.Module):
     """model_zoo/DIEN/src/DIEN.py, AGRUCell: h' = h + a (n - h), r = s(i_r + h_r), n = tanh(i_n + r h_n), with the
     chunks u, r, n of x2h(x) and h2h(h) (u unused).  The kernels read x2h and h2h (functional.gru_sequence)."""

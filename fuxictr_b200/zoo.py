@@ -21,6 +21,7 @@ same RNG consumption) and nothing else.
   FinalNet     model_zoo/FinalNet/src/FinalNet.py
   BST          model_zoo/BST/src/BST.py
   DIEN         model_zoo/DIEN/src/DIEN.py
+  TransAct     model_zoo/TransAct/src/TransAct.py
   ETA, SDIM    model_zoo/LongCTR/ETA/ETA.py, model_zoo/LongCTR/SDIM/SDIM.py
   SIM, TWIN    model_zoo/LongCTR/SIM/SIM.py, model_zoo/LongCTR/TWIN/TWIN.py
   RankModel = the slice of BaseModel a training step touches,
@@ -36,7 +37,7 @@ from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbedding
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
                      FeatureGating, FinalBlock, BehaviorTransformer, DynamicGRU, AttentionLayer, MaskedSumPooling,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, MultiHeadTargetAttention,
-                     MultiHeadTopKAttention, not_in_whitelist)
+                     MultiHeadTopKAttention, TransActTransformer, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
 
@@ -1453,6 +1454,120 @@ class DIEN(RankModel):
 
     def forward_logits(self, inputs):
         return (self._logit_mlp()(self.dnn_input(inputs)),)
+
+    def forward(self, inputs):
+        return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}
+
+
+class TransAct(RankModel):
+    """model_zoo/TransAct/src/TransAct.py, TransAct: per (target, sequence) field pair (a tuple of fields: their
+    embeddings side by side) a TransActTransformer over the L = max_len early-fusion tokens [sequence | target], whose
+    output [last first_k_cols slots | out_linear(max over L)] replaces the pair's sequence fields; then DCNv2's parallel
+    structure, mlp(cat([CrossNetV2(x), parallel_dnn(x)])), on x = [remaining embeddings in FeatureMap order | the
+    transformer outputs in pair order].  The key-padding mask comes from the first sequence field's ids (0 = padding);
+    an empty history keeps its last slot.  Unknown keyword arguments are accepted and ignored, as the reference's
+    **kwargs are.  Refused: shapes outside functional.transact_bound, md % num_heads != 0 (the reference's assert),
+    use_time_window_mask=True and first_k_cols outside [1, max_len] (neither trains in the reference), a DCN input
+    whose width the reference's formula gets wrong, lazy tables and enable_sharding(want_fm=True)."""
+    _routes_sharded_front = True
+
+    def __init__(self, feature_map, model_id="TransAct", gpu=-1, hidden_activations="ReLU", dcn_cross_layers=3,
+                 dcn_hidden_units=[256, 128, 64], mlp_hidden_units=[], num_heads=1, transformer_layers=1,
+                 transformer_dropout=0, dim_feedforward=512, learning_rate=1e-3, embedding_dim=64, net_dropout=0,
+                 batch_norm=False, target_item_field=[("item_id", "cate_id")],
+                 sequence_item_field=[("click_history", "cate_history")], first_k_cols=1, use_time_window_mask=False,
+                 time_window_ms=86400000, concat_max_pool=True, embedding_regularizer=None, net_regularizer=None,
+                 **kwargs):
+        # a tuple of fields may arrive as a list (a JSON or YAML config)
+        as_list = lambda v: [tuple(f) if isinstance(f, list) else f for f in (v if isinstance(v, list) else [v])]  # noqa
+        targets, sequences = as_list(target_item_field), as_list(sequence_item_field)
+        if use_time_window_mask:
+            raise NotImplementedError("TransAct use_time_window_mask=True is not supported: the reference's forward "
+                                      "never passes time_interval_seq, so its mask compares None with an int")
+        specs = feature_map.features
+        dims, width = [], feature_map.sum_emb_out_dim()
+        for sequence, target in zip(sequences, targets):
+            snames, tnames = list(_flatten([sequence])), list(_flatten([target]))
+            md = embedding_dim * (len(snames) + len(tnames))
+            L = int(specs[snames[0]]["max_len"])
+            if not 1 <= first_k_cols <= L:
+                raise NotImplementedError("TransAct first_k_cols=%d is not supported: it must lie in [1, max_len = %d] "
+                                          "(the reference sizes its output for first_k_cols slots but takes at most "
+                                          "max_len)" % (first_k_cols, L))
+            assert md % num_heads == 0, "embed_dim must be divisible by num_heads"
+            bound = F2.transact_bound(L, md, num_heads, len(snames) + len(tnames))
+            if bound is not None:
+                raise NotImplementedError("TransAct kernels: " + bound)
+            dims.append(md)
+            width += (first_k_cols + int(concat_max_pool)) * md - embedding_dim * len(snames)
+        names = list(_flatten(sequences))
+        if len(set(names)) != len(names) or any(specs[f]["type"] != "sequence" for f in names):
+            raise NotImplementedError("TransAct: every sequence field must be a sequence feature of one pair only (the "
+                                      "reference sizes the DCN input for each pair's fields but pops each once)")
+        super(TransAct, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                       embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                       **kwargs)
+        self.target_item_field, self.sequence_item_field = targets, sequences
+        self.feature_map = feature_map
+        self.embedding_dim = embedding_dim
+        self.embedding_layer = FeatureEmbeddingDict(feature_map, embedding_dim)
+        self.transformer_encoders = nn.ModuleList()
+        for md in dims:
+            self.transformer_encoders.append(
+                TransActTransformer(md, dim_feedforward=dim_feedforward, num_heads=num_heads,
+                                    dropout=transformer_dropout, transformer_layers=transformer_layers,
+                                    use_time_window_mask=use_time_window_mask, time_window_ms=time_window_ms,
+                                    first_k_cols=first_k_cols, concat_max_pool=concat_max_pool))
+        self.crossnet = CrossNetV2(width, dcn_cross_layers)
+        self.parallel_dnn = MLP_Block(input_dim=width, output_dim=None, hidden_units=dcn_hidden_units,
+                                      hidden_activations=hidden_activations, output_activation=None,
+                                      dropout_rates=net_dropout, batch_norm=batch_norm)
+        self.mlp = MLP_Block(input_dim=width + dcn_hidden_units[-1], output_dim=1, hidden_units=mlp_hidden_units,
+                             hidden_activations=hidden_activations, output_activation=self.output_activation)
+        self._finish(kwargs, learning_rate)
+
+    def enable_sharding(self, group, batch_local, matrix_width, idx_dtype=torch.float64, want_fm=False):
+        """RankModel.enable_sharding without the FM term, which TransAct does not have."""
+        if want_fm:
+            raise ValueError("TransAct has no FM term: enable_sharding(..., want_fm=False)")
+        return super(TransAct, self).enable_sharding(group, batch_local, matrix_width, idx_dtype=idx_dtype,
+                                                     want_fm=False)
+
+    def _logit_mlp(self):
+        """mlp without its output Sigmoid (the same modules, not registered a second time)."""
+        ent = self.__dict__.get("_logit_head")
+        if ent is None:
+            ent = MLP_Block.__new__(MLP_Block)
+            nn.Module.__init__(ent)
+            mods = list(self.mlp.mlp)
+            ent.mlp = nn.Sequential(*(mods[:-1] if type(mods[-1]) == nn.Sigmoid else mods))
+            self.__dict__["_logit_head"] = ent
+        return ent
+
+    def dcn_input(self, inputs):
+        """The DCN input (B, width): the embeddings left after the sequence fields are dropped, in FeatureMap order,
+        then each pair's transformer output."""
+        X = self.get_inputs(inputs)
+        front = getattr(self, "_sharded_front", None)
+        if front is not None:       # row-sharded tables: (B, D) / (B, L, D) views of the landed rows
+            from .sharded import sharded_front
+            landed, _ = sharded_front(front, self._batch_matrix(inputs))
+            views = front.field_views(landed)
+            emb = OrderedDict((name, views[name]) for name in self.feature_map.features.keys() if name in views)
+        else:
+            emb = self.embedding_layer(X)
+        outs = []
+        for enc, target, sequence in zip(self.transformer_encoders, self.target_item_field, self.sequence_item_field):
+            tnames, snames = list(_flatten([target])), list(_flatten([sequence]))
+            outs.append(enc.run([emb[n] for n in snames], [emb[n] for n in tnames], X[snames[0]]))
+        for name in _flatten(self.sequence_item_field):
+            if self.feature_map.features[name]["type"] == "sequence":
+                emb.pop(name, None)
+        return torch.cat(list(emb.values()) + outs, dim=-1)
+
+    def forward_logits(self, inputs):
+        x = self.dcn_input(inputs)
+        return (self._logit_mlp()(torch.cat([self.crossnet(x), self.parallel_dnn(x)], dim=-1)),)
 
     def forward(self, inputs):
         return {"y_pred": self.output_activation(self.forward_logits(inputs)[0])}

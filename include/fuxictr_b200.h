@@ -649,6 +649,66 @@ B2_API int b2_bst_pool_bwd(const float* g, int64_t ld_g, const uint8_t* valid, i
                            float* dx, void* stream);
 
 /*
+ * TransAct (model_zoo/TransAct/src/TransAct.py): a post-norm nn.TransformerEncoder over the L = max_len early-fusion
+ * tokens of a (target, sequence) pair.  All row-major fp32.  Token b L + t of X (B L, md), md = D (ns + nt), is
+ * [seq_0[b, t] .. seq_{ns-1}[b, t] | tgt_0[b] .. tgt_{nt-1}[b]].  valid (B, L) bytes: 1 where the first sequence
+ * field's id is non-zero, and the last slot of a sample with no such slot (TransActTransformer.adjust_mask).  A layer
+ * on X, with the caller's GEMMs (bias in their epilogues) and bst.cu's add-norm:
+ *   QKV = X W_in^T + b_in (B L, 3 md)            columns [Q | K | V], head h the columns h dh .. h dh + dh - 1
+ *   ctx = b2_transact_attn_fwd(QKV)              per head: dropout(softmax((q scale) k^T + mask)) v, scale =
+ *                                                sqrt(1 / dh) as the caller rounds it; key j masked iff !valid[b, j]
+ *   s   = b2_bst_addnorm_fwd(ctx W_o^T + b_o, X)  norm1(X + dropout1(.))
+ *   out = b2_bst_addnorm_fwd(FFN(s), s)           norm2(s + dropout2(W2 dropout(relu(W1 s + b1)) + b2))
+ * The attention skips padded query rows: their ctx, dQ, dK and dV rows are 0 (the model zeroes those rows, and as
+ * keys they are masked in every layer).  Saved for the backward: QKV, ctx and the softmax max and sum per (b, h, i)
+ * (stat_max, stat_sum (B, H, L)); no (B H, L, L) tensor is stored.  Attention dropout drops weight (b, h, i, j) with
+ * the mask of "Dropout masks" over the (B H L, L) weights, at counter offset snapshot offset + drop_layer.  Every
+ * output with an aux argument (row pitch ld_aux) also receives its GEMM operand copy: bf16 rounding (aux_dtype
+ * B2_BF16) or 3xTF32 small part (B2_F32).
+ * Range: 1 <= L <= B2_TRANSACT_MAX_LEN, 1 <= md <= B2_TRANSACT_MAX_DIM, 1 <= heads <= B2_TRANSACT_MAX_HEADS dividing
+ * md with dh = md / heads <= B2_TRANSACT_MAX_HEAD_DIM, ns, nt >= 1 with ns + nt <= B2_TRANSACT_MAX_PARTS,
+ * 1 <= k <= L, batch >= 0 (0: no launch) with batch L < 2^31.  Shared memory holds tiles of 32 rows of dh (+ 1)
+ * floats, independent of L.  Outside the range, or given a NULL pointer, every entry point returns B2_E_INVALID.
+ * b2_transact_tokens_fwd: X "=" from ns sequence views seq[f] (B, L, D; sample b at seq[f] + b seq_ld[f], its tokens
+ *   contiguous) and nt target views tgt[f] (B, D; row pitch tgt_ld[f]) (host arrays of ns / nt entries), and valid
+ *   "=" from ids (B, L; row pitch ld_ids; B2_F64, B2_I64, B2_I32 or B2_F32), in one launch.
+ * b2_transact_tokens_bwd: from G (B L, md): dseq[f] (B, L, D) "=" and dtgt[f] (B, D) "=" the sum over t (host arrays
+ *   of device pointers, contiguous); no float atomics.
+ * b2_transact_attn_fwd: ctx (B L, md) and the statistics "=".
+ * b2_transact_attn_bwd: dQKV (B L, 3 md) "=" [dQ | dK | dV] from dctx and the saved tensors, in two launches: dQ
+ *   query-block outer (also delta (B, H, L) "=" dO_i . O_i, a workspace), then dK and dV key-block outer; no float
+ *   atomics.
+ * b2_transact_out_fwd: last (B, k md) "=" the last k slots of y (B L, md), 0 where padded; maxv (B, md) "=" the max
+ *   over L of y with padded slots at -1e9 and argmax (B, md) its slot, the first on ties (NULL, NULL: no pooling).
+ * b2_transact_out_bwd: dy (B L, md) "=" from dlast and dmax (NULL: no pooling) through argmax; 0 at padded slots.
+ */
+#define B2_TRANSACT_MAX_LEN 256
+#define B2_TRANSACT_MAX_DIM 512
+#define B2_TRANSACT_MAX_HEAD_DIM 256
+#define B2_TRANSACT_MAX_HEADS 16
+#define B2_TRANSACT_MAX_PARTS 8
+B2_API int b2_transact_tokens_fwd(const float* const* seq, const int64_t* seq_ld, int ns, const float* const* tgt,
+                                  const int64_t* tgt_ld, int nt, const void* ids, int ids_dtype, int64_t ld_ids,
+                                  int64_t batch, int L, int D, float* tok, void* tok_aux, int aux_dtype,
+                                  int64_t ld_aux, uint8_t* valid, void* stream);
+B2_API int b2_transact_tokens_bwd(const float* g, int64_t batch, int L, int D, int ns, int nt, float* const* dseq,
+                                  float* const* dtgt, void* stream);
+B2_API int b2_transact_attn_fwd(const float* qkv, const uint8_t* valid, int64_t batch, int L, int md, int heads,
+                                float scale, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                                float drop_scale, float* ctx, void* ctx_aux, int aux_dtype, int64_t ld_aux,
+                                float* stat_max, float* stat_sum, void* stream);
+B2_API int b2_transact_attn_bwd(const float* qkv, const uint8_t* valid, const float* ctx, const float* dctx,
+                                const float* stat_max, const float* stat_sum, int64_t batch, int L, int md, int heads,
+                                float scale, const int64_t* drop_rng, int64_t drop_layer, uint32_t drop_thresh,
+                                float drop_scale, float* delta, float* dqkv, void* dqkv_aux, int aux_dtype,
+                                int64_t ld_aux, void* stream);
+B2_API int b2_transact_out_fwd(const float* y, const uint8_t* valid, int64_t batch, int L, int md, int k, float* last,
+                               float* maxv, int32_t* argmax, void* max_aux, int aux_dtype, int64_t ld_aux,
+                               void* stream);
+B2_API int b2_transact_out_bwd(const float* dlast, const float* dmax, const int32_t* argmax, const uint8_t* valid,
+                               int64_t batch, int L, int md, int k, float* dy, void* stream);
+
+/*
  * DIEN, the Deep Interest Evolution Network (model_zoo/DIEN/src/DIEN.py): the interest extractor (nn.GRU), the
  * attention between the interests and the target, and the interest-evolution GRU (AUGRU, AGRU or nn.GRU) over a
  * behaviour sequence.  All row-major fp32.
