@@ -19,6 +19,7 @@
 // atomics.  Each kernel waits for its predecessor (programmatic dependent launch) before its first read and never
 // triggers its successor early.
 #include "b2_common.cuh"
+#include "lsh_common.cuh"
 
 #define LSH_THREADS 256
 #define LSH_WARPS (LSH_THREADS / 32)
@@ -30,30 +31,6 @@ static int lsh_check(int64_t batch, int L, int d) {
   B2_REQUIRE(batch >= 0, "LSH: negative batch %lld", (long long) batch);
   B2_REQUIRE(batch * (L + 1) < ((int64_t) 1 << 31), "LSH: batch (L + 1) must stay below 2^31");
   return B2_OK;
-}
-
-// Code word w (bits [32 w, min(32 w + 32, nbits))) of row v under R (d rows of pitch ldr; column c0 + j is bit j).
-__device__ __forceinline__ uint32_t lsh_word(const float* __restrict__ v, const float* sR, int d, int ldr, int c0,
-                                             int nbits) {
-  float acc[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-  for (int i = 0; i < d; ++i) {
-    const float vi = __ldg(v + i);
-    const float* r = sR + i * ldr + c0;
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < nbits) acc[j] = fmaf(vi, r[j], acc[j]);
-  }
-  uint32_t code = 0;
-#pragma unroll
-  for (int j = 0; j < 32; ++j)
-    if (j < nbits && acc[j] > 0.f) code |= 1u << j;
-  return code;
-}
-
-__device__ __forceinline__ void lsh_stage(const float* __restrict__ R, int n, float* sR) {
-  for (int e = threadIdx.x; e < n; e += blockDim.x) sR[e] = __ldg(R + e);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -3373,6 +3373,197 @@ def sdim_interest(item_emb, mask, rotations, short_seq_len, l2_norm, num_heads, 
 
 
 # --------------------------------------------------------------------------------------
+# LongCTR interest block: MIRRN's three SimHash retrievals and FilterLayer2 blocks
+# --------------------------------------------------------------------------------------
+MIRRN_FILTER_DROPOUT = 0.1      # FilterLayer2's out_dropout, hard-coded in MIRRN.__init__
+MIRRN_LN_EPS = 1e-12            # FilterLayer2's TF-style LayerNorm
+
+
+def mirrn_bound(d, L, topk, hash_bits, batch=1):
+    """None when the MIRRN kernels cover item width d, history length L, topk and hash_bits, else the bound it
+    breaks."""
+    msg = _lsh_common_bound(batch, d, L)
+    if msg is not None:
+        return msg
+    if d % 4:
+        return "the item width d (item_info_dim) must be a multiple of 4 (FilterLayer2's four blocks), got %d" % d
+    if not 1 <= hash_bits <= _lib.B2_MIRRN_MAX_BITS:
+        return "hash_bits must lie in [1, %d], got %d" % (_lib.B2_MIRRN_MAX_BITS, hash_bits)
+    if not 1 <= topk <= _lib.B2_LSH_MAX_TOPK:
+        return "topk must lie in [1, %d], got %d" % (_lib.B2_LSH_MAX_TOPK, topk)
+    k = min(topk, L)
+    G = 256 // d
+    retrieve = 4 * 3 * d * hash_bits + 8 * G * d + 8 * d + 12 * (hash_bits + 2) + 24 + 3 * L
+    if retrieve > _lib.B2_LSH_MAX_SMEM:
+        return "d hash_bits = %d needs more shared memory than a CTA has" % (d * hash_bits)
+    if 8 * k * d + 8 * k + 8 * G * d > _lib.B2_LSH_MAX_SMEM:
+        return "k d = %d needs more shared memory than a CTA has" % (k * d)
+    return None
+
+
+def mirrn_filter_table(k):
+    """First column h (k,) float64 of FilterLayer2's circulant at FFT length k: irfft(rfft(u) (a + i b), n=k, ortho)
+    = a u + b (H u) with (H u)_t = sum_s h[(t - s) mod k] u_s and h[m] = -(2 / k) sum_{f=1}^{ceil(k/2)-1}
+    sin(2 pi f m / k).  The DC and Nyquist bins drop out of the sum because irfft ignores their imaginary parts."""
+    m = torch.arange(k, dtype=torch.float64)
+    h = torch.zeros(k, dtype=torch.float64)
+    for f in range(1, (k + 1) // 2):
+        h -= torch.sin(2 * math.pi * f * m / k)
+    return h * (2.0 / k)
+
+
+_MIRRN_TABLES = {}
+
+
+def _mirrn_table(k, dev):
+    key = (k, str(dev))
+    h = _MIRRN_TABLES.get(key)
+    if h is None:
+        h = _MIRRN_TABLES[key] = mirrn_filter_table(k).float().to(dev)
+    return h
+
+
+class _MirrnInterest(torch.autograd.Function):
+    """MIRRN.forward's interest block (MIRRN.py:149-196) over item_feat_emb x (B, L + 1, d) as one node: the short
+    target attention over the window; three SimHash retrievals (b2_mirrn_retrieve_fwd); per retrieval the gathered
+    rows plus 0.02 pos[L - idx] through FilterLayer2 (b2_mirrn_filter_fwd, then b2_bst_addnorm_fwd with eps 1e-12 and
+    the Philox dropout), their mean over the k slots (b2_mirrn_mean_fwd); the long target attention over the three
+    interests, unmasked.  Returns (target, short interest, long interest, positions (B, 3, k)).  The backward runs the
+    attentions', add-norms' and filters' backwards and one assembly launch (b2_mirrn_assemble_bwd) that writes dx
+    once."""
+
+    @staticmethod
+    def forward(ctx, x, mask_u8, R, r_stride, cfg, pos_table, *params):
+        S, k, heads, use_scale, drop = cfg
+        x = _f32c(x)
+        B, L1, d = x.shape
+        L = L1 - 1
+        dev = x.device
+        ctx.empty = B == 0
+        if B == 0:                  # nothing to launch; every gradient is empty or zero
+            ctx.shape = (L, d)
+            empty = torch.empty((0, d), dtype=torch.float32, device=dev)
+            pos = torch.empty((0, 3, k), dtype=torch.int32, device=dev)
+            ctx.mark_non_differentiable(pos)
+            return empty, empty.clone(), empty.clone(), pos
+        ws, wl = params[:4], params[4:8]
+        cws, gammas, betas = params[8:11], params[11:14], params[14:17]
+        target = x[:, L].contiguous()
+        hs, ms = _short_window(x, mask_u8, S)
+        short, sctx = _mhta_fwd(target, hs, ms, heads, _mhta_scale(ws, d, heads, use_scale), ws)
+        pos = torch.empty((B, 3, k), dtype=torch.int32, device=dev)
+        _lib.call("b2_mirrn_retrieve_fwd", _ptr(x), _ptr(mask_u8), _ptr(R), r_stride, B, L, d, R.shape[-1], k,
+                  _ptr(pos), _stream())
+        htab = _mirrn_table(k, dev)
+        pos_table = _f32c(pos_table)
+        cws = tuple(_f32c(w) for w in cws)
+        u = torch.empty((3, B * k, d), dtype=torch.float32, device=dev)
+        y = torch.empty_like(u)
+        _lib.call("b2_mirrn_filter_fwd", _ptr(x), _ptr(pos), _ptr(pos_table), pos_table.shape[0], *map(_ptr, cws),
+                  _ptr(htab), B, L, d, k, _ptr(u), _ptr(y), _stream())
+        z = torch.empty_like(u)
+        mean = torch.empty((3, B * k), dtype=torch.float32, device=dev)
+        rstd = torch.empty_like(mean)
+        for q in range(3):
+            _lib.call("b2_bst_addnorm_fwd", _ptr(y[q]), _ptr(u[q]), B * k, d, _ptr(gammas[q]), _ptr(betas[q]),
+                      MIRRN_LN_EPS, *_drop_args(drop[q]), _ptr(z[q]), *_aux_args(None), _ptr(mean[q]), _ptr(rstd[q]),
+                      _stream())
+        interests = torch.empty((B, 3, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_mirrn_mean_fwd", _ptr(z), B, d, k, _ptr(interests), _stream())
+        long, lctx = _mhta_fwd(target, interests, None, heads, _mhta_scale(wl, d, heads, use_scale), wl)
+        ctx.parts = (sctx, lctx, S, k, L, pos, u, y, mean, rstd, htab, drop, pos_table)
+        ctx.params = (cws, gammas, betas)
+        ctx.leaves = (params[8:11], pos_table)
+        ctx.mark_non_differentiable(pos)
+        return target, short, long, pos
+
+    @staticmethod
+    def backward(ctx, g_target, g_short, g_long, _):
+        if ctx.empty:
+            L, d = ctx.shape
+            dx = torch.zeros((0, L + 1, d), dtype=torch.float32, device=g_target.device)
+            return (dx,) + (None,) * 22
+        sctx, lctx, S, k, L, pos, u, y, mean, rstd, htab, drop, pos_table = ctx.parts
+        cws, gammas, betas = ctx.params
+        dt_s, dx_s, dws = _mhta_bwd(sctx, _f32c(g_short))
+        dt_l, dint, dwl = _mhta_bwd(lctx, _f32c(g_long))
+        B, d = dt_s.shape
+        dev = dt_s.device
+        dz = torch.empty((3, B * k, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_mirrn_mean_bwd", _ptr(dint), B, d, k, _ptr(dz), _stream())
+        dgam = [_grad_buffer(p, zero=True) for p in gammas]
+        dbet = [_grad_buffer(p, zero=True) for p in betas]
+        dy = torch.empty_like(dz)
+        dropping = any(dq is not None for dq in drop)
+        dres = torch.empty_like(dz) if dropping else dy     # without dropout the residual's gradient is dy itself
+        for q in range(3):
+            _lib.call("b2_bst_addnorm_bwd", _ptr(y[q]), _ptr(u[q]), _ptr(dz[q]), None, B * k, d, _ptr(gammas[q]),
+                      _ptr(mean[q]), _ptr(rstd[q]), *_drop_args(drop[q]), _ptr(dy[q]), *_aux_args(None),
+                      _ptr(dres[q] if dropping else None), _ptr(dgam[q]), _ptr(dbet[q]), _stream())
+        dcw = [_grad_buffer(p, zero=True) for p in ctx.leaves[0]]
+        dpos = _grad_buffer(ctx.leaves[1], zero=True)
+        du = torch.empty_like(dz)
+        _lib.call("b2_mirrn_filter_bwd", _ptr(dy), _ptr(dres), _ptr(u), _ptr(pos), pos_table.shape[0],
+                  *map(_ptr, cws), _ptr(htab), B, L, d, k, _ptr(du), *map(_ptr, dcw), _ptr(dpos), _stream())
+        g_target = _f32c(g_target)
+        dx = torch.empty((B, L + 1, d), dtype=torch.float32, device=dev)
+        _lib.call("b2_mirrn_assemble_bwd", _ptr(g_target), _ptr(dt_s), _ptr(dt_l), _ptr(dx_s), S, _ptr(du),
+                  _ptr(pos), B, L, d, k, _ptr(dx), _stream())
+        return (dx, None, None, None, None, dpos) + dws + dwl + tuple(dcw) + tuple(dgam) + tuple(dbet)
+
+
+def mirrn_interest(item_emb, mask, rotations, short_seq_len, topk, num_heads, use_scale, short_weights, long_weights,
+                   pos_table, complex_weights, ln_weights, ln_biases, dropout=0.0):
+    """MIRRN's interest block: item_emb (B, L + 1, d) (the last position the target), mask (B, L) (non-zero = valid),
+    rotations (d, hash_bits) shared by the three retrievals or (3, d, hash_bits) one set per retrieval (target, short,
+    global); short_weights and long_weights the (W_q, W_k, W_v, W_o) of the two attentions; pos_table (max_len + 1, d)
+    the position embedding; complex_weights, ln_weights, ln_biases the three FilterLayer2 blocks' complex_weight
+    (4, d / 4, d / 4, 2) and LayerNorm weight and bias (d).  dropout: the blocks' out_dropout probability, one for
+    all three or one per block (0: none), drawn from the Philox masks (block q at layer q of one snapshot).  Returns
+    (target, short interest, long interest, positions): three (B, d) and the retrieved history positions (B, 3, k)
+    int32, k = min(topk, L), each row in ascending position order.  Ties at equal distance go to the lower
+    position."""
+    _require_cuda(rotations, pos_table)
+    mask_u8, B, L, d = _longctr_inputs("MIRRN", item_emb, mask, short_seq_len)
+    R = rotations
+    if R.dim() == 2:
+        R3 = R.unsqueeze(0)
+    elif R.dim() == 3 and R.shape[0] == 3:
+        R3 = R
+    else:
+        R3 = None
+    if R3 is None or R3.shape[1] != d:
+        raise ValueError("MIRRN: rotations%s must be (d, hash_bits) or (3, d, hash_bits) with d = %d"
+                         % (tuple(R.shape), d))
+    R3 = _f32c(R3)
+    r_stride = 0 if R.dim() == 2 else R3[0].numel()
+    bound = mirrn_bound(d, L, topk, R3.shape[-1], B)
+    if bound is not None:
+        raise NotImplementedError("MIRRN kernels: " + bound)
+    if pos_table.dim() != 2 or pos_table.shape[1] != d:
+        raise ValueError("MIRRN: pos_table%s must be (max_len + 1, %d)" % (tuple(pos_table.shape), d))
+    if L >= pos_table.shape[0]:
+        raise ValueError("MIRRN: the history length L = %d exceeds max_len = %d (the position embedding has rows "
+                         "0 .. max_len and the reference indexes row L - idx)" % (L, pos_table.shape[0] - 1))
+    filt = tuple(complex_weights) + tuple(ln_weights) + tuple(ln_biases)
+    if len(filt) != 9 or any(tuple(w.shape) != (4, d // 4, d // 4, 2) for w in complex_weights) \
+            or any(w.numel() != d for w in tuple(ln_weights) + tuple(ln_biases)):
+        raise ValueError("MIRRN: three complex_weight (4, d / 4, d / 4, 2) and three LayerNorm weights and biases (d) "
+                         "are needed, d = %d" % d)
+    for w in tuple(short_weights) + tuple(long_weights) + filt:
+        _require_cuda(w)
+    ps = [float(p) for p in dropout] if isinstance(dropout, (list, tuple)) else [float(dropout)] * 3
+    if len(ps) != 3:
+        raise ValueError("MIRRN: dropout must be one probability or one per filter block (3), got %d" % len(ps))
+    drop = [None] * 3
+    if any(p > 0 for p in ps):
+        snap = dropout_snapshot(item_emb.device, 3)
+        drop = [(snap, q) + dropout_consts(p) if p > 0 else None for q, p in enumerate(ps)]
+    cfg = (short_seq_len - 1, min(topk, L), num_heads, use_scale, drop)
+    return _MirrnInterest.apply(item_emb, mask_u8, R3, r_stride, cfg, pos_table, *short_weights, *long_weights, *filt)
+
+
+# --------------------------------------------------------------------------------------
 # LongCTR interest blocks: SIM's soft-search retrieval and TWIN's top-k attention
 # --------------------------------------------------------------------------------------
 def _topk_common_bound(batch, d, L, topk):

@@ -1009,6 +1009,31 @@ class MultiHeadTopKAttention(nn.Module):
                                   "functional.twin_interest on item_feat_emb (B, L + 1, d) with the target last")
 
 
+class FilterLayer2(nn.Module):
+    """model_zoo/LongCTR/MIRRN/MIRRN.py, FilterLayer2: LN(dropout(irfft(rfft(u) W, n=k)) + u) over the k retrieved rows
+    u (B, k, d), FFTs along the slot axis.  The reference's einsum keeps the diagonal of each of the n_block blocks of
+    complex_weight, so the filter is one complex weight per channel and needs no FFT on the device
+    (functional.mirrn_filter_table).  complex_weight (n_block, d / n_block, d / n_block, 2), out_dropout and the
+    TF-style LayerNorm child (eps 1e-12, nn.LayerNorm's formula) keep the reference's registration order, state_dict
+    keys and initial draws.  It runs inside MIRRN's interest block (functional.mirrn_interest), which needs
+    n_block = 4."""
+
+    def __init__(self, max_length, hidden_size, hidden_dropout_prob, n_block):
+        super(FilterLayer2, self).__init__()
+        if n_block != 4 or hidden_size % n_block:
+            raise NotImplementedError("FilterLayer2 kernels: n_block must be 4 and divide hidden_size, got n_block %d, "
+                                      "hidden_size %d" % (n_block, hidden_size))
+        self.complex_weight = nn.Parameter(
+            torch.randn(n_block, hidden_size // n_block, hidden_size // n_block, 2, dtype=torch.float32) * 0.02)
+        self.out_dropout = nn.Dropout(hidden_dropout_prob)
+        self.LayerNorm = nn.LayerNorm(hidden_size, eps=F2.MIRRN_LN_EPS)
+        self.n = n_block
+
+    def forward(self, input_tensor):
+        raise NotImplementedError("FilterLayer2 runs inside MIRRN's interest block: call functional.mirrn_interest on "
+                                  "item_feat_emb (B, L + 1, d) with the target last")
+
+
 class MultiHeadSelfAttention(nn.Module):
     """model_zoo/AutoInt/src/AutoInt.py, MultiHeadSelfAttention: field-wise multi-head self-attention with an optional
     residual (X, or X W_res^T when input_dim != attention_dim), LayerNorm and a final ReLU.  One autograd node per layer

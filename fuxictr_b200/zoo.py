@@ -23,6 +23,7 @@ same RNG consumption) and nothing else.
   DIEN         model_zoo/DIEN/src/DIEN.py
   TransAct     model_zoo/TransAct/src/TransAct.py
   ETA, SDIM    model_zoo/LongCTR/ETA/ETA.py, model_zoo/LongCTR/SDIM/SDIM.py
+  MIRRN        model_zoo/LongCTR/MIRRN/MIRRN.py
   SIM, TWIN    model_zoo/LongCTR/SIM/SIM.py, model_zoo/LongCTR/TWIN/TWIN.py
   RankModel = the slice of BaseModel a training step touches,
              fuxictr/pytorch/models/rank_model.py:84-189, 307-323, 435-448
@@ -37,7 +38,7 @@ from .layers import (fused_front, front_plan, FeatureEmbedding, FeatureEmbedding
                      SerialMaskNet, ParallelMaskNet, MultiHeadSelfAttention, WuKongLayer, wukong_stack,
                      FeatureGating, FinalBlock, BehaviorTransformer, DynamicGRU, AttentionLayer, MaskedSumPooling,
                      DIN_Attention, Dice, CompressedInteractionNet, LogisticRegression, MultiHeadTargetAttention,
-                     MultiHeadTopKAttention, TransActTransformer, not_in_whitelist)
+                     MultiHeadTopKAttention, TransActTransformer, FilterLayer2, not_in_whitelist)
 from .arena import ParamArena, FusedAdam
 from . import functional as F2
 
@@ -1893,6 +1894,79 @@ class TWIN(_LongCTRModel):
         """(target, short, long, positions) of functional.twin_interest."""
         return F2.twin_interest(item_feat_emb, mask, self.short_seq_len, self.topk, self.short_attention.num_heads,
                                 _mhta_weights(self.short_attention), self.long_attention.weights())
+
+    def dnn_input(self, inputs):
+        emb_out, item_feat_emb, mask = self._item_inputs(inputs)
+        target, short, long, _ = self.interest(item_feat_emb, mask)
+        return torch.cat(([emb_out] if emb_out is not None else []) + [target, short, long], dim=-1)
+
+
+class MIRRN(_LongCTRModel):
+    """model_zoo/LongCTR/MIRRN/MIRRN.py, MIRRN: a short target attention over the last short_seq_len - 1 history items;
+    three SimHash retrievals of the topk history items nearest the target, the masked mean of the last 16 items and
+    the masked mean of the whole history, each kept in position order, shifted by 0.02 pos[L - idx], filtered by a
+    FilterLayer2 and averaged over the k slots; a long target attention over those three interests; the DNN reads
+    [batch embeddings, target, short, long].  The interest block is one autograd node on the kernels
+    (functional.mirrn_interest); ties at equal distance go to the lower history position.  Each FilterLayer2's
+    dropout (its own out_dropout.p, 0.1 as the reference hard-codes it) runs in training mode on the Philox masks.
+    reuse_hash=False draws three (d, hash_bits) rotations with torch.randn on the device every forward, in the order
+    target, short, global.  The frozen random_rotations stay outside the optimizer.  Unknown keyword arguments are
+    accepted and ignored.
+    Refusals: see _LongCTRModel, an item width not divisible by 4 (the reference fails at its first forward), a batch
+    with L > max_len, and shapes outside functional.mirrn_bound."""
+
+    def __init__(self, feature_map, model_id="MIRRN", gpu=-1, dnn_hidden_units=[512, 128, 64],
+                 dnn_activations="ReLU", attention_dim=64, num_heads=1, use_scale=True, attention_dropout=0,
+                 reuse_hash=True, hash_bits=32, topk=50, max_len=1000, learning_rate=1e-3, embedding_dim=10,
+                 net_dropout=0, batch_norm=False, short_seq_len=50, accumulation_steps=1, embedding_regularizer=None,
+                 net_regularizer=None, **kwargs):
+        super(MIRRN, self).__init__(feature_map, model_id=model_id, gpu=gpu,
+                                    embedding_regularizer=embedding_regularizer, net_regularizer=net_regularizer,
+                                    **kwargs)
+        self._longctr_init(feature_map, embedding_dim, short_seq_len, attention_dropout, accumulation_steps)
+        if self.item_info_dim % 4:
+            raise ValueError("MIRRN: item_info_dim = %d (the sum of the item features' embedding dims) must be "
+                             "divisible by 4, FilterLayer2's block count; the reference fails at its first forward"
+                             % self.item_info_dim)
+        bound = F2.mirrn_bound(self.item_info_dim, 1, topk, hash_bits)
+        if bound is not None:
+            raise NotImplementedError("MIRRN kernels: " + bound)
+        self.reuse_hash = reuse_hash
+        self.hash_bits = hash_bits
+        self.topk = topk
+        self.max_len = max_len
+        self.embedding_layer = FeatureEmbedding(feature_map, embedding_dim)
+        self.short_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                        attention_dropout, use_scale)
+        self.pos = nn.Embedding(max_len + 1, self.item_info_dim)
+        self.random_rotations = nn.Parameter(torch.randn(self.item_info_dim, self.hash_bits), requires_grad=False)
+        self.MHFT_block = nn.ModuleList([FilterLayer2(topk, self.item_info_dim, F2.MIRRN_FILTER_DROPOUT, 4)
+                                         for _ in range(3)])
+        self.long_attention = MultiHeadTargetAttention(self.item_info_dim, attention_dim, num_heads,
+                                                       attention_dropout, use_scale)
+        input_dim = feature_map.sum_emb_out_dim() + self.item_info_dim * 2
+        self.dnn = MLP_Block(input_dim=input_dim, output_dim=1, hidden_units=dnn_hidden_units,
+                             hidden_activations=dnn_activations, output_activation=self.output_activation,
+                             dropout_rates=net_dropout, batch_norm=batch_norm)
+        self._finish(kwargs, learning_rate)
+
+    def interest(self, item_feat_emb, mask):
+        """(target, short, long, positions) of functional.mirrn_interest."""
+        if mask.shape[1] > self.max_len:
+            raise ValueError("MIRRN: the history length L = %d exceeds max_len = %d (the reference's pos embedding "
+                             "has rows 0 .. max_len)" % (mask.shape[1], self.max_len))
+        if self.reuse_hash:
+            rotations = self.random_rotations
+        else:
+            rotations = torch.stack([torch.randn(self.item_info_dim, self.hash_bits, device=item_feat_emb.device)
+                                     for _ in range(3)])
+        blocks = self.MHFT_block
+        p = [b.out_dropout.p if self.training else 0.0 for b in blocks]
+        return F2.mirrn_interest(item_feat_emb, mask, rotations, self.short_seq_len, self.topk,
+                                 self.short_attention.num_heads, self.short_attention.scale is not None,
+                                 _mhta_weights(self.short_attention), _mhta_weights(self.long_attention),
+                                 self.pos.weight, [b.complex_weight for b in blocks],
+                                 [b.LayerNorm.weight for b in blocks], [b.LayerNorm.bias for b in blocks], p)
 
     def dnn_input(self, inputs):
         emb_out, item_feat_emb, mask = self._item_inputs(inputs)

@@ -807,6 +807,49 @@ B2_API int b2_sdim_assemble_bwd(const float* dt0, const float* dt1, const float*
                                 int d, int num_hashes, int l2norm, float* dx, void* stream);
 
 /*
+ * MIRRN (model_zoo/LongCTR/MIRRN/MIRRN.py): three SimHash retrievals over a long behaviour sequence and a FilterLayer2
+ * block on each.  x is item_feat_emb (B, L + 1, d) row-major fp32: positions [0, L) the history h, position L the
+ * target t; mask (B, L) bytes, non-zero = valid.  k = min(topk, L).  The retrieved rows, their filter outputs and
+ * their gradients u, y, du (3, B, k, d) hold retrieval q's rows as the contiguous (B k, d) block q.
+ * b2_mirrn_retrieve_fwd: queries t, the masked mean of h[:, L - min(16, L):] and the masked mean of all of h (each
+ *   hashed from its masked sum: the division by count + 1e-9 keeps every sign).  Bit j of a row is row . R_q[:, j] > 0
+ *   in fp32 FMA over ascending columns, R_q = R + q r_stride (r_stride 0: one (d, bits) set for all three, and the
+ *   history is hashed once).  dist_l = popc(code_l ^ code_q), 1 + bits where mask is 0.  topk_pos (B, 3, k) int32
+ *   "=" per query the k smallest, ties to the lower position, in ascending position order.
+ * b2_mirrn_filter_fwd: u[q, b, s] "=" x[b, p] + 0.02 pos_table[L - p] (p = topk_pos[b, q, s]; pos_table (pos_rows, d)
+ *   with pos_rows > L), y[q, b, s, c] "=" a_c u[q, b, s, c] + b_c sum_r htab[(s - r) mod k] u[q, b, r, c], with
+ *   (a_c, b_c) = cw_q[n, j, j, 0:2], c = n (d / 4) + j, cw_q the (4, d / 4, d / 4, 2) complex_weight of block q, htab
+ *   (k) the first column of the filter's circulant.  LN(u + dropout(y)) is b2_bst_addnorm_fwd on each block q.
+ * b2_mirrn_filter_bwd: from dy (the add-norm's da) and dres (its dres; dy itself without dropout): du "=" dres +
+ *   a dy - b (H dy); dcw_q[n, j, j, 0] "+=" sum dy u, dcw_q[n, j, j, 1] "+=" sum dy (H u), dpos[L - p] "+=" 0.02 du
+ *   (caller zeroes; float atomics: one per CTA and channel for dcw, one per element for dpos).
+ * b2_mirrn_mean_fwd / _bwd: out (B, 3, d) "=" the mean of z (3, B, k, d) over the k slots; dz "=" g / k.
+ * b2_mirrn_assemble_bwd: dx (B, L + 1, d) "=", every row written once, no atomics.  Row L = dt0 + dt1 + dt2 (each
+ *   (B, d)); rows [L - S, L) add dshort (B, S, d); row p adds du[q, b, s] for every (q, s) with topk_pos[b, q, s] = p,
+ *   in the order q = 0, 1, 2.
+ * Range: d a multiple of 4 in [4, B2_LSH_MAX_DIM], 1 <= L <= B2_LSH_MAX_LEN, 1 <= k <= min(L, B2_LSH_MAX_TOPK),
+ * 1 <= bits <= B2_MIRRN_MAX_BITS, batch (L + 1) < 2^31, batch >= 0 (0: no launch), 1 <= S <= L, and shared memory
+ * within B2_LSH_MAX_SMEM bytes: retrieval 4 nsets d bits + 8 (256 / d) d + 8 d + 12 (bits + 2) + 24 + 3 L (nsets 1 or
+ * 3), filter forward 4 k d + 8 k, backward 8 k d + 8 k + 8 (256 / d) d.  Outside the range, or given a NULL pointer,
+ * every entry point returns B2_E_INVALID.
+ */
+#define B2_MIRRN_MAX_BITS 64
+B2_API int b2_mirrn_retrieve_fwd(const float* x, const uint8_t* mask, const float* R, int64_t r_stride, int64_t batch,
+                                 int L, int d, int bits, int k, int32_t* topk_pos, void* stream);
+B2_API int b2_mirrn_filter_fwd(const float* x, const int32_t* topk_pos, const float* pos_table, int pos_rows,
+                               const float* cw0, const float* cw1, const float* cw2, const float* htab, int64_t batch,
+                               int L, int d, int k, float* u, float* y, void* stream);
+B2_API int b2_mirrn_filter_bwd(const float* dy, const float* dres, const float* u, const int32_t* topk_pos,
+                               int pos_rows, const float* cw0, const float* cw1, const float* cw2, const float* htab,
+                               int64_t batch, int L, int d, int k, float* du, float* dcw0, float* dcw1, float* dcw2,
+                               float* dpos, void* stream);
+B2_API int b2_mirrn_mean_fwd(const float* z, int64_t batch, int d, int k, float* out, void* stream);
+B2_API int b2_mirrn_mean_bwd(const float* g, int64_t batch, int d, int k, float* dz, void* stream);
+B2_API int b2_mirrn_assemble_bwd(const float* dt0, const float* dt1, const float* dt2, const float* dshort, int S,
+                                 const float* du, const int32_t* topk_pos, int64_t batch, int L, int d, int k,
+                                 float* dx, void* stream);
+
+/*
  * SIM / TWIN: learned-score top-k retrieval over a long behaviour sequence, SIM's soft-search GSU
  * (model_zoo/LongCTR/SIM/SIM.py) and TWIN's MultiHeadTopKAttention (model_zoo/LongCTR/TWIN/TWIN.py).  x is
  * item_feat_emb (B, L + 1, d) row-major fp32: positions [0, L) the history, position L the target; mask (B, L) bytes,
