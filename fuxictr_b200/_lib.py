@@ -36,6 +36,7 @@ B2_DIEN_GRU, B2_DIEN_AUGRU, B2_DIEN_AGRU = 0, 1, 2
 B2_LSH_MAX_DIM, B2_LSH_MAX_LEN, B2_LSH_MAX_TOPK, B2_LSH_MAX_SMEM = 256, 4096, 256, 227 * 1024 - 1024
 B2_ETA_MAX_BITS, B2_SDIM_MAX_BITS, B2_SDIM_MAX_HASHES = 64, 24, 32
 B2_MIRRN_MAX_BITS = 64
+B2_LONGCTR_PAD_PRE, B2_LONGCTR_PAD_POST, B2_LONGCTR_MAX_LEN, B2_LONGCTR_MAX_COLS = 0, 1, 1 << 20, 64
 B2_TOPK_MAX_DIM, B2_TOPK_MAX_LEN, B2_TOPK_MAX_K, B2_TOPK_MAX_SMEM = 256, 4096, 256, 220 * 1024
 FM_PRODUCT_SUM, FM_BI_INTERACTION, FM_INNER_PRODUCT = 0, 1, 2
 
@@ -270,6 +271,8 @@ SIGNATURES = {
     "b2_mirrn_mean_bwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "b2_mirrn_assemble_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64,
                                       c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b2_longctr_collate": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
+                                   c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2_sim_retrieve_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_sim_gsu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -850,6 +850,32 @@ B2_API int b2_mirrn_assemble_bwd(const float* dt0, const float* dt1, const float
                                  float* dx, void* stream);
 
 /*
+ * LongCTR input (model_zoo/LongCTR/longctr_dataloader.py, BatchCollator): the triple (batch_dict, item_dict, mask)
+ * built on the device from a store of user histories and item features held in HBM.
+ * b2_longctr_collate: batch (rows, row_stride) int64 or int32 (batch_dtype B2_I64 | B2_I32), the columns col_user,
+ *   col_item and col_seq_len holding each sample's user_index u, item_index t and seq_len.  The histories are CSR:
+ *   offsets (num_users + 1) int64, hist the flat int32 item ids, user u's history hist[offsets[u], offsets[u + 1]).
+ *   item_info (num_items, num_cols) row-major int32.  With n = min(seq_len, len(history of u)) and k = min(n, L),
+ *   slots [0, L) hold keras pad_sequences(maxlen = L, value = 0, padding = truncating = p) of the first n history
+ *   items: the last k, right-aligned (B2_LONGCTR_PAD_PRE), or the first k, left-aligned (B2_LONGCTR_PAD_POST), 0
+ *   elsewhere; slot L holds t.  mask (rows, L) fp32 "=" (id > 0) over slots [0, L); items (num_cols, rows (L + 1))
+ *   int64 "=", items[c, b (L + 1) + l] = item_info[id, c] (positional: a padding slot copies row 0).  One launch.
+ *   The caller guarantees 0 <= u < num_users, 0 <= t < num_items, seq_len >= 0 and every history id in
+ *   [0, num_items); these are not checked on the device.
+ * Range: 0 <= rows < 2^31 (0: no launch), 0 <= L <= B2_LONGCTR_MAX_LEN, 1 <= num_cols <= B2_LONGCTR_MAX_COLS, the
+ * three columns inside a row, num_users, num_items >= 1, mask may be NULL when L = 0.  Outside the range, or given a
+ * NULL pointer, returns B2_E_INVALID.
+ */
+#define B2_LONGCTR_PAD_PRE 0
+#define B2_LONGCTR_PAD_POST 1
+#define B2_LONGCTR_MAX_LEN (1 << 20)
+#define B2_LONGCTR_MAX_COLS 64
+B2_API int b2_longctr_collate(const void* batch, int batch_dtype, int64_t rows, int64_t row_stride, int col_user,
+                              int col_item, int col_seq_len, const int64_t* offsets, const int32_t* hist,
+                              int64_t num_users, const int32_t* item_info, int64_t num_items, int num_cols, int L,
+                              int padding, float* mask, int64_t* items, void* stream);
+
+/*
  * SIM / TWIN: learned-score top-k retrieval over a long behaviour sequence, SIM's soft-search GSU
  * (model_zoo/LongCTR/SIM/SIM.py) and TWIN's MultiHeadTopKAttention (model_zoo/LongCTR/TWIN/TWIN.py).  x is
  * item_feat_emb (B, L + 1, d) row-major fp32: positions [0, L) the history, position L the target; mask (B, L) bytes,
